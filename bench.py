@@ -1,6 +1,6 @@
-"""bench.py — VLP hot path throughput on B200 (driver contract: one JSON line on stdout from rank 0).
+"""bench.py — VLP hot path throughput on H100 (one JSON line on stdout from rank 0).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--config caption|vqa|ccmix] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--config caption|vqa|ccmix] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 Workloads (BASELINE.json `configs`), all BERT-base 12L/768H, 100 regions x 2048 + 20 tokens (L = 123), bf16, dropout 0.1 (the
@@ -18,8 +18,14 @@ scaling).  One step = one batch per GPU.
           pinned host memory -> device (bf16 features + 3 integers per sample for the mask, double-buffered on a copy stream) and the
           loss is read back to the host, all inside the timed region (host wall clock).
   optimizer : the same step including vlp_b200.optimization.BertAdam.step() (fused multi-tensor kernel), reported beside `value`.
-  roofline : dominant kernel family (tcgen05 GEMM), algorithmic FLOPs / CUDA-event time of its launches inside one real step.
+  roofline : dominant kernel family (wgmma GEMM), algorithmic FLOPs / CUDA-event time of its launches inside one real step.
   cpu_baseline : the fp32 oracle port (same unfused eager op sequence as the reference) on the host cores, bounded sample.
+
+  --dump-outputs DIR : after the timed steps, write what the last timed step returned to its caller as float32 .npy files: loss.npy
+          and, per parameter, grad.<name>.npy (all of a small gradient; of a larger one the DUMP_SAMPLE elements at the sorted flat
+          indices torch.randperm(numel, generator=g)[:DUMP_SAMPLE], g = torch.Generator().manual_seed(DUMP_SEED) drawn from in
+          named_parameters() order).  Inputs, weights and dropout seeds depend only on the arguments, so two builds can be compared
+          output for output.
 """
 import argparse
 import ctypes as C
@@ -55,7 +61,8 @@ def load_peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"], "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (dense BF16, 700 W card); not measured here
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
@@ -196,6 +203,35 @@ def step_fn(model, b, tasks):
     return loss
 
 
+DUMP_SAMPLE = 65536  # elements kept of each gradient larger than this (about 20 MB in all for BERT-base)
+DUMP_SEED = 20240607
+
+
+def dump_outputs(out_dir, loss, model):
+    """Write the loss and every parameter gradient of the last step (see --dump-outputs in the module docstring)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    total = 0
+
+    def save(name, t):
+        nonlocal total
+        a = t.detach().float().cpu().numpy()
+        total += a.nbytes
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+    save("loss", loss.reshape(()))
+    gen = torch.Generator().manual_seed(DUMP_SEED)
+    for name, p in model.named_parameters():
+        if p.grad is None:
+            continue
+        g = p.grad.reshape(-1)
+        if g.numel() > DUMP_SAMPLE:
+            idx = torch.randperm(g.numel(), generator=gen)[:DUMP_SAMPLE].sort().values
+            g = g[idx.to(g.device)]
+        save(f"grad.{name}", g)
+    assert total <= 64 << 20, f"--dump-outputs wrote {total} bytes"
+
+
 def pct(sorted_vals, q):
     return sorted_vals[min(len(sorted_vals) - 1, int(q * len(sorted_vals)))]
 
@@ -210,6 +246,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the optimizer-inclusive, exposed-communication and profile passes")
     ap.add_argument("--no-graph", action="store_true", help="drive every step from Python instead of replaying the captured CUDA graph (N = 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's loss and gradients as .npy files to DIR")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference_arm(args)
@@ -264,6 +301,8 @@ def main():
             opt.step()
         return loss
 
+    last = {}
+
     def timed_loop(n, opt=None, graphed=None):
         """n steps on the device-resident batch; returns (total ms, sorted per-step ms) from one CUDA event per step.
         graphed: a vlp_b200.graph.GraphedStep replayed instead of the Python-driven step (same kernels, same work)."""
@@ -274,11 +313,11 @@ def main():
         evs[0].record()
         for i in range(n):
             if graphed is not None:
-                graphed()
+                last["loss"] = graphed()
                 if opt is not None:
                     opt.step()
             else:
-                one_step(dev_batch, opt)
+                last["loss"] = one_step(dev_batch, opt)
             evs[i + 1].record()
         torch.cuda.synchronize()
         barrier()
@@ -329,8 +368,8 @@ def main():
             one_step(dev_batch)
 
     # The step (forward + backward + the reducer's collectives when N > 1) is captured once as a CUDA graph and replayed
-    # (vlp_b200.graph; same kernels, fresh dropout masks per replay): Python needs ~6 ms per step to enqueue the ~330 launches, and
-    # with N processes sharing the host it becomes the bottleneck (2 GPUs: 7.14 ms per step even with the all-reduce switched off).
+    # (vlp_b200.graph; same kernels, fresh dropout masks per replay): Python needs several ms per step to enqueue the ~330 launches,
+    # and with N processes sharing the host it can become the bottleneck.
     # torch-DDP runs (VLP_BENCH_DP=torch_ddp) and VLP_BENCH_GRAPH=0 stay Python-driven.
     use_graph = (not args.no_graph) and os.environ.get("VLP_BENCH_GRAPH", "1") != "0" and \
         (world == 1 or (reducer is not None and os.environ.get("VLP_BENCH_GRAPH_DP", "1") == "1"))
@@ -356,6 +395,8 @@ def main():
     with ClockSampler(local_rank) as clocks:
         ms_total, per_step = timed_loop(args.steps, graphed=gstep)
     launches = (gstep.launches_per_replay * args.steps) if gstep is not None else (L.lib().vlpk_launch_count() - launches0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["loss"], model)
     eager = None
     if gstep is not None and not args.no_extras:
         # the same loop driven from Python, for reference (host enqueue ~ device time: any host hiccup shows up here)
@@ -522,13 +563,8 @@ def main():
     keep_b = B * d.heads * d.seq_len * 16
     hbm_bytes = {"ln_fwd": prof["ln_fwd"]["work_per_step"], "ln_bwd": prof["ln_bwd"]["work_per_step"],
                  "attn_fwd": nl * (Mrows * Hh * 2 * 4 + keep_b), "attn_bwd": nl * (Mrows * Hh * 2 * 7 + keep_b)}
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")
-    if os.path.exists(tp):
-        tj = json.load(open(tp))
-        traffic, traffic_src = tj["gemm_dram_bytes_per_launch_avg"], "static: " + tj["source"]
-    roofline = {"bound": "tensor", "kernel": "vlpk::gemm_kernel (tcgen05 GEMM family: fwd/dgrad/wgrad)", "achieved": achieved, "peak": peak_tf,
-                "unit": "TFLOP/s", "frac": achieved / peak_tf, "traffic": traffic, "traffic_source": traffic_src,
+    roofline = {"bound": "tensor", "kernel": "vlpk::gemm_kernel (wgmma GEMM family: fwd/dgrad/wgrad)", "achieved": achieved, "peak": peak_tf,
+                "unit": "TFLOP/s", "frac": achieved / peak_tf,
                 "peak_source": f"MEASURED_PEAKS.json {'bf16_tflops_sustained' if capped else 'bf16_tflops (burst)'} ({peaks['source']}); "
                                f"{'run was power-capped / clocked down' if capped else 'run stayed at full clocks, no power cap'}",
                 "launches_per_step": gemm_n, "flops_per_launch_avg": gemm_fl / max(gemm_n, 1), "avg_launch_us": gemm_ms * 1e3 / max(gemm_n, 1),
@@ -547,7 +583,7 @@ def main():
             "config": {"workload": cfgw["workload"], "name": args.config, "global_batch": B * world, "seq_len": d.seq_len,
                        "parallelism": f"dp{world}" + ("" if world == 1 else (" torch-DDP" if reducer is None else
                                                                                " NCCL all-reduce of flat bf16 gradient arenas overlapped with backward")),
-                       "l2": "per-step working set (2.3 GB saved activations + 0.23 GB weights) is far larger than the 126 MB L2; no explicit flush",
+                       "l2": "per-step working set (2.3 GB saved activations + 0.23 GB weights) is far larger than the 50 MB L2; no explicit flush",
                        "timing": "CUDA events on the launch stream (one per step), barrier + synchronize both sides, max over ranks",
                        "launch": ("CUDA-graph replay of the captured step (vlp_b200.graph.GraphedStep): identical kernels, device-side seed counter "
                                   "bumped per replay for fresh dropout masks" if use_graph else "Python-driven launches")},

@@ -1,4 +1,4 @@
-/* vlpk.h — C ABI of libvlpk.so, the B200-native (sm_100a) replacement for VLP's data-parallel hot path.
+/* vlpk.h — C ABI of libvlpk.so, the H100-native (sm_90a) replacement for VLP's data-parallel hot path.
  *
  * The reference (LuoweiZhou/VLP) has no FFI layer: its operator API is the nn.Module surface of
  * pytorch_pretrained_bert/modeling.py.  Each entry point below replaces the eager-PyTorch body of one of
@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define VLPK_VERSION 101
+#define VLPK_VERSION 102
 
 /* dtype tags for vlpk_mask_pack */
 #define VLPK_BF16 0
@@ -107,14 +107,12 @@ typedef struct VlpkBwdScratch {
 
 int vlpk_version(void);
 const char* vlpk_last_error(void);
-/* bring-up / A-B testing only: force the GEMM CTA-group size (0 = cost model, 1 = single CTA tiles, 2 = CTA pairs). */
-void vlpk_debug_set_cta_group(int cg);
 /* Leave n SMs out of the persistent GEMM grids (and of the tile cost model) from now on; 0 restores the full machine.  For
  * data-parallel callers while a collective that owns SMs (NCCL all-reduce of the previous gradient arena) runs beside the
  * backward GEMMs: a grid sized for all SMs would have its last CTAs wait behind the collective's. */
 void vlpk_set_reserved_sms(int n);
-/* host-only: the (tile N, CTA-group size, split-K) the cost model picks for a GEMM; out3 = {bn, cg, splits}.  No GPU needed. */
-int vlpk_debug_plan_gemm(int M, int N, int K, int a_mn, int b_mn, int nseg, int seg_rows, int epi, int bn, int splits, int* out3);
+/* host-only: the (tile N, split-K) the cost model picks for a GEMM; out2 = {bn, splits}.  No GPU needed. */
+int vlpk_debug_plan_gemm(int M, int N, int K, int a_mn, int b_mn, int nseg, int seg_rows, int epi, int bn, int splits, int* out2);
 /* A-B testing only: switch a host-side scheduling choice at run time.  "wgrad_stream" (default 1, env VLPK_WGRAD_STREAM=0 turns it
  * off): the weight-gradient GEMM of each Linear's backward runs on a side stream behind its dgrad.  < 0: unknown name. */
 int vlpk_debug_set_option(const char* name, int value);

@@ -1,4 +1,4 @@
-"""ORACLE SUPPORT — imports the UNMODIFIED reference modules from /root/reference (build container only).
+"""ORACLE SUPPORT — imports the UNMODIFIED reference modules from the checkout at $VLP_REFERENCE_ROOT (golden-data generation only).
 
 `import pytorch_pretrained_bert` fails on a modern stack: file_utils.py:20-21 needs boto3/botocore,
 __init__.py:5-6 pulls optimization.py (torch._six, removed in torch 2) and optimization_fp16.py (apex).
@@ -7,7 +7,7 @@ modules, register an empty package object whose __path__ points at the reference
 __init__ is bypassed) and import pytorch_pretrained_bert.modeling.  Without apex the reference falls back to
 its own pure-PyTorch BertLayerNorm (modeling.py:179-192) — that is the arithmetic being pinned.
 
-Never imported by the product; never available on the GPU box (no /root/reference there).
+Never imported by the product or the tests: the tests compare with what oracle/make_golden.py stored under tests/golden/.
 """
 import os
 import pickle
@@ -15,16 +15,16 @@ import sys
 import tempfile
 import types
 
-REF_ROOT = os.environ.get("VLP_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("VLP_REFERENCE_ROOT", "")
 
 
 def available():
-    return os.path.isdir(os.path.join(REF_ROOT, "pytorch_pretrained_bert"))
+    return bool(REF_ROOT) and os.path.isdir(os.path.join(REF_ROOT, "pytorch_pretrained_bert"))
 
 
 def import_reference_modeling():
     if not available():
-        raise RuntimeError(f"reference not found under {REF_ROOT}")
+        raise RuntimeError(f"reference checkout not found (set VLP_REFERENCE_ROOT; got {REF_ROOT!r})")
     for name in ("boto3", "botocore", "botocore.exceptions"):
         sys.modules.setdefault(name, types.ModuleType(name))
     sys.modules["botocore.exceptions"].ClientError = Exception

@@ -2,14 +2,13 @@
 
 CPU restatement (plain PyTorch, fp32, eager, one op per reference op) of the algorithm on VLP's hot path,
 written from the reference's description of the computation; each function cites the reference lines it
-follows (paths relative to /root/reference).  Only tests/, __graft_entry__.smoke() and bench.py's CPU
+follows (paths relative to the reference checkout).  Only tests/, __graft_entry__.smoke() and bench.py's CPU
 baseline / `--impl reference` arm may import this module; vlp_b200 never does.
 
 Pinning: the reference ships no tests or golden vectors for this path (SURVEY.md §4, §8c), so this
 restatement is pinned against the reference ITSELF: oracle/make_golden.py imports the unmodified
-reference modules in the build container, runs them on the seeded inputs of vlp_b200/synth.py and commits
-their outputs under tests/golden/; tests/test_oracle.py checks this file against those vectors (and,
-when /root/reference is present, against the live reference).
+reference modules (checkout at $VLP_REFERENCE_ROOT), runs them on the seeded inputs of vlp_b200/synth.py and
+commits their outputs under tests/golden/; tests/test_oracle.py checks this file against those vectors.
 
 The model is a flat state dict with the reference's parameter names (SURVEY.md §8b); no nn.Module is
 involved, so nothing here can be mistaken for — or silently substituted into — the product path.

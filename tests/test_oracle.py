@@ -43,12 +43,17 @@ def test_oracle_matches_reference_golden(name, golden_dir):
     assert rel(aux["logits"], gold["logits"]) < 1e-5
     assert rel(aux["pooled"], gold["pooled"]) < 1e-5
     n = 0
+    # Some gradients are zero in exact arithmetic (the key bias: softmax ignores a per-row constant) and hold only fp32 round-off,
+    # whose pattern depends on the host's vector units; those must stay at round-off level relative to the gradient scale.
+    scale = max(float(fp["full"].norm()) if "full" in fp else fp["norm"] for fp in gold["grads"].values())
     for k, fp in gold["grads"].items():
         g = sd[k].grad
         assert g is not None, k
         if "full" in fp:
             if fp["full"].norm() == 0:
                 assert g.norm() == 0, k
+            elif fp["full"].norm() <= 1e-7 * scale:
+                assert g.norm() <= 1e-7 * scale, k
             else:
                 assert rel(g, fp["full"]) < 1e-4, k
         else:
@@ -78,21 +83,16 @@ def test_oracle_greedy_decode_matches_reference_golden(golden_dir):
     assert rel(scores, gold["scores"]) < 1e-5
 
 
-def test_oracle_matches_live_reference_when_present():
-    """In the build container the reference itself is importable: compare once more, live, incl. a fresh seed."""
-    from oracle import ref_shim
-    if not ref_shim.available():
-        pytest.skip("/root/reference not present (GPU box)")
+def test_oracle_matches_reference_loss_on_another_seed(golden_dir):
+    """One more case with fresh seeds (weights 3, ragged mixed-mask batch 99) vs the reference's stored loss
+    (oracle/make_golden.py run_mix_seed3)."""
+    gold = torch.load(os.path.join(golden_dir, "mix_seed3.pt"))
     dims = synth.SMALL_L123
     sd = synth.make_state_dict(dims, seed=3)
     batch = synth.make_batch(dims, 3, seed=99, mode="mix", ragged=True)
-    model = ref_shim.build_reference_model(dims, sd).eval()
     with torch.no_grad():
-        ref = model(batch["img"], batch["vis_pe"], batch["input_ids"], batch["segment_ids"], batch["input_mask"], batch["masked_ids"], None,
-                    batch["is_next"], masked_pos=batch["masked_pos"], masked_weights=batch["masked_weights"], task_idx=batch["task_idx"],
-                    vis_masked_pos=batch["vis_masked_pos"], mask_image_regions=False, drop_worst_ratio=0.0)
         got = O.pretraining_loss(sd, dims, batch)
-    assert abs(float(got[0]) - float(ref[0])) < 1e-5
+    assert abs(float(got[0]) - float(gold["loss"])) < 1e-5
 
 
 def _run_bertadam_oracle():

@@ -1,4 +1,4 @@
-"""Parity tests proper (GPU): the sm_100a path behind the reference's Python surface vs (a) the reference's own
+"""Parity tests proper (GPU): the sm_90a path behind the reference's Python surface vs (a) the reference's own
 outputs stored under tests/golden/ and (b) the fp32 oracle run live on the host CPU.
 
 Stated tolerance for bf16 kernels vs the fp32 reference (BASELINE.md §3 / SURVEY.md §8c, derived from the reference's

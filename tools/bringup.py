@@ -1,5 +1,5 @@
 """GPU bring-up harness: runs each kernel family in its own subprocess (a device trap must not take the
-other checks down), compares with plain PyTorch fp32 math, and writes gpurun_out/bringup.log.
+other checks down), compares with plain PyTorch fp32 math, and prints one report per case.
 
     python tools/bringup.py            # run everything
     python tools/bringup.py gemm_kk    # one case in-process
@@ -41,13 +41,9 @@ def gemm(M, N, K, A, B, a_mn=0, b_mn=0, bias=None, epi=0, aux=None, splits=1, bn
 
 
 def case_gemm_kk():
-    return _both_cta_groups(_gemm_kk)
-
-
-def _gemm_kk():
     ok = True
     torch.manual_seed(0)
-    for (M, N, K, bn) in [(128, 128, 64, 128), (300, 256, 192, 128), (300, 256, 192, 256), (1000, 768, 768, 0), (7872, 2304, 768, 0)]:
+    for (M, N, K, bn) in [(128, 128, 64, 128), (300, 256, 192, 128), (300, 256, 192, 0), (1000, 768, 768, 0), (7872, 2304, 768, 0)]:
         A = torch.randn(M, K, device=DEV).to(BF)
         B = torch.randn(N, K, device=DEV).to(BF)
         bias = torch.randn(N, device=DEV).to(BF)
@@ -63,10 +59,6 @@ def _gemm_kk():
 
 
 def case_gemm_epi():
-    return _both_cta_groups(_gemm_epi)
-
-
-def _gemm_epi():
     ok = True
     torch.manual_seed(1)
     M, N, K = 520, 512, 256
@@ -85,25 +77,12 @@ def _gemm_epi():
     return ok
 
 
-def _both_cta_groups(fn):
-    """Run a GEMM case with single-CTA tiles, with cta_group::2 CTA pairs, and with the cost model's own choice."""
-    ok = True
-    for cg in (1, 2, 0):
-        L.lib().vlpk_debug_set_cta_group(cg)
-        print(f" cta_group {'auto' if cg == 0 else cg}")
-        try:
-            ok &= fn()
-        finally:
-            L.lib().vlpk_debug_set_cta_group(0)
-    return ok
-
-
 def case_gemm_dgrad():
     torch.manual_seed(2)
 
     def run():
         ok = True
-        for (M, N, K, bn) in [(300, 256, 128, 128), (300, 512, 320, 256), (1000, 768, 3072, 0)]:
+        for (M, N, K, bn) in [(300, 256, 128, 128), (300, 512, 320, 0), (1000, 768, 3072, 0)]:
             # D[M,N] = A[M,K] B[N,K]^T with B stored as [K,N] row-major (MN-major)
             A = torch.randn(M, K, device=DEV).to(BF)
             Bs = (torch.randn(K, N, device=DEV) * 0.1).to(BF)
@@ -117,7 +96,7 @@ def case_gemm_dgrad():
         ok &= report("dgrad *aux", gemm(M, N, K, A, Bs, b_mn=1, epi=4, aux=aux), ref * aux.float())
         return ok
 
-    return _both_cta_groups(run)
+    return run()
 
 
 def case_gemm_wgrad():
@@ -125,7 +104,7 @@ def case_gemm_wgrad():
 
     def run():
         ok = True
-        for (T, Nf, Kf, splits, bn) in [(128, 128, 128, 1, 128), (500, 256, 384, 1, 128), (500, 256, 512, 3, 256), (7872, 768, 768, 8, 0),
+        for (T, Nf, Kf, splits, bn) in [(128, 128, 128, 1, 128), (500, 256, 384, 1, 128), (500, 256, 512, 3, 0), (7872, 768, 768, 8, 0),
                                         (640, 768, 1608, 2, 0)]:
             dY = (torch.randn(T, Nf, device=DEV) * 0.1).to(BF)
             X = torch.randn(T, Kf, device=DEV).to(BF)
@@ -134,7 +113,7 @@ def case_gemm_wgrad():
             ok &= report(f"wgrad T{T} N{Nf} K{Kf} s{splits} bn{bn}", D, ref)
         return ok
 
-    return _both_cta_groups(run)
+    return run()
 
 
 def _mask_bits(mask01):
@@ -351,12 +330,7 @@ def case_rowops():
 
 
 def case_perf():
-    for cg in (1, 2, 0):
-        L.lib().vlpk_debug_set_cta_group(cg)
-        print(f" cta_group {'auto' if cg == 0 else cg}")
-        _perf(cg == 0)
-    L.lib().vlpk_debug_set_cta_group(0)
-    return True
+    return _perf(True)
 
 
 def _perf(extras):
@@ -377,7 +351,7 @@ def _perf(extras):
         ms = e0.elapsed_time(e1) / iters
         print(f"  {name:36s} {ms * 1e3:9.1f} us  {flops / ms / 1e9:8.1f} TFLOP/s")
 
-    for (N, K, bn) in [(2304, 768, 0), (768, 768, 0), (3072, 768, 0), (768, 3072, 0), (768, 768, 128), (768, 768, 256), (3072, 768, 128), (3072, 768, 256)]:
+    for (N, K, bn) in [(2304, 768, 0), (768, 768, 0), (3072, 768, 0), (768, 3072, 0), (768, 768, 128), (3072, 768, 128)]:
         A = torch.randn(M, K, device=DEV).to(BF); B = torch.randn(N, K, device=DEV).to(BF); D = torch.zeros(M, N, device=DEV, dtype=BF)
         timeit(lambda: gemm(M, N, K, A, B, bn=bn, D0=D), 2.0 * M * N * K, f"fwd  {M}x{N}x{K} bn{bn}")
         if extras:
@@ -421,17 +395,12 @@ if __name__ == "__main__":
         torch.cuda.synchronize()
         print(f"== {name}: {'PASS' if ok else 'FAIL'}")
         sys.exit(0 if ok else 1)
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/bringup.log", "w") as log:
-        for name in CASES:
-            t0 = time.time()
-            try:
-                r = subprocess.run(["timeout", "180", sys.executable, __file__, name], capture_output=True, text=True)
-                out = r.stdout + ("\n[stderr]\n" + r.stderr[-3000:] if r.returncode != 0 else "")
-                rc = r.returncode
-            except Exception as e:  # pragma: no cover
-                out, rc = repr(e), -1
-            msg = f"{out}\n[{name}] rc={rc} {time.time() - t0:.1f}s\n"
-            log.write(msg)
-            log.flush()
-            print(msg)
+    for name in CASES:
+        t0 = time.time()
+        try:
+            r = subprocess.run(["timeout", "180", sys.executable, __file__, name], capture_output=True, text=True)
+            out = r.stdout + ("\n[stderr]\n" + r.stderr[-3000:] if r.returncode != 0 else "")
+            rc = r.returncode
+        except Exception as e:  # pragma: no cover
+            out, rc = repr(e), -1
+        print(f"{out}\n[{name}] rc={rc} {time.time() - t0:.1f}s\n", flush=True)

@@ -4,7 +4,7 @@ B = 64 (M = 7872 token rows): 4 forward, 4 dgrad, 4 wgrad.  Same box, same clock
            the large shapes), time / 16 — the host runs ahead, so this is device time per launch including launch gaps, not host latency;
   "cold"   : one launch after a 512 MB buffer was rewritten, event to event — INCLUDES the host's launch latency (ours: ctypes + tensor-map
            encoding ~ 8 us, cuBLAS ~ 4 us), kept for continuity with the first table of this round.
-Writes a markdown table (default gpurun_out/r02_gemm_vs_cublas.md).
+Prints a markdown table (and writes it to the optional path argument).
 
     python tools/gemm_vs_cublas.py [out.md]
 """
@@ -63,7 +63,7 @@ def vgemm(Mg, N, K, A, B, a_mn=0, b_mn=0, bias=None, epi=0, aux=None, splits=1, 
 
 
 def main():
-    out_path = sys.argv[1] if len(sys.argv) > 1 else "gpurun_out/r02_gemm_vs_cublas.md"
+    out_path = sys.argv[1] if len(sys.argv) > 1 else None
     torch.manual_seed(0)
     flush = torch.empty(512 * 1024 * 1024 // 4, device=DEV, dtype=torch.float32)
     rows = []
@@ -127,8 +127,9 @@ def main():
     flops = sum(r[4] for r in rows)
     lines.append(f"| **sum (one layer fwd+bwd)** | | {tot[2]:.1f} | {tot[3]:.1f} | {flops / tot[2] / 1e6:.0f} | {flops / tot[3] / 1e6:.0f} | {tot[3] / tot[2]:.2f} | {tot[0]:.1f} | {tot[1]:.1f} | |")
     text = "\n".join(lines) + "\n"
-    os.makedirs(os.path.dirname(out_path) or ".", exist_ok=True)
-    open(out_path, "w").write(text)
+    if out_path:
+        os.makedirs(os.path.dirname(out_path) or ".", exist_ok=True)
+        open(out_path, "w").write(text)
     print(text)
 
 

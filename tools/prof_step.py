@@ -1,9 +1,9 @@
 """One training step of the benchmarked configuration between cudaProfilerStart/Stop, for ncu --profile-from-start off.
 
-    ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv \
+    ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --csv --log-file launches.csv \
         python tools/prof_step.py [--layers 12] [--config caption]
     ncu --profile-from-start off --set full --clock-control none --import-source on -k regex:'gemm_kernel|attn_|ln_res' \
-        -o gpurun_out/prof python tools/prof_step.py --layers 2
+        -o prof python tools/prof_step.py --layers 2
 
 --layers 2 keeps every kernel shape of the BERT-base step (the layers are identical) while a --set full capture stays short.
 """

@@ -56,7 +56,6 @@ _P = c_void_p
 _SIGS = {
     "vlpk_version": (c_int, []),
     "vlpk_last_error": (C.c_char_p, []),
-    "vlpk_debug_set_cta_group": (None, [c_int]),
     "vlpk_debug_set_option": (c_int, [C.c_char_p, c_int]),
     "vlpk_set_reserved_sms": (None, [c_int]),
     "vlpk_debug_plan_gemm": (c_int, [c_int] * 10 + [C.POINTER(c_int)]),

@@ -88,10 +88,7 @@ int wgrad_linear(int M, int N, int K, const void* dy, int64_t lddy, const void* 
 // One process drives one GPU, so a single side stream per process is enough; fork / join with events (capturable in a CUDA graph).
 // Backward: the weight-gradient GEMM of each Linear runs behind its dgrad (VLPK_WGRAD_STREAM=0 / option "wgrad_stream" disables):
 // inside one layer the two only share their INPUT; both are persistent one-CTA-per-SM kernels, so the wgrad's CTAs start on the SMs
-// the dgrad's partial last wave leaves idle (93 pair-tiles on 74 CTA pairs for the N = 768 shapes) instead of after its last tile.
-// (A forward use — precomputing the dropout keep-bits of all sites on this stream while the GEMMs leave the integer pipes idle —
-// was measured on the B200 and dropped: attention gained 0.22 ms per step, but the LayerNorm kernels became slower reading bytes than
-// evaluating Philox, and the generator's CTAs contended with the issue-bound kernels: +0.08 ms net.)
+// the dgrad's partial last wave leaves idle (372 tiles on 132 SMs for the N = 768 shapes) instead of after its last tile.
 struct SideStream {
   cudaStream_t stream = nullptr;
   cudaEvent_t fork = nullptr, join = nullptr;
@@ -99,7 +96,7 @@ struct SideStream {
   bool failed = false;
 };
 
-int g_wgrad_stream = -1;  // -1: take VLPK_WGRAD_STREAM from the environment on first use, default on (measured +1 % on the B200 step)
+int g_wgrad_stream = -1;  // -1: take VLPK_WGRAD_STREAM from the environment on first use, default on
 
 SideStream* side_stream() {
   static SideStream side;
@@ -123,7 +120,7 @@ SideStream* wgrad_side() {
 }
 
 // One Linear's backward: weight gradient + input gradient, which only share their inputs.  Default: wgrad then dgrad on `main`
-// (the order validated on the B200).  With the side stream: dgrad first on `main` (it is on the critical path and takes the
+// With the side stream: dgrad first on `main` (it is on the critical path and takes the
 // SMs), then the wgrad on the side stream, whose CTAs fill the SMs the dgrad's partial last wave leaves idle and overlap whatever
 // `main` issues next.  wgrad_join(main) must follow before the wgrad's inputs are overwritten.
 template <class WgradFn, class DgradFn>
@@ -381,20 +378,19 @@ __global__ void relu_bwd_kernel(bf16* __restrict__ dpre, const bf16* __restrict_
 extern "C" {
 
 int vlpk_version(void) { return VLPK_VERSION; }
-void vlpk_debug_set_cta_group(int cg) { debug_set_cta_group(cg); }
 int vlpk_debug_set_option(const char* name, int value) {
   VLPK_CHECK_ARG(name != nullptr, "set_option: null name");
   if (strcmp(name, "wgrad_stream") == 0) { g_wgrad_stream = value ? 1 : 0; return 0; }
   set_error("set_option: unknown option '%s'", name);
   return -1;
 }
-int vlpk_debug_plan_gemm(int M, int N, int K, int a_mn, int b_mn, int nseg, int seg_rows, int epi, int bn, int splits, int* out3) {
+int vlpk_debug_plan_gemm(int M, int N, int K, int a_mn, int b_mn, int nseg, int seg_rows, int epi, int bn, int splits, int* out2) {
   GemmDesc g;
   g.M = M; g.N = N; g.K = K;
   g.a_mn = a_mn != 0; g.b_mn = b_mn != 0;
   g.nseg = nseg; g.b_seg_rows = seg_rows;
   g.epi = epi; g.bn = bn; g.splits = splits;
-  return plan_gemm(g, &out3[0], &out3[1], &out3[2]);
+  return plan_gemm(g, &out2[0], &out2[1]);
 }
 void vlpk_set_reserved_sms(int n) { set_reserved_sms(n); }
 const char* vlpk_last_error(void) { return get_error(); }
@@ -662,9 +658,6 @@ int vlpk_encoder_bwd(const VlpkShape* s, int n_layers, const VlpkLayerWeights* w
   const long long n = static_cast<long long>(s->B) * s->Lq * s->H;
   // The inter-layer gradient lives in ws->dx.  layer_bwd may run in place (dx == dy): dy is consumed
   // entirely by its first kernel (LN2 backward) and dx is written only by its last (QKV dgrad).
-  // (Moving the zero-fill and the fp32 -> bf16 conversion of the gradient arena onto an auxiliary stream, layer by layer beside the
-  // backward GEMMs, was measured on the B200: no change in step time — the GEMMs are L2-bandwidth bound, so the extra traffic costs
-  // them what it saves — and 60 more API calls per step on the host.  Both stay single calls made by the caller.)
   const void* cur_dy = dys[n_layers - 1];
   for (int i = n_layers - 1; i >= 0; --i) {
     void* out = (i == 0) ? dx0 : ws->dx;

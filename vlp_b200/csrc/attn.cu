@@ -3,17 +3,19 @@
 // Reference semantics (pytorch_pretrained_bert/modeling.py:279-302):
 //   S = Q K^T / sqrt(64) + mask_add ; P = softmax(S) ; P = dropout(P) ; ctx = P V
 // where mask_add is 0 / -10000 (modeling.py:832).  One whole sequence (123 -> 128 rows) is a single
-// 128-row UMMA tile, so S and P live only in TMEM / registers / shared memory: the reference's
+// 128-row tile, so S and P live only in registers / shared memory: the reference's
 // [B,12,L,L] score tensor (written + read ~6x per layer, SURVEY.md §8a a5) never touches HBM.
 //
-// One CTA per (head, batch), 8 warps: two threads per tile row (TMEM lane), each owning half of the key columns.
-//   fwd : TMA Q,K,V -> S=QK^T (tcgen05, TMEM) -> scale+bitmask+softmax in registers -> Philox dropout
-//         -> P (bf16, swizzled smem) -> O=PV (tcgen05, V read MN-major straight from its [kv,d] tile)
+// One CTA per (head, batch), two warpgroups: warpgroup g owns query rows [64 g, 64 g + 64) and all 128 key columns, so
+// every row reduction stays inside a quad of threads (wgmma accumulator layout, see wgmma.cuh).
+//   fwd : TMA Q,K,V -> S=QK^T (wgmma, registers) -> scale+bitmask+softmax in registers -> Philox dropout
+//         -> P (bf16, registers) -> O=PV (wgmma with A from registers, V read MN-major straight from its [kv,d] tile)
 //         -> O/rowsum -> TMA store.  Saves only logsumexp per row for backward.
 //   bwd : recompute S,P from Q,K + logsumexp; dP=dO V^T; dS=P*(dP-delta)/8; dV=P^T dO; dK=dS^T Q; dQ=dS K
-//         — five UMMAs, all operands fed from the same five TMA tiles via K-major / MN-major descriptors.
+//         — five wgmma chains, all operands fed from the same TMA tiles via K-major / MN-major descriptors.
 #include "attn.cuh"
 #include "host.cuh"
+#include "rowops.cuh"
 
 namespace vlpk {
 
@@ -22,6 +24,7 @@ static constexpr int TL = 128;        // tile rows (max sequence length)
 static constexpr int TILE_B = TL * 128;  // bytes of one [128 x 64] bf16 tile
 static constexpr float LOG2E = 1.4426950408889634f;
 static constexpr float LN2 = 0.6931471805599453f;
+static constexpr int ATT_THREADS = 256;
 
 struct AttnTmaps {
   CUtensorMap q, k, v, o;         // fwd: o = ctx ; bwd: o = dO (load)
@@ -37,87 +40,81 @@ struct AttnArgs {
   const __nv_bfloat16* do_ptr;  // bwd: dO, same layout
   long long ld_o;
   DropoutCfg drop;
-  float* dbias;  // bwd, optional: [3 * heads * 64] fp32, += column sums of dQ | dK | dV (gradient of the q/k/v biases)
   unsigned char* keep_out;  // fwd, optional: packed dropout keep-decisions, 16 bytes per (sequence, head, query row)
+  float* dbias_part;  // bwd, optional: [B][3 * heads * 64] fp32 per-sequence column sums of dQ | dK | dV (q/k/v bias gradients)
 };
 
-__device__ __forceinline__ void sw_write16(uint8_t* tile, int row, int chunk, uint4 v) {
-  *reinterpret_cast<uint4*>(tile + row * 128 + ((chunk ^ (row & 7)) << 4)) = v;
+// bf16 pair (columns col, col + 1) into a [rows x 64] bf16 tile stored with the 128-byte swizzle of the TMA boxes
+__device__ __forceinline__ void sw_write_pair(uint8_t* tile, int row, int col, uint32_t v) {
+  *reinterpret_cast<uint32_t*>(tile + row * 128 + (((col >> 3) ^ (row & 7)) << 4) + (col & 7) * 2) = v;
 }
 
-// Scaled + masked score in the log2 domain for 32 columns starting at col0.
-// bit set -> attend (add 0) ; bit clear -> add -10000 (reference additive mask) ; col >= Lkv -> -inf.
-__device__ __forceinline__ void score_chunk(const uint32_t (&r)[32], uint32_t mbits, int col0, int Lkv, float (&t)[32]) {
-  const float sc = 0.125f * LOG2E;
-  const float neg = -10000.0f * LOG2E;
-#pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    float x = __uint_as_float(r[j]) * sc + (((mbits >> j) & 1u) ? 0.f : neg);
-    t[j] = (col0 + j < Lkv) ? x : -INFINITY;
+// Per-thread view of one warpgroup's accumulator rows: element i of an m64nN fragment lies in row fr + 8 * ((i >> 1) & 1) of
+// the warpgroup's 64 rows and column 8 * (i >> 2) + fc + (i & 1).
+struct Frag {
+  int fr, fc;
+  __device__ __forceinline__ Frag() {
+    const int t = threadIdx.x & 127, lane = threadIdx.x & 31;
+    fr = (t >> 5) * 16 + (lane >> 2);
+    fc = (lane & 3) * 2;
   }
+};
+
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-// Fast variant for a 32-column chunk in which every row of the warp attends to every column and all columns exist (the image-region
-// prefix of VLP's sequences: 3 of the 4 chunks of every row, seq2seq or bidirectional): one multiply per element.
-__device__ __forceinline__ void score_chunk_plain(const uint32_t (&r)[32], float (&t)[32]) {
-  const float sc = 0.125f * LOG2E;
+// Keep-decisions of the 128 key columns of query rows r (h = 0) and r + 8 (h = 1): word w bit j = column 32 w + j, i.e. byte g of
+// word w = dropout_keep8(seed, site, (row_elem0 + 32 w + 8 g) / 8).  The four threads of a quad each evaluate one word per row
+// (or read the forward's bytes) and exchange them.
+__device__ __forceinline__ void attn_keep_words(const DropoutCfg& d, uint64_t dseed, const uint64_t (&row_elem0)[2], uint32_t (&kw)[2][4]) {
+  const int lane = threadIdx.x & 31, qi = lane & 3;
 #pragma unroll
-  for (int j = 0; j < 32; ++j) t[j] = __uint_as_float(r[j]) * sc;
-}
-// warp-uniform: may this chunk take the plain path?
-__device__ __forceinline__ bool chunk_is_plain(uint32_t mbits, int col0, int Lkv) {
-  return (col0 + 32 <= Lkv) && __all_sync(0xffffffffu, mbits == 0xFFFFFFFFu);
-}
-
-// keep-decisions of this thread's 64 key columns of one query row: two 32-bit words (bit j of word c = column c*32 + j)
-__device__ __forceinline__ void attn_keep_words(const DropoutCfg& d, uint64_t dseed, uint64_t row_elem0, int hf, uint32_t (&kw)[2]) {
-  kw[0] = kw[1] = 0xFFFFFFFFu;
-  if (d.p <= 0.f) return;
-  if (d.bits != nullptr) {
-    const uint2 v = __ldg(reinterpret_cast<const uint2*>(d.bits + ((row_elem0 + hf * 64) >> 3)));
-    kw[0] = v.x;
-    kw[1] = v.y;
-  } else {
+  for (int h = 0; h < 2; ++h) {
+    uint32_t mine = 0xFFFFFFFFu;
+    if (d.p > 0.f) {
+      if (d.bits != nullptr) {
+        mine = __ldg(reinterpret_cast<const uint32_t*>(d.bits + (row_elem0[h] >> 3)) + qi);
+      } else {
+        mine = 0;
 #pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      uint32_t w = 0;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) w |= dropout_keep8(dseed, d.site, (row_elem0 + hf * 64 + c * 32 + g * 8) >> 3, d.thresh16) << (8 * g);
-      kw[c] = w;
+        for (int g = 0; g < 4; ++g) mine |= dropout_keep8(dseed, d.site, (row_elem0[h] + qi * 32 + g * 8) >> 3, d.thresh16) << (8 * g);
+      }
     }
+#pragma unroll
+    for (int w = 0; w < 4; ++w) kw[h][w] = __shfl_sync(0xffffffffu, mine, (lane & ~3) | w);
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// forward: persistent, warp-specialised.  Each CTA walks (sequence, head) items item = blockIdx.x, + gridDim.x, ...; two CTAs
-// per SM (99 KB smem, 256 TMEM columns each) hide each other's residual latencies.
-//   warps 0-7  softmax : warp w owns TMEM lane quadrant w & 3 (32 query rows) and key-column half w >> 2
-//   warp  8    control : one lane issues every TMA load and every tcgen05.mma and runs ahead of the softmax warps
-// TMEM: two 128-column buffers X[0], X[1]; item i uses X[i & 1] for S_i = Q K^T and, once every softmax thread has consumed S_i,
-// for O_i = P V (columns [0,64)).  Pipeline across items (i = item in flight in the softmax warps):
-//   control : ... S_{i+1} issued as soon as Q,K_{i+1} have landed and X[(i+1)&1] has been drained by epilogue(i-1) — i.e. in the
-//             MIDDLE of item i — so the softmax warps never wait for a QK^T;  Q,K_{i+1} are fetched the moment S_i has retired,
-//             V_{i+1} the moment P_i V_i has retired.
-//   softmax : wait S_i -> pass 1 (row max) -> epilogue(i-1) (O_{i-1} / rowsum -> bf16 -> TMA store; its P V retired long ago)
-//             -> pass 2 (exp, Philox dropout, P_i -> smem) -> arrive "P_i ready".
-// ------------------------------------------------------------------------------------------------
-static constexpr int ATT_SOFTMAX_THREADS = 256;
-static constexpr int ATT_THREADS = ATT_SOFTMAX_THREADS + 32;
+// Scaled + masked score in the log2 domain: bit set -> attend (add 0) ; bit clear -> add -10000 (reference additive mask) ;
+// col >= Lkv -> -inf.
+__device__ __forceinline__ float score(float s, const uint32_t (&mw)[4], int col, int Lkv) {
+  const float x = s * (0.125f * LOG2E) + (((mw[col >> 5] >> (col & 31)) & 1u) ? 0.f : -10000.0f * LOG2E);
+  return col < Lkv ? x : -INFINITY;
+}
 
+__device__ __forceinline__ void load_mask_words(const AttnArgs& a, int b, int row, uint32_t (&mw)[4]) {
+  const int mr = (a.mask_rows == 1) ? 0 : min(row, a.mask_rows - 1);
+  const uint4 m4 = __ldg(reinterpret_cast<const uint4*>(a.mask_bits + (static_cast<size_t>(b) * a.mask_rows + mr) * 4));
+  mw[0] = m4.x; mw[1] = m4.y; mw[2] = m4.z; mw[3] = m4.w;
+}
+
+// ------------------------------------------------------------------------------------------------
+// forward  (256 threads, 48 KB smem: Q | K | V; the Q tile is reused as output staging)
+// ------------------------------------------------------------------------------------------------
 struct FwdSmem {
   static constexpr int OFF_Q = 0;
   static constexpr int OFF_K = TILE_B;
   static constexpr int OFF_V = 2 * TILE_B;
-  static constexpr int OFF_P = 3 * TILE_B;        // 2 atoms x 16 KB
-  static constexpr int OFF_O = 5 * TILE_B;        // output staging for the TMA store
-  static constexpr int OFF_RED = 6 * TILE_B;      // float[6][128]: partial row max | bf16-sum | exact sum, per column half
-  static constexpr int OFF_BAR = OFF_RED + 6 * 128 * 4;
-  static constexpr int NUM_BARS = 10;
-  static constexpr int TOTAL = OFF_BAR + NUM_BARS * 8 + 16;
+  static constexpr int OFF_BAR = 3 * TILE_B;
+  static constexpr int TOTAL = OFF_BAR + 16;
   static constexpr int DYN = TOTAL + 1024;
 };
-
-__device__ __forceinline__ void softmax_bar_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 __global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a) {
   extern __shared__ uint8_t smem_raw[];
@@ -125,24 +122,15 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_kernel(const __grid_c
   uint8_t* sQ = smem + FwdSmem::OFF_Q;
   uint8_t* sK = smem + FwdSmem::OFF_K;
   uint8_t* sV = smem + FwdSmem::OFF_V;
-  uint8_t* sP = smem + FwdSmem::OFF_P;
-  uint8_t* sO = smem + FwdSmem::OFF_O;
-  float* s_max = reinterpret_cast<float*>(smem + FwdSmem::OFF_RED);
-  float* s_rsum = s_max + 256;
-  float* s_lsum = s_max + 512;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + FwdSmem::OFF_BAR);
-  uint64_t* bar_qk = &bars[0];      // TMA: Q,K of the next item landed
-  uint64_t* bar_v = &bars[1];       // TMA: V landed
-  uint64_t* bar_s = &bars[2];       // [2] MMA: S in X[j] complete (also: Q,K buffers free)
-  uint64_t* bar_o = &bars[4];       // [2] MMA: O in X[j] complete (also: V and P buffers free)
-  uint64_t* bar_p = &bars[6];       // softmax (256 arrivals): P written, S fully consumed
-  uint64_t* bar_x = &bars[7];       // [2] softmax (256 arrivals): O read out of X[j] -> buffer free for the next S
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(&bars[9]);
+  uint64_t* bar_qk = &bars[0];
+  uint64_t* bar_v = &bars[1];
 
   pdl_launch_dependents();
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int n_items = a.B * a.heads;
-  const int my_items = (n_items - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
+  const int h = blockIdx.x, b = blockIdx.y;
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const Frag f;
+  const int qi = tid & 3;
 
   if (tid == 0) {
     tma_prefetch_desc(&tm.q);
@@ -151,235 +139,122 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_kernel(const __grid_c
     tma_prefetch_desc(&tm.o);
     mbar_init(bar_qk, 1);
     mbar_init(bar_v, 1);
-    mbar_init(&bar_s[0], 1);
-    mbar_init(&bar_s[1], 1);
-    mbar_init(&bar_o[0], 1);
-    mbar_init(&bar_o[1], 1);
-    mbar_init(bar_p, ATT_SOFTMAX_THREADS);
-    mbar_init(&bar_x[0], ATT_SOFTMAX_THREADS);
-    mbar_init(&bar_x[1], ATT_SOFTMAX_THREADS);
     fence_mbar_init();
   }
-  if (warp == 8) {
-    __syncwarp();
-    tmem_alloc<256>(tmem_slot);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   pdl_wait();
-
-  if (warp == 8) {
-    // ===================================== control warp ==========================================
-    if (lane == 0 && my_items > 0) {
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, 128, false, false);
-      constexpr uint32_t idesc_o = umma_idesc_bf16(128, HD, false, true);
-      auto load_qk = [&](int it) {
-        const int item = blockIdx.x + it * gridDim.x;
-        const int b = item / a.heads, h = item - b * a.heads;
-        mbar_arrive_expect_tx(bar_qk, 2 * TILE_B);
-        tma_load_3d(sQ, &tm.q, bar_qk, h * HD, 0, b);
-        tma_load_3d(sK, &tm.k, bar_qk, h * HD, 0, b);
-      };
-      auto load_v = [&](int it) {
-        const int item = blockIdx.x + it * gridDim.x;
-        const int b = item / a.heads, h = item - b * a.heads;
-        mbar_arrive_expect_tx(bar_v, TILE_B);
-        tma_load_3d(sV, &tm.v, bar_v, h * HD, 0, b);
-      };
-      auto issue_s = [&](int it) {   // S_it = Q K^T into X[it & 1]
-        const int j = it & 1;
-        mbar_wait(bar_qk, it & 1);                        // Q,K of item `it` landed
-        mbar_wait(&bar_x[j], ((it >> 1) & 1) ^ 1);        // X[j] drained by epilogue(it - 2) (passes at once for it < 2)
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < HD / 16; ++k)
-          umma_f16(tmem + j * 128, umma_smem_desc_sw128(smem_u32(sQ) + k * 32, 16, 1024),
-                   umma_smem_desc_sw128(smem_u32(sK) + k * 32, 16, 1024), idesc_s, k > 0 ? 1u : 0u);
-        umma_commit(&bar_s[j]);
-      };
-      load_qk(0);
-      load_v(0);
-      issue_s(0);
-      for (int it = 0; it < my_items; ++it) {
-        const int j = it & 1;
-        const uint32_t ph = (it >> 1) & 1;
-        if (it + 1 < my_items) {
-          mbar_wait(&bar_s[j], ph);          // S_it retired: the Q,K buffers may be refilled
-          load_qk(it + 1);
-          issue_s(it + 1);
-        }
-        mbar_wait(bar_p, it & 1);            // P_it in shared memory, S_it consumed by every softmax thread
-        mbar_wait(bar_v, it & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int k = 0; k < TL / 16; ++k)
-          umma_f16(tmem + j * 128, umma_smem_desc_sw128(smem_u32(sP) + (k >> 2) * TILE_B + (k & 3) * 32, 16, 1024),
-                   umma_smem_desc_sw128(smem_u32(sV) + k * 2048, 8192, 1024), idesc_o, k > 0 ? 1u : 0u);
-        umma_commit(&bar_o[j]);
-        if (it + 1 < my_items) {
-          mbar_wait(&bar_o[j], ph);          // P_it V_it retired: V (and P) may be overwritten
-          load_v(it + 1);
-        }
-      }
-    }
-  } else {
-    // ===================================== softmax warps =========================================
-    const int q4 = warp & 3, hf = warp >> 2;
-    const int row = q4 * 32 + lane;
-    const uint32_t t_lane = static_cast<uint32_t>(q4 * 32) << 16;
-    const uint64_t dseed = drop_seed(a.drop);
-    float inv_prev = 0.f;   // 1 / rowsum of the item whose epilogue is still pending
-    int b_prev = 0, h_prev = 0;
-
-    // O_{it} / rowsum -> bf16 -> staging -> TMA store; frees X[it & 1]
-    auto epilogue = [&](int it, int b, int h, float inv) {
-      const int j = it & 1;
-      mbar_wait(&bar_o[j], (it >> 1) & 1);
-      __syncwarp();
-      tc_fence_after();
-      uint32_t r[32];
-      tmem_ld32(tmem + j * 128 + t_lane + hf * 32, r);   // this thread's 32 of the 64 output columns
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(&bar_x[j]);
-      if (tid == 0) tma_store_wait_read<0>();            // the previous item's store has finished reading the staging tile
-      softmax_bar_sync();
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        uint32_t pk[4];
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj)
-          pk[jj] = pack_bf16x2(__uint_as_float(r[g * 8 + 2 * jj]) * inv, __uint_as_float(r[g * 8 + 2 * jj + 1]) * inv);
-        sw_write16(sO, row, hf * 4 + g, make_uint4(pk[0], pk[1], pk[2], pk[3]));
-      }
-      fence_proxy_async_smem();
-      softmax_bar_sync();
-      if (tid == 0) {
-        tma_store_3d(&tm.o, sO, h * HD, 0, b);
-        tma_store_commit();
-      }
-    };
-
-    for (int it = 0; it < my_items; ++it) {
-      const int item = blockIdx.x + it * gridDim.x;
-      const int b = item / a.heads, h = item - b * a.heads;
-      const int j = it & 1;
-      const uint32_t tS = tmem + j * 128;
-      uint32_t mb[2];
-      {
-        const int mr = (a.mask_rows == 1) ? 0 : min(row, a.mask_rows - 1);
-        const uint2 m2 = __ldg(reinterpret_cast<const uint2*>(a.mask_bits + (static_cast<size_t>(b) * a.mask_rows + mr) * 4 + hf * 2));
-        mb[0] = m2.x; mb[1] = m2.y;
-      }
-      mbar_wait(&bar_s[j], (it >> 1) & 1);
-      __syncwarp();
-      tc_fence_after();
-      // pass 1: partial row max over this thread's 64 columns (log2 domain), exchanged through shared memory
-      float tmax = -INFINITY;
-      uint32_t plain_m = 0;   // bit c: chunk c of this warp takes the plain path
-#pragma unroll 1
-      for (int c = 0; c < 2; ++c) {
-        uint32_t r[32];
-        tmem_ld32(tS + t_lane + hf * 64 + c * 32, r);
-        const bool pl = chunk_is_plain(mb[c], hf * 64 + c * 32, a.Lkv);
-        plain_m |= (pl ? 1u : 0u) << c;
-        tmem_ld_wait();
-        if (pl) {
-          float m = __uint_as_float(r[0]);
-#pragma unroll
-          for (int jj = 1; jj < 32; ++jj) m = fmaxf(m, __uint_as_float(r[jj]));
-          tmax = fmaxf(tmax, m * (0.125f * LOG2E));          // the scale is positive: max commutes with it
-        } else {
-          float t[32];
-          score_chunk(r, mb[c], hf * 64 + c * 32, a.Lkv, t);
-#pragma unroll
-          for (int jj = 0; jj < 32; ++jj) tmax = fmaxf(tmax, t[jj]);
-        }
-      }
-      s_max[hf * 128 + row] = tmax;
-      softmax_bar_sync();
-      tmax = fmaxf(s_max[row], s_max[128 + row]);   // Lkv >= 1 guarantees at least one finite column in half 0
-      // the previous item's output: its P V retired long ago; this also guarantees that P / V of item it-1 are no longer read
-      if (it > 0) epilogue(it - 1, b_prev, h_prev, inv_prev);
-      // pass 2: exponentiate, partial row sums, dropout, write un-normalised P (bf16) as the A operand of P V
-      float rsum = 0.f, lsum = 0.f;
-      const uint64_t row_elem0 = ((static_cast<uint64_t>(b) * a.heads + h) * a.Lq + min(row, a.Lq - 1)) * TL;
-      uint32_t kw[2];
-      attn_keep_words(a.drop, dseed, row_elem0, hf, kw);
-      if (a.keep_out != nullptr && row < a.Lq) *reinterpret_cast<uint2*>(a.keep_out + ((row_elem0 + hf * 64) >> 3)) = make_uint2(kw[0], kw[1]);
-#pragma unroll 1
-      for (int c = 0; c < 2; ++c) {
-        uint32_t r[32];
-        float t[32];
-        tmem_ld32(tS + t_lane + hf * 64 + c * 32, r);
-        tmem_ld_wait();
-        if ((plain_m >> c) & 1u) score_chunk_plain(r, t); else score_chunk(r, mb[c], hf * 64 + c * 32, a.Lkv, t);
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const uint32_t keep = (kw[c] >> (8 * g)) & 0xFFu;
-          uint32_t pk[4];
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            const float x0 = fast_ex2(t[g * 8 + 2 * jj] - tmax), x1 = fast_ex2(t[g * 8 + 2 * jj + 1] - tmax);
-            lsum += x0 + x1;                                       // exact sum -> logsumexp (backward recomputes P from it)
-            const float e0 = bf16_round(x0), e1 = bf16_round(x1);  // the tensor core sees bf16 P: normalise O by the sum of
-            rsum += e0 + e1;                                       // exactly those values
-            const float p0 = ((keep >> (2 * jj)) & 1u) ? e0 * a.drop.scale : 0.f;
-            const float p1 = ((keep >> (2 * jj + 1)) & 1u) ? e1 * a.drop.scale : 0.f;
-            pk[jj] = pack_bf16x2(p0, p1);
-          }
-          sw_write16(sP + hf * TILE_B, row, c * 4 + g, make_uint4(pk[0], pk[1], pk[2], pk[3]));
-        }
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(bar_p);
-      s_rsum[hf * 128 + row] = rsum;
-      s_lsum[hf * 128 + row] = lsum;
-      softmax_bar_sync();
-      rsum = s_rsum[row] + s_rsum[128 + row];
-      lsum = s_lsum[row] + s_lsum[128 + row];
-      if (hf == 0 && a.lse != nullptr && row < a.Lq)
-        a.lse[(static_cast<size_t>(b) * a.heads + h) * a.Lq + row] = (tmax + log2f(lsum)) * LN2;
-      inv_prev = 1.0f / rsum;
-      b_prev = b;
-      h_prev = h;
-    }
-    if (my_items > 0) epilogue(my_items - 1, b_prev, h_prev, inv_prev);
-    if (tid == 0) tma_store_wait<0>();
+  if (tid == 0) {
+    mbar_arrive_expect_tx(bar_qk, 2 * TILE_B);
+    tma_load_3d(sQ, &tm.q, bar_qk, h * HD, 0, b);
+    tma_load_3d(sK, &tm.k, bar_qk, h * HD, 0, b);
+    mbar_arrive_expect_tx(bar_v, TILE_B);
+    tma_load_3d(sV, &tm.v, bar_v, h * HD, 0, b);
   }
 
-  tc_fence_before();
+  const int row[2] = {wg * 64 + f.fr, wg * 64 + f.fr + 8};
+  uint32_t mw[2][4];
+  uint64_t row_elem0[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    load_mask_words(a, b, row[hh], mw[hh]);
+    row_elem0[hh] = ((static_cast<uint64_t>(b) * a.heads + h) * a.Lq + min(row[hh], a.Lq - 1)) * TL;
+  }
+
+  // S = Q K^T for this warpgroup's 64 query rows
+  float s[64];
+  mbar_wait(bar_qk, 0);
+  {
+    const uint32_t q0 = smem_u32(sQ) + wg * 8192, k0 = smem_u32(sK);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < HD / 16; ++k)
+      wgmma_m64n128k16_ss<0, 0>(s, wgmma_desc_sw128(q0 + k * 32, 16, 1024), wgmma_desc_sw128(k0 + k * 32, 16, 1024), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+  }
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int i = 0; i < 64; ++i) {
+    const int hh = (i >> 1) & 1;
+    s[i] = score(s[i], mw[hh], 8 * (i >> 2) + f.fc + (i & 1), a.Lkv);
+    mx[hh] = fmaxf(mx[hh], s[i]);
+  }
+  mx[0] = quad_max(mx[0]);  // Lkv >= 1 guarantees a finite maximum
+  mx[1] = quad_max(mx[1]);
+  uint32_t kw[2][4];  // evaluated here rather than up front: keeps them out of the registers live across the S = QK^T wgmma
+  attn_keep_words(a.drop, drop_seed(a.drop), row_elem0, kw);
+  if (a.keep_out != nullptr) {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+      if (row[hh] < a.Lq) reinterpret_cast<uint32_t*>(a.keep_out + (row_elem0[hh] >> 3))[qi] = kw[hh][qi];
+  }
+  // exponentiate, dropout, pack P (bf16) straight into the A fragments of P V
+  float rsum[2] = {0.f, 0.f}, lsum[2] = {0.f, 0.f};
+  uint32_t pa[8][4];
+#pragma unroll
+  for (int i = 0; i < 64; i += 2) {
+    const int hh = (i >> 1) & 1, col = 8 * (i >> 2) + f.fc;
+    const float x0 = fast_ex2(s[i] - mx[hh]), x1 = fast_ex2(s[i + 1] - mx[hh]);
+    lsum[hh] += x0 + x1;                                   // exact sum -> logsumexp (backward recomputes P from it)
+    const float e0 = bf16_round(x0), e1 = bf16_round(x1);  // the tensor core sees bf16 P: normalise O by the sum of
+    rsum[hh] += e0 + e1;                                   // exactly those values
+    const uint32_t keep = kw[hh][col >> 5] >> (col & 31);
+    const float p0 = (keep & 1u) ? e0 * a.drop.scale : 0.f;
+    const float p1 = (keep & 2u) ? e1 * a.drop.scale : 0.f;
+    pa[i >> 3][(i >> 1) & 3] = pack_bf16x2(p0, p1);
+  }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    rsum[hh] = quad_sum(rsum[hh]);
+    lsum[hh] = quad_sum(lsum[hh]);
+    if (qi == 0 && a.lse != nullptr && row[hh] < a.Lq)
+      a.lse[(static_cast<size_t>(b) * a.heads + h) * a.Lq + row[hh]] = (mx[hh] + log2f(lsum[hh])) * LN2;
+  }
+  // O = P V
+  float o[32];
+  mbar_wait(bar_v, 0);
+  {
+    const uint32_t v0 = smem_u32(sV);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < TL / 16; ++k) wgmma_m64n64k16_rs<1>(o, pa[k], wgmma_desc_sw128(v0 + k * 2048, 8192, 1024), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+  }
+  // O / rowsum -> bf16 -> this warpgroup's half of the (dead) Q tile -> one TMA store of the whole tile
+  const float inv[2] = {1.0f / rsum[0], 1.0f / rsum[1]};
+  uint8_t* stg = sQ + wg * 8192;
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    const int hh = (i >> 1) & 1;
+    sw_write_pair(stg, f.fr + 8 * hh, 8 * (i >> 2) + f.fc, pack_bf16x2(o[i] * inv[hh], o[i + 1] * inv[hh]));
+  }
+  fence_proxy_async_smem();
   __syncthreads();
-  tc_fence_after();
-  if (warp == 8) {
-    __syncwarp();
-    tmem_dealloc<256>(tmem);
+  if (tid == 0) {
+    tma_store_3d(&tm.o, sQ, h * HD, 0, b);
+    tma_store_commit();
+    tma_store_wait<0>();
   }
 }
 
 // ------------------------------------------------------------------------------------------------
-// backward  (256 threads, 96 KB smem + 256 TMEM columns -> 2 CTAs per SM)
-//   TMEM: S [0,128) and dP [128,256) are consumed by the softmax-backward phase, then the same columns receive
-//         dV [0,64), dK [64,128), dQ [128,192).   SMEM: one [128 x 128] bf16 buffer holds P (for dV) and then dS (for dK, dQ).
+// backward  (256 threads, 96 KB smem: Q | K | V | dO | a [128 x 128] bf16 buffer holding P (for dV) and then dS (for dK))
 // ------------------------------------------------------------------------------------------------
 struct BwdSmem {
   static constexpr int OFF_Q = 0;            // later dQ staging
   static constexpr int OFF_K = TILE_B;       // later dK staging
   static constexpr int OFF_V = 2 * TILE_B;   // later dV staging
   static constexpr int OFF_DO = 3 * TILE_B;
-  static constexpr int OFF_PD = 4 * TILE_B;  // 2 atoms: P, then dS
-  static constexpr int OFF_RED = 6 * TILE_B; // float[2][128] partial delta exchange
-  static constexpr int OFF_BAR = OFF_RED + 1024;
-  static constexpr int TOTAL = OFF_BAR + 64;
+  static constexpr int OFF_PD = 4 * TILE_B;  // 2 atoms of [128 q x 64 kv]: P, then dS
+  static constexpr int OFF_BAR = 6 * TILE_B;
+  static constexpr int TOTAL = OFF_BAR + 16;
   static constexpr int DYN = TOTAL + 1024;
 };
 
-static constexpr int ATT_BWD_THREADS = 256;
-
-__global__ void __launch_bounds__(ATT_BWD_THREADS, 2) attn_bwd_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a) {
+__global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem + BwdSmem::OFF_Q;
@@ -387,20 +262,12 @@ __global__ void __launch_bounds__(ATT_BWD_THREADS, 2) attn_bwd_kernel(const __gr
   uint8_t* sV = smem + BwdSmem::OFF_V;
   uint8_t* sdO = smem + BwdSmem::OFF_DO;
   uint8_t* sPD = smem + BwdSmem::OFF_PD;
-  float* s_red = reinterpret_cast<float*>(smem + BwdSmem::OFF_RED);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + BwdSmem::OFF_BAR);
-  uint64_t* bar_in = &bars[0];
-  uint64_t* bar_s = &bars[1];
-  uint64_t* bar_v = &bars[2];
-  uint64_t* bar_o = &bars[3];
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(&bars[4]);
+  uint64_t* bar_in = reinterpret_cast<uint64_t*>(smem + BwdSmem::OFF_BAR);
 
   pdl_launch_dependents();
   const int h = blockIdx.x, b = blockIdx.y;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int q4 = warp & 3, hf = warp >> 2;
-  const int row = q4 * 32 + lane;
-  const uint64_t dseed = drop_seed(a.drop);
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const Frag f;
 
   if (tid == 0) {
     tma_prefetch_desc(&tm.q);
@@ -408,177 +275,127 @@ __global__ void __launch_bounds__(ATT_BWD_THREADS, 2) attn_bwd_kernel(const __gr
     tma_prefetch_desc(&tm.v);
     tma_prefetch_desc(&tm.o);
     mbar_init(bar_in, 1);
-    mbar_init(bar_s, 1);
-    mbar_init(bar_v, 1);
-    mbar_init(bar_o, 1);
     fence_mbar_init();
   }
-  if (warp == 0) {
-    __syncwarp();
-    tmem_alloc<256>(tmem_slot);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t tS = tmem, tdP = tmem + 128, tdV = tmem, tdK = tmem + 64, tdQ = tmem + 128;
   pdl_wait();
-
   if (tid == 0) {
     mbar_arrive_expect_tx(bar_in, 4 * TILE_B);
     tma_load_3d(sQ, &tm.q, bar_in, h * HD, 0, b);
     tma_load_3d(sK, &tm.k, bar_in, h * HD, 0, b);
     tma_load_3d(sV, &tm.v, bar_in, h * HD, 0, b);
     tma_load_3d(sdO, &tm.o, bar_in, h * HD, 0, b);
-    mbar_wait(bar_in, 0);
-    tc_fence_after();
-    constexpr uint32_t idesc = umma_idesc_bf16(128, 128, false, false);
-#pragma unroll
-    for (int k = 0; k < HD / 16; ++k)
-      umma_f16(tS, umma_smem_desc_sw128(smem_u32(sQ) + k * 32, 16, 1024),
-               umma_smem_desc_sw128(smem_u32(sK) + k * 32, 16, 1024), idesc, k > 0 ? 1u : 0u);
-#pragma unroll
-    for (int k = 0; k < HD / 16; ++k)
-      umma_f16(tdP, umma_smem_desc_sw128(smem_u32(sdO) + k * 32, 16, 1024),
-               umma_smem_desc_sw128(smem_u32(sV) + k * 32, 16, 1024), idesc, k > 0 ? 1u : 0u);
-    umma_commit(bar_s);
   }
 
-  const bool row_ok = row < a.Lq;
-  uint32_t mb[2];
+  const int row[2] = {wg * 64 + f.fr, wg * 64 + f.fr + 8};
+  uint32_t mw[2][4];
+  uint64_t row_elem0[2];
+  float lse2[2];
+  bool row_ok[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    load_mask_words(a, b, row[hh], mw[hh]);
+    row_elem0[hh] = ((static_cast<uint64_t>(b) * a.heads + h) * a.Lq + min(row[hh], a.Lq - 1)) * TL;
+    row_ok[hh] = row[hh] < a.Lq;
+    lse2[hh] = row_ok[hh] ? a.lse[(static_cast<size_t>(b) * a.heads + h) * a.Lq + row[hh]] * LOG2E : 0.f;
+  }
+  uint32_t kw[2][4];  // dropout keep mask of this thread's rows (forward's bytes when available, else Philox evaluated once)
+  attn_keep_words(a.drop, drop_seed(a.drop), row_elem0, kw);
+
+  // S = Q K^T and dP = dO V^T for this warpgroup's 64 query rows
+  float s[64], dp[64];
+  mbar_wait(bar_in, 0);
   {
-    const int mr = (a.mask_rows == 1) ? 0 : min(row, a.mask_rows - 1);
-    const uint2 m2 = __ldg(reinterpret_cast<const uint2*>(a.mask_bits + (static_cast<size_t>(b) * a.mask_rows + mr) * 4 + hf * 2));
-    mb[0] = m2.x; mb[1] = m2.y;
+    const uint32_t q0 = smem_u32(sQ) + wg * 8192, k0 = smem_u32(sK), do0 = smem_u32(sdO) + wg * 8192, v0 = smem_u32(sV);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < HD / 16; ++k)
+      wgmma_m64n128k16_ss<0, 0>(s, wgmma_desc_sw128(q0 + k * 32, 16, 1024), wgmma_desc_sw128(k0 + k * 32, 16, 1024), k > 0 ? 1u : 0u);
+#pragma unroll
+    for (int k = 0; k < HD / 16; ++k)
+      wgmma_m64n128k16_ss<0, 0>(dp, wgmma_desc_sw128(do0 + k * 32, 16, 1024), wgmma_desc_sw128(v0 + k * 32, 16, 1024), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    reg_fence(dp);
   }
-  const float lse2 = row_ok ? a.lse[(static_cast<size_t>(b) * a.heads + h) * a.Lq + row] * LOG2E : 0.f;
-
-  mbar_wait(bar_s, 0);
-  __syncwarp();
-  tc_fence_after();
-  const uint32_t t_lane = static_cast<uint32_t>(q4 * 32) << 16;
-  // pass A: delta_r = sum_j P_rj dP_rj with the SAME recomputed P that pass B multiplies with, so that sum_j dS_rj = 0 holds
-  // to fp32 round-off.  (The usual shortcut delta = dO . O inherits the bf16 rounding of O; when keys / values share a large
-  // common component — VLP's 100 near-identical region rows at initialisation — that error is amplified by |mean| / |spread|
-  // and reached 10-20 % in dQ/dK on the VQA parity case.)
-  float delta = 0.f;
-  uint32_t kw[2];  // dropout keep mask of this thread's 64 columns (forward's bytes when available, else Philox evaluated once)
-  attn_keep_words(a.drop, dseed, ((static_cast<uint64_t>(b) * a.heads + h) * a.Lq + min(row, a.Lq - 1)) * TL, hf, kw);
-  uint32_t plain_m = 0;
-#pragma unroll 1
-  for (int c = 0; c < 2; ++c) {
-    uint32_t r[32], d[32];
-    float t[32];
-    tmem_ld32(tS + t_lane + hf * 64 + c * 32, r);
-    tmem_ld32(tdP + t_lane + hf * 64 + c * 32, d);
-    const bool pl = chunk_is_plain(mb[c], hf * 64 + c * 32, a.Lkv);
-    plain_m |= (pl ? 1u : 0u) << c;
-    tmem_ld_wait();
-    if (pl) score_chunk_plain(r, t); else score_chunk(r, mb[c], hf * 64 + c * 32, a.Lkv, t);
-    const uint32_t kbc = kw[c];
+  // P (recomputed from the logsumexp; 0 for columns >= Lkv and rows >= Lq) and the dropout-masked dP.
+  // delta_r = sum_j P_rj dP_rj with the SAME recomputed P that dS multiplies with, so that sum_j dS_rj = 0 holds to fp32
+  // round-off.  (The usual shortcut delta = dO . O inherits the bf16 rounding of O; when keys / values share a large common
+  // component — VLP's 100 near-identical region rows at initialisation — that error is amplified by |mean| / |spread| and
+  // reached 10-20 % in dQ/dK on the VQA parity case.)
+  float delta[2] = {0.f, 0.f};
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      const uint32_t keep = (kbc >> (8 * g)) & 0xFFu;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float p = row_ok ? fast_ex2(t[g * 8 + j] - lse2) : 0.f;
-        const float dpm = ((keep >> j) & 1u) ? __uint_as_float(d[g * 8 + j]) * a.drop.scale : 0.f;
-        delta = fmaf(p, dpm, delta);
-      }
-    }
+  for (int i = 0; i < 64; ++i) {
+    const int hh = (i >> 1) & 1, col = 8 * (i >> 2) + f.fc + (i & 1);
+    const float p = row_ok[hh] ? fast_ex2(score(s[i], mw[hh], col, a.Lkv) - lse2[hh]) : 0.f;
+    const bool kp = (kw[hh][col >> 5] >> (col & 31)) & 1u;
+    const float dpm = kp ? dp[i] * a.drop.scale : 0.f;
+    delta[hh] = fmaf(p, dpm, delta[hh]);
+    s[i] = p;
+    dp[i] = dpm;
   }
-  s_red[hf * 128 + row] = delta;
-  __syncthreads();
-  delta = s_red[row] + s_red[128 + row];
-  uint32_t dsp[32];  // this thread's 64 dS values (bf16 pairs), parked in registers until P has been consumed
+  delta[0] = quad_sum(delta[0]);
+  delta[1] = quad_sum(delta[1]);
+  uint32_t dsa[8][4];  // dS (bf16) as the A fragments of dQ = dS K
 #pragma unroll
-  for (int c = 0; c < 2; ++c) {
-    uint32_t r[32], d[32];
-    float t[32];
-    tmem_ld32(tS + t_lane + hf * 64 + c * 32, r);
-    tmem_ld32(tdP + t_lane + hf * 64 + c * 32, d);
-    tmem_ld_wait();
-    if ((plain_m >> c) & 1u) score_chunk_plain(r, t); else score_chunk(r, mb[c], hf * 64 + c * 32, a.Lkv, t);
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      const uint32_t keep = (kw[c] >> (8 * g)) & 0xFFu;
-      uint32_t pk[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float pv[2], dv[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int jj = g * 8 + 2 * j + e;
-          const float p = row_ok ? fast_ex2(t[jj] - lse2) : 0.f;  // exp2(-inf) = 0 for columns >= Lkv
-          const bool kp = (keep >> (2 * j + e)) & 1u;
-          const float dpm = kp ? __uint_as_float(d[jj]) * a.drop.scale : 0.f;
-          pv[e] = kp ? p * a.drop.scale : 0.f;
-          dv[e] = p * (dpm - delta) * 0.125f;
-        }
-        pk[j] = pack_bf16x2(pv[0], pv[1]);
-        dsp[c * 16 + g * 4 + j] = pack_bf16x2(dv[0], dv[1]);
-      }
-      sw_write16(sPD + hf * TILE_B, row, c * 4 + g, make_uint4(pk[0], pk[1], pk[2], pk[3]));
-    }
+  for (int i = 0; i < 64; i += 2) {
+    const int hh = (i >> 1) & 1, col = 8 * (i >> 2) + f.fc;
+    const uint32_t keep = kw[hh][col >> 5] >> (col & 31);
+    const float p0 = (keep & 1u) ? s[i] * a.drop.scale : 0.f, p1 = (keep & 2u) ? s[i + 1] * a.drop.scale : 0.f;
+    sw_write_pair(sPD + (col >> 6) * TILE_B, row[hh], col & 63, pack_bf16x2(p0, p1));
+    dsa[i >> 3][(i >> 1) & 3] = pack_bf16x2(s[i] * (dp[i] - delta[hh]) * 0.125f, s[i + 1] * (dp[i + 1] - delta[hh]) * 0.125f);
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
 
-  constexpr uint32_t idesc_mm = umma_idesc_bf16(128, HD, true, true);   // A^T from [q,kv] tile, B from [q,d] tile
-  constexpr uint32_t idesc_km = umma_idesc_bf16(128, HD, false, true);  // A = dS [q,kv], B from [kv,d] tile
-  if (tid == 0) {
-    tc_fence_after();
+  // dV[kv, d] = sum_q Pd[q, kv] dO[q, d] for kv rows [64 wg, 64 wg + 64): A = Pd^T (MN-major), B = dO (MN-major)
+  float dv[32];
+  {
+    const uint32_t p0 = smem_u32(sPD) + wg * TILE_B, do0 = smem_u32(sdO);
+    wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < TL / 16; ++k)  // dV[kv,d] = sum_q Pd[q,kv] dO[q,d]     (overwrites S columns: all S/dP reads are done)
-      umma_f16(tdV, umma_smem_desc_sw128(smem_u32(sPD) + k * 2048, TILE_B, 1024),
-               umma_smem_desc_sw128(smem_u32(sdO) + k * 2048, 8192, 1024), idesc_mm, k > 0 ? 1u : 0u);
-    umma_commit(bar_v);
+    for (int k = 0; k < TL / 16; ++k)
+      wgmma_m64n64k16_ss<1, 1>(dv, wgmma_desc_sw128(p0 + k * 2048, 8192, 1024), wgmma_desc_sw128(do0 + k * 2048, 8192, 1024), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(dv);
   }
-  mbar_wait(bar_v, 0);   // P has been read by the tensor core: the buffer can take dS
-  __syncwarp();
+  __syncthreads();  // both warpgroups have read P: the buffer can take dS
 #pragma unroll
-  for (int c = 0; c < 2; ++c)
+  for (int c = 0; c < 8; ++c)
 #pragma unroll
-    for (int g = 0; g < 4; ++g)
-      sw_write16(sPD + hf * TILE_B, row, c * 4 + g,
-                 make_uint4(dsp[c * 16 + g * 4], dsp[c * 16 + g * 4 + 1], dsp[c * 16 + g * 4 + 2], dsp[c * 16 + g * 4 + 3]));
-  fence_proxy_async_smem();
-  tc_fence_before();
-  __syncthreads();
-  if (tid == 0) {
-    tc_fence_after();
-#pragma unroll
-    for (int k = 0; k < TL / 16; ++k)  // dK[kv,d] = sum_q dS[q,kv] Q[q,d]
-      umma_f16(tdK, umma_smem_desc_sw128(smem_u32(sPD) + k * 2048, TILE_B, 1024),
-               umma_smem_desc_sw128(smem_u32(sQ) + k * 2048, 8192, 1024), idesc_mm, k > 0 ? 1u : 0u);
-#pragma unroll
-    for (int k = 0; k < TL / 16; ++k)  // dQ[q,d] = sum_kv dS[q,kv] K[kv,d]
-      umma_f16(tdQ, umma_smem_desc_sw128(smem_u32(sPD) + (k >> 2) * TILE_B + (k & 3) * 32, 16, 1024),
-               umma_smem_desc_sw128(smem_u32(sK) + k * 2048, 8192, 1024), idesc_km, k > 0 ? 1u : 0u);
-    umma_commit(bar_o);
-  }
-  mbar_wait(bar_o, 0);
-  __syncwarp();
-  tc_fence_after();
-  // all MMAs retired: Q/K/V tiles are dead, reuse them as output staging; each thread converts 32 of the 64 columns
-#pragma unroll
-  for (int o = 0; o < 3; ++o) {
-    const uint32_t tsrc = (o == 0) ? tdQ : (o == 1 ? tdK : tdV);
-    uint8_t* stg = (o == 0) ? sQ : (o == 1 ? sK : sV);
-    uint32_t r[32];
-    tmem_ld32(tsrc + t_lane + hf * 32, r);
-    tmem_ld_wait();
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      uint32_t pk[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) pk[j] = pack_bf16x2(__uint_as_float(r[g * 8 + 2 * j]), __uint_as_float(r[g * 8 + 2 * j + 1]));
-      sw_write16(stg, row, hf * 4 + g, make_uint4(pk[0], pk[1], pk[2], pk[3]));
+    for (int e = 0; e < 4; ++e) {
+      const int hh = e & 1, col = 16 * c + 8 * (e >> 1) + f.fc;
+      sw_write_pair(sPD + (col >> 6) * TILE_B, row[hh], col & 63, dsa[c][e]);
     }
+  fence_proxy_async_smem();
+  __syncthreads();
+
+  // dK[kv, d] = sum_q dS[q, kv] Q[q, d]  (A = dS^T from shared memory) ; dQ[q, d] = sum_kv dS[q, kv] K[kv, d]  (A = dS registers)
+  float dk[32], dq[32];
+  {
+    const uint32_t p0 = smem_u32(sPD) + wg * TILE_B, q0 = smem_u32(sQ), k0 = smem_u32(sK);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < TL / 16; ++k)
+      wgmma_m64n64k16_ss<1, 1>(dk, wgmma_desc_sw128(p0 + k * 2048, 8192, 1024), wgmma_desc_sw128(q0 + k * 2048, 8192, 1024), k > 0 ? 1u : 0u);
+#pragma unroll
+    for (int k = 0; k < TL / 16; ++k) wgmma_m64n64k16_rs<1>(dq, dsa[k], wgmma_desc_sw128(k0 + k * 2048, 8192, 1024), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(dk);
+    reg_fence(dq);
+  }
+  __syncthreads();  // every wgmma has read Q / K / V: reuse them as output staging
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    const int r = wg * 64 + f.fr + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + f.fc;
+    sw_write_pair(sQ, r, col, pack_bf16x2(dq[i], dq[i + 1]));
+    sw_write_pair(sK, r, col, pack_bf16x2(dk[i], dk[i + 1]));
+    sw_write_pair(sV, r, col, pack_bf16x2(dv[i], dv[i + 1]));
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
   if (tid == 0) {
     tma_store_3d(&tm.dq, sQ, h * HD, 0, b);
@@ -586,22 +403,18 @@ __global__ void __launch_bounds__(ATT_BWD_THREADS, 2) attn_bwd_kernel(const __gr
     tma_store_3d(&tm.dv, sV, h * HD, 0, b);
     tma_store_commit();
   }
-  if (a.dbias != nullptr && tid < 192) {
-    // bias gradients of the q/k/v projections = column sums of dQ / dK / dV: fold the staged tiles (rows >= L are exactly zero)
+  if (a.dbias_part != nullptr && tid < 192) {
+    // this sequence's share of the q/k/v bias gradients = column sums of the staged dQ / dK / dV tiles (rows >= L are exactly
+    // zero); written, not added, so that launch_sum_parts can add the sequences in a fixed order
     const int o = tid >> 6, c = tid & 63;
     const uint8_t* stg = (o == 0) ? sQ : (o == 1 ? sK : sV);
     float acc = 0.f;
 #pragma unroll 8
     for (int r = 0; r < TL; ++r)
       acc += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(stg + r * 128 + (((c >> 3) ^ (r & 7)) << 4) + (c & 7) * 2));
-    atomicAdd(a.dbias + o * a.heads * HD + h * HD + c, acc);
+    a.dbias_part[static_cast<size_t>(b) * 3 * a.heads * HD + o * a.heads * HD + h * HD + c] = acc;
   }
   if (tid == 0) tma_store_wait<0>();
-  tc_fence_after();
-  if (warp == 0) {
-    __syncwarp();
-    tmem_dealloc<256>(tmem);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -640,17 +453,15 @@ int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream) {
   a.mask_bits = d.mask_bits; a.mask_rows = d.mask_rows;
   a.lse = d.lse; a.o_ptr = nullptr; a.do_ptr = nullptr; a.ld_o = d.ld_o;
   a.drop = d.drop;
-  a.dbias = nullptr;
   a.keep_out = d.keep_out;
+  a.dbias_part = nullptr;
   static bool attr_set = false;
   if (!attr_set) {
     VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem::DYN));
     attr_set = true;
   }
   LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * d.Lkv * HD, stream);
-  const int n_items = d.B * d.heads;
-  const int slots = 2 * num_sms();   // two CTAs per SM
-  VLPK_CUDA(launch_ex(attn_fwd_kernel, dim3(n_items < slots ? n_items : slots), dim3(ATT_THREADS), FwdSmem::DYN, stream, 1, tm, a));
+  VLPK_CUDA(launch_ex(attn_fwd_kernel, dim3(d.heads, d.B), dim3(ATT_THREADS), FwdSmem::DYN, stream, 1, tm, a));
   return 0;
 }
 
@@ -676,15 +487,23 @@ int launch_attn_bwd(const AttnDesc& d, cudaStream_t stream) {
   a.do_ptr = reinterpret_cast<const __nv_bfloat16*>(d.d_o);
   a.ld_o = d.ld_o;
   a.drop = d.drop;
-  a.dbias = d.dbias;
   a.keep_out = nullptr;
+  a.dbias_part = nullptr;
+  const long long nbias = 3LL * d.heads * HD;
+  if (d.dbias != nullptr) {
+    a.dbias_part = scratch_f32(SCRATCH_ATTN_DBIAS, static_cast<size_t>(d.B) * nbias, stream);
+    if (a.dbias_part == nullptr) return -1;
+  }
   static bool attr_set = false;
   if (!attr_set) {
     VLPK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem::DYN));
     attr_set = true;
   }
-  LaunchScope scope(CAT_ATTN_BWD, 10.0 * d.B * d.heads * d.Lq * d.Lkv * HD, stream);
-  VLPK_CUDA(launch_ex(attn_bwd_kernel, dim3(d.heads, d.B), dim3(ATT_BWD_THREADS), BwdSmem::DYN, stream, 1, tm, a));
+  {
+    LaunchScope scope(CAT_ATTN_BWD, 10.0 * d.B * d.heads * d.Lq * d.Lkv * HD, stream);
+    VLPK_CUDA(launch_ex(attn_bwd_kernel, dim3(d.heads, d.B), dim3(ATT_THREADS), BwdSmem::DYN, stream, 1, tm, a));
+  }
+  if (d.dbias != nullptr) VLPK_TRY(launch_sum_parts(a.dbias_part, d.B, nbias, d.dbias, stream));
   return 0;
 }
 

@@ -26,7 +26,7 @@ struct AttnDesc {
   void* dk = nullptr;
   void* dv = nullptr;  // each [B, L, ld_dqkv]
   int64_t ld_dqkv = 0;
-  float* dbias = nullptr;  // optional [3 * heads * 64] fp32: += column sums of dQ | dK | dV
+  float* dbias = nullptr;  // optional [3 * heads * 64] fp32: += column sums of dQ | dK | dV, summed over sequences in a fixed order
 };
 
 int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream);

@@ -1,7 +1,7 @@
-// vlp_b200 — sm_100a device-side primitives shared by every kernel in this library.
+// vlp_b200 — sm_90a device-side primitives shared by every kernel in this library.
 //
-// Thin inline-PTX wrappers for the Blackwell async machinery (mbarrier, TMA, tcgen05/TMEM),
-// UMMA shared-memory / instruction descriptor builders, a counter-based Philox RNG for
+// Thin inline-PTX wrappers for the Hopper async machinery (mbarrier, TMA, wgmma),
+// the wgmma shared-memory descriptor builder, a counter-based Philox RNG for
 // regenerable dropout masks, and small bf16 pack helpers.  Nothing here is a translation of
 // reference code: the reference (LuoweiZhou/VLP) has no native code at all (SURVEY.md §2.1).
 #pragma once
@@ -9,6 +9,8 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace vlpk {
 
@@ -120,6 +122,12 @@ __device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* m, const vo
                "r"(smem_u32(src)), "r"(c0), "r"(c1)
                : "memory");
 }
+__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, const void* src, int c0, int c1, int c2) {
+  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void tma_store_wait_read() {
@@ -131,80 +139,37 @@ __device__ __forceinline__ void tma_store_wait() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (warpgroup MMA) issue / completion
 // ----------------------------------------------------------------------------------------------
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-  static_assert(NCOLS == 32 || NCOLS == 64 || NCOLS == 128 || NCOLS == 256 || NCOLS == 512, "pow2 cols");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// Orders this warpgroup's register accesses before the wgmma that follow (required before the first wgmma that reads or
+// accumulates into registers written by ordinary instructions).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16 inputs with fp32 accumulate.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed.
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// Keeps the compiler from moving accesses of an accumulator across wgmma_fence / wgmma_wait.
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (lane i <- TMEM lane base+i).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
 // ----------------------------------------------------------------------------------------------
-// UMMA descriptors (bit layout: PTX ISA "tcgen05 matrix/instruction descriptors")
+// wgmma shared-memory matrix descriptor (PTX ISA "Matrix Descriptor Format" for wgmma), 128-byte swizzle:
+//   start address >>4 : bits [0,14)   leading byte offset >>4 : bits [16,30)   stride byte offset >>4 : bits [32,46)
+//   swizzle mode (1 = 128B) : bits [62,64)
+// K-major operand (rows of 64 bf16 = 128 B):  SBO = 1024 (8-row group), LBO unused;  +32 B per K = 16 step.
+// MN-major operand ([k][64 mn] boxes of 8 KB): SBO = 1024 (8-k group), LBO = 8192 (next 64-wide MN box);  +2048 B per K = 16.
 // ----------------------------------------------------------------------------------------------
-// Shared-memory operand descriptor, 128-byte swizzle, sm_100 version field = 1.
-//   start address >>4 : bits [0,14)     leading byte offset >>4 : bits [16,30)
-//   stride byte offset >>4 : bits [32,46)   version : bits [46,48)   layout (2 = SW128) : bits [61,64)
-__device__ __forceinline__ uint64_t umma_smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;
-  d |= 2ull << 61;
+  d |= 1ull << 62;
   return d;
-}
-// Instruction descriptor for kind::f16, bf16 x bf16 -> fp32, M = 128.
-//   c_format(F32=1) bits[4,6)  a_format(BF16=1) bits[7,10)  b_format bits[10,13)
-//   a_major bit 15, b_major bit 16 (0 = K-major, 1 = MN-major)  N>>3 bits[17,23)  M>>4 bits[24,29)
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int m, int n, bool a_mn, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-         (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
 }
 
 // ----------------------------------------------------------------------------------------------

@@ -1,6 +1,6 @@
-// vlp_b200 — persistent, warp-specialised tcgen05 GEMM for sm_100a.
+// vlp_b200 — persistent, warp-specialised wgmma GEMM for sm_90a.
 //
-//   D[M,N] = epilogue( sum_k A[m,k] * B[n,k] )         bf16 operands, fp32 accumulation in TMEM
+//   D[M,N] = epilogue( sum_k A[m,k] * B[n,k] )         bf16 operands, fp32 accumulation in registers
 //
 // Every dense contraction on the VLP hot path goes through this one kernel family
 // (SURVEY.md §8a a1,a2,a5,a6,a8,a9,a18 / Appendix B):
@@ -8,16 +8,14 @@
 //   dgrad    dX = dY W   : A = dY [M,N'] (K-major),          B = weight [N',K'] read MN-major (no transpose copy)
 //   wgrad    dW = dY^T X : A = dY read MN-major, B = X read MN-major, split-K, fp32 TMA reduce-add
 //
-// Structure (320 threads per CTA; CG = 1: one CTA per tile of 128 x BN, CG = 2: a CTA pair (cluster of 2, one
-// TPC) per tile of 256 x BN with tcgen05 cta_group::2 — each CTA stages its own 128 rows of A and HALF of B, so the
-// L2->SM and shared-memory traffic per MMA flop drop by 1/3 and 1/2 respectively; the first GPU profile showed the
-// single-CTA 128x256 tile to be operand-feed bound at ~50 % of the MMA rate):
-//   warp 0      TMA producer   : cp.async.bulk.tensor -> 128B-swizzled smem ring (STAGES deep)
-//   warp 1      MMA issuer     : (leader CTA) tcgen05.mma M=128*CG, N=BN, K=16 x4 per 64-wide k-block, accumulators
-//                                double-buffered in TMEM (2 x BN columns) so epilogue(i) overlaps mainloop(i+1)
-//   warps 2..9  epilogue       : two groups of 4 warps (one per TMEM lane quadrant) split the column boxes;
-//                                tcgen05.ld -> registers -> fused pointwise op -> swizzled smem staging
-//                                -> TMA store (or TMA reduce-add for split-K weight gradients)
+// Structure (288 threads per CTA, one CTA per SM, one 128 x 128 output tile at a time):
+//   warp 8          TMA producer   : one elected lane issues cp.async.bulk.tensor into a 128B-swizzled smem ring (STAGES deep)
+//   warpgroups 0,1  MMA + epilogue : each owns 64 rows of the tile: wgmma m64n128k16 (x4 per 64-wide k-block) into a register
+//                                    accumulator, then the fused pointwise op -> swizzled smem staging -> TMA store (or TMA
+//                                    reduce-add for split-K weight gradients).  While one warpgroup drains its epilogue the
+//                                    producer keeps filling the ring for the next tile.
+// Tiles are 128 wide only: a 256-wide tile needs a 128-register accumulator per thread, and a 9-warp (or 12-warp) block is
+// capped at 168 registers, so its epilogues spill.
 #include "gemm.cuh"
 
 #include <cstdlib>
@@ -26,11 +24,12 @@
 
 namespace vlpk {
 
-static constexpr int BM = 128;  // rows per CTA == TMEM lanes
+static constexpr int BM = 128;  // rows per CTA tile (two warpgroups x 64)
 static constexpr int BK = 64;   // k-block: 64 bf16 = one 128-byte swizzle span
-static constexpr int NUM_THREADS = 320;
-static constexpr int STG_BYTES = BM * 128;  // one staging buffer: 128 rows x 128 bytes
-static constexpr uint32_t PEER_MASK = 0xFEFFFFFFu;  // shared::cluster address of the same offset in CTA 0 of the pair
+static constexpr int NUM_THREADS = 288;
+static constexpr int STG_BYTES = 64 * 128;  // one staging box: 64 rows x 128 bytes
+static constexpr int SMEM_MAX = 232448;     // 227 KB: the per-block opt-in limit of sm_90
+static constexpr int BN = 128;              // tile columns (see above)
 
 struct GemmTmaps {
   CUtensorMap a;
@@ -43,6 +42,7 @@ struct GemmArgs {
   int M, N, K;
   int b_seg_rows;
   int splits;
+  int split_slices;  // EPI_REDUCE_F32: split s reduce-adds into slice s of the 3-D output map (else all into slice 0)
   const __nv_bfloat16* bias[3];
   const __nv_bfloat16* aux;
   long long ld_aux;
@@ -51,258 +51,99 @@ struct GemmArgs {
   float* colsum;  // optional [N] fp32: += column sums of the (bf16-rounded) output tile, i.e. the bias gradient of a dgrad output
 };
 
-template <int BN, int CG, int STAGES>
+template <int STAGES>
 struct SmemLayout {
-  static constexpr int A_BYTES = BM * BK * 2;         // 16 KB : this CTA's 128 rows of A
-  static constexpr int B_BYTES = (BN / CG) * BK * 2;  // this CTA's share of B
+  static constexpr int A_BYTES = BM * BK * 2;  // 16 KB
+  static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int OFF_STG = STAGES * STAGE_BYTES;  // 4 staging buffers (2 per epilogue group)
-  static constexpr int OFF_BIAS = OFF_STG + 4 * STG_BYTES;
-  static constexpr int OFF_BAR = OFF_BIAS + BN * 4;
-  static constexpr int NUM_BARS = 2 * STAGES + 4;
-  static constexpr int OFF_TMEM = OFF_BAR + NUM_BARS * 8;
-  static constexpr int TOTAL = OFF_TMEM + 16;
+  static constexpr int OFF_STG = STAGES * STAGE_BYTES;  // 4 staging boxes (2 per MMA warpgroup)
+  static constexpr int OFF_BAR = OFF_STG + 4 * STG_BYTES;
+  static constexpr int NUM_BARS = 2 * STAGES;
+  static constexpr int TOTAL = OFF_BAR + NUM_BARS * 8;
   static constexpr int DYN_BYTES = TOTAL + 1024;  // slack for manual 1024-byte alignment
-  static_assert(DYN_BYTES <= 232448, "shared memory budget exceeded");
+  static_assert(DYN_BYTES <= SMEM_MAX, "shared memory budget exceeded");
 };
 
-// Accumulator stage stride / allocation in TMEM columns (allocations must be powers of two: BN = 192 rounds up to 256).
-template <int BN>
-struct TmemGeom {
-  static constexpr int ACC_STRIDE = (BN <= 128) ? 128 : 256;
-  static constexpr int COLS = 2 * ACC_STRIDE;
-};
-
-template <int BN, int CG>
 struct StageCount {
-  // everything left of the 227 KB after the 4 staging buffers, bias tile, barriers and alignment slack
-  static constexpr int value = (232448 - 1024 - 4 * STG_BYTES - BN * 4 - 256) / (BM * BK * 2 + (BN / CG) * BK * 2);
+  // everything left of the 227 KB after the 4 staging boxes, barriers and alignment slack
+  static constexpr int value = (SMEM_MAX - 1024 - 4 * STG_BYTES - 256) / (BM * BK * 2 + BN * BK * 2);
 };
 
-__device__ __forceinline__ void epi_bar_sync(int group) {
-  asm volatile("bar.sync %0, 128;" ::"r"(group + 1) : "memory");
-}
-__device__ __forceinline__ void all_epi_bar_sync() { asm volatile("bar.sync 3, 256;" ::: "memory"); }
-
-__device__ __forceinline__ void stg_write16(uint8_t* stg, int row, int chunk, uint4 v) {
-  *reinterpret_cast<uint4*>(stg + row * 128 + ((chunk ^ (row & 7)) << 4)) = v;
+__device__ __forceinline__ void wg_bar_sync(int cw) {
+  asm volatile("bar.sync %0, 128;" ::"r"(cw + 1) : "memory");
 }
 
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-template <int CG>
-__device__ __forceinline__ void tma_load_2d_cg(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  if (CG == 1) {
-    tma_load_2d(dst, m, bar, c0, c1);
-  } else {
-    // both CTAs of the pair signal the LEADER's barrier (peer bit cleared)
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-        "[%2];" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & PEER_MASK), "r"(c0), "r"(c1)
-        : "memory");
-  }
-}
-
-template <int CG>
-__device__ __forceinline__ void umma_f16_cg(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if (CG == 1) {
-    umma_f16(d_tmem, adesc, bdesc, idesc, accumulate);
-  } else {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-
-// Completion of all prior MMAs -> arrive on `bar` (CG = 2: on the barrier at this offset in BOTH CTAs of the pair).
-template <int CG>
-__device__ __forceinline__ void umma_commit_cg(uint64_t* bar) {
-  if (CG == 1) {
-    umma_commit(bar);
-  } else {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(static_cast<uint16_t>(3))
-                 : "memory");
-  }
-}
-
-// Arrive on the leader CTA's copy of `bar`.
-template <int CG>
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  if (CG == 1) {
-    mbar_arrive(bar);
-  } else {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & PEER_MASK) : "memory");
-  }
-}
-
-template <int NCOLS, int CG>
-__device__ __forceinline__ void tmem_alloc_cg(uint32_t* smem_dst) {
-  if (CG == 1) {
-    tmem_alloc<NCOLS>(smem_dst);
-  } else {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "n"(NCOLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-}
-template <int NCOLS, int CG>
-__device__ __forceinline__ void tmem_dealloc_cg(uint32_t taddr) {
-  if (CG == 1) {
-    tmem_dealloc<NCOLS>(taddr);
-  } else {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-  }
-}
-
-template <int BN, int CG, bool A_MN, bool B_MN, int EPI>
+template <bool A_MN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
-  constexpr int STAGES = StageCount<BN, CG>::value;
-  using L = SmemLayout<BN, CG, STAGES>;
+  constexpr int STAGES = StageCount::value;
+  using L = SmemLayout<STAGES>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::OFF_BAR);
-  uint64_t* full_bar = bars;                    // TMA -> MMA   (leader's copy is the one waited on)
-  uint64_t* empty_bar = bars + STAGES;          // MMA -> TMA   (each CTA's own copy)
-  uint64_t* tfull_bar = bars + 2 * STAGES;      // MMA -> epilogue (each CTA's own copy)
-  uint64_t* tempty_bar = bars + 2 * STAGES + 2; // epilogue -> MMA (leader's copy)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L::OFF_TMEM);
-  float* s_bias = reinterpret_cast<float*>(smem + L::OFF_BIAS);
+  uint64_t* full_bar = bars;            // TMA -> MMA
+  uint64_t* empty_bar = bars + STAGES;  // MMA -> TMA (one arrival per MMA warp)
 
   pdl_launch_dependents();  // the next kernel may be scheduled as SMs free up; it blocks in its own pdl_wait()
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
   const int lane = threadIdx.x & 31;
-  const int rank = (CG == 2) ? static_cast<int>(cluster_ctarank()) : 0;
-  const int cluster_id = blockIdx.x / CG;
-  const int num_clusters = gridDim.x / CG;
 
-  const int num_m = (args.M + BM * CG - 1) / (BM * CG);
+  const int num_m = (args.M + BM - 1) / BM;
   const int num_n = (args.N + BN - 1) / BN;
   const int total_kb = (args.K + BK - 1) / BK;
   const int kb_per = (total_kb + args.splits - 1) / args.splits;
   const int num_work = num_m * num_n * args.splits;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm.a);
     tma_prefetch_desc(&tm.b[0]);
     tma_prefetch_desc(&tm.d0);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 256 * CG);
+      mbar_init(&empty_bar[i], 8);
     }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc_cg<TmemGeom<BN>::COLS, CG>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  if (CG == 2) cluster_sync_all();  // peer barriers must be initialised before any remote arrive / multicast commit
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();  // barrier init, TMEM allocation and descriptor prefetch above overlap the previous kernel's tail
+  pdl_wait();  // barrier init and descriptor prefetch above overlap the previous kernel's tail
 
-  if (warp == 0) {
+  if (wg == 2) {
     // ===================================== TMA producer ========================================
-    // The whole warp walks the loop (all loop state is warp-uniform, so the compiler keeps the TMA operands in uniform
-    // registers); one elected lane issues.  A divergent `if (lane == 0)` body costs an ELECT + R2UR waterfall per instruction.
     {
+      // The whole warp walks the loop (warp-uniform state); one elected lane issues.
       int stage = 0;
       uint32_t phase = 0;
-      for (int w = cluster_id; w < num_work; w += num_clusters) {
+      for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
         const int n_blk = w % num_n;
         const int m_blk = (w / num_n) % num_m;
         const int split = w / (num_n * num_m);
         const int kb0 = split * kb_per;
         const int kb1 = min(total_kb, kb0 + kb_per);
-        const int m0 = (m_blk * CG + rank) * BM;
+        const int m0 = m_blk * BM;
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1u);
           if (elect_one()) {
             uint8_t* sA = smem + stage * L::STAGE_BYTES;
             uint8_t* sB = sA + L::A_BYTES;
-            if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], L::STAGE_BYTES * CG);
+            mbar_arrive_expect_tx(&full_bar[stage], L::STAGE_BYTES);
             if (!A_MN) {
-              tma_load_2d_cg<CG>(sA, &tm.a, &full_bar[stage], kb * BK, m0);
+              tma_load_2d(sA, &tm.a, &full_bar[stage], kb * BK, m0);
             } else {
 #pragma unroll
-              for (int j = 0; j < BM / 64; ++j) tma_load_2d_cg<CG>(sA + j * 8192, &tm.a, &full_bar[stage], m0 + j * 64, kb * BK);
+              for (int j = 0; j < BM / 64; ++j) tma_load_2d(sA + j * 8192, &tm.a, &full_bar[stage], m0 + j * 64, kb * BK);
             }
             if (!B_MN) {
               const int n0 = n_blk * BN;
               const int seg = n0 / args.b_seg_rows;
-              tma_load_2d_cg<CG>(sB, &tm.b[seg], &full_bar[stage], kb * BK, n0 - seg * args.b_seg_rows + rank * (BN / CG));
+              tma_load_2d(sB, &tm.b[seg], &full_bar[stage], kb * BK, n0 - seg * args.b_seg_rows);
             } else {
               const int k0 = kb * BK;
               const int seg = k0 / args.b_seg_rows;
 #pragma unroll
-              for (int j = 0; j < BN / CG / 64; ++j)
-                tma_load_2d_cg<CG>(sB + j * 8192, &tm.b[seg], &full_bar[stage], n_blk * BN + rank * (BN / CG) + j * 64,
-                                   k0 - seg * args.b_seg_rows);
+              for (int j = 0; j < BN / 64; ++j)
+                tma_load_2d(sB + j * 8192, &tm.b[seg], &full_bar[stage], n_blk * BN + j * 64, k0 - seg * args.b_seg_rows);
             }
-          }
-          __syncwarp();
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ====================================== MMA issuer ==========================================
-    // Warp-uniform loop, one elected lane issues the four K=16 MMAs of a k-block and the two commits.  Descriptors are
-    // (constant high word) + (low word = stage base + k * step): one integer add per operand per MMA.
-    if (rank == 0) {
-      constexpr uint32_t idesc = umma_idesc_bf16(BM * CG, BN, A_MN, B_MN);
-      constexpr uint32_t DESC_HI = (1024u >> 4) | (1u << 14) | (2u << 29);  // SBO = 1024 B, descriptor version 1, SWIZZLE_128B
-      constexpr uint32_t A_LBO = A_MN ? (8192u >> 4) : 1u, B_LBO = B_MN ? (8192u >> 4) : 1u;
-      constexpr uint32_t A_KSTEP = A_MN ? (2048u >> 4) : (32u >> 4), B_KSTEP = B_MN ? (2048u >> 4) : (32u >> 4);
-      const uint32_t a_lo0 = ((smem_u32(smem) & 0x3FFFFu) >> 4) | (A_LBO << 16);
-      const uint32_t b_lo0 = a_lo0 - (A_LBO << 16) + (L::A_BYTES >> 4) + (B_LBO << 16);
-      int stage = 0;
-      uint32_t phase = 0;
-      int it = 0;
-      for (int w = cluster_id; w < num_work; w += num_clusters, ++it) {
-        const int split = w / (num_n * num_m);
-        const int kb0 = split * kb_per;
-        const int kb1 = min(total_kb, kb0 + kb_per);
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1u;
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * TmemGeom<BN>::ACC_STRIDE;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t a_lo = a_lo0 + stage * (L::STAGE_BYTES >> 4);
-            const uint32_t b_lo = b_lo0 + stage * (L::STAGE_BYTES >> 4);
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              const uint64_t adesc = (static_cast<uint64_t>(DESC_HI) << 32) | (a_lo + k * A_KSTEP);
-              const uint64_t bdesc = (static_cast<uint64_t>(DESC_HI) << 32) | (b_lo + k * B_KSTEP);
-              umma_f16_cg<CG>(d_tmem, adesc, bdesc, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            }
-            umma_commit_cg<CG>(&empty_bar[stage]);  // smem slot reusable (in both CTAs) once these MMAs have read it
-            if (kb == kb1 - 1) umma_commit_cg<CG>(&tfull_bar[acc]);
           }
           __syncwarp();
           if (++stage == STAGES) {
@@ -313,67 +154,74 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
       }
     }
   } else {
-    // ======================================= epilogue ===========================================
-    const int ew = warp - 2;          // 0..7
-    const int grp = ew >> 2;          // epilogue group: handles column boxes with (box & 1) == grp
-    const int q = warp & 3;           // TMEM lane quadrant this warp may access
-    const int row = q * 32 + lane;    // row of this CTA's 128-row tile owned by this thread
-    const int et = threadIdx.x - 64;  // 0..255
-    const bool store_thread = ((ew & 3) == 0 && lane == 0);
+    // ================================== MMA + epilogue ==========================================
+    const int cw = wg;                             // rows [64 cw, 64 cw + 64) of every tile
+    const int t = threadIdx.x - 128 * wg;          // 0..127
+    const int fr = (t >> 5) * 16 + (lane >> 2);    // first accumulator row of this thread (second: fr + 8)
+    const int fc = (lane & 3) * 2;                 // first accumulator column within each 8-column group
+    const bool store_thread = (t == 0);
     const uint64_t dseed = drop_seed(args.drop);
     // bias exists only for forward Linears (B read K-major, segments tile N)
     constexpr bool HAS_BIAS = !B_MN && (EPI == EPI_STORE || EPI == EPI_GELU || EPI == EPI_RELU);
-    uint8_t* stg0 = smem + L::OFF_STG + grp * 2 * STG_BYTES;
+    uint8_t* stg0 = smem + L::OFF_STG + cw * 2 * STG_BYTES;
     uint8_t* stg1 = stg0 + STG_BYTES;
-    int it = 0;
+    // A rows of this warpgroup: 64 rows x 128 B (K-major) or the second 64-wide M box (MN-major) — 8 KB further either way
+    const uint32_t a_base = smem_u32(smem) + cw * 8192;
+    const uint32_t b_base = smem_u32(smem) + L::A_BYTES;
+    int stage = 0;
+    uint32_t phase = 0;
     uint32_t box_seq = 0;
-    for (int w = cluster_id; w < num_work; w += num_clusters, ++it) {
+    float acc[BN / 2];
+    for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
       const int n_blk = w % num_n;
       const int m_blk = (w / num_n) % num_m;
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1u;
+      const int split = w / (num_n * num_m);
+      const int kb0 = split * kb_per;
+      const int kb1 = min(total_kb, kb0 + kb_per);
       const int n0 = n_blk * BN;
-      const int m0 = (m_blk * CG + rank) * BM;
-      const long long m = m0 + row;
-      const bool row_ok = m < args.M;
+      const int m0 = m_blk * BM + cw * 64;
 
-      if (HAS_BIAS) {
-        const int seg = n0 / args.b_seg_rows;
-        const __nv_bfloat16* bp = args.bias[seg];
-        all_epi_bar_sync();  // previous tile's bias reads are finished
-        for (int i = et; i < BN; i += 256) {
-          const int n = n0 + i;
-          s_bias[i] = (bp != nullptr && n < args.N) ? __bfloat162float(bp[n - seg * args.b_seg_rows]) : 0.f;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = a_base + stage * L::STAGE_BYTES;
+        const uint32_t sb = b_base + stage * L::STAGE_BYTES;
+        reg_fence(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t adesc = A_MN ? wgmma_desc_sw128(sa + k * 2048, 8192, 1024) : wgmma_desc_sw128(sa + k * 32, 16, 1024);
+          const uint64_t bdesc = B_MN ? wgmma_desc_sw128(sb + k * 2048, 8192, 1024) : wgmma_desc_sw128(sb + k * 32, 16, 1024);
+          wgmma_m64n128k16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, (kb > kb0 || k > 0) ? 1u : 0u);
         }
-        all_epi_bar_sync();
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence(acc);
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);  // this warp's share of the slot has been read
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1u;
+        }
       }
 
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      __syncwarp();
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * TmemGeom<BN>::ACC_STRIDE;
-
+      // ---- epilogue: accumulator element i of this thread sits at row fr + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + fc + (i & 1)
       if (EPI == EPI_REDUCE_F32) {
         // fp32 staging: 32 columns = 128 bytes per row; one TMA reduce-add box per 32 columns.
         constexpr int NBOX = BN / 32;
-#pragma unroll 1
-        for (int c = grp; c < NBOX; c += 2) {
-          uint32_t r[32];
-          tmem_ld32(t_row + c * 32, r);
-          tmem_ld_wait();
-          if (c + 2 >= NBOX) {
-            tc_fence_before();
-            mbar_arrive_leader<CG>(&tempty_bar[acc]);
-          }
+#pragma unroll
+        for (int c = 0; c < NBOX; ++c) {
           uint8_t* stg = (box_seq & 1u) ? stg1 : stg0;
           if (store_thread) tma_store_wait_read<1>();
-          epi_bar_sync(grp);
+          wg_bar_sync(cw);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) stg_write16(stg, row, j, make_uint4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]));
+          for (int j = 0; j < 8; ++j) {
+            const int i = c * 16 + 2 * j;
+            const int r = fr + 8 * (j & 1), col = 8 * (j >> 1) + fc;
+            *reinterpret_cast<float2*>(stg + r * 128 + (((col >> 2) ^ (r & 7)) << 4) + (col & 3) * 4) = make_float2(acc[i], acc[i + 1]);
+          }
           fence_proxy_async_smem();
-          epi_bar_sync(grp);
+          wg_bar_sync(cw);
           if (store_thread) {
-            tma_reduce_add_2d(&tm.d0, stg, n0 + c * 32, m0);
+            tma_reduce_add_3d(&tm.d0, stg, n0 + c * 32, m0, args.split_slices ? split : 0);
             tma_store_commit();
           }
           ++box_seq;
@@ -381,249 +229,183 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
       } else {
         // bf16 staging: 64 columns = 128 bytes per row; one TMA store box per 64 columns.
         constexpr int NBOX = BN / 64;
-#pragma unroll 1
-        for (int c = grp; c < NBOX; c += 2) {
-          uint32_t o0[32];  // packed bf16 pairs: primary output, 64 columns
-          uint32_t o1[(EPI == EPI_GELU) ? 32 : 1];
+        const __nv_bfloat16* bp = nullptr;
+        int bias_off = 0;
+        if (HAS_BIAS) {
+          const int seg = n0 / args.b_seg_rows;
+          bp = args.bias[seg];
+          bias_off = seg * args.b_seg_rows;
+        }
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            uint32_t r[32];
-            tmem_ld32(t_row + c * 64 + h * 32, r);
-            tmem_ld_wait();
-            const int nb = n0 + c * 64 + h * 32;  // first global column of this 32-wide slab
+        for (int c = 0; c < NBOX; ++c) {
+          uint8_t* stg = (EPI == EPI_GELU) ? stg0 : ((box_seq & 1u) ? stg1 : stg0);
+          if (store_thread) {
+            if (EPI == EPI_GELU) tma_store_wait_read<0>(); else tma_store_wait_read<1>();
+          }
+          wg_bar_sync(cw);
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            const int i = c * 32 + 2 * j;
+            const int r = fr + 8 * (j & 1), col = 8 * (j >> 1) + fc;
+            const int n = n0 + c * 64 + col;
+            const long long m = m0 + r;
+            float v0 = acc[i], v1 = acc[i + 1];
             if (HAS_BIAS) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) r[j] = __float_as_uint(__uint_as_float(r[j]) + s_bias[c * 64 + h * 32 + j]);
+              if (bp != nullptr && n < args.N) {
+                const float2 bb = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(bp + n - bias_off)));
+                v0 += bb.x;
+                v1 += bb.y;
+              }
             }
+            const int so = r * 128 + (((col >> 3) ^ (r & 7)) << 4) + (col & 7) * 2;
             if (EPI == EPI_GELU) {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                float g0, d0, g1, d1;
-                gelu_and_grad(__uint_as_float(r[2 * j]), g0, d0);
-                gelu_and_grad(__uint_as_float(r[2 * j + 1]), g1, d1);
-                o0[h * 16 + j] = pack_bf16x2(d0, d1);  // gelu'(u): all backward needs from the pre-activation
-                o1[h * 16 + j] = pack_bf16x2(g0, g1);  // gelu(u)
-              }
-            } else if (EPI == EPI_RELU) {
-#pragma unroll
-              for (int g = 0; g < 4; ++g) {
-                uint32_t keep = 0xFFu;
-                if (args.drop.p > 0.f)
-                  keep = dropout_keep8(dseed, args.drop.site, (static_cast<uint64_t>(m) * args.N + nb + g * 8) >> 3, args.drop.thresh16);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  float v0 = fmaxf(__uint_as_float(r[g * 8 + 2 * j]), 0.f);
-                  float v1 = fmaxf(__uint_as_float(r[g * 8 + 2 * j + 1]), 0.f);
-                  v0 = ((keep >> (2 * j)) & 1u) ? v0 * args.drop.scale : 0.f;
-                  v1 = ((keep >> (2 * j + 1)) & 1u) ? v1 * args.drop.scale : 0.f;
-                  o0[h * 16 + g * 4 + j] = pack_bf16x2(v0, v1);
-                }
-              }
+              float g0, d0, g1, d1;
+              gelu_and_grad(v0, g0, d0);
+              gelu_and_grad(v1, g1, d1);
+              *reinterpret_cast<uint32_t*>(stg0 + so) = pack_bf16x2(d0, d1);  // gelu'(u): all backward needs from the pre-activation
+              *reinterpret_cast<uint32_t*>(stg1 + so) = pack_bf16x2(g0, g1);  // gelu(u)
+              continue;
+            }
+            if (EPI == EPI_RELU) {
+              uint32_t keep = 0xFFu;
+              if (args.drop.p > 0.f)
+                keep = dropout_keep8(dseed, args.drop.site, (static_cast<uint64_t>(m) * args.N + (n - fc)) >> 3, args.drop.thresh16);
+              v0 = fmaxf(v0, 0.f);
+              v1 = fmaxf(v1, 0.f);
+              v0 = ((keep >> fc) & 1u) ? v0 * args.drop.scale : 0.f;
+              v1 = ((keep >> (fc + 1)) & 1u) ? v1 * args.drop.scale : 0.f;
             } else if (EPI == EPI_ADD || EPI == EPI_MUL || EPI == EPI_DRELU) {
-#pragma unroll
-              for (int g = 0; g < 4; ++g) {
-                uint4 a = make_uint4(0, 0, 0, 0);
-                if (row_ok && nb + g * 8 + 8 <= args.N) a = __ldg(reinterpret_cast<const uint4*>(args.aux + m * args.ld_aux + nb + g * 8));
-                const uint32_t aw[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  const float2 x = unpack_bf16x2(aw[j]);
-                  float v0 = __uint_as_float(r[g * 8 + 2 * j]), v1 = __uint_as_float(r[g * 8 + 2 * j + 1]);
-                  if (EPI == EPI_ADD) {
-                    v0 += x.x;
-                    v1 += x.y;
-                  } else if (EPI == EPI_MUL) {
-                    v0 *= x.x;
-                    v1 *= x.y;
-                  } else {
-                    v0 = x.x > 0.f ? v0 * args.relu_scale : 0.f;
-                    v1 = x.y > 0.f ? v1 * args.relu_scale : 0.f;
-                  }
-                  o0[h * 16 + g * 4 + j] = pack_bf16x2(v0, v1);
-                }
+              float2 x = make_float2(0.f, 0.f);
+              if (m < args.M && n < args.N) x = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(args.aux + m * args.ld_aux + n)));
+              if (EPI == EPI_ADD) {
+                v0 += x.x;
+                v1 += x.y;
+              } else if (EPI == EPI_MUL) {
+                v0 *= x.x;
+                v1 *= x.y;
+              } else {
+                v0 = x.x > 0.f ? v0 * args.relu_scale : 0.f;
+                v1 = x.y > 0.f ? v1 * args.relu_scale : 0.f;
               }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) o0[h * 16 + j] = pack_bf16x2(__uint_as_float(r[2 * j]), __uint_as_float(r[2 * j + 1]));
             }
+            *reinterpret_cast<uint32_t*>(stg + so) = pack_bf16x2(v0, v1);
           }
-          if (c + 2 >= NBOX) {
-            // this thread's TMEM reads of the accumulator are done: hand it back to the MMA warp
-            tc_fence_before();
-            mbar_arrive_leader<CG>(&tempty_bar[acc]);
+          fence_proxy_async_smem();
+          wg_bar_sync(cw);
+          if (store_thread) {
+            tma_store_2d(&tm.d0, stg, n0 + c * 64, m0);
+            if (EPI == EPI_GELU) tma_store_2d(&tm.d1, stg1, n0 + c * 64, m0);
+            tma_store_commit();
           }
-          if (EPI == EPI_GELU) {
-            if (store_thread) tma_store_wait_read<0>();
-            epi_bar_sync(grp);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              stg_write16(stg0, row, j, make_uint4(o0[4 * j], o0[4 * j + 1], o0[4 * j + 2], o0[4 * j + 3]));
-              stg_write16(stg1, row, j, make_uint4(o1[4 * j], o1[4 * j + 1], o1[4 * j + 2], o1[4 * j + 3]));
-            }
-            fence_proxy_async_smem();
-            epi_bar_sync(grp);
-            if (store_thread) {
-              tma_store_2d(&tm.d0, stg0, n0 + c * 64, m0);
-              tma_store_2d(&tm.d1, stg1, n0 + c * 64, m0);
-              tma_store_commit();
-            }
-          } else {
-            uint8_t* stg = (box_seq & 1u) ? stg1 : stg0;
-            if (store_thread) tma_store_wait_read<1>();
-            epi_bar_sync(grp);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) stg_write16(stg, row, j, make_uint4(o0[4 * j], o0[4 * j + 1], o0[4 * j + 2], o0[4 * j + 3]));
-            fence_proxy_async_smem();
-            epi_bar_sync(grp);
-            if (store_thread) {
-              tma_store_2d(&tm.d0, stg, n0 + c * 64, m0);
-              tma_store_commit();
-            }
-            if (args.colsum != nullptr) {
-              // bias gradient = column sums of this output: fold the staged [128 x 64] bf16 tile (rows beyond M are zero).
-              // Two threads per column take 64 rows each; the buffer is not overwritten before the next-but-one barrier.
-              const int gt = (ew & 3) * 32 + lane;
-              const int col = gt & 63, r0 = (gt >> 6) * 64;
-              float acc_c = 0.f;
+          if (EPI != EPI_GELU && args.colsum != nullptr) {
+            // bias gradient = column sums of this output: fold the staged [64 x 64] bf16 box (rows beyond M are zero).
+            // Two threads per column take 32 rows each; the buffer is not overwritten before the next-but-one barrier.
+            const int col = t & 63, r0 = (t >> 6) * 32;
+            float acc_c = 0.f;
 #pragma unroll 8
-              for (int rr = r0; rr < r0 + 64; ++rr) {
-                const __nv_bfloat16 v = *reinterpret_cast<const __nv_bfloat16*>(stg + rr * 128 + (((col >> 3) ^ (rr & 7)) << 4) + (col & 7) * 2);
-                acc_c += __bfloat162float(v);
-              }
-              if (n0 + c * 64 + col < args.N) atomicAdd(args.colsum + n0 + c * 64 + col, acc_c);
+            for (int rr = r0; rr < r0 + 32; ++rr) {
+              const __nv_bfloat16 v = *reinterpret_cast<const __nv_bfloat16*>(stg + rr * 128 + (((col >> 3) ^ (rr & 7)) << 4) + (col & 7) * 2);
+              acc_c += __bfloat162float(v);
             }
-            ++box_seq;
+            if (n0 + c * 64 + col < args.N) atomicAdd(args.colsum + n0 + c * 64 + col, acc_c);
           }
+          ++box_seq;
         }
       }
     }
     if (store_thread) tma_store_wait<0>();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (CG == 2) cluster_sync_all();  // the peer may still be multicasting commits into / reading from this CTA
-  tc_fence_after();
-  if (warp == 1) {
-    __syncwarp();
-    tmem_dealloc_cg<TmemGeom<BN>::COLS, CG>(tmem_base);
   }
 }
 
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-static int g_force_cg = 0;  // bring-up switch (vlpk_debug_set_cta_group): 0 = auto, 1 / 2 = force
-void debug_set_cta_group(int cg) { g_force_cg = cg; }
-
-template <int BN, int CG, bool A_MN, bool B_MN, int EPI>
+template <bool A_MN, bool B_MN, int EPI>
 static int launch_inst(const GemmTmaps& tm, const GemmArgs& args, int num_work, cudaStream_t stream) {
-  constexpr int STAGES = StageCount<BN, CG>::value;
-  using L = SmemLayout<BN, CG, STAGES>;
-  auto kfn = gemm_kernel<BN, CG, A_MN, B_MN, EPI>;
+  constexpr int STAGES = StageCount::value;
+  using L = SmemLayout<STAGES>;
+  auto kfn = gemm_kernel<A_MN, B_MN, EPI>;
   static bool attr_set = false;  // benign race: idempotent
   if (!attr_set) {
     VLPK_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, L::DYN_BYTES));
     attr_set = true;
   }
-  const int max_clusters = gemm_sms() / CG;
-  const int clusters = num_work < max_clusters ? num_work : max_clusters;
+  const int max_ctas = gemm_sms();
+  const int ctas = num_work < max_ctas ? num_work : max_ctas;
   LaunchScope scope(A_MN ? CAT_GEMM_WGRAD : (B_MN ? CAT_GEMM_DGRAD : CAT_GEMM_FWD), 2.0 * args.M * args.N * args.K, stream);
-  VLPK_CUDA(launch_ex(kfn, dim3(clusters * CG), dim3(NUM_THREADS), L::DYN_BYTES, stream, CG, tm, args));
+  VLPK_CUDA(launch_ex(kfn, dim3(ctas), dim3(NUM_THREADS), L::DYN_BYTES, stream, 1, tm, args));
   return 0;
 }
 
-template <int BN, int CG>
 static int dispatch(const GemmDesc& g, const GemmTmaps& tm, const GemmArgs& args, int num_work, cudaStream_t s) {
   if (!g.a_mn && !g.b_mn) {
     switch (g.epi) {
-      case EPI_STORE: return launch_inst<BN, CG, false, false, EPI_STORE>(tm, args, num_work, s);
-      case EPI_GELU: return launch_inst<BN, CG, false, false, EPI_GELU>(tm, args, num_work, s);
-      case EPI_RELU: return launch_inst<BN, CG, false, false, EPI_RELU>(tm, args, num_work, s);
+      case EPI_STORE: return launch_inst<false, false, EPI_STORE>(tm, args, num_work, s);
+      case EPI_GELU: return launch_inst<false, false, EPI_GELU>(tm, args, num_work, s);
+      case EPI_RELU: return launch_inst<false, false, EPI_RELU>(tm, args, num_work, s);
       default: break;
     }
   } else if (!g.a_mn && g.b_mn) {
     switch (g.epi) {
-      case EPI_STORE: return launch_inst<BN, CG, false, true, EPI_STORE>(tm, args, num_work, s);
-      case EPI_ADD: return launch_inst<BN, CG, false, true, EPI_ADD>(tm, args, num_work, s);
-      case EPI_MUL: return launch_inst<BN, CG, false, true, EPI_MUL>(tm, args, num_work, s);
-      case EPI_DRELU: return launch_inst<BN, CG, false, true, EPI_DRELU>(tm, args, num_work, s);
-      case EPI_REDUCE_F32: return launch_inst<BN, CG, false, true, EPI_REDUCE_F32>(tm, args, num_work, s);  // split-K dgrad (MLM head)
+      case EPI_STORE: return launch_inst<false, true, EPI_STORE>(tm, args, num_work, s);
+      case EPI_ADD: return launch_inst<false, true, EPI_ADD>(tm, args, num_work, s);
+      case EPI_MUL: return launch_inst<false, true, EPI_MUL>(tm, args, num_work, s);
+      case EPI_DRELU: return launch_inst<false, true, EPI_DRELU>(tm, args, num_work, s);
+      case EPI_REDUCE_F32: return launch_inst<false, true, EPI_REDUCE_F32>(tm, args, num_work, s);  // split-K dgrad (MLM head)
       default: break;
     }
   } else if (g.a_mn && g.b_mn) {
-    if (g.epi == EPI_REDUCE_F32) return launch_inst<BN, CG, true, true, EPI_REDUCE_F32>(tm, args, num_work, s);
-    if (g.epi == EPI_STORE) return launch_inst<BN, CG, true, true, EPI_STORE>(tm, args, num_work, s);        // bf16 wgrad, no split-K
+    if (g.epi == EPI_REDUCE_F32) return launch_inst<true, true, EPI_REDUCE_F32>(tm, args, num_work, s);
+    if (g.epi == EPI_STORE) return launch_inst<true, true, EPI_STORE>(tm, args, num_work, s);        // bf16 wgrad, no split-K
   }
   set_error("gemm: unsupported (a_mn=%d, b_mn=%d, epi=%d) combination", (int)g.a_mn, (int)g.b_mn, g.epi);
   return -1;
 }
 
-template <int CG>
-static int dispatch_fwd192(const GemmDesc& g, const GemmTmaps& tm, const GemmArgs& args, int num_work, cudaStream_t s) {
-  switch (g.epi) {
-    case EPI_STORE: return launch_inst<192, CG, false, false, EPI_STORE>(tm, args, num_work, s);
-    case EPI_GELU: return launch_inst<192, CG, false, false, EPI_GELU>(tm, args, num_work, s);
-    case EPI_RELU: return launch_inst<192, CG, false, false, EPI_RELU>(tm, args, num_work, s);
-    default: break;
-  }
-  set_error("gemm: 192-wide tile requested for an unsupported epilogue %d", g.epi);
-  return -1;
-}
-
-// Cost model used to pick (tile N, CTA pairing, split-K): rounds of the persistent loop x per-tile cost, where the
-// mainloop cost per k-block is proportional to the operand bytes each SM pulls from L2 (128 rows of A + BN/CG rows of B)
-// and the epilogue cost to the BN columns each CTA drains.
-static double tile_cost(int M, int N, int total_kb, int bn, int cg, int splits, bool reduce) {
-  const int num_m = (M + BM * cg - 1) / (BM * cg);
-  const int num_n = (N + bn - 1) / bn;
+// Cost model used to pick split-K: rounds of the persistent loop x per-tile cost, where the mainloop cost per k-block is
+// proportional to the operand bytes each SM pulls from L2 (128 rows of A + BN rows of B) and the epilogue cost to the BN
+// columns each CTA drains.
+static double tile_cost(int M, int N, int total_kb, int splits, bool reduce) {
+  const int num_m = (M + BM - 1) / BM;
+  const int num_n = (N + BN - 1) / BN;
   const long long tiles = static_cast<long long>(num_m) * num_n * splits;
-  const int slots = gemm_sms() / cg;
+  const int slots = gemm_sms();
   const long long rounds = (tiles + slots - 1) / slots;
   const int kb_per = (total_kb + splits - 1) / splits;
-  const double mainloop = kb_per * (128.0 + double(bn) / cg);
-  const double epi = (reduce ? 3.0 : 1.5) * bn;
+  const double mainloop = kb_per * (128.0 + double(BN));
+  const double epi = (reduce ? 3.0 : 1.5) * BN;
   return rounds * (mainloop + epi + 60.0);
 }
 
-// Tile N, CTA-group size and split-K for one GEMM (pure host logic; exposed to the CPU tests as vlpk_debug_plan_gemm).
-int plan_gemm(const GemmDesc& g, int* bn_out, int* cg_out, int* splits_out) {
+// Tile N (always BN) and split-K for one GEMM (pure host logic; exposed to the CPU tests as vlpk_debug_plan_gemm).
+int plan_gemm(const GemmDesc& g, int* bn_out, int* splits_out) {
   const int seg_rows = g.nseg > 1 ? g.b_seg_rows : (g.b_mn ? g.K : g.N);
   const int total_kb = (g.K + BK - 1) / BK;
   const bool reduce = (g.epi == EPI_REDUCE_F32);
-  int bn = 128, cg = 1, splits = 1;
-  {
-    double best = 1e300;
-    for (int cbn : {128, 192, 256}) {
-      if (cbn == 192 && (g.b_mn || g.a_mn)) continue;  // 192-wide tiles are instantiated for forward (K-major) GEMMs only
-      if (g.bn != 0 && cbn != g.bn) continue;
-      if (g.nseg > 1 && !g.b_mn && seg_rows % cbn != 0) continue;
-      for (int ccg : {1, 2}) {
-        if (g_force_cg != 0 && ccg != g_force_cg) continue;
-        if (g.b_mn && (cbn / ccg) % 64 != 0) continue;  // MN-major B: a CTA's share is made of whole 64-wide boxes
-        const int max_s = reduce ? (total_kb / 8 > 0 ? total_kb / 8 : 1) : 1;
-        for (int s = 1; s <= max_s; ++s) {
-          if (reduce && g.splits > 0 && s != (g.splits < max_s ? g.splits : max_s)) continue;
-          const double c = tile_cost(g.M, g.N, total_kb, cbn, ccg, s, reduce);
-          if (c < best) {
-            best = c;
-            bn = cbn;
-            cg = ccg;
-            splits = s;
-          }
+  VLPK_CHECK_ARG(g.bn == 0 || g.bn == BN, "gemm: no valid tile configuration (bn=%d; tiles are %d wide)", g.bn, BN);
+  VLPK_CHECK_ARG(g.nseg == 1 || seg_rows % (g.b_mn ? BK : BN) == 0, "gemm: segment rows %d not tile aligned", seg_rows);
+  int splits = 1;
+  if (reduce) {
+    const int max_s = total_kb / 8 > 0 ? total_kb / 8 : 1;
+    if (g.splits > 0) {
+      splits = g.splits < max_s ? g.splits : max_s;
+    } else {
+      double best = 1e300;
+      for (int s = 1; s <= max_s; ++s) {
+        const double c = tile_cost(g.M, g.N, total_kb, s, reduce);
+        if (c < best) {
+          best = c;
+          splits = s;
         }
       }
     }
-    VLPK_CHECK_ARG(best < 1e300, "gemm: no valid tile configuration (bn=%d, segments of %d rows)", g.bn, seg_rows);
   }
-  if (g.nseg > 1) VLPK_CHECK_ARG(seg_rows % (g.b_mn ? BK : bn) == 0, "gemm: segment rows %d not tile aligned", seg_rows);
   if (splits > total_kb) splits = total_kb;
   {
     const int kb_per = (total_kb + splits - 1) / splits;
     splits = (total_kb + kb_per - 1) / kb_per;  // no empty splits
   }
-  *bn_out = bn;
-  *cg_out = cg;
+  *bn_out = BN;
   *splits_out = splits;
   return 0;
 }
@@ -637,9 +419,9 @@ int launch_gemm(const GemmDesc& g, cudaStream_t stream) {
   VLPK_CHECK_ARG(g.splits <= 1 || reduce, "gemm: split-K needs EPI_REDUCE_F32");
   VLPK_CHECK_ARG(g.b_rows == 0 || (g.nseg == 1 && g.b_rows <= (g.b_mn ? g.K : g.N)), "gemm: b_rows=%d needs a single B segment", g.b_rows);
 
-  // ---- choose tile N, CTA-group size and split-K
-  int bn = 128, cg = 1, splits = 1;
-  VLPK_TRY(plan_gemm(g, &bn, &cg, &splits));
+  // ---- choose tile N and split-K
+  int bn = BN, splits = 1;
+  VLPK_TRY(plan_gemm(g, &bn, &splits));
 
   GemmTmaps tm;
   memset(&tm, 0, sizeof(tm));
@@ -651,7 +433,7 @@ int launch_gemm(const GemmDesc& g, cudaStream_t stream) {
   for (int s = 0; s < g.nseg; ++s) {
     if (!g.b_mn) {
       const int rows = g.nseg > 1 ? seg_rows : (g.b_rows > 0 ? g.b_rows : g.N);
-      VLPK_TRY(make_tmap_2d(&tm.b[s], TM_BF16, g.B[s], g.K, rows, g.ldb, BK, bn / cg));
+      VLPK_TRY(make_tmap_2d(&tm.b[s], TM_BF16, g.B[s], g.K, rows, g.ldb, BK, bn));
     } else {
       const int rows = g.nseg > 1 ? seg_rows : (g.b_rows > 0 ? g.b_rows : g.K);
       VLPK_TRY(make_tmap_2d(&tm.b[s], TM_BF16, g.B[s], g.N, rows, g.ldb, 64, BK));
@@ -659,13 +441,20 @@ int launch_gemm(const GemmDesc& g, cudaStream_t stream) {
   }
   for (int s = g.nseg; s < 3; ++s) tm.b[s] = tm.b[0];
   if (reduce) {
-    VLPK_TRY(make_tmap_2d(&tm.d0, TM_F32, g.D0, g.N, g.M, g.ldd0, 32, BM));
+    // 3-D map [slices][M][N]: one slice, or one per split when the caller sums the splits itself
+    VLPK_CHECK_ARG(g.split_stride == 0 || (g.split_stride % 4 == 0 && g.split_stride >= static_cast<int64_t>(g.M) * g.ldd0),
+                   "gemm: split_stride %lld must be a multiple of 4 and cover M x ldd0", (long long)g.split_stride);
+    const uint64_t dims[3] = {static_cast<uint64_t>(g.N), static_cast<uint64_t>(g.M), static_cast<uint64_t>(g.split_stride ? splits : 1)};
+    const uint64_t strides[2] = {static_cast<uint64_t>(g.ldd0) * 4,
+                                 static_cast<uint64_t>(g.split_stride ? g.split_stride : static_cast<int64_t>(g.M) * g.ldd0) * 4};
+    const uint32_t box[3] = {32, 64, 1};
+    VLPK_TRY(make_tmap(&tm.d0, TM_F32, 3, g.D0, dims, strides, box));
     tm.d1 = tm.d0;
   } else {
-    VLPK_TRY(make_tmap_2d(&tm.d0, TM_BF16, g.D0, g.N, g.M, g.ldd0, 64, BM));
+    VLPK_TRY(make_tmap_2d(&tm.d0, TM_BF16, g.D0, g.N, g.M, g.ldd0, 64, 64));
     if (g.epi == EPI_GELU) {
       VLPK_CHECK_ARG(g.D1 != nullptr, "gemm: EPI_GELU needs D1");
-      VLPK_TRY(make_tmap_2d(&tm.d1, TM_BF16, g.D1, g.N, g.M, g.ldd1, 64, BM));
+      VLPK_TRY(make_tmap_2d(&tm.d1, TM_BF16, g.D1, g.N, g.M, g.ldd1, 64, 64));
     } else {
       tm.d1 = tm.d0;
     }
@@ -682,6 +471,7 @@ int launch_gemm(const GemmDesc& g, cudaStream_t stream) {
   a.K = g.K;
   a.b_seg_rows = seg_rows;
   a.splits = splits;
+  a.split_slices = (reduce && g.split_stride > 0) ? 1 : 0;
   for (int s = 0; s < 3; ++s) a.bias[s] = (s < g.nseg) ? g.bias[s] : nullptr;
   a.aux = g.aux;
   a.ld_aux = g.ld_aux;
@@ -689,14 +479,10 @@ int launch_gemm(const GemmDesc& g, cudaStream_t stream) {
   a.colsum = g.colsum;
   a.drop = g.drop;
 
-  const int num_m = (g.M + BM * cg - 1) / (BM * cg);
+  const int num_m = (g.M + BM - 1) / BM;
   const int num_n = (g.N + bn - 1) / bn;
   const int num_work = num_m * num_n * splits;
-  if (bn == 192) return cg == 2 ? dispatch_fwd192<2>(g, tm, a, num_work, stream) : dispatch_fwd192<1>(g, tm, a, num_work, stream);
-  if (bn == 256 && cg == 2) return dispatch<256, 2>(g, tm, a, num_work, stream);
-  if (bn == 256 && cg == 1) return dispatch<256, 1>(g, tm, a, num_work, stream);
-  if (bn == 128 && cg == 2) return dispatch<128, 2>(g, tm, a, num_work, stream);
-  return dispatch<128, 1>(g, tm, a, num_work, stream);
+  return dispatch(g, tm, a, num_work, stream);
 }
 
 }  // namespace vlpk

@@ -1,4 +1,4 @@
-// vlp_b200 — host-side description of one tcgen05 GEMM launch (see gemm.cu).
+// vlp_b200 — host-side description of one wgmma GEMM launch (see gemm.cu).
 #pragma once
 #include "common.cuh"
 
@@ -44,12 +44,14 @@ struct GemmDesc {
   DropoutCfg drop = {0.f, 1.f, 0u, 0ull, 0ull, nullptr};
   float* colsum = nullptr;  // optional [N] fp32: += column sums of the output (bias gradient of a dgrad output)
   int splits = 1;  // split-K (EPI_REDUCE_F32 only); 0 = choose automatically
-  int bn = 0;      // tile N (0 = auto)
+  // EPI_REDUCE_F32: 0 = every split reduce-adds into D0 (the order of the additions varies from run to run); > 0 = split s adds
+  // into its own slice D0 + s * split_stride (zeroed by the caller), which the caller then sums in a fixed order
+  int64_t split_stride = 0;
+  int bn = 0;      // tile N (0 = auto; 128 is the only width)
 };
 
 // Returns 0 on success, <0 on argument error, >0 cudaError_t.  Message via vlpk::set_error.
 int launch_gemm(const GemmDesc& g, cudaStream_t stream);
-void debug_set_cta_group(int cg);
-int plan_gemm(const GemmDesc& g, int* bn_out, int* cg_out, int* splits_out);
+int plan_gemm(const GemmDesc& g, int* bn_out, int* splits_out);
 
 }  // namespace vlpk

@@ -3,7 +3,7 @@
 //
 // The reference materialises fp32 logits [B*P, 28996] and runs softmax / NLL as separate passes; through torch on this stack
 // the three GEMMs additionally fall on legacy 2-byte-aligned kernels because 28996 is not a multiple of 8.  Here:
-//   forward : logits (bf16, leading dimension padded to a multiple of 8) from the tcgen05 GEMM with the bias in its epilogue —
+//   forward : logits (bf16, leading dimension padded to a multiple of 8) from the wgmma GEMM with the bias in its epilogue —
 //             the decoder weight is read in place, its 4 missing rows are zero-filled by TMA — then ONE pass per row for the
 //             online log-sum-exp and the loss;
 //   backward: dlogits = (softmax - onehot) * dloss in one pass (bf16), bias gradient by column sums, dh by a split-K GEMM over the
@@ -154,7 +154,22 @@ int launch_decoder_ce_bwd(const DecoderCeArgs& a, cudaStream_t s) {
     g.D0 = a.dh; g.ldd0 = a.H;
     g.epi = EPI_REDUCE_F32;
     g.splits = 0;
-    VLPK_TRY(launch_gemm(g, s));
+    int bn = 0;
+    VLPK_TRY(plan_gemm(g, &bn, &g.splits));
+    if (g.splits > 1) {
+      // dh feeds every activation gradient of the backward pass, so its sum must not depend on the order in which the splits
+      // finish: each split adds into its own zeroed slice and the slices are summed in a fixed order
+      const long long n = static_cast<long long>(a.R) * a.H;
+      float* part = scratch_f32(SCRATCH_SPLITK, static_cast<size_t>(n) * g.splits, s);
+      if (part == nullptr) return -1;
+      VLPK_CUDA(cudaMemsetAsync(part, 0, static_cast<size_t>(n) * g.splits * sizeof(float), s));
+      g.D0 = part;
+      g.split_stride = n;
+      VLPK_TRY(launch_gemm(g, s));
+      VLPK_TRY(launch_sum_parts(part, g.splits, n, a.dh, s));
+    } else {
+      VLPK_TRY(launch_gemm(g, s));
+    }
   }
   GemmDesc g;  // dW[V,H] (bf16) = dlogits^T h: both operands read MN-major, K = R fits one or a few k-blocks, direct store
   g.M = a.V; g.N = a.H; g.K = a.R;

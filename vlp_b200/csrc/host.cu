@@ -72,6 +72,39 @@ int make_tmap(CUtensorMap* out, TmapDtype dt, int rank, const void* base, const 
   return 0;
 }
 
+float* scratch_f32(int slot, size_t n, cudaStream_t s) {
+  struct Buf {
+    int dev, slot;
+    float* p;
+    size_t n;
+  };
+  static std::mutex mu;
+  static std::vector<Buf> bufs;  // superseded buffers stay allocated (graphs may still reference them)
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) {
+    set_error("scratch: no CUDA device");
+    return nullptr;
+  }
+  std::lock_guard<std::mutex> lk(mu);
+  Buf* best = nullptr;
+  for (auto& b : bufs)
+    if (b.dev == dev && b.slot == slot && (best == nullptr || b.n > best->n)) best = &b;
+  if (best != nullptr && best->n >= n) return best->p;
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(s, &cs) != cudaSuccess || cs != cudaStreamCaptureStatusNone) {
+    set_error("scratch: %zu floats needed for slot %d while a CUDA graph is being captured; run the step once before capturing", n, slot);
+    return nullptr;
+  }
+  float* p = nullptr;
+  const size_t want = best != nullptr && 2 * best->n > n ? 2 * best->n : n;
+  if (cudaMalloc(&p, want * sizeof(float)) != cudaSuccess) {
+    set_error("scratch: cudaMalloc of %zu floats failed", want);
+    return nullptr;
+  }
+  bufs.push_back(Buf{dev, slot, p, want});
+  return p;
+}
+
 bool pdl_enabled() {
   static int v = -1;
   if (v < 0) {
@@ -85,8 +118,8 @@ int num_sms() {
   static int n = 0;
   if (n == 0) {
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;  // no device visible (host-only planning): an H100 SXM
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }
@@ -97,9 +130,8 @@ int num_sms() {
 static int g_reserved_sms = 0;
 void set_reserved_sms(int n) { g_reserved_sms = n > 0 ? n : 0; }
 int gemm_sms() {
-  int n = num_sms() - g_reserved_sms;
-  if (n < 2) n = 2;
-  return n & ~1;  // CTA pairs
+  const int n = num_sms() - g_reserved_sms;
+  return n < 1 ? 1 : n;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -55,8 +55,14 @@ inline int make_tmap_2d(CUtensorMap* out, TmapDtype dt, const void* base, uint64
   return make_tmap(out, dt, 2, base, dims, strides, box);
 }
 
+// Library-owned fp32 device scratch for the ordered reductions, one buffer per slot and device.  Grow-only, and a buffer is
+// never freed, so CUDA graphs captured earlier keep valid pointers; growing is refused (nullptr, error set) while `s` is being
+// captured — the first call of a shape must run outside capture, as a graph's warm-up does.
+enum ScratchSlot { SCRATCH_ATTN_DBIAS = 0, SCRATCH_SPLITK = 1, SCRATCH_SLOTS = 2 };
+float* scratch_f32(int slot, size_t n, cudaStream_t s);
+
 int num_sms();
-// SMs available to the persistent GEMM grids: num_sms() minus what vlpk_set_reserved_sms put aside (default 0), even.
+// SMs available to the persistent GEMM grids: num_sms() minus what vlpk_set_reserved_sms put aside (default 0), at least 1.
 int gemm_sms();
 void set_reserved_sms(int n);
 

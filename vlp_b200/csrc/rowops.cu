@@ -620,6 +620,27 @@ int launch_colsum(const void* x, long long ld, long long M, int N, float* out, c
   return 0;
 }
 
+// out[i] += sum over p of part[p * n + i], added in the order p = 0, 1, ... : the fixed-order second stage of a reduction
+// whose first stage wrote one partial per CTA (attention bias gradients) or per split (split-K), so that the result does not
+// depend on the order in which those CTAs finish.
+__global__ void __launch_bounds__(256) sum_parts_kernel(const float* __restrict__ part, int parts, long long n, float* __restrict__ out) {
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    float t = 0.f;
+    for (int p = 0; p < parts; ++p) t += part[p * n + i];
+    out[i] += t;
+  }
+}
+
+int launch_sum_parts(const float* part, int parts, long long n, float* out, cudaStream_t s) {
+  VLPK_CHECK_ARG(part != nullptr && out != nullptr && parts >= 1 && n >= 1, "sum_parts: parts=%d n=%lld", parts, n);
+  long long blocks = (n + 255) / 256;
+  if (blocks > 4LL * num_sms()) blocks = 4LL * num_sms();
+  LaunchScope scope(CAT_MISC, 4.0 * n * (parts + 2), s);
+  sum_parts_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(part, parts, n, out);
+  VLPK_CUDA(cudaGetLastError());
+  return 0;
+}
+
 // Test support: the keep-decisions the kernels take for dropout site `site` under `seed`, element by element (1 = keep), produced by
 // the same dropout_keep8() every fused epilogue / row kernel calls — tests feed these masks to the fp32 oracle to check the
 // dropout-on (training) configuration numerically.

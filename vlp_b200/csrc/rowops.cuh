@@ -63,6 +63,8 @@ int launch_mask_pack(const void* mask, int dtype, int mode, int B, int rows, int
                      uint32_t* out, cudaStream_t s);
 int launch_mask_synth(const int* len_b, const int* mode, int len_a, int B, int L, uint32_t* out, cudaStream_t s);
 int launch_colsum(const void* x, long long ld, long long M, int N, float* out, cudaStream_t s);
+// out[i] += sum_{p < parts} part[p * n + i], in the order p = 0, 1, ... (the same bits on every run)
+int launch_sum_parts(const float* part, int parts, long long n, float* out, cudaStream_t s);
 int launch_f32_to_bf16(const float* x, void* y, long long n, cudaStream_t s);
 int launch_dropout_mask(const DropoutCfg& d, long long n, unsigned char* out, cudaStream_t s);
 

@@ -1,7 +1,7 @@
 """Data-parallel gradient all-reduce for the VLP hot path (SURVEY.md §8e / a19: the path shards by batch; the one collective
 is the mean of all gradients per step — `DistributedDataParallel` in the reference, vlp/run_img2txt_dist.py:386).
 
-torch DDP works unchanged on vlp_b200 modules.  This module is the B200-first alternative used by bench.py: the fused
+torch DDP works unchanged on vlp_b200 modules.  This module is the H100-first alternative used by bench.py: the fused
 encoder backward already produces each layer group's gradients as ONE contiguous bf16 arena, so the arena itself is handed to
 NCCL (`all_reduce`, AVG, asynchronously, the moment the group's backward finishes) while earlier groups are still computing —
 no per-parameter bucket copies, no autograd hooks, no graph walk for unused parameters.

@@ -1,9 +1,9 @@
 """Whole-step CUDA-graph replay of the VLP training step (forward + backward through the module surface).
 
-The fused hot path issues ~330 kernel launches per 6.7 ms step (12 x BertLayer forward/backward, region projections, embeddings,
-heads); driven from Python — torch modules, autograd Functions, ctypes calls — the host needs ~5.9 ms per step to enqueue them, i.e.
-it is barely ahead of the device and every hiccup (GC, loader work, H2D bookkeeping) stalls the GPU: the round-2 end-to-end number sat
-14 % below the device-resident one.  `GraphedStep` captures the launch sequence of one step once and replays it:
+The fused hot path issues ~330 kernel launches per step (12 x BertLayer forward/backward, region projections, embeddings, heads);
+driven from Python — torch modules, autograd Functions, ctypes calls — the host needs several milliseconds per step to enqueue them,
+so every hiccup (GC, loader work, H2D bookkeeping) can stall the GPU.  `GraphedStep` captures the launch sequence of one step once and
+replays it:
 
     gstep = GraphedStep(model, example_batch, step)      # step(model, batch) -> loss ; must call loss.backward() itself
     for batch in loader:                                  # batch: dict of CUDA tensors (e.g. from staging.BatchStager.get())

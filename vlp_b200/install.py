@@ -3,7 +3,7 @@
 The reference drivers import their model classes with
     from pytorch_pretrained_bert.modeling import BertForPreTrainingLossMask      (vlp/run_img2txt_dist.py:24)
     from pytorch_pretrained_bert.modeling import BertForSeq2SeqDecoder           (vlp/decode_img2txt.py:20)
-`install()` makes those names resolve to the B200-native classes of vlp_b200.vlp_modules, either by rebinding them in
+`install()` makes those names resolve to the H100-native classes of vlp_b200.vlp_modules, either by rebinding them in
 an already-imported reference `modeling` module or — when the reference package cannot be imported on this stack
 (boto3 / torch._six / apex, SURVEY.md §8c) — by registering vlp_b200.vlp_modules itself as `pytorch_pretrained_bert.modeling`.
 """

@@ -1,4 +1,4 @@
-"""BertAdam on B200 — same constructor, param-group keys, state keys and schedule functions as the reference's
+"""BertAdam on H100 — same constructor, param-group keys, state keys and schedule functions as the reference's
 pytorch_pretrained_bert/optimization.py:32-182 (imported by vlp/run_img2txt_dist.py:25, built at :422-426), with `step()`
 executed by two launches of libvlpk.so (`vlpk_bertadam_step`, csrc/optim.cu) over ALL parameters instead of the reference's
 Python loop of ~400 tensors x (norm + host read-back + 6 elementwise kernels).
@@ -222,7 +222,7 @@ class BertAdam(Optimizer):
         n = len(tab)
         chunk = L.lib().vlpk_bertadam_chunk()
         # The descriptor table travels through PINNED host memory: an asynchronous copy from pageable memory synchronises the host
-        # with the stream, i.e. with the whole backward that is still in flight — a pipeline bubble of ~1 ms per step on a B200.
+        # with the stream, i.e. with the whole backward that is still in flight — a pipeline bubble every step.
         # Three rotating slots: a slot is rewritten two steps after its copy was enqueued (the copy has long completed by then).
         slot = self._pinned.setdefault((device, n), {"i": 0, "bufs": [None, None, None]})
         k = slot["i"] = (slot["i"] + 1) % 3

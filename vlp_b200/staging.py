@@ -1,9 +1,9 @@
-"""Input staging for the B200 hot path (SURVEY.md §8f-4): what sits between the data loader and `model(...)`.
+"""Input staging for the H100 hot path (SURVEY.md §8f-4): what sits between the data loader and `model(...)`.
 
 The reference loader (vlp/seq2seq_loader.py:229-359, stacked by vlp/loader_utils.py) hands the training loop, per step and per GPU,
 fp32 region features [B,100,2048] + [B,100,1607] and an int64 [B,123,123] self-attention mask — 1.58 MB per sample, 101 MB per
 64-sample batch — which run_img2txt_dist.py:463 copies synchronously (`t.to(device)`).  At 6.7 ms per step that copy is a
-quarter of the PCIe budget and the int64 mask is pure redundancy.  This module provides the B200-first replacement:
+quarter of the PCIe budget and the int64 mask is pure redundancy.  This module provides the H100-first replacement:
 
   * `mask_descriptor` / `PackedAttentionMask.synthesize`: the mask travels as three integers per sample (len_a, len_b, mode) and
     is synthesised on the device, directly in the 128-bit-per-row packed form the attention kernels consume (`vlpk_mask_synth`,

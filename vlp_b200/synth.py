@@ -1,7 +1,7 @@
 """Deterministic synthetic weights and batches in the exact tuple layout VLP's loader produces.
 
 The hot path's input contract is the 12-tuple returned by Preprocess4Seq2seq.__call__
-(/root/reference/vlp/seq2seq_loader.py:229-359, stacked by vlp/loader_utils.py:17-24); SURVEY.md §8d
+(the reference's vlp/seq2seq_loader.py:229-359, stacked by vlp/loader_utils.py:17-24); SURVEY.md §8d
 specifies the synthetic generators used for parity and benchmarking.  Everything is generated on CPU
 from a torch.Generator so that the same seed gives bit-identical tensors in every process (tests,
 bench, oracle, golden-vector script).

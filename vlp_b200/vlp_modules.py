@@ -1,7 +1,7 @@
-"""The reference's nn.Module surface, rebuilt on the sm_100a kernels of libvlpk.so.
+"""The reference's nn.Module surface, rebuilt on the sm_90a kernels of libvlpk.so.
 
 Same class names, constructor / forward signatures, attribute paths and state_dict keys as
-/root/reference/pytorch_pretrained_bert/modeling.py, so vlp/run_img2txt_dist.py, vlp/decode_img2txt.py and
+the reference's pytorch_pretrained_bert/modeling.py, so vlp/run_img2txt_dist.py, vlp/decode_img2txt.py and
 vlp/eval_vqa2.py can call these classes unchanged (see vlp_b200/install.py and INTEGRATION.md).  The module
 tree exists to own the named parameters; the arithmetic of the hot path — region projections, embeddings,
 the BertLayer stack and their backward — runs in hand-written CUDA through vlp_b200.ops.  There is no eager
