@@ -1,0 +1,265 @@
+"""Tile-local checks for the GEMM and attention kernels: fp64 references of the same bf16 inputs, an elementwise rounding bound,
+a per-block rel-L2 bound and NaN guard bands around every output.
+
+A global rel-L2 over a whole output dilutes a defect in one tile by the square root of the tile count, so a box that is never
+written, a missing k-block or a wrong 64-row half passes it at production sizes.  Here every output is held to
+
+    |got - ref| <= r * |ref| + a * E          (elementwise; r = one bf16 rounding for bf16 outputs, 0 for fp32 outputs)
+    ||got - ref||_blk / ||ref||_blk <= bound  (per 128 x 128 GEMM tile, per (sequence, head) attention block)
+
+where E is the magnitude the kernel's fp32 sums run over: |A| |B|^T for a GEMM (times the epilogue's Lipschitz factor), P |V| for
+the attention context and |P|^T |dO| for dV.  Failures name the worst block, its error and its bound.  Every function here runs on
+whatever device its tensors live on; nothing needs a GPU except the helpers that call the library (replayed dropout masks).
+"""
+import math
+
+import torch
+
+BF = torch.bfloat16
+F64 = torch.float64
+
+# ---- bounds ------------------------------------------------------------------------------------------------------------------
+# Kept at >= 2x the worst value observed on the H100 (80 GB HBM3) with the kernels at this commit; DESIGN.md §6 lists the ceilings.
+R_BF16 = 2.0 ** -8            # one bf16 rounding (relative)
+GEMM_A = 2.0 ** -16           # fp32 accumulation, per unit of |A||B|^T
+GEMM_TILE_BF16 = 6e-3         # rel-L2 of one 128 x 128 tile, bf16 output
+GEMM_TILE_F32 = 2e-5          # rel-L2 of one 128 x 128 tile, fp32 output
+ATTN_A = 2.0 ** -7            # P is rounded to bf16 before P V / P^T dO / dS K: one rounding of every summand, with 2x slack
+ATTN_FWD_BLOCK = 6e-3         # rel-L2 of ctx per (sequence, head)
+ATTN_LSE = 2e-5               # |lse - ref| <= ATTN_LSE * (1 + |ref|)
+ATTN_BWD_BLOCK = 2e-2         # rel-L2 of dq / dk / dv per (sequence, head)
+SUM_REL = 1e-5                # fp32 column sums (bias gradients): |got - ref| <= SUM_REL * sum |x|
+
+TILE = 128
+
+# NaN bit patterns of the guard bands (quiet NaN with a payload no arithmetic produces)
+_GUARD = {BF: (torch.int16, 0x7FA5), torch.float32: (torch.int32, 0x7FA5A5A5)}
+
+
+class CheckError(AssertionError):
+    pass
+
+
+# ---- guard bands -------------------------------------------------------------------------------------------------------------
+def guarded(rows, cols, ld=None, dtype=BF, extra_rows=2, col0=0, device="cuda"):
+    """A [rows, cols] view with leading dimension `ld` (default cols) that starts `col0` elements into its row, inside a buffer
+    with `extra_rows` more rows.  The whole buffer, the view included, is filled with a NaN bit pattern: an element the kernel
+    should write and does not stays NaN, and assert_guard_intact() checks that everything outside the view is bit-identical."""
+    ld = cols + col0 if ld is None else ld
+    assert ld >= col0 + cols
+    ity, pat = _GUARD[dtype]
+    n = (rows + extra_rows) * ld
+    buf = torch.empty(n, dtype=dtype, device=device)
+    buf.view(ity).fill_(pat)
+    view = buf.as_strided((rows, cols), (ld, 1), col0)
+    band = torch.ones(n, dtype=torch.bool, device=device)
+    band.as_strided((rows, cols), (ld, 1), col0).fill_(False)
+    view._guard = (buf, band, ity, pat)
+    return view
+
+
+def guard_fill(view, values):
+    """Write `values` into a guarded view (prior contents of a reduce-add target) without touching the band."""
+    view.copy_(values.to(view.dtype))
+    return view
+
+
+def assert_guard_intact(view, name="output"):
+    buf, band, ity, pat = view._guard
+    bad = (buf.view(ity) != pat) & band
+    if bool(bad.any()):
+        idx = int(bad.nonzero()[0, 0])
+        ld = view.stride(0)
+        raise CheckError(f"{name}: {int(bad.sum())} guard element(s) overwritten outside the [{view.shape[0]}, {view.shape[1]}] view "
+                         f"(first at buffer row {idx // ld}, column {idx % ld}; ld {ld}, view starts at column {view.storage_offset()})")
+
+
+# ---- references --------------------------------------------------------------------------------------------------------------
+def gelu64(u):
+    return 0.5 * u * (1.0 + torch.erf(u / math.sqrt(2.0)))
+
+
+def gelu_grad64(u):
+    return 0.5 * (1.0 + torch.erf(u / math.sqrt(2.0))) + u * torch.exp(-0.5 * u * u) / math.sqrt(2.0 * math.pi)
+
+
+def gemm_ref(A, B):
+    """A [M,K], B [N,K] (any float dtype, logical K-major views) -> (A B^T, |A| |B|^T) in fp64."""
+    A64, B64 = A.to(F64), B.to(F64)
+    return A64 @ B64.t(), A64.abs() @ B64.abs().t()
+
+
+def epilogue_ref(epi, acc, E, bias=None, aux=None, prior=None, keep=None, scale=1.0):
+    """fp64 reference of each gemm.cuh epilogue on top of acc = A B^T.  Returns {output name: (ref, E scaled by the epilogue's
+    Lipschitz factor)}; `keep` (0/1, same shape) and `scale` are the dropout keep mask and 1/(1-p) (RELU) or the relu scale
+    (DRELU)."""
+    u = acc if bias is None else acc + bias.to(F64)
+    x = None if aux is None else aux.to(F64)
+    if epi == 0:       # STORE
+        return {"d0": (u, E)}
+    if epi == 1:       # GELU: D0 = gelu'(u), D1 = gelu(u)
+        return {"d0": (gelu_grad64(u), E), "d1": (gelu64(u), E)}
+    if epi == 2:       # RELU (+ dropout)
+        k = torch.ones_like(u) if keep is None else keep.to(F64)
+        return {"d0": (torch.relu(u) * k * scale, E * scale)}
+    if epi == 3:       # ADD
+        return {"d0": (acc + x, E)}
+    if epi == 4:       # MUL
+        return {"d0": (acc * x, E * x.abs())}
+    if epi == 5:       # DRELU
+        return {"d0": (torch.where(x > 0, acc * scale, torch.zeros_like(acc)), E * scale)}
+    if epi == 6:       # REDUCE_F32: prior contents + product; the prior is one more summand of the fp32 sum
+        p = torch.zeros_like(acc) if prior is None else prior.to(F64)
+        return {"d0": (p + acc, E + p.abs())}
+    raise ValueError(epi)
+
+
+def attn_ref(q, k, v, allow, keep=None, p=0.0):
+    """fp64 attention forward with the reference semantics (modeling.py:279-302): additive -10000 where `allow` is False, scale
+    1/8, keys >= Lkv absent (k/v carry exactly Lkv rows), dropout keep mask scaled by 1/(1-p).
+    q [B,h,Lq,64], k/v [B,h,Lkv,64], allow [B,Lq,Lkv] bool.  Returns dict(ctx, lse, P, Pd, E)."""
+    q, k, v = q.to(F64), k.to(F64), v.to(F64)
+    s = q @ k.transpose(-1, -2) / 8.0 + (~allow[:, None]).to(F64) * -10000.0
+    P = torch.softmax(s, -1)
+    Pd = P if keep is None else P * keep.to(F64) / (1.0 - p)
+    return {"ctx": Pd @ v, "lse": torch.logsumexp(s, -1), "P": P, "Pd": Pd, "E": Pd @ v.abs()}
+
+
+def attn_bwd_ref(q, k, v, allow, dO, keep=None, p=0.0):
+    """fp64 gradients of attn_ref's ctx for upstream dO [B,h,Lq,64]: dict(dq, dk, dv, E_dq, E_dk, E_dv).
+    dS = P (dP - sum_j P dP); its magnitude E_dS = P (|dP| + sum_j P |dP|) carries into E_dq = E_dS |K| / 8 and E_dk."""
+    f = attn_ref(q, k, v, allow, keep, p)
+    q, k, v, dO = q.to(F64), k.to(F64), v.to(F64), dO.to(F64)
+    P, Pd = f["P"], f["Pd"]
+    dPd = dO @ v.transpose(-1, -2)
+    dP = dPd if keep is None else dPd * keep.to(F64) / (1.0 - p)
+    dS = P * (dP - (P * dP).sum(-1, keepdim=True))
+    E_dS = P * (dP.abs() + (P * dP.abs()).sum(-1, keepdim=True))
+    return {"dq": dS @ k / 8.0, "dk": dS.transpose(-1, -2) @ q / 8.0, "dv": Pd.transpose(-1, -2) @ dO,
+            "E_dq": E_dS @ k.abs() / 8.0, "E_dk": E_dS.transpose(-1, -2) @ q.abs() / 8.0,
+            "E_dv": Pd.abs().transpose(-1, -2) @ dO.abs(), "fwd": f}
+
+
+def bits_to_allow(bits, Lq, Lkv):
+    """int32 [B, rows, 4] attend bitmask (rows 1 = broadcast) -> bool [B, Lq, Lkv] as the kernels read it (bits >= Lkv ignored)."""
+    b = bits.to(torch.int64) & 0xFFFFFFFF
+    cols = torch.arange(Lkv, device=bits.device)
+    allow = ((b[:, :, cols // 32] >> (cols % 32)) & 1).bool()
+    return allow.expand(bits.shape[0], Lq, Lkv) if bits.shape[1] == 1 else allow[:, :Lq]
+
+
+# ---- bounds ------------------------------------------------------------------------------------------------------------------
+def _fmt_ratio(err, bound):
+    return err / bound if bound > 0 else (0.0 if err == 0 else math.inf)
+
+
+def check_elementwise(name, got, ref, E, r, a, where=None):
+    """|got - ref| <= r |ref| + a E everywhere (NaN fails).  Raises CheckError naming the worst element (and through
+    `where(row, col)` its tile or block).  Returns the largest share of the a E term used, max((|got - ref| - r |ref|)+ / (a E)):
+    the r term is the exact worst case of the final rounding, a is the tolerance being calibrated (a = 0: the full ratio)."""
+    g = got.to(F64)
+    diff = (g - ref).abs()
+    bound = r * ref.abs() + a * E
+    ratio = torch.where(bound > 0, diff / bound.clamp_min(1e-300), torch.where(diff == 0, torch.zeros_like(diff), torch.full_like(diff, math.inf)))
+    ratio = torch.where(torch.isnan(g), torch.full_like(ratio, math.inf), ratio)
+    worst = float(ratio.max()) if ratio.numel() else 0.0
+    if not worst <= 1.0:
+        flat = int(ratio.reshape(-1).argmax())
+        idx = []
+        for s in reversed(ratio.shape):
+            idx.append(flat % s)
+            flat //= s
+        idx = tuple(reversed(idx))
+        n_bad = int((ratio > 1.0).sum())
+        loc = where(*idx) if where is not None else f"index {idx}"
+        raise CheckError(f"{name}: {n_bad} element(s) over the elementwise bound; worst at {loc}: got {float(g[idx]):.6g} ref "
+                         f"{float(ref[idx]):.6g} |err| {float(diff[idx]):.3e} > bound {float(bound[idx]):.3e} "
+                         f"(r={r:.3g}, a={a:.3g}, E={float(E[idx]):.3e})")
+    if a == 0 or not ratio.numel():
+        return worst
+    aE = a * E
+    used = torch.where(aE > 0, (diff - r * ref.abs()).clamp_min(0) / aE.clamp_min(1e-300), torch.zeros_like(aE))
+    return float(used.max())
+
+
+def tile_rel_l2(got, ref, tile=TILE):
+    """Per-tile rel-L2 of a 2-D output: (err [tm, tn], ref norm [tm, tn])."""
+    M, N = ref.shape
+    tm, tn = -(-M // tile), -(-N // tile)
+    d = torch.zeros(tm * tile, tn * tile, dtype=F64, device=ref.device)
+    rr = torch.zeros_like(d)
+    d[:M, :N] = got.to(F64) - ref
+    rr[:M, :N] = ref
+    d2 = d.view(tm, tile, tn, tile).pow(2).sum((1, 3))
+    r2 = rr.view(tm, tile, tn, tile).pow(2).sum((1, 3))
+    return d2.sqrt(), r2.sqrt()
+
+
+def _check_blocks(name, err, nrm, bound, label):
+    """err / nrm per block <= bound (a scalar or one bound per block), skipping blocks whose reference is zero.  Returns the
+    worst rel / bound."""
+    bound = torch.as_tensor(bound, dtype=F64, device=err.device).expand_as(err)
+    live = nrm > 0
+    rel = torch.where(live, err / nrm.clamp_min(1e-300), torch.zeros_like(err))
+    rel = torch.where(torch.isnan(err) & live, torch.full_like(rel, math.inf), rel)
+    ratio = rel / bound
+    worst = float(ratio.max()) if ratio.numel() else 0.0
+    if not worst <= 1.0:
+        idx = tuple(int(i) for i in (ratio == ratio.max()).nonzero()[0]) if not math.isnan(worst) else (0,) * rel.dim()
+        n_bad = int((ratio > 1.0).sum())
+        raise CheckError(f"{name}: {n_bad} block(s) over the rel-L2 bound; worst {label(*idx)} rel-L2 {float(rel[idx]):.3e} > bound "
+                         f"{float(bound[idx]):.3e}")
+    return worst
+
+
+def check_gemm(name, got, ref, E, a=GEMM_A, tile_bound=None):
+    """One GEMM output against its fp64 reference.  Returns (elementwise worst / bound, tile worst / bound)."""
+    f32 = got.dtype == torch.float32
+    r = 0.0 if f32 else R_BF16
+    tb = tile_bound if tile_bound is not None else (GEMM_TILE_F32 if f32 else GEMM_TILE_BF16)
+    assert got.shape == ref.shape, (got.shape, ref.shape)
+    e = check_elementwise(name, got, ref, E, r, a, where=lambda i, j: f"row {i} col {j} (tile m={i // TILE} n={j // TILE})")
+    err, nrm = tile_rel_l2(got, ref)
+    t = _check_blocks(name, err, nrm, tb, lambda i, j: f"tile m={i} n={j} (rows {i * TILE}.., cols {j * TILE}..)")
+    return e, t
+
+
+def heads_view(t, B, L, heads):
+    """[B*L, ld] or [B, L, ld] rows with head-major columns -> [B, heads, L, 64]."""
+    return t.reshape(B, L, -1)[..., :heads * 64].reshape(B, L, heads, 64).permute(0, 2, 1, 3)
+
+
+def check_attn_block(name, got, ref, E, block_bound, a=ATTN_A, conditioned=False):
+    """got/ref/E [B, heads, L, 64]: elementwise bound (r = one bf16 rounding) and rel-L2 per (sequence, head).
+    conditioned=True (backward): a block's bound is at least R_BF16 ||E|| / ||ref||.  dq = dS K / 8 with dS rounded to bf16 for
+    the tensor core; when the keys share a common component, or a row attends to nothing and P is nearly one-hot, the exact dq
+    cancels far below |dS| |K| and one rounding of dS is that much larger relative to it."""
+    B, h = ref.shape[:2]
+    e = check_elementwise(name, got, ref, E, R_BF16, a, where=lambda b, hh, i, j: f"b={b} h={hh} row {i} col {j}")
+    d = (got.to(F64) - ref).pow(2).sum((2, 3)).sqrt()
+    n = ref.pow(2).sum((2, 3)).sqrt()
+    bound = block_bound
+    if conditioned:
+        bound = torch.maximum(torch.full_like(n, block_bound), R_BF16 * E.pow(2).sum((2, 3)).sqrt() / n.clamp_min(1e-300))
+    t = _check_blocks(name, d, n, bound, lambda b, hh: f"block b={b} h={hh}")
+    return e, t
+
+
+def check_lse(name, got, ref, tol=ATTN_LSE):
+    """|lse - ref| <= tol (1 + |ref|); got/ref [B, heads, Lq]."""
+    diff = (got.to(F64) - ref).abs()
+    bound = tol * (1.0 + ref.abs())
+    ratio = torch.where(torch.isnan(diff), torch.full_like(diff, math.inf), diff / bound)
+    worst = float(ratio.max())
+    if not worst <= 1.0:
+        b, h, i = (int(x) for x in (ratio == ratio.max()).nonzero()[0]) if not math.isnan(worst) else (0, 0, 0)
+        raise CheckError(f"{name}: worst at b={b} h={h} row {i}: got {float(got[b, h, i]):.8g} ref {float(ref[b, h, i]):.8g} "
+                         f"|err| {float(diff[b, h, i]):.3e} > bound {float(bound[b, h, i]):.3e}")
+    return worst
+
+
+def check_colsum(name, got, x):
+    """fp32 column sums (a bias gradient) of x [M, N] against the fp64 sums: |got - ref| <= SUM_REL * sum |x| per column."""
+    x64 = x.to(F64)
+    ref, mag = x64.sum(0), x64.abs().sum(0)
+    return check_elementwise(name, got.to(F64), ref, mag, 0.0, SUM_REL, where=lambda j: f"column {j}")
