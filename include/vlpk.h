@@ -243,6 +243,14 @@ int vlpk_decoder_ce_fwd(int R, int V, int H, const void* h, const void* w, const
  * dw [V,H] bf16 (overwritten), dbias [Vp] fp32 (ZEROED by the caller). */
 int vlpk_decoder_ce_bwd(int R, int V, int H, const void* h, const void* w, const int64_t* labels, const void* logits, const float* lse,
                         const float* dloss, void* dlogits, float* dh, void* dw, float* dbias, void* stream);
+/* The same pair with the label-smoothed loss of LabelSmoothingLoss (loss.py:12-48, crit_mask_lm_smoothed, modeling.py:995-999,
+ * 1104-1106) in place of the cross-entropy; arguments as above plus eps in (0, 1] (V >= 3, otherwise rc < 0 and nothing runs).
+ * Target of a row with label t: q_0 = 0, q_t = 1 - eps, eps / (V - 2) elsewhere.  Label 0 (the reference's ignore index) and labels
+ * outside [0,V) are ignored positions: loss 0, dlogits row 0.  loss = KL(q || softmax(logits)), dlogits = (softmax - q) * dloss. */
+int vlpk_decoder_ce_ls_fwd(int R, int V, int H, float eps, const void* h, const void* w, const void* bias_pad, const int64_t* labels,
+                           void* logits, float* lse, float* loss, void* stream);
+int vlpk_decoder_ce_ls_bwd(int R, int V, int H, float eps, const void* h, const void* w, const int64_t* labels, const void* logits,
+                           const float* lse, const float* dloss, void* dlogits, float* dh, void* dw, float* dbias, void* stream);
 
 /* ---- optimizer (SURVEY.md §8f-1) ----------------------------------------------------------------------------------------
  * One parameter tensor of a BertAdam step.  64 bytes; the table is read by the kernels from DEVICE memory. */

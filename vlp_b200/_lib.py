@@ -102,6 +102,8 @@ _SIGS = {
                                  C.POINTER(VlpkBwdScratch), c_float, c_float, C.POINTER(VlpkDropout), _P]),
     "vlpk_decoder_ce_fwd": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
     "vlpk_decoder_ce_bwd": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "vlpk_decoder_ce_ls_fwd": (c_int, [c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "vlpk_decoder_ce_ls_bwd": (c_int, [c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "vlpk_bertadam_chunk": (c_int, []),
     "vlpk_bertadam_step": (c_int, [_P, _P, _P, _P, c_int, _P, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, _P]),
     "vlpk_profile_enable": (None, [c_int]),

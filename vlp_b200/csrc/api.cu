@@ -697,6 +697,33 @@ int vlpk_decoder_ce_bwd(int R, int V, int H, const void* h, const void* w, const
   return launch_decoder_ce_bwd(a, S(stream));
 }
 
+int vlpk_decoder_ce_ls_fwd(int R, int V, int H, float eps, const void* h, const void* w, const void* bias_pad, const int64_t* labels,
+                           void* logits, float* lse, float* loss, void* stream) {
+  VLPK_CHECK_ARG(eps > 0.f && eps <= 1.f && V >= 3, "decoder_ce_ls: label smoothing %g with V=%d (needs 0 < eps <= 1, V >= 3)",
+                 static_cast<double>(eps), V);
+  DecoderCeArgs a;
+  a.R = R; a.V = V; a.H = H; a.eps = eps;
+  a.h = h; a.w = w; a.bias_pad = bias_pad;
+  a.labels = reinterpret_cast<const long long*>(labels);
+  a.logits = logits; a.dlogits = logits;  // (alignment check only)
+  a.lse = lse; a.loss = loss;
+  return launch_decoder_ce_fwd(a, S(stream));
+}
+
+int vlpk_decoder_ce_ls_bwd(int R, int V, int H, float eps, const void* h, const void* w, const int64_t* labels, const void* logits,
+                           const float* lse, const float* dloss, void* dlogits, float* dh, void* dw, float* dbias, void* stream) {
+  VLPK_CHECK_ARG(eps > 0.f && eps <= 1.f && V >= 3, "decoder_ce_ls: label smoothing %g with V=%d (needs 0 < eps <= 1, V >= 3)",
+                 static_cast<double>(eps), V);
+  DecoderCeArgs a;
+  a.R = R; a.V = V; a.H = H; a.eps = eps;
+  a.h = h; a.w = w;
+  a.labels = reinterpret_cast<const long long*>(labels);
+  a.logits = const_cast<void*>(logits);
+  a.lse = const_cast<float*>(lse);
+  a.dloss = dloss; a.dlogits = dlogits; a.dh = dh; a.dw = dw; a.dbias = dbias;
+  return launch_decoder_ce_bwd(a, S(stream));
+}
+
 int vlpk_bertadam_chunk(void) { return ADAM_CHUNK; }
 
 int vlpk_bertadam_step(const VlpkAdamTensor* tensors_host, const VlpkAdamTensor* tensors_dev, const int32_t* chunk_prefix_host,

@@ -21,6 +21,9 @@ struct DecoderCeArgs {
   float* dh = nullptr;           // [R,H]  fp32, zeroed by the caller (split-K reduce-add target)
   void* dw = nullptr;            // [V,H]  bf16, overwritten
   float* dbias = nullptr;        // [Vp]   fp32, zeroed by the caller
+  // label smoothing (LabelSmoothingLoss, ignore index 0): 0 = plain cross-entropy; otherwise eps in (0, 1] and V >= 3, the target
+  // is q_0 = 0, q_label = 1 - eps, q_j = eps / (V - 2) elsewhere, and label 0 is an ignored position as well
+  float eps = 0.f;
 };
 
 int launch_decoder_ce_fwd(const DecoderCeArgs& a, cudaStream_t s);

@@ -388,12 +388,18 @@ class EmbedFn(torch.autograd.Function):
 # ------------------------------------------------------------------------------------------------
 class DecoderCEFn(torch.autograd.Function):
     """loss[r] = CE(h[r] W^T + bias, labels[r]) (modeling.py:478-482 + 1108-1109) without fp32 logits; also returns the bf16
-    logits [R,V] (non-differentiable view, kept for `last_prediction_scores`)."""
+    logits [R,V] (non-differentiable view, kept for `last_prediction_scores`).
+
+    label_smoothing > 0 selects the smoothed loss of crit_mask_lm_smoothed instead (modeling.py:995-999, 1104-1106): per row the
+    KL divergence from the target q (q_0 = 0, q_label = 1 - eps, eps / (V - 2) elsewhere) to softmax(logits), with label 0 ignored
+    (vlpk_decoder_ce_ls_fwd/bwd).  0 keeps the cross-entropy calls."""
 
     @staticmethod
-    def forward(ctx, h, w, bias, labels, dp_hook=None):
+    def forward(ctx, h, w, bias, labels, dp_hook=None, label_smoothing=0.0):
         _require_cuda(h, "decoder input")
         ctx.dp_hook = dp_hook
+        eps = float(label_smoothing)
+        ctx.eps = eps
         R, H = h.shape
         V = w.shape[0]
         Vp = (V + 7) // 8 * 8
@@ -404,8 +410,12 @@ class DecoderCEFn(torch.autograd.Function):
         logits = torch.empty(R, Vp, device=h.device, dtype=BF16)
         lse = torch.empty(R, device=h.device, dtype=torch.float32)
         loss = torch.empty(R, device=h.device, dtype=torch.float32)
-        L.call("vlpk_decoder_ce_fwd", R, V, H, hc.data_ptr(), wc.data_ptr(), bias_pad.data_ptr(), labels.data_ptr(), logits.data_ptr(),
-               lse.data_ptr(), loss.data_ptr(), L.stream())
+        if eps:
+            L.call("vlpk_decoder_ce_ls_fwd", R, V, H, eps, hc.data_ptr(), wc.data_ptr(), bias_pad.data_ptr(), labels.data_ptr(),
+                   logits.data_ptr(), lse.data_ptr(), loss.data_ptr(), L.stream())
+        else:
+            L.call("vlpk_decoder_ce_fwd", R, V, H, hc.data_ptr(), wc.data_ptr(), bias_pad.data_ptr(), labels.data_ptr(), logits.data_ptr(),
+                   lse.data_ptr(), loss.data_ptr(), L.stream())
         ctx.save_for_backward(hc, wc, labels, logits, lse)
         ctx.meta = (h.dtype, w.dtype, bias.dtype)
         scores = logits[:, :V]
@@ -425,12 +435,16 @@ class DecoderCEFn(torch.autograd.Function):
         dh = torch.zeros(R, H, device=dev, dtype=torch.float32)
         dw = torch.empty(V, H, device=dev, dtype=BF16)
         dbias = torch.zeros(Vp, device=dev, dtype=torch.float32)
-        L.call("vlpk_decoder_ce_bwd", R, V, H, hc.data_ptr(), wc.data_ptr(), labels.data_ptr(), logits.data_ptr(), lse.data_ptr(), dl.data_ptr(),
-               dlogits.data_ptr(), dh.data_ptr(), dw.data_ptr(), dbias.data_ptr(), L.stream())
+        if ctx.eps:
+            L.call("vlpk_decoder_ce_ls_bwd", R, V, H, ctx.eps, hc.data_ptr(), wc.data_ptr(), labels.data_ptr(), logits.data_ptr(),
+                   lse.data_ptr(), dl.data_ptr(), dlogits.data_ptr(), dh.data_ptr(), dw.data_ptr(), dbias.data_ptr(), L.stream())
+        else:
+            L.call("vlpk_decoder_ce_bwd", R, V, H, hc.data_ptr(), wc.data_ptr(), labels.data_ptr(), logits.data_ptr(), lse.data_ptr(),
+                   dl.data_ptr(), dlogits.data_ptr(), dh.data_ptr(), dw.data_ptr(), dbias.data_ptr(), L.stream())
         dwp = dw.to(wdt)
         if ctx.dp_hook is not None:
             ctx.dp_hook.on_decoder_weight_grad(dwp)      # data parallelism: this (tied) gradient is complete FIRST — reduce it now
-        return dh.to(hdt), dwp, dbias[:V].to(bdt), None, None
+        return dh.to(hdt), dwp, dbias[:V].to(bdt), None, None, None
 
 
 def layer_cached_fwd(hidden, kv_cache, pos, mask_bits, heads, I, params):

@@ -541,6 +541,47 @@ class _RegionProjections:
         return v, pe
 
 
+class LabelSmoothingLoss(nn.modules.loss._Loss):
+    """Label-smoothed masked-LM loss, the reference's crit_mask_lm_smoothed (loss.py:12-48; same constructor and `one_hot` buffer).
+
+    The target of a position with label t is q_ignore = 0, q_t = 1 - eps and s = eps / (V - 2) for every other word; a position whose
+    label is `ignore_index` (or lies outside [0, V)) has loss 0.  forward(output, target) takes log-probabilities [B, P, V] and returns
+    the per-position KL divergence sum_j q_j (log q_j - output_j) [B, P], evaluated in closed form without the dense [B*P, V] target:
+        K - (1 - eps) output_t - s (sum_j output_j - output_ignore - output_t),   K = xlogy(1 - eps, 1 - eps) + (V - 2) s log s.
+    The buffer keeps checkpoints key-compatible with the reference; the loss uses constants computed from eps at construction, which
+    a cast of the module (model.bfloat16()) does not round.  The fused head (ops.DecoderCEFn) evaluates the same loss with
+    ignore_index 0."""
+
+    def __init__(self, label_smoothing=0, tgt_vocab_size=0, ignore_index=0, size_average=None, reduce=None, reduction="mean"):
+        if not 0.0 < label_smoothing <= 1.0:
+            raise ValueError(f"label_smoothing must be in (0, 1], got {label_smoothing}")
+        if tgt_vocab_size < 3:
+            raise ValueError(f"tgt_vocab_size must be at least 3, got {tgt_vocab_size}")
+        super().__init__(size_average=size_average, reduce=reduce, reduction=reduction)
+        self.ignore_index = ignore_index
+        self.label_smoothing = float(label_smoothing)
+        self.smoothing_value = label_smoothing / (tgt_vocab_size - 2)
+        self.confidence = 1.0 - label_smoothing
+        self.tgt_vocab_size = tgt_vocab_size
+        one_hot = torch.full((tgt_vocab_size,), self.smoothing_value)
+        one_hot[ignore_index] = 0
+        self.register_buffer("one_hot", one_hot.unsqueeze(0))
+        c, s = self.confidence, self.smoothing_value
+        self.kl_const = (c * math.log(c) if c > 0 else 0.0) + (tgt_vocab_size - 2) * s * math.log(s)
+
+    def forward(self, output, target):
+        V = self.tgt_vocab_size
+        if output.size(2) != V:
+            raise ValueError(f"LabelSmoothingLoss: {output.size(2)} classes, built for {V}")
+        logp = output.reshape(-1, V)
+        t = target.reshape(-1)
+        live = (t != self.ignore_index) & (t >= 0) & (t < V)
+        lp_t = logp.gather(1, torch.where(live, t, torch.zeros_like(t)).unsqueeze(1)).squeeze(1)
+        rest = logp.sum(1) - logp[:, self.ignore_index] - lp_t
+        loss = self.kl_const - self.confidence * lp_t - self.smoothing_value * rest
+        return torch.where(live, loss, torch.zeros_like(loss)).view(target.shape)
+
+
 class BertForPreTrainingLossMask(PreTrainedBertModel, _RegionProjections):
     """modeling.py:982-1143."""
 
@@ -553,14 +594,16 @@ class BertForPreTrainingLossMask(PreTrainedBertModel, _RegionProjections):
         self.num_labels = num_labels
         self.len_vis_input = len_vis_input
         self.enable_butd = enable_butd
-        if getattr(config, "label_smoothing", None):
-            raise NotImplementedError("vlp_b200: label_smoothing is out of scope (default 0, run_img2txt_dist.py:78)")
-        self.crit_mask_lm_smoothed = None
+        if getattr(config, "label_smoothing", None):         # modeling.py:995-999
+            self.crit_mask_lm_smoothed = LabelSmoothingLoss(config.label_smoothing, config.vocab_size, ignore_index=0, reduction="none")
+        else:
+            self.crit_mask_lm_smoothed = None
         self._build_region_projections(config, enable_butd)
         self._load_fc7(required=False)
         self.tasks = tasks
-        # decoder + bias + cross-entropy through vlpk_decoder_ce_fwd/bwd (csrc/head.cu).  False selects the torch evaluation of the
-        # same ops, kept only as the comparison arm of tests/test_fused_head_gpu.py.
+        # decoder + bias + cross-entropy through vlpk_decoder_ce_fwd/bwd (csrc/head.cu), or the label-smoothed loss through
+        # vlpk_decoder_ce_ls_fwd/bwd.  False selects the torch evaluation of the same ops, kept only as the comparison arm of
+        # tests/test_fused_head_gpu.py and tests/test_label_smoothing_gpu.py.
         self.fused_mlm_head = os.environ.get("VLP_FUSED_HEAD", "1") != "0"
         self._vlpk_dp_hook = None      # data parallelism (vlp_b200/dp.py): receives the tied decoder weight's gradient as soon as it exists
         if tasks == "vqa2":
@@ -613,18 +656,22 @@ class BertForPreTrainingLossMask(PreTrainedBertModel, _RegionProjections):
             if self.fused_mlm_head:                          # decoder + bias + CE in libvlpk, SURVEY.md §8f-3
                 pred = self.cls.predictions
                 hid = pred.transform(gathered.to(pred.decoder.weight.dtype))
+                eps = self.crit_mask_lm_smoothed.label_smoothing if self.crit_mask_lm_smoothed is not None else 0.0
                 loss_flat, scores = ops.DecoderCEFn.apply(hid.reshape(-1, hid.size(-1)), pred.decoder.weight, pred.bias,
-                                                          masked_lm_labels.reshape(-1), self._vlpk_dp_hook)
+                                                          masked_lm_labels.reshape(-1), self._vlpk_dp_hook, eps)
                 self.last_prediction_scores = scores.view(*masked_lm_labels.shape, -1)
                 masked_lm_loss = loss_flat.view_as(masked_lm_labels)
             else:
                 prediction_scores_masked, _ = self.cls(gathered, pooled_output, task_idx=task_idx)
                 self.last_prediction_scores = prediction_scores_masked
-                # same per-position CE as crit_mask_lm(scores.transpose(1, 2).float(), labels) (modeling.py:1108-1109), evaluated on
-                # the contiguous [B*P, V] view so that the softmax reduces over the unit-stride dimension
-                V = prediction_scores_masked.size(-1)
-                masked_lm_loss = F.cross_entropy(prediction_scores_masked.reshape(-1, V).float(), masked_lm_labels.reshape(-1),
-                                                 reduction="none").view_as(masked_lm_labels)
+                if self.crit_mask_lm_smoothed is not None:   # modeling.py:1104-1106
+                    masked_lm_loss = self.crit_mask_lm_smoothed(F.log_softmax(prediction_scores_masked.float(), dim=-1), masked_lm_labels)
+                else:
+                    # same per-position CE as crit_mask_lm(scores.transpose(1, 2).float(), labels) (modeling.py:1108-1109), evaluated
+                    # on the contiguous [B*P, V] view so that the softmax reduces over the unit-stride dimension
+                    V = prediction_scores_masked.size(-1)
+                    masked_lm_loss = F.cross_entropy(prediction_scores_masked.reshape(-1, V).float(), masked_lm_labels.reshape(-1),
+                                                     reduction="none").view_as(masked_lm_labels)
             masked_lm_loss = loss_mask_and_normalize(masked_lm_loss.float(), masked_weights, drop_worst_ratio)
 
         if mask_image_regions:                               # Selfie-like pretext, modeling.py:1113-1131
