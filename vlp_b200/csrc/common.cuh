@@ -75,6 +75,15 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (++spins > (1u << 28)) { __trap(); }
   }
 }
+// The same bounded spin for code that must not contain a trap: a trap inside a setmaxnreg.inc region makes ptxas
+// allocate that region under the launch register count.  A timeout sets `timed_out`, after which every later wait
+// returns at once; the caller traps once it has left the region.
+__device__ __forceinline__ void mbar_wait_flag(uint64_t* bar, uint32_t parity, bool& timed_out) {
+  uint32_t spins = 0;
+  while (!timed_out && !mbar_try_wait(bar, parity)) {
+    if (++spins > (1u << 28)) timed_out = true;
+  }
+}
 
 // ----------------------------------------------------------------------------------------------
 // Programmatic dependent launch: a kernel launched with the programmatic-stream-serialization attribute may start while
@@ -149,6 +158,12 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
+// Register reallocation between warpgroups: every warp of the warpgroup executes it, and the block's producer / consumer
+// counts must fit the register file together.
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 // Keeps the compiler from moving accesses of an accumulator across wgmma_fence / wgmma_wait.
 template <int N>
 __device__ __forceinline__ void reg_fence(float (&d)[N]) {

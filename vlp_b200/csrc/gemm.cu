@@ -8,14 +8,24 @@
 //   dgrad    dX = dY W   : A = dY [M,N'] (K-major),          B = weight [N',K'] read MN-major (no transpose copy)
 //   wgrad    dW = dY^T X : A = dY read MN-major, B = X read MN-major, split-K, fp32 TMA reduce-add
 //
-// Structure (288 threads per CTA, one CTA per SM, one 128 x 128 output tile at a time):
-//   warp 8          TMA producer   : one elected lane issues cp.async.bulk.tensor into a 128B-swizzled smem ring (STAGES deep)
-//   warpgroups 0,1  MMA + epilogue : each owns 64 rows of the tile: wgmma m64n128k16 (x4 per 64-wide k-block) into a register
-//                                    accumulator, then the fused pointwise op -> swizzled smem staging -> TMA store (or TMA
-//                                    reduce-add for split-K weight gradients).  While one warpgroup drains its epilogue the
-//                                    producer keeps filling the ring for the next tile.
-// Tiles are 128 wide only: a 256-wide tile needs a 128-register accumulator per thread, and a 9-warp (or 12-warp) block is
-// capped at 168 registers, so its epilogues spill.
+// Structure (384 threads per CTA, one CTA per SM, 128 x 128 output tiles, two in flight):
+//   warpgroup 0     TMA producer   : one elected lane of warp 0 issues cp.async.bulk.tensor into a 128B-swizzled smem ring
+//                                    (STAGES deep), tile after tile in the CTA's work order.
+//   warpgroups 1,2  MMA + epilogue : ping-pong consumers.  Consumer c takes every other tile of the CTA's work sequence and
+//                                    owns all 128 rows of it: two wgmma m64n128k16 per k16 step (rows 0-63 and 64-127 of the
+//                                    A stage) into a 2 x 64 register accumulator, one wgmma group kept in flight across
+//                                    k-blocks, then the fused pointwise op -> swizzled smem staging -> TMA store (or TMA
+//                                    reduce-add for split-K weight gradients).  One consumer's epilogue runs while the other
+//                                    consumer's mainloop keeps the tensor pipe busy.
+// Each ring stage is read by exactly one consumer.  The producer signals a stage on the full barrier of the consumer whose
+// tile it belongs to (one set of full barriers per consumer), so each consumer waits only on phases of its own k-blocks and
+// can never mistake a phase of the other consumer's k-blocks for one of its own.  A consumer steps its ring position over
+// the k-blocks of the other consumer's tiles.
+// Registers: a 12-warp block is capped at 168 per thread, too few for a 128-register accumulator plus an epilogue.  The
+// producer warpgroup gives registers back (setmaxnreg 24) and the consumers take them (setmaxnreg 240):
+// 128 x 24 + 256 x 240 = 64 512 of the 65 536-register file.  ptxas allocates the consumer code under the 240 only if
+// that code contains no trap, so the consumers use the flagging mbar_wait_flag and trap after their loop.
+// Tiles are 128 wide only: a 256-wide tile would need a 256-register accumulator per consumer thread.
 #include "gemm.cuh"
 
 #include <cstdlib>
@@ -24,10 +34,13 @@
 
 namespace vlpk {
 
-static constexpr int BM = 128;  // rows per CTA tile (two warpgroups x 64)
+static constexpr int BM = 128;  // rows per tile (one consumer warpgroup: two m64 wgmma row halves)
 static constexpr int BK = 64;   // k-block: 64 bf16 = one 128-byte swizzle span
-static constexpr int NUM_THREADS = 288;
+static constexpr int NUM_THREADS = 384;
+static constexpr int PRODUCER_REGS = 24;
+static constexpr int CONSUMER_REGS = 240;
 static constexpr int STG_BYTES = 64 * 128;  // one staging box: 64 rows x 128 bytes
+static constexpr int STG_PER_CONSUMER = 4;  // staging boxes per consumer warpgroup (a 4-deep store ring; GELU: 2 pairs)
 static constexpr int SMEM_MAX = 232448;     // 227 KB: the per-block opt-in limit of sm_90
 static constexpr int BN = 128;              // tile columns (see above)
 
@@ -56,17 +69,17 @@ struct SmemLayout {
   static constexpr int A_BYTES = BM * BK * 2;  // 16 KB
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int OFF_STG = STAGES * STAGE_BYTES;  // 4 staging boxes (2 per MMA warpgroup)
-  static constexpr int OFF_BAR = OFF_STG + 4 * STG_BYTES;
-  static constexpr int NUM_BARS = 2 * STAGES;
+  static constexpr int OFF_STG = STAGES * STAGE_BYTES;  // STG_PER_CONSUMER staging boxes per consumer warpgroup
+  static constexpr int OFF_BAR = OFF_STG + 2 * STG_PER_CONSUMER * STG_BYTES;
+  static constexpr int NUM_BARS = 3 * STAGES;  // full (one set per consumer) + empty
   static constexpr int TOTAL = OFF_BAR + NUM_BARS * 8;
   static constexpr int DYN_BYTES = TOTAL + 1024;  // slack for manual 1024-byte alignment
   static_assert(DYN_BYTES <= SMEM_MAX, "shared memory budget exceeded");
 };
 
 struct StageCount {
-  // everything left of the 227 KB after the 4 staging boxes, barriers and alignment slack
-  static constexpr int value = (SMEM_MAX - 1024 - 4 * STG_BYTES - 256) / (BM * BK * 2 + BN * BK * 2);
+  // everything left of the 227 KB after the staging boxes, barriers and alignment slack
+  static constexpr int value = (SMEM_MAX - 1024 - 2 * STG_PER_CONSUMER * STG_BYTES - 256) / (BM * BK * 2 + BN * BK * 2);
 };
 
 __device__ __forceinline__ void wg_bar_sync(int cw) {
@@ -82,11 +95,11 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::OFF_BAR);
-  uint64_t* full_bar = bars;            // TMA -> MMA
-  uint64_t* empty_bar = bars + STAGES;  // MMA -> TMA (one arrival per MMA warp)
+  uint64_t* full_bar = bars;                // TMA -> consumer c: full_bar[c * STAGES + stage]
+  uint64_t* empty_bar = bars + 2 * STAGES;  // consumer -> TMA (one arrival per warp of the consuming warpgroup)
 
   pdl_launch_dependents();  // the next kernel may be scheduled as SMs free up; it blocks in its own pdl_wait()
-  const int wg = threadIdx.x >> 7;
+  const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);  // warp-uniform as far as the compiler can tell
   const int lane = threadIdx.x & 31;
 
   const int num_m = (args.M + BM - 1) / BM;
@@ -99,22 +112,23 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
     tma_prefetch_desc(&tm.a);
     tma_prefetch_desc(&tm.b[0]);
     tma_prefetch_desc(&tm.d0);
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 8);
-    }
+    for (int i = 0; i < 2 * STAGES; ++i) mbar_init(&full_bar[i], 1);
+    for (int i = 0; i < STAGES; ++i) mbar_init(&empty_bar[i], 4);
     fence_mbar_init();
   }
   __syncthreads();
   pdl_wait();  // barrier init and descriptor prefetch above overlap the previous kernel's tail
 
-  if (wg == 2) {
+  if (wg == 0) {
     // ===================================== TMA producer ========================================
-    {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (threadIdx.x < 32) {
       // The whole warp walks the loop (warp-uniform state); one elected lane issues.
       int stage = 0;
       uint32_t phase = 0;
-      for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
+      int item = 0;  // index in this CTA's work sequence: even items go to consumer 0, odd ones to consumer 1
+      for (int w = blockIdx.x; w < num_work; w += gridDim.x, ++item) {
+        uint64_t* fb = full_bar + (item & 1) * STAGES;
         const int n_blk = w % num_n;
         const int m_blk = (w / num_n) % num_m;
         const int split = w / (num_n * num_m);
@@ -126,23 +140,23 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
           if (elect_one()) {
             uint8_t* sA = smem + stage * L::STAGE_BYTES;
             uint8_t* sB = sA + L::A_BYTES;
-            mbar_arrive_expect_tx(&full_bar[stage], L::STAGE_BYTES);
+            mbar_arrive_expect_tx(&fb[stage], L::STAGE_BYTES);
             if (!A_MN) {
-              tma_load_2d(sA, &tm.a, &full_bar[stage], kb * BK, m0);
+              tma_load_2d(sA, &tm.a, &fb[stage], kb * BK, m0);
             } else {
 #pragma unroll
-              for (int j = 0; j < BM / 64; ++j) tma_load_2d(sA + j * 8192, &tm.a, &full_bar[stage], m0 + j * 64, kb * BK);
+              for (int j = 0; j < BM / 64; ++j) tma_load_2d(sA + j * 8192, &tm.a, &fb[stage], m0 + j * 64, kb * BK);
             }
             if (!B_MN) {
               const int n0 = n_blk * BN;
               const int seg = n0 / args.b_seg_rows;
-              tma_load_2d(sB, &tm.b[seg], &full_bar[stage], kb * BK, n0 - seg * args.b_seg_rows);
+              tma_load_2d(sB, &tm.b[seg], &fb[stage], kb * BK, n0 - seg * args.b_seg_rows);
             } else {
               const int k0 = kb * BK;
               const int seg = k0 / args.b_seg_rows;
 #pragma unroll
               for (int j = 0; j < BN / 64; ++j)
-                tma_load_2d(sB + j * 8192, &tm.b[seg], &full_bar[stage], n_blk * BN + j * 64, k0 - seg * args.b_seg_rows);
+                tma_load_2d(sB + j * 8192, &tm.b[seg], &fb[stage], n_blk * BN + j * 64, k0 - seg * args.b_seg_rows);
             }
           }
           __syncwarp();
@@ -155,79 +169,108 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
     }
   } else {
     // ================================== MMA + epilogue ==========================================
-    const int cw = wg;                             // rows [64 cw, 64 cw + 64) of every tile
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int cw = wg - 1;                         // consumer index: items cw, cw + 2, ... of this CTA's work sequence
     const int t = threadIdx.x - 128 * wg;          // 0..127
-    const int fr = (t >> 5) * 16 + (lane >> 2);    // first accumulator row of this thread (second: fr + 8)
+    const int fr = (t >> 5) * 16 + (lane >> 2);    // first accumulator row of this thread in each 64-row half (second: fr + 8)
     const int fc = (lane & 3) * 2;                 // first accumulator column within each 8-column group
     const bool store_thread = (t == 0);
     const uint64_t dseed = drop_seed(args.drop);
     // bias exists only for forward Linears (B read K-major, segments tile N)
     constexpr bool HAS_BIAS = !B_MN && (EPI == EPI_STORE || EPI == EPI_GELU || EPI == EPI_RELU);
-    uint8_t* stg0 = smem + L::OFF_STG + cw * 2 * STG_BYTES;
-    uint8_t* stg1 = stg0 + STG_BYTES;
-    // A rows of this warpgroup: 64 rows x 128 B (K-major) or the second 64-wide M box (MN-major) — 8 KB further either way
-    const uint32_t a_base = smem_u32(smem) + cw * 8192;
+    uint8_t* stg_base = smem + L::OFF_STG + cw * STG_PER_CONSUMER * STG_BYTES;
+    // A rows 64 h .. 64 h + 63 of a stage: 64 rows x 128 B (K-major) or the h-th 64-wide M box (MN-major) — 8 KB apart
+    const uint32_t a_base = smem_u32(smem);
     const uint32_t b_base = smem_u32(smem) + L::A_BYTES;
-    int stage = 0;
-    uint32_t phase = 0;
+    uint64_t* fb = full_bar + cw * STAGES;
+    int stage = 0;        // ring stage of the next k-block, counted over both consumers' k-blocks
+    uint32_t phases = 0;  // bit s: parity of this consumer's next wait on fb[s]
     uint32_t box_seq = 0;
-    float acc[BN / 2];
-    for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
+    bool timed_out = false;  // a full-barrier wait gave up: trap after the loop (see mbar_wait_flag)
+    float acc[2][BN / 2];  // rows 0-63 and 64-127 of the tile
+    // Defined here so that the accumulator is live only in the consumer branch (reg_fence reads it before the first wgmma,
+    // whose accumulate flag is 0): otherwise it would be live from kernel entry, under the producer's register count.
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[0][i] = acc[1][i] = 0.f;
+    for (int w = blockIdx.x + cw * gridDim.x; w < num_work; w += 2 * gridDim.x) {
+      const int w_other = w - static_cast<int>(gridDim.x);
+      if (w_other >= static_cast<int>(blockIdx.x)) {
+        // step over the k-blocks of the other consumer's tile, which precedes this one in the ring
+        const int split_o = w_other / (num_n * num_m);
+        const int kb0_o = split_o * kb_per;
+        stage = (stage + min(total_kb, kb0_o + kb_per) - kb0_o) % STAGES;
+      }
       const int n_blk = w % num_n;
       const int m_blk = (w / num_n) % num_m;
       const int split = w / (num_n * num_m);
       const int kb0 = split * kb_per;
       const int kb1 = min(total_kb, kb0 + kb_per);
       const int n0 = n_blk * BN;
-      const int m0 = m_blk * BM + cw * 64;
 
+      // One wgmma group stays in flight: a stage is released once the group after the one that read it has been issued.
+      int prev_stage = 0;
       for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
+        mbar_wait_flag(&fb[stage], (phases >> stage) & 1u, timed_out);
+        phases ^= 1u << stage;
         const uint32_t sa = a_base + stage * L::STAGE_BYTES;
         const uint32_t sb = b_base + stage * L::STAGE_BYTES;
-        reg_fence(acc);
+        reg_fence(acc[0]);
+        reg_fence(acc[1]);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k) {
-          const uint64_t adesc = A_MN ? wgmma_desc_sw128(sa + k * 2048, 8192, 1024) : wgmma_desc_sw128(sa + k * 32, 16, 1024);
           const uint64_t bdesc = B_MN ? wgmma_desc_sw128(sb + k * 2048, 8192, 1024) : wgmma_desc_sw128(sb + k * 32, 16, 1024);
-          wgmma_m64n128k16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, (kb > kb0 || k > 0) ? 1u : 0u);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t sah = sa + h * 8192;
+            const uint64_t adesc = A_MN ? wgmma_desc_sw128(sah + k * 2048, 8192, 1024) : wgmma_desc_sw128(sah + k * 32, 16, 1024);
+            wgmma_m64n128k16_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[h], adesc, bdesc, (kb > kb0 || k > 0) ? 1u : 0u);
+          }
         }
         wgmma_commit();
-        wgmma_wait<0>();
-        reg_fence(acc);
-        if (lane == 0) mbar_arrive(&empty_bar[stage]);  // this warp's share of the slot has been read
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1u;
-        }
+        wgmma_wait<1>();
+        reg_fence(acc[0]);
+        reg_fence(acc[1]);
+        if (kb > kb0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);  // this warp's share of the previous slot has been read
+        prev_stage = stage;
+        if (++stage == STAGES) stage = 0;
       }
+      wgmma_wait<0>();
+      reg_fence(acc[0]);
+      reg_fence(acc[1]);
+      if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
 
-      // ---- epilogue: accumulator element i of this thread sits at row fr + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + fc + (i & 1)
+      // ---- epilogue, one 64-row half h at a time: accumulator element acc[h][i] of this thread sits at row
+      //      64 h + fr + 8 * ((i >> 1) & 1), column 8 * (i >> 2) + fc + (i & 1)
       if (EPI == EPI_REDUCE_F32) {
-        // fp32 staging: 32 columns = 128 bytes per row; one TMA reduce-add box per 32 columns.
+        // fp32 staging: 32 columns = 128 bytes per row; one TMA reduce-add box per 64 rows x 32 columns.
         constexpr int NBOX = BN / 32;
 #pragma unroll
-        for (int c = 0; c < NBOX; ++c) {
-          uint8_t* stg = (box_seq & 1u) ? stg1 : stg0;
-          if (store_thread) tma_store_wait_read<1>();
-          wg_bar_sync(cw);
+        for (int h = 0; h < 2; ++h) {
+          const int m0 = m_blk * BM + h * 64;
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int i = c * 16 + 2 * j;
-            const int r = fr + 8 * (j & 1), col = 8 * (j >> 1) + fc;
-            *reinterpret_cast<float2*>(stg + r * 128 + (((col >> 2) ^ (r & 7)) << 4) + (col & 3) * 4) = make_float2(acc[i], acc[i + 1]);
+          for (int c = 0; c < NBOX; ++c) {
+            uint8_t* stg = stg_base + (box_seq % STG_PER_CONSUMER) * STG_BYTES;
+            if (store_thread) tma_store_wait_read<STG_PER_CONSUMER - 1>();
+            wg_bar_sync(cw);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int i = c * 16 + 2 * j;
+              const int r = fr + 8 * (j & 1), col = 8 * (j >> 1) + fc;
+              *reinterpret_cast<float2*>(stg + r * 128 + (((col >> 2) ^ (r & 7)) << 4) + (col & 3) * 4) = make_float2(acc[h][i], acc[h][i + 1]);
+            }
+            fence_proxy_async_smem();
+            wg_bar_sync(cw);
+            if (store_thread) {
+              tma_reduce_add_3d(&tm.d0, stg, n0 + c * 32, m0, args.split_slices ? split : 0);
+              tma_store_commit();
+            }
+            ++box_seq;
           }
-          fence_proxy_async_smem();
-          wg_bar_sync(cw);
-          if (store_thread) {
-            tma_reduce_add_3d(&tm.d0, stg, n0 + c * 32, m0, args.split_slices ? split : 0);
-            tma_store_commit();
-          }
-          ++box_seq;
         }
       } else {
-        // bf16 staging: 64 columns = 128 bytes per row; one TMA store box per 64 columns.
+        // bf16 staging: 64 columns = 128 bytes per row; one TMA store box per 64 rows x 64 columns.  GELU stores two outputs
+        // per box position, from a pair of staging boxes; its two pairs alternate like the single boxes of the other epilogues.
         constexpr int NBOX = BN / 64;
         const __nv_bfloat16* bp = nullptr;
         int bias_off = 0;
@@ -237,83 +280,95 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
           bias_off = seg * args.b_seg_rows;
         }
 #pragma unroll
-        for (int c = 0; c < NBOX; ++c) {
-          uint8_t* stg = (EPI == EPI_GELU) ? stg0 : ((box_seq & 1u) ? stg1 : stg0);
-          if (store_thread) {
-            if (EPI == EPI_GELU) tma_store_wait_read<0>(); else tma_store_wait_read<1>();
-          }
-          wg_bar_sync(cw);
+        for (int h = 0; h < 2; ++h) {
+          const int m0 = m_blk * BM + h * 64;
+          // Each half recomputes its column offsets, bias addresses and dropout seed: shared by both halves, they would
+          // stay live through the first half's epilogue next to the 128-register accumulator and spill.
+          int nh = n0;
+          const __nv_bfloat16* bph = bp;
+          uint64_t dsh = dseed;
+          asm volatile("" : "+r"(nh), "+l"(bph), "+l"(dsh));
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int i = c * 32 + 2 * j;
-            const int r = fr + 8 * (j & 1), col = 8 * (j >> 1) + fc;
-            const int n = n0 + c * 64 + col;
-            const long long m = m0 + r;
-            float v0 = acc[i], v1 = acc[i + 1];
-            if (HAS_BIAS) {
-              if (bp != nullptr && n < args.N) {
-                const float2 bb = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(bp + n - bias_off)));
-                v0 += bb.x;
-                v1 += bb.y;
+          for (int c = 0; c < NBOX; ++c) {
+            uint8_t* stg = (EPI == EPI_GELU) ? stg_base + (box_seq & 1u) * 2 * STG_BYTES : stg_base + (box_seq % STG_PER_CONSUMER) * STG_BYTES;
+            uint8_t* stg_g = stg + STG_BYTES;  // EPI_GELU: gelu(u) next to gelu'(u)
+            if (store_thread) {
+              if (EPI == EPI_GELU) tma_store_wait_read<STG_PER_CONSUMER / 2 - 1>(); else tma_store_wait_read<STG_PER_CONSUMER - 1>();
+            }
+            wg_bar_sync(cw);
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+              const int i = c * 32 + 2 * j;
+              const int r = fr + 8 * (j & 1), col = 8 * (j >> 1) + fc;
+              const int n = nh + c * 64 + col;
+              const long long m = m0 + r;
+              float v0 = acc[h][i], v1 = acc[h][i + 1];
+              if (HAS_BIAS) {
+                if (bph != nullptr && n < args.N) {
+                  const float2 bb = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(bph + n - bias_off)));
+                  v0 += bb.x;
+                  v1 += bb.y;
+                }
               }
-            }
-            const int so = r * 128 + (((col >> 3) ^ (r & 7)) << 4) + (col & 7) * 2;
-            if (EPI == EPI_GELU) {
-              float g0, d0, g1, d1;
-              gelu_and_grad(v0, g0, d0);
-              gelu_and_grad(v1, g1, d1);
-              *reinterpret_cast<uint32_t*>(stg0 + so) = pack_bf16x2(d0, d1);  // gelu'(u): all backward needs from the pre-activation
-              *reinterpret_cast<uint32_t*>(stg1 + so) = pack_bf16x2(g0, g1);  // gelu(u)
-              continue;
-            }
-            if (EPI == EPI_RELU) {
-              uint32_t keep = 0xFFu;
-              if (args.drop.p > 0.f)
-                keep = dropout_keep8(dseed, args.drop.site, (static_cast<uint64_t>(m) * args.N + (n - fc)) >> 3, args.drop.thresh16);
-              v0 = fmaxf(v0, 0.f);
-              v1 = fmaxf(v1, 0.f);
-              v0 = ((keep >> fc) & 1u) ? v0 * args.drop.scale : 0.f;
-              v1 = ((keep >> (fc + 1)) & 1u) ? v1 * args.drop.scale : 0.f;
-            } else if (EPI == EPI_ADD || EPI == EPI_MUL || EPI == EPI_DRELU) {
-              float2 x = make_float2(0.f, 0.f);
-              if (m < args.M && n < args.N) x = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(args.aux + m * args.ld_aux + n)));
-              if (EPI == EPI_ADD) {
-                v0 += x.x;
-                v1 += x.y;
-              } else if (EPI == EPI_MUL) {
-                v0 *= x.x;
-                v1 *= x.y;
-              } else {
-                v0 = x.x > 0.f ? v0 * args.relu_scale : 0.f;
-                v1 = x.y > 0.f ? v1 * args.relu_scale : 0.f;
+              const int so = r * 128 + (((col >> 3) ^ (r & 7)) << 4) + (col & 7) * 2;
+              if (EPI == EPI_GELU) {
+                float g0, d0, g1, d1;
+                gelu_and_grad(v0, g0, d0);
+                gelu_and_grad(v1, g1, d1);
+                *reinterpret_cast<uint32_t*>(stg + so) = pack_bf16x2(d0, d1);    // gelu'(u): all backward needs from the pre-activation
+                *reinterpret_cast<uint32_t*>(stg_g + so) = pack_bf16x2(g0, g1);  // gelu(u)
+                continue;
               }
+              if (EPI == EPI_RELU) {
+                uint32_t keep = 0xFFu;
+                if (args.drop.p > 0.f)
+                  keep = dropout_keep8(dsh, args.drop.site, (static_cast<uint64_t>(m) * args.N + (n - fc)) >> 3, args.drop.thresh16);
+                v0 = fmaxf(v0, 0.f);
+                v1 = fmaxf(v1, 0.f);
+                v0 = ((keep >> fc) & 1u) ? v0 * args.drop.scale : 0.f;
+                v1 = ((keep >> (fc + 1)) & 1u) ? v1 * args.drop.scale : 0.f;
+              } else if (EPI == EPI_ADD || EPI == EPI_MUL || EPI == EPI_DRELU) {
+                float2 x = make_float2(0.f, 0.f);
+                if (m < args.M && n < args.N) x = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(args.aux + m * args.ld_aux + n)));
+                if (EPI == EPI_ADD) {
+                  v0 += x.x;
+                  v1 += x.y;
+                } else if (EPI == EPI_MUL) {
+                  v0 *= x.x;
+                  v1 *= x.y;
+                } else {
+                  v0 = x.x > 0.f ? v0 * args.relu_scale : 0.f;
+                  v1 = x.y > 0.f ? v1 * args.relu_scale : 0.f;
+                }
+              }
+              *reinterpret_cast<uint32_t*>(stg + so) = pack_bf16x2(v0, v1);
             }
-            *reinterpret_cast<uint32_t*>(stg + so) = pack_bf16x2(v0, v1);
-          }
-          fence_proxy_async_smem();
-          wg_bar_sync(cw);
-          if (store_thread) {
-            tma_store_2d(&tm.d0, stg, n0 + c * 64, m0);
-            if (EPI == EPI_GELU) tma_store_2d(&tm.d1, stg1, n0 + c * 64, m0);
-            tma_store_commit();
-          }
-          if (EPI != EPI_GELU && args.colsum != nullptr) {
-            // bias gradient = column sums of this output: fold the staged [64 x 64] bf16 box (rows beyond M are zero).
-            // Two threads per column take 32 rows each; the buffer is not overwritten before the next-but-one barrier.
-            const int col = t & 63, r0 = (t >> 6) * 32;
-            float acc_c = 0.f;
+            fence_proxy_async_smem();
+            wg_bar_sync(cw);
+            if (store_thread) {
+              tma_store_2d(&tm.d0, stg, nh + c * 64, m0);
+              if (EPI == EPI_GELU) tma_store_2d(&tm.d1, stg_g, nh + c * 64, m0);
+              tma_store_commit();
+            }
+            if (EPI != EPI_GELU && args.colsum != nullptr) {
+              // bias gradient = column sums of this output: fold the staged [64 x 64] bf16 box (rows beyond M are zero).
+              // Two threads per column take 32 rows each; the box is not overwritten before the barrier STG_PER_CONSUMER boxes on.
+              const int col = t & 63, r0 = (t >> 6) * 32;
+              float acc_c = 0.f;
 #pragma unroll 8
-            for (int rr = r0; rr < r0 + 32; ++rr) {
-              const __nv_bfloat16 v = *reinterpret_cast<const __nv_bfloat16*>(stg + rr * 128 + (((col >> 3) ^ (rr & 7)) << 4) + (col & 7) * 2);
-              acc_c += __bfloat162float(v);
+              for (int rr = r0; rr < r0 + 32; ++rr) {
+                const __nv_bfloat16 v = *reinterpret_cast<const __nv_bfloat16*>(stg + rr * 128 + (((col >> 3) ^ (rr & 7)) << 4) + (col & 7) * 2);
+                acc_c += __bfloat162float(v);
+              }
+              if (nh + c * 64 + col < args.N) atomicAdd(args.colsum + nh + c * 64 + col, acc_c);
             }
-            if (n0 + c * 64 + col < args.N) atomicAdd(args.colsum + n0 + c * 64 + col, acc_c);
+            ++box_seq;
           }
-          ++box_seq;
         }
       }
     }
     if (store_thread) tma_store_wait<0>();
+    if (timed_out) __trap();
   }
 }
 
