@@ -111,6 +111,12 @@ const char* vlpk_last_error(void);
  * data-parallel callers while a collective that owns SMs (NCCL all-reduce of the previous gradient arena) runs beside the
  * backward GEMMs: a grid sized for all SMs would have its last CTAs wait behind the collective's. */
 void vlpk_set_reserved_sms(int n);
+/* Deterministic mode (process-wide, default 0; no launch, cheap enough to call before every library call).  When on, every
+ * reduction whose fp32 additions could happen in a run-dependent order (atomics from several blocks, split-K reduce-add, the
+ * embedding-table scatter of repeated ids) writes partials that are summed in a fixed order, and the split-K counts no longer
+ * depend on vlpk_set_reserved_sms: on one GPU, gradients and BertAdam results are bitwise reproducible.  Slower; the default path
+ * is unchanged.  Python selects it with torch.use_deterministic_algorithms(True). */
+void vlpk_set_deterministic(int on);
 /* host-only: the (tile N, split-K) the cost model picks for a GEMM; out2 = {bn, splits}.  No GPU needed. */
 int vlpk_debug_plan_gemm(int M, int N, int K, int a_mn, int b_mn, int nseg, int seg_rows, int epi, int bn, int splits, int* out2);
 /* A-B testing only: switch a host-side scheduling choice at run time.  "wgrad_stream" (default 1, env VLPK_WGRAD_STREAM=0 turns it

@@ -1,6 +1,6 @@
 """C-ABI call sequences shared by the GPU parity tests and by the CPU marshalling dry-run.
 
-`dry_run()` replaces the library call by a ctypes conversion of the arguments against the prototypes declared in
+`dry_run()` replaces the library call (`_lib.invoke`, behind `_lib.call`'s deterministic-mode check) by a ctypes conversion of the arguments against the prototypes declared in
 vlp_b200/_lib.py (the mirror of include/vlpk.h), so that the host-side marshalling of a GPU test — structs, pointer
 arithmetic, argument order and count — is exercised by the `-m "not gpu"` suite without launching anything.  It computes
 nothing: buffers keep whatever torch.empty returned.
@@ -26,12 +26,12 @@ def dry_run():
         proto(lambda *a: 0)(*args)      # raises ctypes.ArgumentError / TypeError on any mismatch
         calls.append(name)
 
-    saved = (L.call, L.stream, ops._require_cuda)
-    L.call, L.stream, ops._require_cuda = fake_call, (lambda: 0), (lambda t, what: None)
+    saved = (L.invoke, L.stream, ops._require_cuda, L._deterministic)
+    L.invoke, L.stream, ops._require_cuda = fake_call, (lambda: 0), (lambda t, what: None)
     try:
         yield calls
     finally:
-        L.call, L.stream, ops._require_cuda = saved
+        L.invoke, L.stream, ops._require_cuda, L._deterministic = saved   # the library itself never saw the dry run's mode changes
 
 
 def _rn(gen, dev, *shape, scale=1.0, shift=0.0):

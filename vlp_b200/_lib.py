@@ -58,6 +58,7 @@ _SIGS = {
     "vlpk_last_error": (C.c_char_p, []),
     "vlpk_debug_set_option": (c_int, [C.c_char_p, c_int]),
     "vlpk_set_reserved_sms": (None, [c_int]),
+    "vlpk_set_deterministic": (None, [c_int]),
     "vlpk_debug_plan_gemm": (c_int, [c_int] * 10 + [C.POINTER(c_int)]),
     "vlpk_mask_pack": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_i64, c_i64, _P, _P]),
     "vlpk_mask_synth": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P]),
@@ -154,5 +155,22 @@ def stream():
     return torch.cuda.current_stream().cuda_stream
 
 
+# The library's deterministic mode as last sent (its default is off).  `call` follows torch.use_deterministic_algorithms: the
+# switch is read before every library call and forwarded when it has changed since the last one.
+_deterministic = False
+
+
 def call(name, *args):
-    check(getattr(lib(), name)(*args), name)
+    global _deterministic
+    det = torch.are_deterministic_algorithms_enabled()
+    if det != _deterministic:
+        invoke("vlpk_set_deterministic", int(det))
+        _deterministic = det
+    invoke(name, *args)
+
+
+def invoke(name, *args):
+    """One library call, no mode check; raises on a non-zero return code."""
+    rc = getattr(lib(), name)(*args)
+    if rc is not None:
+        check(rc, name)

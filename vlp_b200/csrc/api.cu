@@ -81,6 +81,7 @@ int wgrad_linear(int M, int N, int K, const void* dy, int64_t lddy, const void* 
   g.D0 = dw; g.ldd0 = lddw;
   g.epi = EPI_REDUCE_F32;
   g.splits = 0;  // chosen together with the tile shape by launch_gemm's cost model
+  if (deterministic()) return launch_gemm_split_slices(g, SCRATCH_WGRAD, st);
   return launch_gemm(g, st);
 }
 
@@ -271,7 +272,12 @@ int ffn_bwd_impl(const VlpkShape* s, const VlpkLayerWeights* w, const VlpkLayerA
   // ---- output.dense: dW2 += dt2^T hmid ; dU = (dt2 W2) * gelu'(u)   [gelu'(u) was stored by the forward epilogue in acts.u]
   VLPK_TRY(linear_bwd_pair(
       st, [&](cudaStream_t q) { return wgrad_linear(M, H, I, dt2, H, a->hmid, I, g->w2, I, q); },
-      [&](cudaStream_t q) { return dgrad_linear(M, H, I, dt2, H, w->w2, I, ws->du, I, EPI_MUL, a->u, I, q, g->b1); }));  // + db1 = column sums of dU
+      [&](cudaStream_t q) {
+        // db1 = column sums of dU: fused into the dgrad's epilogue (atomics), or in deterministic mode a separate ordered column sum
+        if (!deterministic()) return dgrad_linear(M, H, I, dt2, H, w->w2, I, ws->du, I, EPI_MUL, a->u, I, q, g->b1);
+        VLPK_TRY(dgrad_linear(M, H, I, dt2, H, w->w2, I, ws->du, I, EPI_MUL, a->u, I, q));
+        return launch_colsum(ws->du, I, M, I, g->b1, q);
+      }));
   // ---- intermediate.dense: dW1 += dU^T y1 ; dy1 = dU W1 + dz2 (residual branch of LN2)
   VLPK_TRY(linear_bwd_pair(
       st, [&](cudaStream_t q) { return wgrad_linear(M, I, H, ws->du, I, a->y1, H, g->w1, H, q); },
@@ -393,6 +399,7 @@ int vlpk_debug_plan_gemm(int M, int N, int K, int a_mn, int b_mn, int nseg, int 
   return plan_gemm(g, &out2[0], &out2[1]);
 }
 void vlpk_set_reserved_sms(int n) { set_reserved_sms(n); }
+void vlpk_set_deterministic(int on) { set_deterministic(on != 0); }
 const char* vlpk_last_error(void) { return get_error(); }
 
 int vlpk_mask_pack(const void* mask, int dtype, int mode, int B, int rows, int kv, int64_t stride_b, int64_t stride_r, uint32_t* out,
@@ -782,6 +789,7 @@ int vlpk_gemm(int M, int N, int K, int a_mn, const void* A, int64_t lda, int b_m
   g.D0 = D0; g.ldd0 = ldd0; g.D1 = D1; g.ldd1 = ldd1;
   g.aux = static_cast<const bf16*>(aux); g.ld_aux = ld_aux;
   g.epi = epi; g.splits = splits; g.bn = bn;
+  if (deterministic() && epi == EPI_REDUCE_F32) return launch_gemm_split_slices(g, SCRATCH_SPLITK, S(stream));
   return launch_gemm(g, S(stream));
 }
 

@@ -31,6 +31,7 @@
 #include <cstdlib>
 
 #include "host.cuh"
+#include "rowops.cuh"
 
 namespace vlpk {
 
@@ -424,7 +425,8 @@ static double tile_cost(int M, int N, int total_kb, int splits, bool reduce) {
   const int num_m = (M + BM - 1) / BM;
   const int num_n = (N + BN - 1) / BN;
   const long long tiles = static_cast<long long>(num_m) * num_n * splits;
-  const int slots = gemm_sms();
+  // deterministic mode: the split count decides how a weight gradient is summed, so it must not follow vlpk_set_reserved_sms
+  const int slots = deterministic() ? num_sms() : gemm_sms();
   const long long rounds = (tiles + slots - 1) / slots;
   const int kb_per = (total_kb + splits - 1) / splits;
   const double mainloop = kb_per * (128.0 + double(BN));
@@ -538,6 +540,24 @@ int launch_gemm(const GemmDesc& g, cudaStream_t stream) {
   const int num_n = (g.N + bn - 1) / bn;
   const int num_work = num_m * num_n * splits;
   return dispatch(g, tm, a, num_work, stream);
+}
+
+int launch_gemm_split_slices(GemmDesc g, int slot, cudaStream_t stream) {
+  VLPK_CHECK_ARG(g.epi == EPI_REDUCE_F32 && g.split_stride == 0, "gemm: split slices are for EPI_REDUCE_F32 into one D0");
+  int bn = 0, splits = 1;
+  VLPK_TRY(plan_gemm(g, &bn, &splits));
+  if (splits == 1) return launch_gemm(g, stream);  // one reduce-add per element: already order-free
+  VLPK_CHECK_ARG(g.ldd0 == g.N, "gemm: split slices need a dense D0 (ldd0 %lld != N %d)", (long long)g.ldd0, g.N);
+  const long long n = static_cast<long long>(g.M) * g.N;
+  float* part = scratch_f32(slot, static_cast<size_t>(n) * splits, stream);
+  if (part == nullptr) return -1;
+  VLPK_CUDA(cudaMemsetAsync(part, 0, static_cast<size_t>(n) * splits * sizeof(float), stream));
+  float* out = static_cast<float*>(g.D0);
+  g.D0 = part;
+  g.splits = splits;
+  g.split_stride = n;
+  VLPK_TRY(launch_gemm(g, stream));
+  return launch_sum_parts(part, splits, n, out, stream);
 }
 
 }  // namespace vlpk

@@ -53,5 +53,8 @@ struct GemmDesc {
 // Returns 0 on success, <0 on argument error, >0 cudaError_t.  Message via vlpk::set_error.
 int launch_gemm(const GemmDesc& g, cudaStream_t stream);
 int plan_gemm(const GemmDesc& g, int* bn_out, int* splits_out);
+// EPI_REDUCE_F32 with the split count plan_gemm picks, summed in a fixed order: with more than one split, each split reduce-adds
+// into its own zeroed slice of scratch slot `slot` and the slices are then added to D0 (fp32, +=, ldd0 == N) in split order.
+int launch_gemm_split_slices(GemmDesc g, int slot, cudaStream_t stream);
 
 }  // namespace vlpk

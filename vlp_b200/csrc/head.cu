@@ -218,22 +218,8 @@ int launch_decoder_ce_bwd(const DecoderCeArgs& a, cudaStream_t s) {
     g.D0 = a.dh; g.ldd0 = a.H;
     g.epi = EPI_REDUCE_F32;
     g.splits = 0;
-    int bn = 0;
-    VLPK_TRY(plan_gemm(g, &bn, &g.splits));
-    if (g.splits > 1) {
-      // dh feeds every activation gradient of the backward pass, so its sum must not depend on the order in which the splits
-      // finish: each split adds into its own zeroed slice and the slices are summed in a fixed order
-      const long long n = static_cast<long long>(a.R) * a.H;
-      float* part = scratch_f32(SCRATCH_SPLITK, static_cast<size_t>(n) * g.splits, s);
-      if (part == nullptr) return -1;
-      VLPK_CUDA(cudaMemsetAsync(part, 0, static_cast<size_t>(n) * g.splits * sizeof(float), s));
-      g.D0 = part;
-      g.split_stride = n;
-      VLPK_TRY(launch_gemm(g, s));
-      VLPK_TRY(launch_sum_parts(part, g.splits, n, a.dh, s));
-    } else {
-      VLPK_TRY(launch_gemm(g, s));
-    }
+    // dh feeds every activation gradient of the backward pass, so its sum must not depend on the order in which the splits finish
+    VLPK_TRY(launch_gemm_split_slices(g, SCRATCH_SPLITK, s));
   }
   GemmDesc g;  // dW[V,H] (bf16) = dlogits^T h: both operands read MN-major, K = R fits one or a few k-blocks, direct store
   g.M = a.V; g.N = a.H; g.K = a.R;

@@ -134,6 +134,10 @@ int gemm_sms() {
   return n < 1 ? 1 : n;
 }
 
+static bool g_deterministic = false;
+bool deterministic() { return g_deterministic; }
+void set_deterministic(bool on) { g_deterministic = on; }
+
 // ------------------------------------------------------------------------------------------------
 // launch accounting / profiling
 // ------------------------------------------------------------------------------------------------

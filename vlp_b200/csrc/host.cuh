@@ -58,13 +58,28 @@ inline int make_tmap_2d(CUtensorMap* out, TmapDtype dt, const void* base, uint64
 // Library-owned fp32 device scratch for the ordered reductions, one buffer per slot and device.  Grow-only, and a buffer is
 // never freed, so CUDA graphs captured earlier keep valid pointers; growing is refused (nullptr, error set) while `s` is being
 // captured — the first call of a shape must run outside capture, as a graph's warm-up does.
-enum ScratchSlot { SCRATCH_ATTN_DBIAS = 0, SCRATCH_SPLITK = 1, SCRATCH_SLOTS = 2 };
+// A slot is only ever used by kernels on one stream at a time: the weight-gradient GEMMs, which may run on the side stream,
+// have their own slot.
+enum ScratchSlot {
+  SCRATCH_ATTN_DBIAS = 0,  // attention q/k/v bias gradient, one partial per sequence
+  SCRATCH_SPLITK = 1,      // split-K slices of the MLM head's dh (main stream)
+  SCRATCH_WGRAD = 2,       // deterministic mode: split-K slices of weight gradients (main or wgrad side stream)
+  SCRATCH_ORDERED = 3,     // deterministic mode: per-block partials of column sums, LayerNorm dγ/dβ, token types, Σg²
+  SCRATCH_SORT = 4,        // deterministic mode: sorted (id, row) pairs and sort temporaries of the table scatter
+  SCRATCH_SLOTS = 5
+};
 float* scratch_f32(int slot, size_t n, cudaStream_t s);
 
 int num_sms();
 // SMs available to the persistent GEMM grids: num_sms() minus what vlpk_set_reserved_sms put aside (default 0), at least 1.
 int gemm_sms();
 void set_reserved_sms(int n);
+
+// Deterministic mode (vlpk_set_deterministic): every reduction whose operands could be added in a run-dependent order (fp32
+// atomics from several blocks, TMA reduce-add from several split-K splits) writes per-block / per-split partials that are then
+// summed in a fixed order.  Off by default; the default path's kernels and launches are unchanged.
+bool deterministic();
+void set_deterministic(bool on);
 
 // Launch with optional cluster dimension and programmatic dependent launch (VLPK_PDL=0 disables the latter).
 bool pdl_enabled();

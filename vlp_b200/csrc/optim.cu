@@ -8,6 +8,7 @@
 //                           m = b1 m + (1-b1) g ; v = b2 v + (1-b2) g^2 ; u = m / (sqrt(v) + e) + wd p ; p -= lr u
 //                           — no bias correction, decoupled weight decay (optimization.py:150-172).
 // Parameters may be bf16 (then an fp32 master copy carries the arithmetic and the bf16 parameter is its rounding) or fp32.
+// Deterministic mode: step 1 writes one partial per chunk and a third kernel adds each tensor's partials in a fixed order.
 // Work decomposition: chunk c -> tensor t by binary search in an exclusive prefix of per-tensor chunk counts, so tensors of
 // any size mix (a 28996x768 embedding next to 768-element biases) and the grid is sized from the SM count.
 // Algorithmic HBM bytes per element: gradient read twice (2 x 2 B bf16) + master/m/v read+write (24 B) + parameter write (2 B).
@@ -71,6 +72,8 @@ __device__ __forceinline__ void store8_bf16(__nv_bfloat16* p, long long i, const
 
 __device__ __forceinline__ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
+// ORDERED (deterministic mode): chunk c writes its sum to sq[c] instead of adding it to sq[tensor].
+template <bool ORDERED>
 __global__ void __launch_bounds__(ADAM_THREADS)
 adam_sqnorm_kernel(const VlpkAdamTensor* __restrict__ T, const int* __restrict__ prefix, int n_tensors, int n_chunks,
                    float* __restrict__ sq) {
@@ -112,10 +115,26 @@ adam_sqnorm_kernel(const VlpkAdamTensor* __restrict__ T, const int* __restrict__
       float tot = lane < ADAM_THREADS / 32 ? s_part[lane] : 0.f;
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, o);
-      if (lane == 0) atomicAdd(sq + t, tot);
+      if (lane == 0) {
+        if constexpr (ORDERED) sq[c] = tot;
+        else atomicAdd(sq + t, tot);
+      }
     }
     __syncthreads();  // s_part is reused by the next chunk
   }
+}
+
+// sq[t] = sum of tensor t's chunk partials: one warp per tensor, lane l adds chunks l, l + 32, ... in turn, then a fixed butterfly.
+__global__ void __launch_bounds__(ADAM_THREADS)
+adam_sqnorm_sum_kernel(const int* __restrict__ prefix, int n_tensors, const float* __restrict__ part, float* __restrict__ sq) {
+  const int t = blockIdx.x * (ADAM_THREADS / 32) + (threadIdx.x >> 5);
+  if (t >= n_tensors) return;
+  const int lane = threadIdx.x & 31;
+  float acc = 0.f;
+  for (int c = __ldg(prefix + t) + lane; c < __ldg(prefix + t + 1); c += 32) acc += part[c];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if (lane == 0) sq[t] = acc;
 }
 
 __device__ __forceinline__ void adam_elem(float g, float& m, float& v, float& p, float coef, float wd, const AdamHyper& h) {
@@ -204,9 +223,20 @@ int launch_bertadam(const VlpkAdamTensor* th, const VlpkAdamTensor* td, const in
   const int n_chunks = ph[n_tensors];
   const int grid = n_chunks < num_sms() * 8 ? n_chunks : num_sms() * 8;
   VLPK_CUDA(cudaMemsetAsync(sqnorm_dev, 0, sizeof(float) * n_tensors, s));
-  if (h.max_grad_norm > 0.f) {
+  if (h.max_grad_norm > 0.f && !deterministic()) {
     LaunchScope scope(CAT_MISC, 0.0, s);
-    adam_sqnorm_kernel<<<grid, ADAM_THREADS, 0, s>>>(td, pd, n_tensors, n_chunks, sqnorm_dev);
+    adam_sqnorm_kernel<false><<<grid, ADAM_THREADS, 0, s>>>(td, pd, n_tensors, n_chunks, sqnorm_dev);
+    VLPK_CUDA(cudaGetLastError());
+  } else if (h.max_grad_norm > 0.f) {
+    float* part = scratch_f32(SCRATCH_ORDERED, static_cast<size_t>(n_chunks), s);
+    if (part == nullptr) return -1;
+    {
+      LaunchScope scope(CAT_MISC, 0.0, s);
+      adam_sqnorm_kernel<true><<<grid, ADAM_THREADS, 0, s>>>(td, pd, n_tensors, n_chunks, part);
+      VLPK_CUDA(cudaGetLastError());
+    }
+    LaunchScope scope(CAT_MISC, 0.0, s);
+    adam_sqnorm_sum_kernel<<<(n_tensors + ADAM_THREADS / 32 - 1) / (ADAM_THREADS / 32), ADAM_THREADS, 0, s>>>(pd, n_tensors, part, sqnorm_dev);
     VLPK_CUDA(cudaGetLastError());
   }
   {

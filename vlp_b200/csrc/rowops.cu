@@ -122,7 +122,8 @@ static constexpr int LNB_WARPS = 16;
 // index of (chunk i, lane l, element j) of a per-warp [NCH*256] accumulator: two float4 halves, lanes adjacent
 __device__ __forceinline__ int lnb_idx(int i, int half, int lane) { return ((i * 2 + half) * 32 + lane) * 4; }
 
-template <int NCH>
+// ORDERED (deterministic mode): each block writes its column sums to a.part instead of adding them atomically.
+template <int NCH, bool ORDERED>
 __global__ void __launch_bounds__(LNB_WARPS * 32, 1) ln_res_drop_bwd_kernel(LnArgs a) {
   pdl_launch_dependents();
   pdl_wait();
@@ -240,9 +241,16 @@ __global__ void __launch_bounds__(LNB_WARPS * 32, 1) ln_res_drop_bwd_kernel(LnAr
       vb += s_ln[(w * 3 + 1) * W + idx];
       vt += s_ln[(w * 3 + 2) * W + idx];
     }
-    if (a.dgamma != nullptr) atomicAdd(a.dgamma + c, vg);
-    if (a.dbeta != nullptr) atomicAdd(a.dbeta + c, vb);
-    if (a.dbias != nullptr) atomicAdd(a.dbias + c, vt);
+    if constexpr (ORDERED) {
+      const long long slab = static_cast<long long>(gridDim.x) * a.H, o = static_cast<long long>(blockIdx.x) * a.H + c;
+      if (a.dgamma != nullptr) a.part[o] = vg;
+      if (a.dbeta != nullptr) a.part[slab + o] = vb;
+      if (a.dbias != nullptr) a.part[2 * slab + o] = vt;
+    } else {
+      if (a.dgamma != nullptr) atomicAdd(a.dgamma + c, vg);
+      if (a.dbeta != nullptr) atomicAdd(a.dbeta + c, vb);
+      if (a.dbias != nullptr) atomicAdd(a.dbias + c, vt);
+    }
   }
 }
 
@@ -287,14 +295,33 @@ int launch_ln_res_drop_bwd(const LnArgs& a, cudaStream_t s) {
   const size_t smem = static_cast<size_t>(LNB_WARPS * 3 + 1) * nch * 256 * sizeof(float);
   static bool attr_set = false;
   if (!attr_set) {
-    VLPK_CUDA(cudaFuncSetAttribute(ln_res_drop_bwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (LNB_WARPS * 3 + 1) * 1 * 1024));
-    VLPK_CUDA(cudaFuncSetAttribute(ln_res_drop_bwd_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (LNB_WARPS * 3 + 1) * 2 * 1024));
-    VLPK_CUDA(cudaFuncSetAttribute(ln_res_drop_bwd_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (LNB_WARPS * 3 + 1) * 3 * 1024));
-    VLPK_CUDA(cudaFuncSetAttribute(ln_res_drop_bwd_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (LNB_WARPS * 3 + 1) * 4 * 1024));
+    VLPK_CUDA(cudaFuncSetAttribute(ln_res_drop_bwd_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (LNB_WARPS * 3 + 1) * 1 * 1024));
+    VLPK_CUDA(cudaFuncSetAttribute(ln_res_drop_bwd_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (LNB_WARPS * 3 + 1) * 2 * 1024));
+    VLPK_CUDA(cudaFuncSetAttribute(ln_res_drop_bwd_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (LNB_WARPS * 3 + 1) * 3 * 1024));
+    VLPK_CUDA(cudaFuncSetAttribute(ln_res_drop_bwd_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (LNB_WARPS * 3 + 1) * 4 * 1024));
+    VLPK_CUDA(cudaFuncSetAttribute(ln_res_drop_bwd_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (LNB_WARPS * 3 + 1) * 1 * 1024));
+    VLPK_CUDA(cudaFuncSetAttribute(ln_res_drop_bwd_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (LNB_WARPS * 3 + 1) * 2 * 1024));
+    VLPK_CUDA(cudaFuncSetAttribute(ln_res_drop_bwd_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (LNB_WARPS * 3 + 1) * 3 * 1024));
+    VLPK_CUDA(cudaFuncSetAttribute(ln_res_drop_bwd_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (LNB_WARPS * 3 + 1) * 4 * 1024));
     attr_set = true;
   }
-  LaunchScope scope(CAT_LN_BWD, 2.0 * a.M * a.H * ((a.res ? 3 : 2) + (a.dz ? 1 : 0) + (a.dt ? 1 : 0)) + 8.0 * a.M, s);
-  VLPK_DISPATCH_NCH(a.H, VLPK_CUDA(launch_ex(ln_res_drop_bwd_kernel<NCH>, dim3(static_cast<unsigned>(grid)), dim3(LNB_WARPS * 32), smem, s, 1, a)));
+  if (!deterministic()) {
+    LaunchScope scope(CAT_LN_BWD, 2.0 * a.M * a.H * ((a.res ? 3 : 2) + (a.dz ? 1 : 0) + (a.dt ? 1 : 0)) + 8.0 * a.M, s);
+    VLPK_DISPATCH_NCH(a.H, VLPK_CUDA(launch_ex(ln_res_drop_bwd_kernel<NCH, false>, dim3(static_cast<unsigned>(grid)), dim3(LNB_WARPS * 32), smem, s, 1, a)));
+    return 0;
+  }
+  // per-block partials, then a fixed-order sum over the blocks (the grid depends only on M and the device)
+  const long long n = grid * a.H;
+  LnArgs b = a;
+  b.part = scratch_f32(SCRATCH_ORDERED, static_cast<size_t>(3 * n), s);
+  if (b.part == nullptr) return -1;
+  {
+    LaunchScope scope(CAT_LN_BWD, 2.0 * a.M * a.H * ((a.res ? 3 : 2) + (a.dz ? 1 : 0) + (a.dt ? 1 : 0)) + 8.0 * a.M, s);
+    VLPK_DISPATCH_NCH(a.H, VLPK_CUDA(launch_ex(ln_res_drop_bwd_kernel<NCH, true>, dim3(static_cast<unsigned>(grid)), dim3(LNB_WARPS * 32), smem, s, 1, b)));
+  }
+  float* outs[3] = {a.dgamma, a.dbeta, a.dbias};
+  for (int k = 0; k < 3; ++k)
+    if (outs[k] != nullptr) VLPK_TRY(launch_sum_parts(b.part + k * n, static_cast<int>(grid), a.H, outs[k], s));
   return 0;
 }
 
@@ -359,7 +386,8 @@ __global__ void __launch_bounds__(256) embed_fwd_kernel(EmbedArgs a) {
   if (lane == 0 && a.stats != nullptr) a.stats[rowi] = make_float2(mean, rstd);
 }
 
-template <int NCH>
+// ORDERED (deterministic mode): each block writes its column sums to a.part instead of adding them atomically.
+template <int NCH, bool ORDERED>
 __global__ void __launch_bounds__(256) embed_bwd_kernel(EmbedArgs a) {
   const uint64_t dseed = drop_seed(a.drop);
   extern __shared__ float s_red[];  // [wpb][2][H]
@@ -436,8 +464,14 @@ __global__ void __launch_bounds__(256) embed_bwd_kernel(EmbedArgs a) {
       vg += s_red[(w * 2 + 0) * a.H + c];
       vb += s_red[(w * 2 + 1) * a.H + c];
     }
-    atomicAdd(a.dgamma + c, vg);
-    atomicAdd(a.dbeta + c, vb);
+    if constexpr (ORDERED) {
+      const long long o = static_cast<long long>(blockIdx.x) * a.H + c;
+      a.part[o] = vg;
+      a.part[static_cast<long long>(gridDim.x) * a.H + o] = vb;
+    } else {
+      atomicAdd(a.dgamma + c, vg);
+      atomicAdd(a.dbeta + c, vb);
+    }
   }
 }
 
@@ -473,16 +507,33 @@ int launch_embed_bwd(const EmbedArgs& a, cudaStream_t s) {
   const size_t smem = static_cast<size_t>(wpb) * 2 * a.H * sizeof(float);
   static bool attr_set = false;
   if (!attr_set) {
-    VLPK_CUDA(cudaFuncSetAttribute(embed_bwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 1024 * 4));
-    VLPK_CUDA(cudaFuncSetAttribute(embed_bwd_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 1024 * 4));
-    VLPK_CUDA(cudaFuncSetAttribute(embed_bwd_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 1024 * 4));
-    VLPK_CUDA(cudaFuncSetAttribute(embed_bwd_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 1024 * 4));
+    VLPK_CUDA(cudaFuncSetAttribute(embed_bwd_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 1024 * 4));
+    VLPK_CUDA(cudaFuncSetAttribute(embed_bwd_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 1024 * 4));
+    VLPK_CUDA(cudaFuncSetAttribute(embed_bwd_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 1024 * 4));
+    VLPK_CUDA(cudaFuncSetAttribute(embed_bwd_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 1024 * 4));
+    VLPK_CUDA(cudaFuncSetAttribute(embed_bwd_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 1024 * 4));
+    VLPK_CUDA(cudaFuncSetAttribute(embed_bwd_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 1024 * 4));
+    VLPK_CUDA(cudaFuncSetAttribute(embed_bwd_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 1024 * 4));
+    VLPK_CUDA(cudaFuncSetAttribute(embed_bwd_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 1024 * 4));
     attr_set = true;
   }
-  LaunchScope scope(CAT_EMBED, 2.0 * M * a.H * 5, s);
-  VLPK_DISPATCH_NCH(a.H, embed_bwd_kernel<NCH><<<static_cast<unsigned>(grid), wpb * 32, smem, s>>>(a));
-  VLPK_CUDA(cudaGetLastError());
-  return 0;
+  if (!deterministic()) {
+    LaunchScope scope(CAT_EMBED, 2.0 * M * a.H * 5, s);
+    VLPK_DISPATCH_NCH(a.H, embed_bwd_kernel<NCH, false><<<static_cast<unsigned>(grid), wpb * 32, smem, s>>>(a));
+    VLPK_CUDA(cudaGetLastError());
+    return 0;
+  }
+  const long long n = grid * a.H;
+  EmbedArgs b = a;
+  b.part = scratch_f32(SCRATCH_ORDERED, static_cast<size_t>(2 * n), s);
+  if (b.part == nullptr) return -1;
+  {
+    LaunchScope scope(CAT_EMBED, 2.0 * M * a.H * 5, s);
+    VLPK_DISPATCH_NCH(a.H, embed_bwd_kernel<NCH, true><<<static_cast<unsigned>(grid), wpb * 32, smem, s>>>(b));
+    VLPK_CUDA(cudaGetLastError());
+  }
+  VLPK_TRY(launch_sum_parts(b.part, static_cast<int>(grid), a.H, a.dgamma, s));
+  return launch_sum_parts(b.part + n, static_cast<int>(grid), a.H, a.dbeta, s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -578,7 +629,9 @@ int launch_mask_synth(const int* len_b, const int* mode, int len_a, int B, int L
 // Block = 8 column-groups (8 columns = 16 bytes each) x 32 row-lanes over a [COLSUM_ROWS x 64] slab: every 128-byte
 // line is consumed whole by 8 adjacent threads, each thread keeps 8 independent 16-byte loads in flight, and the
 // 32 row-lane partials are folded through shared memory before one atomicAdd per column per block.
+// ORDERED (deterministic mode): block (x, y) writes its sums to out[y * N + c] instead of adding them to out[c].
 static constexpr int COLSUM_ROWS = 256;
+template <bool ORDERED>
 __global__ void __launch_bounds__(256) colsum_kernel(const __nv_bfloat16* __restrict__ x, long long ld, long long M, int N,
                                                       float* __restrict__ out) {
   __shared__ float s_part[32][65];
@@ -606,7 +659,11 @@ __global__ void __launch_bounds__(256) colsum_kernel(const __nv_bfloat16* __rest
 #pragma unroll
     for (int i = 0; i < 32; ++i) t += s_part[i][threadIdx.x];
     const int c = blockIdx.x * 64 + threadIdx.x;
-    if (c < N) atomicAdd(out + c, t);
+    if constexpr (ORDERED) {
+      if (c < N) out[static_cast<long long>(blockIdx.y) * N + c] = t;
+    } else {
+      if (c < N) atomicAdd(out + c, t);
+    }
   }
 }
 
@@ -614,10 +671,20 @@ int launch_colsum(const void* x, long long ld, long long M, int N, float* out, c
   VLPK_CHECK_ARG(N % 8 == 0 && ld % 8 == 0, "colsum: N=%d ld=%lld must be multiples of 8", N, ld);
   VLPK_CHECK_ARG(M > 0 && !misaligned(x, 15) && !misaligned(out, 3), "colsum: M=%lld, x must be 16-byte aligned", M);
   dim3 grid((N + 63) / 64, static_cast<unsigned>((M + COLSUM_ROWS - 1) / COLSUM_ROWS));
-  LaunchScope scope(CAT_MISC, 2.0 * M * N, s);
-  colsum_kernel<<<grid, 256, 0, s>>>(static_cast<const __nv_bfloat16*>(x), ld, M, N, out);
-  VLPK_CUDA(cudaGetLastError());
-  return 0;
+  if (!deterministic()) {
+    LaunchScope scope(CAT_MISC, 2.0 * M * N, s);
+    colsum_kernel<false><<<grid, 256, 0, s>>>(static_cast<const __nv_bfloat16*>(x), ld, M, N, out);
+    VLPK_CUDA(cudaGetLastError());
+    return 0;
+  }
+  float* part = scratch_f32(SCRATCH_ORDERED, static_cast<size_t>(grid.y) * N, s);
+  if (part == nullptr) return -1;
+  {
+    LaunchScope scope(CAT_MISC, 2.0 * M * N, s);
+    colsum_kernel<true><<<grid, 256, 0, s>>>(static_cast<const __nv_bfloat16*>(x), ld, M, N, part);
+    VLPK_CUDA(cudaGetLastError());
+  }
+  return launch_sum_parts(part, static_cast<int>(grid.y), N, out, s);
 }
 
 // out[i] += sum over p of part[p * n + i], added in the order p = 0, 1, ... : the fixed-order second stage of a reduction

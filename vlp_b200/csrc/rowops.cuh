@@ -26,6 +26,7 @@ struct LnArgs {
   float* dgamma = nullptr;            // [H] fp32 accumulators (atomicAdd)
   float* dbeta = nullptr;
   float* dbias = nullptr;             // [H] column sum of dt = gradient of the dense bias
+  float* part = nullptr;              // deterministic mode (set by the launcher): [3][grid][H] per-block dgamma | dbeta | dbias
 };
 
 int launch_ln_res_drop_fwd(const LnArgs& a, cudaStream_t s);
@@ -54,6 +55,7 @@ struct EmbedArgs {
   __nv_bfloat16* dz = nullptr;  // [B*L,H] grad wrt the pre-LN sum
   float* dgamma = nullptr;
   float* dbeta = nullptr;
+  float* part = nullptr;  // deterministic mode (set by the launcher): [2][grid][H] per-block dgamma | dbeta
 };
 
 int launch_embed_fwd(const EmbedArgs& a, cudaStream_t s);

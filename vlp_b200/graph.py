@@ -17,6 +17,8 @@ replay.  Shapes are frozen: a batch of another shape needs its own GraphedStep.
 
 Constraints (checked or documented): all parameters' `.grad` are produced by the graph (zero_grad(set_to_none=True) semantics — gradient
 accumulation across replays needs an explicit add outside the graph); `step` must not synchronise with the host (no `.item()`).
+Deterministic mode (torch.use_deterministic_algorithms(True), see DESIGN.md "Run-to-run reproducibility") selects other kernels, so a
+GraphedStep replays the mode it was captured in (its warm-up runs in that mode too) and refuses to replay under the other one.
 Data parallelism: `step` may include `dp.GradientAllReducer.finish()` — the arena all-reduces issued from the backward hooks and the
 tail reductions are NCCL kernels on torch.distributed's streams and are captured with their stream dependencies like everything
 else (every rank must capture and replay in lock-step; pass capture_error_mode="thread_local").
@@ -33,6 +35,7 @@ class GraphedStep:
         """capture_error_mode: passed to torch.cuda.graph; use "thread_local" when other threads issue CUDA calls during the capture
         (torch.distributed's NCCL watchdog polling earlier collectives)."""
         self.model = model
+        self.deterministic = torch.are_deterministic_algorithms_enabled()
         dev = next(model.parameters()).device
         self.static = {}
         for k, v in example_batch.items():
@@ -77,6 +80,9 @@ class GraphedStep:
                 dst.copy_(src, non_blocking=True)
 
     def __call__(self, batch=None):
+        if torch.are_deterministic_algorithms_enabled() != self.deterministic:
+            raise RuntimeError(f"vlp_b200.graph: this step was captured with deterministic algorithms "
+                               f"{'on' if self.deterministic else 'off'}; capture another GraphedStep to replay it in the other mode")
         if batch is not None:
             self.load(batch)
         self._seed.add_(1)                               # fresh dropout masks from the frozen launch sequence
