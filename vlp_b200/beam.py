@@ -5,6 +5,8 @@ bookkeeping on the device — top-k, back pointers (integer floor division: the 
 floats on torch >= 1.6 and breaks `gather`, SURVEY.md §2 #7), the per-layer K/V caches reordered by the back pointers, and the final
 best-hypothesis selection + back-tracking (:1431-1472) as vectorised tensor ops: no host synchronisation inside or after the loop
 (the optional duplicate-n-gram filter is the one host-side piece, as in the reference).
+Per-sample `task_idx` (the relaxed MLM head, relax_projection > 1) is expanded to the B*K beam rows with the other inputs; the
+reference does not expand it (:1297 vs :1325-1373), so its relaxed beam search only runs at B = 1.
 Every step runs the fused layers on the two new rows (token, [MASK]) against the K/V caches (`dec.use_kv_cache`), or — reference
 data flow — against the re-encoded prefix.
 """
@@ -94,6 +96,8 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
                 prev_layers = [_expand_beams(x[:, :-1, :], K) for x in new_layers]
             token_type_ids, position_ids = _expand_beams(token_type_ids, K), _expand_beams(position_ids, K)
             attention_mask, mask_ids = _expand_beams(attention_mask, K), _expand_beams(mask_ids, K)
+            if torch.is_tensor(task_idx) and task_idx.dim() == 1 and task_idx.shape[0] == B:
+                task_idx = _expand_beams(task_idx, K)                      # per-sample ids follow their beams (relaxed head)
         elif caches is not None:
             parent = (back + torch.arange(B, device=dev).unsqueeze(1) * K).reshape(-1)      # beam i continues hypothesis parent[i]
             caches = [c.index_select(0, parent) for c in caches]

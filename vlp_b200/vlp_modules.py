@@ -7,8 +7,9 @@ tree exists to own the named parameters; the arithmetic of the hot path — regi
 the BertLayer stack and their backward — runs in hand-written CUDA through vlp_b200.ops.  There is no eager
 PyTorch re-implementation of those ops here: without the library (or without a GPU) they raise.
 
-What intentionally stays in PyTorch (SURVEY.md §8a a12, a14, a15): the pooler, the MLM head
-(192 rows x 28 996 vocab, 0.6 % of FLOPs) and the VQA head, plus the scalar loss arithmetic.
+What intentionally stays in PyTorch (SURVEY.md §8a a12, a14, a15): the pooler, the MLM head's transform (also the relaxed
+per-task transform of relax_projection > 1 and its task select, BertLMPredictionHead.select_task) and the VQA head, plus the scalar
+loss arithmetic; the MLM decoder + bias + loss run in the fused head kernels.
 """
 import copy
 import json
@@ -101,8 +102,12 @@ def _check_supported(config):
         raise NotImplementedError("vlp_b200: attention head size must be 64 (BERT-base geometry)")
     if config.hidden_size % 128 != 0 or config.intermediate_size % 64 != 0:
         raise NotImplementedError("vlp_b200: hidden_size must be a multiple of 128 and intermediate_size of 64")
-    if getattr(config, "relax_projection", 0) and config.relax_projection > 1:
-        raise NotImplementedError("vlp_b200: relax_projection > 1 is not supported")
+
+
+def _relax(config):
+    """Number of per-task head slices, n (reference modeling.py:426-427, 451-454): config.relax_projection when it is > 1, else 1."""
+    n = getattr(config, "relax_projection", 0) or 0
+    return n if n > 1 else 1
 
 
 class BertLayerNorm(nn.Module):
@@ -333,18 +338,23 @@ class BertPooler(nn.Module):
 
 
 class BertPredictionHeadTransform(nn.Module):
+    """modeling.py:420-435.  With config.relax_projection = n > 1 the transform is Linear(H, nH) -> GELU -> LayerNorm(nH): one H-wide
+    slice per task, normalised together."""
+
     def __init__(self, config):
         super().__init__()
         self.transform_act_fn = ACT2FN[config.hidden_act] if isinstance(config.hidden_act, str) else config.hidden_act
-        self.dense = nn.Linear(config.hidden_size, config.hidden_size)
-        self.LayerNorm = BertLayerNorm(config.hidden_size, eps=1e-5)
+        hid_size = config.hidden_size * _relax(config)
+        self.dense = nn.Linear(config.hidden_size, hid_size)
+        self.LayerNorm = BertLayerNorm(hid_size, eps=1e-5)
 
     def forward(self, hidden_states):
         return self.LayerNorm(self.transform_act_fn(self.dense(hidden_states)))
 
 
 class BertLMPredictionHead(nn.Module):
-    """modeling.py:438-482: transform + decoder tied to the word embeddings + output-only bias."""
+    """modeling.py:438-482: transform + decoder tied to the word embeddings + output-only bias.  With relax_projection = n > 1 each
+    sample keeps the H-wide slice of the [B, P, nH] transform output named by its task_idx (select_task) before the decoder."""
 
     def __init__(self, config, bert_model_embedding_weights):
         super().__init__()
@@ -352,9 +362,53 @@ class BertLMPredictionHead(nn.Module):
         self.decoder = nn.Linear(bert_model_embedding_weights.size(1), bert_model_embedding_weights.size(0), bias=False)
         self.decoder.weight = bert_model_embedding_weights
         self.bias = nn.Parameter(torch.zeros(bert_model_embedding_weights.size(0)))
+        n = _relax(config)
+        self.relax_projection = n if n > 1 else 0
+
+    def check_task_idx(self, task_idx):
+        """Host-side validation of task_idx for a relaxed head (no-op otherwise); never synchronises with the device.  None, a
+        non-integer id, or a CPU tensor / Python int outside [0, n) raise ValueError.  Device-resident ids are not range-checked: an id
+        outside [0, n) selects an all-zero slice, so that sample's logits are the decoder bias alone."""
+        n = self.relax_projection
+        if n <= 1:
+            return
+        if task_idx is None:
+            raise ValueError(f"vlp_b200: relax_projection = {n} needs task_idx (one id in [0, {n}) per sample)")
+        if isinstance(task_idx, bool) or not (isinstance(task_idx, int) or torch.is_tensor(task_idx)):
+            raise ValueError(f"vlp_b200: task_idx must be an int or an integer tensor, got {type(task_idx).__name__}")
+        if torch.is_tensor(task_idx):
+            if task_idx.is_floating_point() or task_idx.is_complex() or task_idx.dtype == torch.bool or task_idx.dim() > 1:
+                raise ValueError(f"vlp_b200: task_idx must be a 0-d or 1-d integer tensor, got {task_idx.dtype} {tuple(task_idx.shape)}")
+            if task_idx.is_cuda or task_idx.numel() == 0:
+                return
+            lo, hi = int(task_idx.min()), int(task_idx.max())
+        else:
+            lo = hi = task_idx
+        if lo < 0 or hi >= n:
+            raise ValueError(f"vlp_b200: task_idx values must lie in [0, {n}), got [{lo}, {hi}]")
+
+    def select_task(self, hidden_states, task_idx):
+        """[B, P, nH] -> [B, P, H]: sample b keeps slice task_idx[b], the reference's view(B, P, n, H)[arange(B), :, task_idx, :]
+        (modeling.py:471-476); returns its input unchanged for a plain head.  task_idx is an int, a 0-d tensor or a [B] tensor.
+
+        Evaluated as a multiply by the one-hot of task_idx and a sum over the n slices: the forward value is exact (one non-zero term),
+        and the backward is a broadcast multiply, with no scatter or atomics, so deterministic mode needs nothing special.  The one-hot
+        is a comparison with arange(n), not F.one_hot, which asserts on the device for an id outside [0, n)."""
+        n = self.relax_projection
+        if n <= 1:
+            return hidden_states
+        self.check_task_idx(task_idx)
+        B, P, nH = hidden_states.shape
+        t = torch.as_tensor(task_idx, device=hidden_states.device).reshape(-1)
+        if t.numel() not in (1, B):
+            raise ValueError(f"vlp_b200: task_idx has {t.numel()} ids for a batch of {B}")
+        one_hot = (t.unsqueeze(1) == torch.arange(n, device=t.device)).to(hidden_states.dtype)          # [B or 1, n]
+        x = hidden_states.reshape(B, P, n, nH // n)
+        return (x * one_hot.view(-1, 1, n, 1)).sum(2)
 
     def forward(self, hidden_states, task_idx=None):
         hidden_states = self.transform(hidden_states.to(self.decoder.weight.dtype))
+        hidden_states = self.select_task(hidden_states, task_idx)
         return self.decoder(hidden_states) + self.bias
 
 
@@ -388,7 +442,11 @@ class PreTrainedBertModel(nn.Module):
     @classmethod
     def from_pretrained(cls, pretrained_model_name, state_dict=None, cache_dir=None, *inputs, **kwargs):
         """Same kwargs as the reference (config_path, type_vocab_size, relax_projection, task_idx, max_position_embeddings,
-        fp32_embedding, label_smoothing, drop_prob) and the same state_dict remaps (modeling.py:648-732).
+        fp32_embedding, label_smoothing, drop_prob) and the same state_dict remaps (modeling.py:648-732): TF-era gamma/beta names, the
+        segment-type and position tables, and the MLM head transform between relaxed and plain layouts — a relaxed checkpoint loaded
+        into a plain model keeps slice config.task_idx (slice 0 when it is unset; as in the reference a falsy task_idx kwarg, 0
+        included, leaves the config's value), a plain checkpoint loaded into a relaxed model is repeated n times, and two different
+        relax counts > 1 raise ValueError (the reference asserts).
         `pretrained_model_name` must be a local directory holding bert_config.json (+ pytorch_model.bin unless state_dict is given)."""
         if not os.path.isdir(pretrained_model_name):
             raise EnvironmentError(f"vlp_b200.from_pretrained: '{pretrained_model_name}' is not a local directory (no network / archive download)")
@@ -436,6 +494,28 @@ class PreTrainedBertModel(nn.Module):
                 state_dict[k] = old.repeat(reps, 1)[:config.max_position_embeddings].clone()
             else:
                 state_dict[k] = old[:config.max_position_embeddings]
+        k = "cls.predictions.transform.dense.weight"         # relaxed <-> plain MLM head transform (modeling.py:704-732)
+        H = config.hidden_size
+        n_config = _relax(config)
+        if k in state_dict and n_config * H != state_dict[k].shape[0]:
+            if state_dict[k].shape[0] % H != 0:
+                raise ValueError(f"from_pretrained: {k} has {state_dict[k].shape[0]} rows, not a multiple of hidden_size {H}")
+            n_state = state_dict[k].shape[0] // H
+            if n_state > 1 and n_config > 1:
+                raise ValueError(f"from_pretrained: a checkpoint with relax_projection {n_state} cannot load into relax_projection {n_config}")
+            vectors = ("cls.predictions.transform.dense.bias", "cls.predictions.transform.LayerNorm.weight",
+                       "cls.predictions.transform.LayerNorm.bias")
+            if n_state == 1:                                 # plain checkpoint, relaxed model: every task starts from the same head
+                state_dict[k] = state_dict[k].unsqueeze(0).repeat(n_config, 1, 1).reshape(n_config * H, H)
+                for kk in vectors:
+                    state_dict[kk] = state_dict[kk].unsqueeze(0).repeat(n_config, 1).view(-1)
+            else:                                            # relaxed checkpoint, plain model: keep slice config.task_idx (else 0)
+                t = config.task_idx if getattr(config, "task_idx", None) is not None and 0 <= config.task_idx <= 3 else 0
+                if t >= n_state:
+                    raise ValueError(f"from_pretrained: task_idx {t} names no slice of a relax_projection {n_state} checkpoint")
+                state_dict[k] = state_dict[k].view(n_state, H, H).select(0, t)
+                for kk in vectors:
+                    state_dict[kk] = state_dict[kk].view(n_state, H).select(0, t)
         prefix_fix = "" if hasattr(model, "bert") else "bert."
         if prefix_fix:
             state_dict = {(kk[len(prefix_fix):] if kk.startswith(prefix_fix) else kk): v for kk, v in state_dict.items()}
@@ -622,6 +702,8 @@ class BertForPreTrainingLossMask(PreTrainedBertModel, _RegionProjections):
     def forward(self, vis_feats, vis_pe, input_ids, token_type_ids=None, attention_mask=None, masked_lm_labels=None, ans_labels=None,
                 next_sentence_label=None, masked_pos=None, masked_weights=None, task_idx=None, vis_masked_pos=[], mask_image_regions=False,
                 drop_worst_ratio=0.2, vqa_inference=False):
+        if not vqa_inference and masked_pos is not None and masked_pos.numel() > 0:
+            self.cls.predictions.check_task_idx(task_idx)      # before anything is launched
         vis_feats, vis_pe = self.project_regions(vis_feats, vis_pe)
 
         if vqa_inference:                                    # modeling.py:1039-1047
@@ -655,7 +737,7 @@ class BertForPreTrainingLossMask(PreTrainedBertModel, _RegionProjections):
             gathered = torch.gather(sequence_output, 1, masked_pos.unsqueeze(2).expand(-1, -1, sequence_output.size(-1)))
             if self.fused_mlm_head:                          # decoder + bias + CE in libvlpk, SURVEY.md §8f-3
                 pred = self.cls.predictions
-                hid = pred.transform(gathered.to(pred.decoder.weight.dtype))
+                hid = pred.select_task(pred.transform(gathered.to(pred.decoder.weight.dtype)), task_idx)
                 eps = self.crit_mask_lm_smoothed.label_smoothing if self.crit_mask_lm_smoothed is not None else 0.0
                 loss_flat, scores = ops.DecoderCEFn.apply(hid.reshape(-1, hid.size(-1)), pred.decoder.weight, pred.bias,
                                                           masked_lm_labels.reshape(-1), self._vlpk_dp_hook, eps)
@@ -723,6 +805,7 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         return [torch.empty(batch, rows, 2 * H, device=device, dtype=torch.bfloat16) for _ in self.bert.encoder.layer]
 
     def forward(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, sample_mode="greedy"):
+        self.cls.predictions.check_task_idx(task_idx)          # before anything is launched
         with torch.no_grad():
             vis_feats, vis_pe = self.project_regions(vis_feats, vis_pe)
             if self.search_beam_size > 1:
