@@ -45,13 +45,19 @@ typedef struct VlpkDropout {
   const uint64_t* seed_dev; /* optional device counter added to `seed` at run time (CUDA-graph replays) */
 } VlpkDropout;
 
+/* Key slots.  Attention over Lkv keys lays its per-row data out in S = 128 * ceil(Lkv / 128) key slots (128, 256, 384 or 512): a
+ * packed mask row has S / 32 u32 words, an attention keep-bit row S / 8 bytes, and the attention dropout element of (sequence b, head
+ * h, query q, key j) is ((b * heads + h) * Lq + q) * S + j.  For Lkv <= 128 this is the 128-slot layout of earlier versions. */
 typedef struct VlpkShape {
   int32_t B;     /* sequences */
-  int32_t Lq;    /* query rows per sequence  (<= 128) */
-  int32_t Lkv;   /* key/value rows per sequence (<= 128); == Lq except incremental decode */
+  int32_t Lq;    /* query rows per sequence  (<= 128, or <= kv_slots) */
+  int32_t Lkv;   /* key/value rows per sequence (<= 128, or <= 512 with kv_slots); == Lq except incremental decode */
   int32_t H;     /* hidden size (multiple of 64) */
   int32_t heads; /* H / 64 */
   int32_t I;     /* intermediate size */
+  int32_t kv_slots; /* 0: Lq, Lkv <= 128 and masks / keep-bits in the 128-slot layout; else S = 128 * ceil(Lkv / 128), which every mask
+                     * and keep-bit buffer passed with this shape must have.  Added after version 102: a C caller that builds VlpkShape
+                     * itself must zero it (e.g. `VlpkShape s = {0}`). */
 } VlpkShape;
 
 /* One BertLayer's parameters (modeling.py:244-372), bf16, nn.Linear layout [out,in]. */
@@ -87,9 +93,9 @@ typedef struct VlpkLayerActs {
   float* stats2; /* [B*Lq, 2] */
   void* kv;      /* incremental decode only: [B*Lkv, 2H] key|value projections; else NULL */
   /* Optional (NULL = attention backward re-evaluates Philox): packed keep-decisions of the attention-probability dropout, 1 bit per
-   * element (byte i = elements 8i..8i+7, numbering as in vlpk_debug_dropout_mask; 128 key slots per query row).  Written by the
-   * forward attention kernel, read by the backward one. */
-  unsigned char* drop_attn; /* [B*heads*Lq*16] */
+   * element (byte i = elements 8i..8i+7, numbering as in vlpk_debug_dropout_mask; S key slots per query row, S = 128 when
+   * kv_slots = 0).  Written by the forward attention kernel, read by the backward one. */
+  unsigned char* drop_attn; /* [B*heads*Lq*S/8] */
 } VlpkLayerActs;
 
 /* Scratch for backward, shared by all layers (bf16). */
@@ -120,17 +126,20 @@ void vlpk_set_deterministic(int on);
 /* host-only: the (tile N, split-K) the cost model picks for a GEMM; out2 = {bn, splits}.  No GPU needed. */
 int vlpk_debug_plan_gemm(int M, int N, int K, int a_mn, int b_mn, int nseg, int seg_rows, int epi, int bn, int splits, int* out2);
 /* A-B testing only: switch a host-side scheduling choice at run time.  "wgrad_stream" (default 1, env VLPK_WGRAD_STREAM=0 turns it
- * off): the weight-gradient GEMM of each Linear's backward runs on a side stream behind its dgrad.  < 0: unknown name. */
+ * off): the weight-gradient GEMM of each Linear's backward runs on a side stream behind its dgrad.  "attn_tiled" (default 0, test
+ * support): the KV-tiled attention kernels, which otherwise run only when Lq or Lkv > 128, run at every length.  < 0: unknown name. */
 int vlpk_debug_set_option(const char* name, int value);
 
-/* get_extended_attention_mask (modeling.py:807-833) -> per-row 128-bit "attend" bitmask.
- * mask: [B, rows, kv] with element strides (stride_b, stride_r, 1); rows may be 1 (2-D mask). out: [B, rows, 4] u32. */
+/* get_extended_attention_mask (modeling.py:807-833) -> per-row S-bit "attend" bitmask, S = 128 * ceil(kv / 128), kv <= 512.
+ * mask: [B, rows, kv] with element strides (stride_b, stride_r, 1); rows may be 1 (2-D mask). out: [B, rows, S / 32] u32 (bits >= kv
+ * are 0; for kv <= 128, [B, rows, 4] exactly as in earlier versions). */
 int vlpk_mask_pack(const void* mask, int dtype, int mode, int B, int rows, int kv, int64_t stride_b, int64_t stride_r,
                    uint32_t* out, void* stream);
 
 /* Input staging (SURVEY.md §8f-4): the loader's self-attention mask (vlp/seq2seq_loader.py:291-301) synthesised on the device from
  * three integers per sample instead of shipping [B,L,L] int64: len_a region tokens (same for the batch), len_b[b] text tokens,
- * mode[b] (0 = bidirectional, 1 = seq2seq).  Output: the packed bitmask vlpk_mask_pack would produce from the loader's matrix. */
+ * mode[b] (0 = bidirectional, 1 = seq2seq), L <= 512.  Output: [B, L, S / 32] u32, the packed bitmask vlpk_mask_pack would produce
+ * from the loader's matrix. */
 int vlpk_mask_synth(const int32_t* len_b, const int32_t* mode, int len_a, int B, int L, uint32_t* out, void* stream);
 
 /* y[M,N] = dropout(act(x[M,K] w[N,K]^T + b)) — vis_embed / vis_pe_embed Linears (modeling.py:1003-1018, 1035-1036).
@@ -175,13 +184,22 @@ int vlpk_ln_res_drop_bwd(int64_t M, int H, const void* t, const void* res, const
                          void* dz, void* dt, float* dgamma, float* dbeta, float* dbias, const VlpkDropout* drop, uint64_t site,
                          void* stream);
 
-/* softmax(QK^T/8 + mask) V per (sequence, head) — BertSelfAttention core (modeling.py:279-302). */
+/* softmax(QK^T/8 + mask) V per (sequence, head) — BertSelfAttention core (modeling.py:279-302).  Masks in the 128-slot layout:
+ * Lq, Lkv <= 128.  The _wide forms take the key-slot count of the mask (and dropout numbering) as kv_slots, with VlpkShape's meaning:
+ * 0 = 128-slot layout with Lq, Lkv <= 128; else 128 * ceil(Lkv / 128) for Lkv <= 512. */
 int vlpk_attn_core_fwd(int B, int heads, int Lq, int Lkv, const void* q, int64_t ld_q, const void* k, const void* v, int64_t ld_kv,
                        const uint32_t* mask_bits, int mask_rows, void* ctx, int64_t ld_ctx, float* lse, const VlpkDropout* drop,
                        uint64_t site, void* stream);
 int vlpk_attn_core_bwd(int B, int heads, int L, const void* q, const void* k, const void* v, int64_t ld_qkv, const uint32_t* mask_bits,
                        int mask_rows, const void* ctx, const void* dctx, int64_t ld_ctx, const float* lse, void* dq, void* dk,
                        void* dv, int64_t ld_dqkv, const VlpkDropout* drop, uint64_t site, void* stream);
+int vlpk_attn_core_fwd_wide(int B, int heads, int Lq, int Lkv, const void* q, int64_t ld_q, const void* k, const void* v, int64_t ld_kv,
+                            const uint32_t* mask_bits, int mask_rows, void* ctx, int64_t ld_ctx, float* lse, const VlpkDropout* drop,
+                            uint64_t site, int kv_slots, void* stream);
+int vlpk_attn_core_bwd_wide(int B, int heads, int L, const void* q, const void* k, const void* v, int64_t ld_qkv,
+                            const uint32_t* mask_bits, int mask_rows, const void* ctx, const void* dctx, int64_t ld_ctx, const float* lse,
+                            void* dq, void* dk, void* dv, int64_t ld_dqkv, const VlpkDropout* drop, uint64_t site, int kv_slots,
+                            void* stream);
 
 /* BertAttention.forward (modeling.py:326-330): QKV projection + attention core + output projection + LN.
  * x_kv == NULL or == x: self-attention over x (training / encoder path).
@@ -224,7 +242,7 @@ int vlpk_mha_incr_fwd(const VlpkShape* s, const VlpkLayerWeights* w, const void*
 int vlpk_layer_cached_fwd(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, void* kv_cache, int cache_rows, int pos,
                           const uint32_t* mask_bits, int mask_rows, VlpkLayerActs* a, uint64_t layer_id, void* stream);
 /* Host-only: bytes the caller must provide for a shape.  out3 = { all VlpkLayerActs buffers of ONE layer (without the optional
- * drop_attn keep-bytes: B*heads*Lq*16),
+ * drop_attn keep-bytes: B*heads*Lq*S/8),
  * all VlpkBwdScratch buffers (shared by the layers), the fp32 VlpkLayerGrads accumulators of ONE layer }. */
 int vlpk_workspace_bytes(const VlpkShape* s, size_t* out3);
 
@@ -300,8 +318,9 @@ int vlpk_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 int vlpk_colsum(const void* x, int64_t ld, int64_t M, int N, float* out, void* stream);
 /* Test support: out[i] = 1 if element i of dropout site `site` is kept under `drop` (p, seed), else 0 — the decision every fused
  * kernel takes through the same counter-based Philox function.  Element numbering per site: LayerNorm / embedding / Linear+ReLU
- * sites: row * width + column; attention site: ((b * heads + h) * Lq + query) * 128 + key.  Sites: layer * 8 + {0 attention
+ * sites: row * width + column; attention site: ((b * heads + h) * Lq + query) * S + key.  Sites: layer * 8 + {0 attention
  * probabilities, 1 attention-output dropout, 2 FFN-output dropout}; 1<<20 embeddings; (1<<21)+{1 vis_embed, 2 vis_pe_embed}.
+ * (attention: S key slots per query row, see VlpkShape; 128 for Lkv <= 128.)
  * n must be a multiple of 8. */
 int vlpk_debug_dropout_mask(const VlpkDropout* drop, uint64_t site, int64_t n, unsigned char* out, void* stream);
 int vlpk_add_bf16(void* dst, const void* a, const void* b, int64_t n, void* stream);

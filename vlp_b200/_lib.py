@@ -20,8 +20,9 @@ class VlpkDropout(C.Structure):
 
 
 class VlpkShape(C.Structure):
+    # kv_slots: 0 = the 128-slot layout (Lq, Lkv <= 128); else 128 * ceil(Lkv / 128), see ops.kv_slots.  Left at 0 by the six-field form.
     _fields_ = [("B", C.c_int32), ("Lq", C.c_int32), ("Lkv", C.c_int32), ("H", C.c_int32), ("heads", C.c_int32),
-                ("I", C.c_int32)]
+                ("I", C.c_int32), ("kv_slots", C.c_int32)]
 
 
 WEIGHT_FIELDS = ["wq", "wk", "wv", "bq", "bk", "bv", "wo", "bo", "ln1_g", "ln1_b", "w1", "b1", "w2", "b2", "ln2_g", "ln2_b"]
@@ -77,6 +78,10 @@ _SIGS = {
                                    C.POINTER(VlpkDropout), c_u64, _P]),
     "vlpk_attn_core_bwd": (c_int, [c_int, c_int, c_int, _P, _P, _P, c_i64, _P, c_int, _P, _P, c_i64, _P, _P, _P, _P, c_i64,
                                    C.POINTER(VlpkDropout), c_u64, _P]),
+    "vlpk_attn_core_fwd_wide": (c_int, [c_int, c_int, c_int, c_int, _P, c_i64, _P, _P, c_i64, _P, c_int, _P, c_i64, _P,
+                                        C.POINTER(VlpkDropout), c_u64, c_int, _P]),
+    "vlpk_attn_core_bwd_wide": (c_int, [c_int, c_int, c_int, _P, _P, _P, c_i64, _P, c_int, _P, _P, c_i64, _P, _P, _P, _P, c_i64,
+                                        C.POINTER(VlpkDropout), c_u64, c_int, _P]),
     "vlpk_mha_fwd": (c_int, [C.POINTER(VlpkShape), C.POINTER(VlpkLayerWeights), _P, _P, _P, c_int, C.POINTER(VlpkLayerActs),
                              c_float, c_float, C.POINTER(VlpkDropout), c_u64, _P]),
     "vlpk_ffn_fwd": (c_int, [C.POINTER(VlpkShape), C.POINTER(VlpkLayerWeights), C.POINTER(VlpkLayerActs), c_float,

@@ -48,7 +48,7 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
     out_len = token_type_ids.shape[1]
     dev = input_ids.device
     prev_emb, prev_layers = None, None
-    caches = dec.new_kv_caches(B, dev) if getattr(dec, "use_kv_cache", False) else None
+    caches = dec.new_kv_caches(B, dev, out_len) if getattr(dec, "use_kv_cache", False) else None
     curr_ids = input_ids
     mask_ids = input_ids[:, :1] * 0 + dec.mask_word_id
     total_scores, beam_eos, step_ids, step_ptrs = [], [], [], []

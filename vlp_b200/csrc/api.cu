@@ -35,8 +35,14 @@ inline DropoutCfg mk_drop(const VlpkDropout* d, float p, uint64_t site) {
 
 int check_shape(const VlpkShape* s) {
   VLPK_CHECK_ARG(s != nullptr, "null shape");
-  VLPK_CHECK_ARG(s->B > 0 && s->Lq > 0 && s->Lkv > 0 && s->Lq <= 128 && s->Lkv <= 128,
-                 "shape: B=%d Lq=%d Lkv=%d (sequence length must be in [1,128])", s->B, s->Lq, s->Lkv);
+  if (s->kv_slots == 0) {
+    VLPK_CHECK_ARG(s->B > 0 && s->Lq > 0 && s->Lkv > 0 && s->Lq <= 128 && s->Lkv <= 128,
+                   "shape: B=%d Lq=%d Lkv=%d (sequence length must be in [1,128])", s->B, s->Lq, s->Lkv);
+  } else {
+    VLPK_CHECK_ARG(s->B > 0 && s->Lq > 0 && s->Lkv > 0 && s->Lkv <= 512 && s->kv_slots == (s->Lkv + 127) / 128 * 128 && s->Lq <= s->kv_slots,
+                   "shape: B=%d Lq=%d Lkv=%d kv_slots=%d (sequence length must be in [1,512], kv_slots = 128 * ceil(Lkv / 128) >= Lq)",
+                   s->B, s->Lq, s->Lkv, s->kv_slots);
+  }
   VLPK_CHECK_ARG(s->H > 0 && s->H % 64 == 0 && s->heads * 64 == s->H, "shape: H=%d heads=%d (head_dim must be 64)", s->H,
                  s->heads);
   VLPK_CHECK_ARG(s->I > 0 && s->I % 64 == 0, "shape: I=%d must be a multiple of 64", s->I);
@@ -160,7 +166,7 @@ int mha_fwd_impl(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, c
   const bool incr = (cache == nullptr && x_kv != nullptr && x_kv != x);
   const DropoutCfg none = make_dropout(0.f, 0, 0);
   AttnDesc ad;
-  ad.B = s->B; ad.heads = s->heads; ad.Lq = s->Lq; ad.Lkv = s->Lkv;
+  ad.B = s->B; ad.heads = s->heads; ad.Lq = s->Lq; ad.Lkv = s->Lkv; ad.kv_slots = s->kv_slots;
   ad.mask_bits = bits; ad.mask_rows = mask_rows;
   ad.o = a->ctx; ad.ld_o = H; ad.lse = a->lse;
   ad.drop = mk_drop(drop, p_attn, site_of(layer_id, SITE_ATTN));
@@ -311,7 +317,7 @@ int mha_bwd_impl(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, c
       [&](cudaStream_t q) { return dgrad_linear(M, H, H, dt1, H, w->wo, H, ws->dctx, H, EPI_STORE, nullptr, 0, q); }));
   // ---- attention core
   AttnDesc ad;
-  ad.B = s->B; ad.heads = s->heads; ad.Lq = s->Lq; ad.Lkv = s->Lkv;
+  ad.B = s->B; ad.heads = s->heads; ad.Lq = s->Lq; ad.Lkv = s->Lkv; ad.kv_slots = s->kv_slots;
   ad.q = a->qkv; ad.k = static_cast<const bf16*>(a->qkv) + H; ad.v = static_cast<const bf16*>(a->qkv) + 2 * H;
   ad.ld_q = 3 * H; ad.ld_kv = 3 * H;
   ad.o = a->ctx; ad.ld_o = H; ad.d_o = ws->dctx;
@@ -387,6 +393,7 @@ int vlpk_version(void) { return VLPK_VERSION; }
 int vlpk_debug_set_option(const char* name, int value) {
   VLPK_CHECK_ARG(name != nullptr, "set_option: null name");
   if (strcmp(name, "wgrad_stream") == 0) { g_wgrad_stream = value ? 1 : 0; return 0; }
+  if (strcmp(name, "attn_tiled") == 0) { set_attn_tiled(value != 0); return 0; }
   set_error("set_option: unknown option '%s'", name);
   return -1;
 }
@@ -539,12 +546,12 @@ int vlpk_ln_res_drop_bwd(int64_t M, int H, const void* t, const void* res, const
   return launch_ln_res_drop_bwd(a, S(stream));
 }
 
-int vlpk_attn_core_fwd(int B, int heads, int Lq, int Lkv, const void* q, int64_t ld_q, const void* k, const void* v, int64_t ld_kv,
-                       const uint32_t* mask_bits, int mask_rows, void* ctx, int64_t ld_ctx, float* lse, const VlpkDropout* drop,
-                       uint64_t site, void* stream) {
+int vlpk_attn_core_fwd_wide(int B, int heads, int Lq, int Lkv, const void* q, int64_t ld_q, const void* k, const void* v, int64_t ld_kv,
+                            const uint32_t* mask_bits, int mask_rows, void* ctx, int64_t ld_ctx, float* lse, const VlpkDropout* drop,
+                            uint64_t site, int kv_slots, void* stream) {
   VLPK_CHECK_ARG(q && k && v && ctx, "attn_core_fwd: null pointer");
   AttnDesc d;
-  d.B = B; d.heads = heads; d.Lq = Lq; d.Lkv = Lkv;
+  d.B = B; d.heads = heads; d.Lq = Lq; d.Lkv = Lkv; d.kv_slots = kv_slots;
   d.q = q; d.k = k; d.v = v; d.ld_q = ld_q; d.ld_kv = ld_kv;
   d.o = ctx; d.ld_o = ld_ctx;
   d.mask_bits = mask_bits; d.mask_rows = mask_rows; d.lse = lse;
@@ -552,18 +559,31 @@ int vlpk_attn_core_fwd(int B, int heads, int Lq, int Lkv, const void* q, int64_t
   return launch_attn_fwd(d, S(stream));
 }
 
-int vlpk_attn_core_bwd(int B, int heads, int L, const void* q, const void* k, const void* v, int64_t ld_qkv, const uint32_t* mask_bits,
-                       int mask_rows, const void* ctx, const void* dctx, int64_t ld_ctx, const float* lse, void* dq, void* dk, void* dv,
-                       int64_t ld_dqkv, const VlpkDropout* drop, uint64_t site, void* stream) {
+int vlpk_attn_core_fwd(int B, int heads, int Lq, int Lkv, const void* q, int64_t ld_q, const void* k, const void* v, int64_t ld_kv,
+                       const uint32_t* mask_bits, int mask_rows, void* ctx, int64_t ld_ctx, float* lse, const VlpkDropout* drop,
+                       uint64_t site, void* stream) {
+  return vlpk_attn_core_fwd_wide(B, heads, Lq, Lkv, q, ld_q, k, v, ld_kv, mask_bits, mask_rows, ctx, ld_ctx, lse, drop, site, 0, stream);
+}
+
+int vlpk_attn_core_bwd_wide(int B, int heads, int L, const void* q, const void* k, const void* v, int64_t ld_qkv, const uint32_t* mask_bits,
+                            int mask_rows, const void* ctx, const void* dctx, int64_t ld_ctx, const float* lse, void* dq, void* dk, void* dv,
+                            int64_t ld_dqkv, const VlpkDropout* drop, uint64_t site, int kv_slots, void* stream) {
   VLPK_CHECK_ARG(q && k && v && ctx && dctx && lse && dq && dk && dv, "attn_core_bwd: null pointer");
   AttnDesc d;
-  d.B = B; d.heads = heads; d.Lq = L; d.Lkv = L;
+  d.B = B; d.heads = heads; d.Lq = L; d.Lkv = L; d.kv_slots = kv_slots;
   d.q = q; d.k = k; d.v = v; d.ld_q = ld_qkv; d.ld_kv = ld_qkv;
   d.o = const_cast<void*>(ctx); d.ld_o = ld_ctx; d.d_o = dctx;
   d.mask_bits = mask_bits; d.mask_rows = mask_rows; d.lse = const_cast<float*>(lse);
   d.dq = dq; d.dk = dk; d.dv = dv; d.ld_dqkv = ld_dqkv;
   d.drop = mk_drop(drop, drop ? drop->p : 0.f, site);
   return launch_attn_bwd(d, S(stream));
+}
+
+int vlpk_attn_core_bwd(int B, int heads, int L, const void* q, const void* k, const void* v, int64_t ld_qkv, const uint32_t* mask_bits,
+                       int mask_rows, const void* ctx, const void* dctx, int64_t ld_ctx, const float* lse, void* dq, void* dk, void* dv,
+                       int64_t ld_dqkv, const VlpkDropout* drop, uint64_t site, void* stream) {
+  return vlpk_attn_core_bwd_wide(B, heads, L, q, k, v, ld_qkv, mask_bits, mask_rows, ctx, dctx, ld_ctx, lse, dq, dk, dv, ld_dqkv, drop, site, 0,
+                                 stream);
 }
 
 int vlpk_mha_fwd(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, const void* x_kv, const uint32_t* mask_bits, int mask_rows,

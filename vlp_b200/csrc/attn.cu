@@ -1,4 +1,4 @@
-// vlp_b200 — masked-softmax attention core for VLP's [image-region | text-token] sequence (L <= 128).
+// vlp_b200 — masked-softmax attention core for VLP's [image-region | text-token] sequence: single-tile kernels for L <= 128, KV-tiled ones up to 512.
 //
 // Reference semantics (pytorch_pretrained_bert/modeling.py:279-302):
 //   S = Q K^T / sqrt(64) + mask_add ; P = softmax(S) ; P = dropout(P) ; ctx = P V
@@ -418,6 +418,494 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_kernel(const __grid_c
 }
 
 // ------------------------------------------------------------------------------------------------
+// tiled kernels: sequences longer than one tile (Lq or Lkv in (128, 512]), or any length under the "attn_tiled" test option.
+// Key slots S = 128 * ceil(Lkv / 128): a mask row has S / 32 words, a keep-bit row S / 8 bytes, and the dropout element of
+// (b, h, q, key) is ((b * heads + h) * Lq + q) * S + key.  For Lkv <= 128 that is the single-tile kernels' layout.
+//   fwd     : CTA per (head, sequence, 128-row q tile); K/V tiles stream through a two-stage TMA ring; online softmax in the log2
+//             domain, O rescaled in registers.  Same per-element semantics as attn_fwd_kernel.
+//   bwd dq  : CTA per (head, sequence, q tile); pass 1 over the KV tiles: delta_r = sum_j P_rj dP_rj from the recomputed P (as
+//             attn_bwd_kernel); pass 2: dS and dQ = dS K / 8 in registers.  Writes dQ, delta and the dQ column sums.
+//   bwd dkv : CTA per (head, sequence, kv tile); loops over the q tiles: P from lse, dS with delta, dV += P^T dO, dK += dS^T Q in
+//             registers.  Writes dK, dV and their column sums.
+// No floating-point atomics: every output element and every bias partial is written by exactly one CTA.  Recompute cost: QK^T runs
+// 3x and dO V^T 3x (2 in the dq kernel, 1 in the dkv kernel) against 1x each in the single-tile backward.
+// ------------------------------------------------------------------------------------------------
+static constexpr int MAX_SLOTS = 512;
+static bool g_attn_tiled = false;  // test option "attn_tiled": the tiled kernels at every length
+
+void set_attn_tiled(bool on) { g_attn_tiled = on; }
+
+struct AttnTiledArgs {
+  int B, heads, Lq, Lkv;
+  int slots;                  // S: key slots per query row
+  int tiles;                  // bwd: bias partials per sequence (= q tiles = kv tiles)
+  const uint32_t* mask_bits;  // [B, mask_rows, S / 32]
+  int mask_rows;
+  float* lse;                 // [B, heads, Lq]
+  float* delta;               // bwd: [B, heads, Lq], written by the dq kernel, read by the dkv kernel
+  DropoutCfg drop;
+  unsigned char* keep_out;    // fwd, optional: S / 8 bytes per (sequence, head, query row)
+  float* dbias_part;          // bwd, optional: [B * tiles][3 * heads * 64] column sums of dQ | dK | dV per (sequence, tile)
+};
+
+// The 4 mask words of key tile kt for query row `row`.
+__device__ __forceinline__ void load_mask_tile(const AttnTiledArgs& a, int b, int row, int kt, uint32_t (&mw)[4]) {
+  const int mr = (a.mask_rows == 1) ? 0 : min(row, a.mask_rows - 1);
+  const uint4 m4 = __ldg(reinterpret_cast<const uint4*>(a.mask_bits + (static_cast<size_t>(b) * a.mask_rows + mr) * (a.slots >> 5)) + kt);
+  mw[0] = m4.x; mw[1] = m4.y; mw[2] = m4.z; mw[3] = m4.w;
+}
+
+__device__ __forceinline__ uint64_t tiled_row_elem0(const AttnTiledArgs& a, int b, int h, int row) {
+  return ((static_cast<uint64_t>(b) * a.heads + h) * a.Lq + min(row, a.Lq - 1)) * a.slots;
+}
+
+// this thread's column of the bias partial: column sums of a staged [128 x 64] bf16 tile (rows past the sequence are zero)
+__device__ __forceinline__ float staged_colsum(const uint8_t* stg, int c) {
+  float acc = 0.f;
+#pragma unroll 8
+  for (int r = 0; r < TL; ++r)
+    acc += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(stg + r * 128 + (((c >> 3) ^ (r & 7)) << 4) + (c & 7) * 2));
+  return acc;
+}
+
+struct FwdTiledSmem {
+  static constexpr int OFF_Q = 0;        // later output staging
+  static constexpr int OFF_KV = TILE_B;  // 2 stages of K | V
+  static constexpr int OFF_BAR = 5 * TILE_B;
+  static constexpr int TOTAL = OFF_BAR + 24;
+  static constexpr int DYN = TOTAL + 1024;
+};
+
+// One CTA per SM: the running O (32 registers) stays live beside S and P, which does not fit the 128 registers of two CTAs
+__global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_tiled_kernel(const __grid_constant__ AttnTmaps tm, const AttnTiledArgs a) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem + FwdTiledSmem::OFF_Q;
+  uint8_t* sKV = smem + FwdTiledSmem::OFF_KV;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + FwdTiledSmem::OFF_BAR);  // [0] Q, [1 + s] K|V stage s
+
+  pdl_launch_dependents();
+  const int h = blockIdx.x, b = blockIdx.y, q0 = blockIdx.z * TL;
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const Frag f;
+  const int qi = tid & 3;
+  const int nkt = (a.Lkv + TL - 1) / TL;
+
+  if (tid == 0) {
+    tma_prefetch_desc(&tm.q);
+    tma_prefetch_desc(&tm.k);
+    tma_prefetch_desc(&tm.v);
+    tma_prefetch_desc(&tm.o);
+    for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();
+  if (tid == 0) {
+    mbar_arrive_expect_tx(&bars[0], TILE_B);
+    tma_load_3d(sQ, &tm.q, &bars[0], h * HD, q0, b);
+    for (int kt = 0; kt < 2 && kt < nkt; ++kt) {
+      mbar_arrive_expect_tx(&bars[1 + kt], 2 * TILE_B);
+      tma_load_3d(sKV + kt * 2 * TILE_B, &tm.k, &bars[1 + kt], h * HD, kt * TL, b);
+      tma_load_3d(sKV + kt * 2 * TILE_B + TILE_B, &tm.v, &bars[1 + kt], h * HD, kt * TL, b);
+    }
+  }
+
+  const int row[2] = {q0 + wg * 64 + f.fr, q0 + wg * 64 + f.fr + 8};
+  uint64_t row_elem0[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) row_elem0[hh] = tiled_row_elem0(a, b, h, row[hh]);
+  const uint64_t dseed = drop_seed(a.drop);
+
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float mx[2] = {-INFINITY, -INFINITY}, rsum[2] = {0.f, 0.f}, lsum[2] = {0.f, 0.f};  // lsum / rsum: this thread's columns only
+  mbar_wait(&bars[0], 0);
+  for (int kt = 0; kt < nkt; ++kt) {
+    const int st = kt & 1;
+    uint8_t* sK = sKV + st * 2 * TILE_B;
+    uint8_t* sV = sK + TILE_B;
+    uint32_t mw[2][4];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) load_mask_tile(a, b, row[hh], kt, mw[hh]);
+    float s[64];
+    mbar_wait(&bars[1 + st], (kt >> 1) & 1);
+    {
+      const uint32_t qa = smem_u32(sQ) + wg * 8192, k0 = smem_u32(sK);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < HD / 16; ++k)
+        wgmma_m64n128k16_ss<0, 0>(s, wgmma_desc_sw128(qa + k * 32, 16, 1024), wgmma_desc_sw128(k0 + k * 32, 16, 1024), k > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(s);
+    }
+    const int lkv = a.Lkv - kt * TL;  // >= 1: column 0 of every tile is a real key, so the tile maximum is finite
+    float tmx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < 64; ++i) {
+      const int hh = (i >> 1) & 1;
+      s[i] = score(s[i], mw[hh], 8 * (i >> 2) + f.fc + (i & 1), lkv);
+      tmx[hh] = fmaxf(tmx[hh], s[i]);
+    }
+    float alpha[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const float mnew = fmaxf(mx[hh], quad_max(tmx[hh]));
+      alpha[hh] = fast_ex2(mx[hh] - mnew);  // 0 on the first tile (mx = -inf)
+      mx[hh] = mnew;
+      lsum[hh] *= alpha[hh];
+      rsum[hh] *= alpha[hh];
+    }
+    uint32_t kw[2][4];
+    const uint64_t tile_elem0[2] = {row_elem0[0] + kt * TL, row_elem0[1] + kt * TL};
+    attn_keep_words(a.drop, dseed, tile_elem0, kw);
+    if (a.keep_out != nullptr) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+        if (row[hh] < a.Lq) reinterpret_cast<uint32_t*>(a.keep_out + (tile_elem0[hh] >> 3))[qi] = kw[hh][qi];
+    }
+    uint32_t pa[8][4];
+#pragma unroll
+    for (int i = 0; i < 64; i += 2) {
+      const int hh = (i >> 1) & 1, col = 8 * (i >> 2) + f.fc;
+      const float x0 = fast_ex2(s[i] - mx[hh]), x1 = fast_ex2(s[i + 1] - mx[hh]);
+      lsum[hh] += x0 + x1;
+      const float e0 = bf16_round(x0), e1 = bf16_round(x1);
+      rsum[hh] += e0 + e1;
+      const uint32_t keep = kw[hh][col >> 5] >> (col & 31);
+      const float p0 = (keep & 1u) ? e0 * a.drop.scale : 0.f;
+      const float p1 = (keep & 2u) ? e1 * a.drop.scale : 0.f;
+      pa[i >> 3][(i >> 1) & 3] = pack_bf16x2(p0, p1);
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
+    {
+      const uint32_t v0 = smem_u32(sV);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TL / 16; ++k) wgmma_m64n64k16_rs<1>(o, pa[k], wgmma_desc_sw128(v0 + k * 2048, 8192, 1024), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(o);
+    }
+    __syncthreads();  // both warpgroups are done with stage st
+    if (tid == 0 && kt + 2 < nkt) {
+      mbar_arrive_expect_tx(&bars[1 + st], 2 * TILE_B);
+      tma_load_3d(sK, &tm.k, &bars[1 + st], h * HD, (kt + 2) * TL, b);
+      tma_load_3d(sV, &tm.v, &bars[1 + st], h * HD, (kt + 2) * TL, b);
+    }
+  }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    rsum[hh] = quad_sum(rsum[hh]);
+    lsum[hh] = quad_sum(lsum[hh]);
+    if (qi == 0 && a.lse != nullptr && row[hh] < a.Lq)
+      a.lse[(static_cast<size_t>(b) * a.heads + h) * a.Lq + row[hh]] = (mx[hh] + log2f(lsum[hh])) * LN2;
+  }
+  const float inv[2] = {1.0f / rsum[0], 1.0f / rsum[1]};
+  uint8_t* stg = sQ + wg * 8192;  // this warpgroup's own Q rows: only its own S = QK^T read them
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    const int hh = (i >> 1) & 1;
+    sw_write_pair(stg, f.fr + 8 * hh, 8 * (i >> 2) + f.fc, pack_bf16x2(o[i] * inv[hh], o[i + 1] * inv[hh]));
+  }
+  fence_proxy_async_smem();
+  __syncthreads();
+  if (tid == 0) {
+    tma_store_3d(&tm.o, sQ, h * HD, q0, b);
+    tma_store_commit();
+    tma_store_wait<0>();
+  }
+}
+
+// P (recomputed from the logsumexp; 0 for keys >= Lkv and rows >= Lq) and the dropout-masked dP of one 64 x 128 (q, key) block,
+// in place of the S = QK^T and dP = dO V^T accumulators.
+__device__ __forceinline__ void tiled_p_dp(const AttnTiledArgs& a, const Frag& f, float (&s)[64], float (&dp)[64], const uint32_t (&mw)[2][4],
+                                           const uint32_t (&kw)[2][4], const float (&lse2)[2], const bool (&row_ok)[2], int lkv) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) {
+    const int hh = (i >> 1) & 1, col = 8 * (i >> 2) + f.fc + (i & 1);
+    s[i] = row_ok[hh] ? fast_ex2(score(s[i], mw[hh], col, lkv) - lse2[hh]) : 0.f;
+    dp[i] = ((kw[hh][col >> 5] >> (col & 31)) & 1u) ? dp[i] * a.drop.scale : 0.f;
+  }
+}
+
+// S = Q K^T and dP = dO V^T for one warpgroup's 64 query rows against one 128-key tile
+__device__ __forceinline__ void tiled_s_dp(uint32_t qa, uint32_t doa, uint32_t k0, uint32_t v0, float (&s)[64], float (&dp)[64]) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < HD / 16; ++k)
+    wgmma_m64n128k16_ss<0, 0>(s, wgmma_desc_sw128(qa + k * 32, 16, 1024), wgmma_desc_sw128(k0 + k * 32, 16, 1024), k > 0 ? 1u : 0u);
+#pragma unroll
+  for (int k = 0; k < HD / 16; ++k)
+    wgmma_m64n128k16_ss<0, 0>(dp, wgmma_desc_sw128(doa + k * 32, 16, 1024), wgmma_desc_sw128(v0 + k * 32, 16, 1024), k > 0 ? 1u : 0u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  reg_fence(s);
+  reg_fence(dp);
+}
+
+struct BwdDqSmem {
+  static constexpr int OFF_Q = 0;  // later dQ staging
+  static constexpr int OFF_DO = TILE_B;
+  static constexpr int OFF_KV = 2 * TILE_B;  // 2 stages of K | V
+  static constexpr int OFF_BAR = 6 * TILE_B;
+  static constexpr int TOTAL = OFF_BAR + 24;
+  static constexpr int DYN = TOTAL + 1024;
+};
+
+__global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_dq_tiled_kernel(const __grid_constant__ AttnTmaps tm, const AttnTiledArgs a) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem + BwdDqSmem::OFF_Q;
+  uint8_t* sdO = smem + BwdDqSmem::OFF_DO;
+  uint8_t* sKV = smem + BwdDqSmem::OFF_KV;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + BwdDqSmem::OFF_BAR);  // [0] Q | dO, [1 + s] K|V stage s
+
+  pdl_launch_dependents();
+  const int h = blockIdx.x, b = blockIdx.y, qt = blockIdx.z, q0 = qt * TL;
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const Frag f;
+  const int nkt = (a.Lkv + TL - 1) / TL;
+  const int nload = 2 * nkt;  // the KV tiles stream through the ring twice: delta pass, then dQ pass
+
+  if (tid == 0) {
+    tma_prefetch_desc(&tm.q);
+    tma_prefetch_desc(&tm.k);
+    tma_prefetch_desc(&tm.v);
+    tma_prefetch_desc(&tm.o);
+    for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();
+  if (tid == 0) {
+    mbar_arrive_expect_tx(&bars[0], 2 * TILE_B);
+    tma_load_3d(sQ, &tm.q, &bars[0], h * HD, q0, b);
+    tma_load_3d(sdO, &tm.o, &bars[0], h * HD, q0, b);
+    for (int i = 0; i < 2; ++i) {
+      mbar_arrive_expect_tx(&bars[1 + i], 2 * TILE_B);
+      tma_load_3d(sKV + i * 2 * TILE_B, &tm.k, &bars[1 + i], h * HD, (i % nkt) * TL, b);
+      tma_load_3d(sKV + i * 2 * TILE_B + TILE_B, &tm.v, &bars[1 + i], h * HD, (i % nkt) * TL, b);
+    }
+  }
+
+  const int row[2] = {q0 + wg * 64 + f.fr, q0 + wg * 64 + f.fr + 8};
+  uint64_t row_elem0[2];
+  float lse2[2];
+  bool row_ok[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    row_elem0[hh] = tiled_row_elem0(a, b, h, row[hh]);
+    row_ok[hh] = row[hh] < a.Lq;
+    lse2[hh] = row_ok[hh] ? a.lse[(static_cast<size_t>(b) * a.heads + h) * a.Lq + row[hh]] * LOG2E : 0.f;
+  }
+  const uint64_t dseed = drop_seed(a.drop);
+  const uint32_t qa = smem_u32(sQ) + wg * 8192, doa = smem_u32(sdO) + wg * 8192;
+
+  float delta[2] = {0.f, 0.f};
+  float dq[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) dq[i] = 0.f;
+  mbar_wait(&bars[0], 0);
+  for (int it = 0; it < nload; ++it) {
+    const int st = it & 1, kt = it % nkt;
+    uint8_t* sK = sKV + st * 2 * TILE_B;
+    uint8_t* sV = sK + TILE_B;
+    uint32_t mw[2][4], kw[2][4];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) load_mask_tile(a, b, row[hh], kt, mw[hh]);
+    const uint64_t tile_elem0[2] = {row_elem0[0] + kt * TL, row_elem0[1] + kt * TL};
+    attn_keep_words(a.drop, dseed, tile_elem0, kw);
+    float s[64], dp[64];
+    mbar_wait(&bars[1 + st], (it >> 1) & 1);
+    tiled_s_dp(qa, doa, smem_u32(sK), smem_u32(sV), s, dp);
+    tiled_p_dp(a, f, s, dp, mw, kw, lse2, row_ok, a.Lkv - kt * TL);
+    if (it < nkt) {
+#pragma unroll
+      for (int i = 0; i < 64; ++i) delta[(i >> 1) & 1] = fmaf(s[i], dp[i], delta[(i >> 1) & 1]);
+      if (it == nkt - 1) {
+        delta[0] = quad_sum(delta[0]);
+        delta[1] = quad_sum(delta[1]);
+        if ((tid & 3) == 0) {
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh)
+            if (row_ok[hh]) a.delta[(static_cast<size_t>(b) * a.heads + h) * a.Lq + row[hh]] = delta[hh];
+        }
+      }
+    } else {
+      uint32_t dsa[8][4];
+#pragma unroll
+      for (int i = 0; i < 64; i += 2) {
+        const int hh = (i >> 1) & 1;
+        dsa[i >> 3][(i >> 1) & 3] = pack_bf16x2(s[i] * (dp[i] - delta[hh]) * 0.125f, s[i + 1] * (dp[i + 1] - delta[hh]) * 0.125f);
+      }
+      const uint32_t k0 = smem_u32(sK);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TL / 16; ++k) wgmma_m64n64k16_rs<1>(dq, dsa[k], wgmma_desc_sw128(k0 + k * 2048, 8192, 1024), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(dq);
+    }
+    __syncthreads();  // both warpgroups are done with stage st
+    if (tid == 0 && it + 2 < nload) {
+      const int nt = (it + 2) % nkt;
+      mbar_arrive_expect_tx(&bars[1 + st], 2 * TILE_B);
+      tma_load_3d(sK, &tm.k, &bars[1 + st], h * HD, nt * TL, b);
+      tma_load_3d(sV, &tm.v, &bars[1 + st], h * HD, nt * TL, b);
+    }
+  }
+  uint8_t* stg = sQ + wg * 8192;  // this warpgroup's own Q rows
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) sw_write_pair(stg, f.fr + 8 * ((i >> 1) & 1), 8 * (i >> 2) + f.fc, pack_bf16x2(dq[i], dq[i + 1]));
+  fence_proxy_async_smem();
+  __syncthreads();
+  if (tid == 0) {
+    tma_store_3d(&tm.dq, sQ, h * HD, q0, b);
+    tma_store_commit();
+  }
+  if (a.dbias_part != nullptr && tid < HD)
+    a.dbias_part[(static_cast<size_t>(b) * a.tiles + qt) * 3 * a.heads * HD + h * HD + tid] = staged_colsum(sQ, tid);
+  if (tid == 0) tma_store_wait<0>();
+}
+
+struct BwdDkvSmem {
+  static constexpr int OFF_K = 0;        // later dK staging
+  static constexpr int OFF_V = TILE_B;   // later dV staging
+  static constexpr int OFF_QD = 2 * TILE_B;  // 2 stages of Q | dO
+  static constexpr int OFF_P = 6 * TILE_B;   // 2 atoms of [128 q x 64 kv]: dropout-masked P
+  static constexpr int OFF_DS = 8 * TILE_B;  // 2 atoms of [128 q x 64 kv]: dS
+  static constexpr int OFF_BAR = 10 * TILE_B;
+  static constexpr int TOTAL = OFF_BAR + 24;
+  static constexpr int DYN = TOTAL + 1024;
+};
+
+__global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_dkv_tiled_kernel(const __grid_constant__ AttnTmaps tm, const AttnTiledArgs a) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sK = smem + BwdDkvSmem::OFF_K;
+  uint8_t* sV = smem + BwdDkvSmem::OFF_V;
+  uint8_t* sQD = smem + BwdDkvSmem::OFF_QD;
+  uint8_t* sP = smem + BwdDkvSmem::OFF_P;
+  uint8_t* sDS = smem + BwdDkvSmem::OFF_DS;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + BwdDkvSmem::OFF_BAR);  // [0] K | V, [1 + s] Q|dO stage s
+
+  pdl_launch_dependents();
+  const int h = blockIdx.x, b = blockIdx.y, kt = blockIdx.z, kv0 = kt * TL;
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const Frag f;
+  const int nqt = (a.Lq + TL - 1) / TL;
+  const int lkv = a.Lkv - kv0;
+
+  if (tid == 0) {
+    tma_prefetch_desc(&tm.q);
+    tma_prefetch_desc(&tm.k);
+    tma_prefetch_desc(&tm.v);
+    tma_prefetch_desc(&tm.o);
+    for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();  // also orders the reads of delta after the dq kernel
+  if (tid == 0) {
+    mbar_arrive_expect_tx(&bars[0], 2 * TILE_B);
+    tma_load_3d(sK, &tm.k, &bars[0], h * HD, kv0, b);
+    tma_load_3d(sV, &tm.v, &bars[0], h * HD, kv0, b);
+    for (int i = 0; i < 2 && i < nqt; ++i) {
+      mbar_arrive_expect_tx(&bars[1 + i], 2 * TILE_B);
+      tma_load_3d(sQD + i * 2 * TILE_B, &tm.q, &bars[1 + i], h * HD, i * TL, b);
+      tma_load_3d(sQD + i * 2 * TILE_B + TILE_B, &tm.o, &bars[1 + i], h * HD, i * TL, b);
+    }
+  }
+  const uint64_t dseed = drop_seed(a.drop);
+
+  float dk[32], dv[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) dk[i] = dv[i] = 0.f;
+  mbar_wait(&bars[0], 0);
+  for (int qt = 0; qt < nqt; ++qt) {
+    const int st = qt & 1;
+    uint8_t* sQ = sQD + st * 2 * TILE_B;
+    uint8_t* sdO = sQ + TILE_B;
+    const int rl[2] = {wg * 64 + f.fr, wg * 64 + f.fr + 8};  // rows within the q tile
+    const int row[2] = {qt * TL + rl[0], qt * TL + rl[1]};
+    uint32_t mw[2][4], kw[2][4];
+    float lse2[2], delta[2];
+    bool row_ok[2];
+    uint64_t tile_elem0[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      load_mask_tile(a, b, row[hh], kt, mw[hh]);
+      tile_elem0[hh] = tiled_row_elem0(a, b, h, row[hh]) + kv0;
+      row_ok[hh] = row[hh] < a.Lq;
+      const size_t li = (static_cast<size_t>(b) * a.heads + h) * a.Lq + row[hh];
+      lse2[hh] = row_ok[hh] ? a.lse[li] * LOG2E : 0.f;
+      delta[hh] = row_ok[hh] ? a.delta[li] : 0.f;
+    }
+    attn_keep_words(a.drop, dseed, tile_elem0, kw);
+    float s[64], dp[64];
+    mbar_wait(&bars[1 + st], (qt >> 1) & 1);
+    tiled_s_dp(smem_u32(sQ) + wg * 8192, smem_u32(sdO) + wg * 8192, smem_u32(sK), smem_u32(sV), s, dp);
+    tiled_p_dp(a, f, s, dp, mw, kw, lse2, row_ok, lkv);
+#pragma unroll
+    for (int i = 0; i < 64; i += 2) {
+      const int hh = (i >> 1) & 1, col = 8 * (i >> 2) + f.fc;
+      const uint32_t keep = kw[hh][col >> 5] >> (col & 31);
+      const float p0 = (keep & 1u) ? s[i] * a.drop.scale : 0.f, p1 = (keep & 2u) ? s[i + 1] * a.drop.scale : 0.f;
+      sw_write_pair(sP + (col >> 6) * TILE_B, rl[hh], col & 63, pack_bf16x2(p0, p1));
+      sw_write_pair(sDS + (col >> 6) * TILE_B, rl[hh], col & 63,
+                    pack_bf16x2(s[i] * (dp[i] - delta[hh]) * 0.125f, s[i + 1] * (dp[i + 1] - delta[hh]) * 0.125f));
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+    // dV[kv, d] += sum_q Pd[q, kv] dO[q, d] and dK[kv, d] += sum_q dS[q, kv] Q[q, d] for kv rows [64 wg, 64 wg + 64)
+    {
+      const uint32_t p0 = smem_u32(sP) + wg * TILE_B, ds0 = smem_u32(sDS) + wg * TILE_B, do0 = smem_u32(sdO), q0 = smem_u32(sQ);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TL / 16; ++k)
+        wgmma_m64n64k16_ss<1, 1>(dv, wgmma_desc_sw128(p0 + k * 2048, 8192, 1024), wgmma_desc_sw128(do0 + k * 2048, 8192, 1024), 1u);
+#pragma unroll
+      for (int k = 0; k < TL / 16; ++k)
+        wgmma_m64n64k16_ss<1, 1>(dk, wgmma_desc_sw128(ds0 + k * 2048, 8192, 1024), wgmma_desc_sw128(q0 + k * 2048, 8192, 1024), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(dv);
+      reg_fence(dk);
+    }
+    __syncthreads();  // P / dS buffers and stage st are free
+    if (tid == 0 && qt + 2 < nqt) {
+      mbar_arrive_expect_tx(&bars[1 + st], 2 * TILE_B);
+      tma_load_3d(sQ, &tm.q, &bars[1 + st], h * HD, (qt + 2) * TL, b);
+      tma_load_3d(sdO, &tm.o, &bars[1 + st], h * HD, (qt + 2) * TL, b);
+    }
+  }
+  // every wgmma has read K / V: reuse them as output staging
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    const int r = wg * 64 + f.fr + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + f.fc;
+    sw_write_pair(sK, r, col, pack_bf16x2(dk[i], dk[i + 1]));
+    sw_write_pair(sV, r, col, pack_bf16x2(dv[i], dv[i + 1]));
+  }
+  fence_proxy_async_smem();
+  __syncthreads();
+  if (tid == 0) {
+    tma_store_3d(&tm.dk, sK, h * HD, kv0, b);
+    tma_store_3d(&tm.dv, sV, h * HD, kv0, b);
+    tma_store_commit();
+  }
+  if (a.dbias_part != nullptr && tid < 2 * HD) {
+    const int o = 1 + (tid >> 6), c = tid & 63;
+    a.dbias_part[(static_cast<size_t>(b) * a.tiles + kt) * 3 * a.heads * HD + o * a.heads * HD + h * HD + c] =
+        staged_colsum(o == 1 ? sK : sV, c);
+  }
+  if (tid == 0) tma_store_wait<0>();
+}
+
+// ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
 static int make_seq_tmap(CUtensorMap* out, const void* base, int width, int L, int B, int64_t ld, int64_t batch_stride = 0) {
@@ -430,11 +918,74 @@ static int make_seq_tmap(CUtensorMap* out, const void* base, int width, int L, i
 
 static int check_common(const AttnDesc& d) {
   VLPK_CHECK_ARG(d.head_dim == HD, "attention: head_dim %d unsupported (only 64)", d.head_dim);
-  VLPK_CHECK_ARG(d.Lq >= 1 && d.Lq <= TL && d.Lkv >= 1 && d.Lkv <= TL, "attention: Lq=%d Lkv=%d must be in [1,128]",
-                 d.Lq, d.Lkv);
+  if (d.kv_slots == 0) {
+    VLPK_CHECK_ARG(d.Lq >= 1 && d.Lq <= TL && d.Lkv >= 1 && d.Lkv <= TL, "attention: Lq=%d Lkv=%d must be in [1,128]",
+                   d.Lq, d.Lkv);
+  } else {
+    VLPK_CHECK_ARG(d.Lkv >= 1 && d.Lkv <= MAX_SLOTS && d.kv_slots == (d.Lkv + TL - 1) / TL * TL && d.Lq >= 1 && d.Lq <= d.kv_slots,
+                   "attention: Lq=%d Lkv=%d kv_slots=%d (needs Lkv in [1,512], kv_slots = 128 * ceil(Lkv / 128), Lq in [1,kv_slots])",
+                   d.Lq, d.Lkv, d.kv_slots);
+  }
   VLPK_CHECK_ARG(d.B >= 1 && d.heads >= 1, "attention: B=%d heads=%d", d.B, d.heads);
   VLPK_CHECK_ARG(d.mask_bits != nullptr && (d.mask_rows == 1 || d.mask_rows == d.Lq), "attention: mask rows %d",
                  d.mask_rows);
+  return 0;
+}
+
+static bool use_tiled(const AttnDesc& d) { return g_attn_tiled || d.Lq > TL || d.Lkv > TL; }
+
+static AttnTiledArgs tiled_args(const AttnDesc& d) {
+  AttnTiledArgs a;
+  a.B = d.B; a.heads = d.heads; a.Lq = d.Lq; a.Lkv = d.Lkv;
+  a.slots = d.kv_slots != 0 ? d.kv_slots : TL;
+  a.tiles = (d.Lq + TL - 1) / TL;
+  a.mask_bits = d.mask_bits; a.mask_rows = d.mask_rows;
+  a.lse = d.lse; a.delta = nullptr;
+  a.drop = d.drop;
+  a.keep_out = nullptr;
+  a.dbias_part = nullptr;
+  return a;
+}
+
+static int launch_attn_fwd_tiled(const AttnDesc& d, const AttnTmaps& tm, cudaStream_t stream) {
+  AttnTiledArgs a = tiled_args(d);
+  a.keep_out = d.keep_out;
+  static bool attr_set = false;
+  if (!attr_set) {
+    VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdTiledSmem::DYN));
+    attr_set = true;
+  }
+  LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * d.Lkv * HD, stream);
+  VLPK_CUDA(launch_ex(attn_fwd_tiled_kernel, dim3(d.heads, d.B, (d.Lq + TL - 1) / TL), dim3(ATT_THREADS), FwdTiledSmem::DYN, stream, 1, tm, a));
+  return 0;
+}
+
+static int launch_attn_bwd_tiled(const AttnDesc& d, const AttnTmaps& tm, cudaStream_t stream) {
+  AttnTiledArgs a = tiled_args(d);
+  const long long nbias = 3LL * d.heads * HD;
+  a.delta = scratch_f32(SCRATCH_ATTN_DELTA, static_cast<size_t>(d.B) * d.heads * d.Lq, stream);
+  if (a.delta == nullptr) return -1;
+  if (d.dbias != nullptr) {
+    a.dbias_part = scratch_f32(SCRATCH_ATTN_DBIAS, static_cast<size_t>(d.B) * a.tiles * nbias, stream);
+    if (a.dbias_part == nullptr) return -1;
+  }
+  static bool attr_set = false;
+  if (!attr_set) {
+    VLPK_CUDA(cudaFuncSetAttribute(attn_bwd_dq_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdDqSmem::DYN));
+    VLPK_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdDkvSmem::DYN));
+    attr_set = true;
+  }
+  const double flops = 10.0 * d.B * d.heads * d.Lq * d.Lkv * HD;  // algorithmic: the recomputed products are not counted
+  {
+    LaunchScope scope(CAT_ATTN_BWD, 0.4 * flops, stream);
+    VLPK_CUDA(launch_ex(attn_bwd_dq_tiled_kernel, dim3(d.heads, d.B, a.tiles), dim3(ATT_THREADS), BwdDqSmem::DYN, stream, 1, tm, a));
+  }
+  {
+    LaunchScope scope(CAT_ATTN_BWD, 0.6 * flops, stream);
+    VLPK_CUDA(launch_ex(attn_bwd_dkv_tiled_kernel, dim3(d.heads, d.B, (d.Lkv + TL - 1) / TL), dim3(ATT_THREADS), BwdDkvSmem::DYN, stream, 1,
+                        tm, a));
+  }
+  if (d.dbias != nullptr) VLPK_TRY(launch_sum_parts(a.dbias_part, d.B * a.tiles, nbias, d.dbias, stream));
   return 0;
 }
 
@@ -448,6 +999,7 @@ int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream) {
   VLPK_TRY(make_seq_tmap(&tm.v, d.v, width, d.Lkv, d.B, d.ld_kv, d.kv_batch_stride));
   VLPK_TRY(make_seq_tmap(&tm.o, d.o, width, d.Lq, d.B, d.ld_o));
   tm.dq = tm.dk = tm.dv = tm.o;
+  if (use_tiled(d)) return launch_attn_fwd_tiled(d, tm, stream);
   AttnArgs a;
   a.B = d.B; a.heads = d.heads; a.Lq = d.Lq; a.Lkv = d.Lkv;
   a.mask_bits = d.mask_bits; a.mask_rows = d.mask_rows;
@@ -479,6 +1031,7 @@ int launch_attn_bwd(const AttnDesc& d, cudaStream_t stream) {
   VLPK_TRY(make_seq_tmap(&tm.dq, d.dq, width, d.Lq, d.B, d.ld_dqkv));
   VLPK_TRY(make_seq_tmap(&tm.dk, d.dk, width, d.Lkv, d.B, d.ld_dqkv));
   VLPK_TRY(make_seq_tmap(&tm.dv, d.dv, width, d.Lkv, d.B, d.ld_dqkv));
+  if (use_tiled(d)) return launch_attn_bwd_tiled(d, tm, stream);
   AttnArgs a;
   a.B = d.B; a.heads = d.heads; a.Lq = d.Lq; a.Lkv = d.Lkv;
   a.mask_bits = d.mask_bits; a.mask_rows = d.mask_rows;

@@ -6,7 +6,8 @@ namespace vlpk {
 
 struct AttnDesc {
   int B = 0, heads = 0, head_dim = 64;
-  int Lq = 0, Lkv = 0;  // query rows / key-value rows per sequence (<= 128)
+  int Lq = 0, Lkv = 0;  // query rows / key-value rows per sequence (<= 128, or <= 512 with kv_slots)
+  int kv_slots = 0;     // 0: single-tile layout (Lq, Lkv <= 128); else 128 * ceil(Lkv / 128) key slots per mask / keep-bit row
   // Q: [B, Lq, ld_q] ; K,V: [B, Lkv, ld_kv] ; head h occupies columns [h*64, h*64+64) from each base pointer.
   const void* q = nullptr;
   const void* k = nullptr;
@@ -15,11 +16,11 @@ struct AttnDesc {
   int64_t kv_batch_stride = 0;  // elements between consecutive sequences of K / V (0 = Lkv * ld_kv); a K/V cache has cache_rows * ld_kv
   void* o = nullptr;  // ctx [B, Lq, ld_o]   (bwd: forward output, read for delta)
   int64_t ld_o = 0;
-  const uint32_t* mask_bits = nullptr;  // [B, mask_rows, 4] packed by vlpk_mask_pack
+  const uint32_t* mask_bits = nullptr;  // [B, mask_rows, S / 32] packed by vlpk_mask_pack, S = kv_slots (128 when 0)
   int mask_rows = 0;                    // Lq or 1
   float* lse = nullptr;                 // [B, heads, Lq] (fwd: optional output ; bwd: input)
   DropoutCfg drop = {0.f, 1.f, 0u, 0ull, 0ull, nullptr};   // backward: drop.bits = forward's keep_out (or null: re-evaluate Philox)
-  unsigned char* keep_out = nullptr;  // forward, optional: [B*heads*Lq*16] packed keep-decisions of the attention dropout
+  unsigned char* keep_out = nullptr;  // forward, optional: [B*heads*Lq*S/8] packed keep-decisions of the attention dropout
   // backward only
   const void* d_o = nullptr;  // [B, Lq, ld_o]
   void* dq = nullptr;
@@ -29,7 +30,9 @@ struct AttnDesc {
   float* dbias = nullptr;  // optional [3 * heads * 64] fp32: += column sums of dQ | dK | dV, summed over sequences in a fixed order
 };
 
+// Lq, Lkv <= 128: the single-tile kernels; longer sequences (or the "attn_tiled" test option): the KV-tiled kernels.
 int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream);
 int launch_attn_bwd(const AttnDesc& d, cudaStream_t stream);
+void set_attn_tiled(bool on);
 
 }  // namespace vlpk

@@ -66,7 +66,8 @@ enum ScratchSlot {
   SCRATCH_WGRAD = 2,       // deterministic mode: split-K slices of weight gradients (main or wgrad side stream)
   SCRATCH_ORDERED = 3,     // deterministic mode: per-block partials of column sums, LayerNorm dγ/dβ, token types, Σg²
   SCRATCH_SORT = 4,        // deterministic mode: sorted (id, row) pairs and sort temporaries of the table scatter
-  SCRATCH_SLOTS = 5
+  SCRATCH_ATTN_DELTA = 5,  // tiled attention backward: delta_r = sum_j P_rj dP_rj, written by the dq kernel for the dkv kernel
+  SCRATCH_SLOTS = 6
 };
 float* scratch_f32(int slot, size_t n, cudaStream_t s);
 

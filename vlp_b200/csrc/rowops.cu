@@ -4,7 +4,7 @@
 //
 //   ln_res_drop_fwd/bwd : y = LN(dropout(t) + res)           BertSelfOutput / BertOutput, modeling.py:313-317, 353-357
 //   embed_fwd/bwd       : y = dropout(LN(word|vis + pos|vis_pe + type))      BertEmbeddings, modeling.py:217-241
-//   mask_pack           : additive/0-1 attention mask -> 128-bit row bitmask  get_extended_attention_mask, modeling.py:807-833
+//   mask_pack           : additive/0-1 attention mask -> S-bit row bitmask (S = 128 * ceil(kv / 128))  get_extended_attention_mask, modeling.py:807-833
 //   colsum              : bias gradients
 //   f32_to_bf16         : gradient arena conversion
 #include "rowops.cuh"
@@ -550,37 +550,43 @@ __device__ __forceinline__ bool mask_attend<__nv_bfloat16>(__nv_bfloat16 v, int 
 template <>
 __device__ __forceinline__ bool mask_attend<long long>(long long v, int mode) { return v != 0; }
 
-// One warp per mask row: lane j tests elements j, j+32, j+64, j+96 (coalesced 256-byte requests for int64 masks) and the four
-// words come from __ballot_sync.  (Round 1 walked a whole 984-byte row per thread: 49 us for the [64,123,123] int64 mask.)
+// One warp per mask row: lane j tests elements j, j+32, j+64, j+96 of each 128-key chunk (coalesced 256-byte requests for int64
+// masks) and each chunk's four words come from __ballot_sync.  (Round 1 walked a whole 984-byte row per thread: 49 us for the
+// [64,123,123] int64 mask.)  A row has `chunks` = ceil(kv / 128) chunks: S / 32 words with S = 128 * chunks key slots.
 template <typename T>
 __global__ void __launch_bounds__(256) mask_pack_kernel(const T* __restrict__ m, long long sb, long long sr, int B, int rows, int kv,
-                                                              int mode, uint32_t* __restrict__ out) {
+                                                              int chunks, int mode, uint32_t* __restrict__ out) {
   const long long idx = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
   if (idx >= static_cast<long long>(B) * rows) return;  // warp-uniform
   const int lane = threadIdx.x & 31;
   const int b = static_cast<int>(idx / rows), r = static_cast<int>(idx % rows);
   const T* p = m + b * sb + r * sr;
-  uint32_t w[4];
+  for (int c = 0; c < chunks; ++c) {
+    uint32_t w[4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int j = lane + 32 * i;
-    const bool on = (j < kv) && mask_attend<T>(p[j], mode);
-    w[i] = __ballot_sync(0xffffffffu, on);
+    for (int i = 0; i < 4; ++i) {
+      const int j = 128 * c + lane + 32 * i;
+      const bool on = (j < kv) && mask_attend<T>(p[j], mode);
+      w[i] = __ballot_sync(0xffffffffu, on);
+    }
+    if (lane == 0) reinterpret_cast<uint4*>(out)[idx * chunks + c] = make_uint4(w[0], w[1], w[2], w[3]);
   }
-  if (lane == 0) reinterpret_cast<uint4*>(out)[idx] = make_uint4(w[0], w[1], w[2], w[3]);
 }
+
+static constexpr int MASK_MAX_KV = 512;
 
 int launch_mask_pack(const void* mask, int dtype, int mode, int B, int rows, int kv, long long stride_b, long long stride_r,
                      uint32_t* out, cudaStream_t s) {
-  VLPK_CHECK_ARG(B > 0 && rows > 0 && kv > 0 && kv <= 128, "mask_pack: kv=%d must be in [1,128]", kv);
+  VLPK_CHECK_ARG(B > 0 && rows > 0 && kv > 0 && kv <= MASK_MAX_KV, "mask_pack: kv=%d must be in [1,512]", kv);
   VLPK_CHECK_ARG(!misaligned(out, 15), "mask_pack: the bitmask buffer must be 16-byte aligned");
   const long long n = static_cast<long long>(B) * rows;
   const unsigned gridw = static_cast<unsigned>((n + 7) / 8);
+  const int chunks = (kv + 127) / 128;
   LaunchScope scope(CAT_MISC, 0.0, s);
   switch (dtype) {
-    case VLPK_DT_F32: mask_pack_kernel<float><<<gridw, 256, 0, s>>>(static_cast<const float*>(mask), stride_b, stride_r, B, rows, kv, mode, out); break;
-    case VLPK_DT_BF16: mask_pack_kernel<__nv_bfloat16><<<gridw, 256, 0, s>>>(static_cast<const __nv_bfloat16*>(mask), stride_b, stride_r, B, rows, kv, mode, out); break;
-    case VLPK_DT_I64: mask_pack_kernel<long long><<<gridw, 256, 0, s>>>(static_cast<const long long*>(mask), stride_b, stride_r, B, rows, kv, mode, out); break;
+    case VLPK_DT_F32: mask_pack_kernel<float><<<gridw, 256, 0, s>>>(static_cast<const float*>(mask), stride_b, stride_r, B, rows, kv, chunks, mode, out); break;
+    case VLPK_DT_BF16: mask_pack_kernel<__nv_bfloat16><<<gridw, 256, 0, s>>>(static_cast<const __nv_bfloat16*>(mask), stride_b, stride_r, B, rows, kv, chunks, mode, out); break;
+    case VLPK_DT_I64: mask_pack_kernel<long long><<<gridw, 256, 0, s>>>(static_cast<const long long*>(mask), stride_b, stride_r, B, rows, kv, chunks, mode, out); break;
     default: set_error("mask_pack: unsupported dtype %d", dtype); return -1;
   }
   VLPK_CUDA(cudaGetLastError());
@@ -592,33 +598,36 @@ int launch_mask_pack(const void* mask, int dtype, int mode, int B, int rows, int
 // sample do.  len_a = region tokens, len_b = text tokens, st = len_a + 2, en = len_a + len_b + 3 (= tokens incl. [CLS] / 2 x [SEP]):
 //   s2s : every row attends to columns [0, st); rows in [st, en) additionally to columns [st, row]   (causal over the text)
 //   bi  : every row attends to columns [0, en)
+// Rows have ceil(L / 128) chunks of 4 words, as mask_pack writes them.
 __global__ void __launch_bounds__(256) mask_synth_kernel(const int* __restrict__ len_b, const int* __restrict__ mode, int len_a, int B, int L,
-                                                          uint32_t* __restrict__ out) {
+                                                          int chunks, uint32_t* __restrict__ out) {
   const long long idx = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
   if (idx >= static_cast<long long>(B) * L) return;  // warp-uniform
   const int lane = threadIdx.x & 31;
   const int b = static_cast<int>(idx / L), r = static_cast<int>(idx % L);
   const int st = len_a + 2, en = min(len_a + len_b[b] + 3, L);
   const bool s2s = mode[b] != 0;
-  uint32_t w[4];
+  for (int c = 0; c < chunks; ++c) {
+    uint32_t w[4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int j = lane + 32 * i;
-    bool on;
-    if (s2s) on = (j < st) || (r >= st && r < en && j >= st && j <= r);
-    else on = j < en;
-    w[i] = __ballot_sync(0xffffffffu, on && j < L);
+    for (int i = 0; i < 4; ++i) {
+      const int j = 128 * c + lane + 32 * i;
+      bool on;
+      if (s2s) on = (j < st) || (r >= st && r < en && j >= st && j <= r);
+      else on = j < en;
+      w[i] = __ballot_sync(0xffffffffu, on && j < L);
+    }
+    if (lane == 0) reinterpret_cast<uint4*>(out)[idx * chunks + c] = make_uint4(w[0], w[1], w[2], w[3]);
   }
-  if (lane == 0) reinterpret_cast<uint4*>(out)[idx] = make_uint4(w[0], w[1], w[2], w[3]);
 }
 
 int launch_mask_synth(const int* len_b, const int* mode, int len_a, int B, int L, uint32_t* out, cudaStream_t s) {
   VLPK_CHECK_ARG(len_b != nullptr && mode != nullptr && out != nullptr, "mask_synth: null pointer");
-  VLPK_CHECK_ARG(B > 0 && L > 0 && L <= 128 && len_a >= 0 && len_a + 3 <= L, "mask_synth: B=%d L=%d len_a=%d", B, L, len_a);
+  VLPK_CHECK_ARG(B > 0 && L > 0 && L <= MASK_MAX_KV && len_a >= 0 && len_a + 3 <= L, "mask_synth: B=%d L=%d len_a=%d", B, L, len_a);
   VLPK_CHECK_ARG(!misaligned(out, 15), "mask_synth: the bitmask buffer must be 16-byte aligned");
   const long long n = static_cast<long long>(B) * L;
   LaunchScope scope(CAT_MISC, 0.0, s);
-  mask_synth_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(len_b, mode, len_a, B, L, out);
+  mask_synth_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(len_b, mode, len_a, B, L, (L + 127) / 128, out);
   VLPK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -69,8 +69,29 @@ def _require_cuda(t, what):
 # ------------------------------------------------------------------------------------------------
 # attention mask -> bitmask
 # ------------------------------------------------------------------------------------------------
+MAX_SEQ = 512  # longest sequence the attention kernels take (4 key tiles of 128)
+
+
+def key_slots(kv):
+    """S = 128 * ceil(kv / 128): key slots of a packed mask row (S / 32 words) and of an attention keep-bit row (S / 8 bytes)."""
+    return (kv + 127) // 128 * 128
+
+
+def kv_slots(Lq, Lkv):
+    """VlpkShape.kv_slots for a shape: 0 (the 128-slot layout) when both lengths fit one tile, else key_slots(Lkv).  Raises before any
+    launch for lengths the kernels do not take."""
+    if not (1 <= Lq and 1 <= Lkv <= MAX_SEQ and Lq <= key_slots(Lkv)):
+        raise ValueError(f"vlp_b200: sequence length Lq={Lq} Lkv={Lkv} unsupported (attention takes up to {MAX_SEQ})")
+    return 0 if Lq <= 128 and Lkv <= 128 else key_slots(Lkv)
+
+
+def _check_mask_words(mask_bits, Lkv):
+    if mask_bits.shape[-1] * 32 != key_slots(Lkv):
+        raise ValueError(f"vlp_b200: packed mask has {mask_bits.shape[-1]} words per row; {key_slots(Lkv) // 32} needed for {Lkv} keys")
+
+
 def pack_mask(mask, mode="additive"):
-    """[B,1,R,KV] / [B,R,KV] additive (0/-10000) or 0/1 mask -> int32 [B,R,4] 'attend' bitmask (R may be 1)."""
+    """[B,1,R,KV] / [B,R,KV] additive (0/-10000) or 0/1 mask -> int32 [B,R,S/32] 'attend' bitmask (R may be 1), S = key_slots(KV)."""
     _require_cuda(mask, "attention mask")
     if mask.dim() == 4:
         mask = mask[:, 0]
@@ -82,7 +103,9 @@ def pack_mask(mask, mode="additive"):
     if dt is None:
         mask = mask.float()
         dt = 1
-    out = torch.empty(B, R, 4, device=mask.device, dtype=torch.int32)
+    if KV > MAX_SEQ:
+        raise ValueError(f"vlp_b200: attention mask over {KV} keys; the kernels take up to {MAX_SEQ}")
+    out = torch.empty(B, R, key_slots(KV) // 32, device=mask.device, dtype=torch.int32)
     L.call("vlpk_mask_pack", mask.data_ptr(), dt, 0 if mode == "additive" else 1, B, R, KV, R * KV, KV, out.data_ptr(), L.stream())
     return out
 
@@ -126,9 +149,9 @@ class _Acts:
         self.bf = torch.empty(n_layers, per_bf, device=device, dtype=BF16)
         self.f32 = torch.empty(n_layers, per_f, device=device, dtype=torch.float32)
         self.structs = (L.VlpkLayerActs * n_layers)()
-        # training with dropout: 1 bit per attention probability (128 key slots per query row), written by the forward attention
-        # kernel and re-read by the backward one instead of re-evaluating Philox
-        self.bits = torch.empty(n_layers, B * heads * Lq * 16, device=device, dtype=torch.uint8) if drop_bits else None
+        # training with dropout: 1 bit per attention probability (key_slots(Lq) per query row: the training path has Lkv = Lq),
+        # written by the forward attention kernel and re-read by the backward one instead of re-evaluating Philox
+        self.bits = torch.empty(n_layers, B * heads * Lq * key_slots(Lq) // 8, device=device, dtype=torch.uint8) if drop_bits else None
         self.y = []
         for i in range(n_layers):
             st = self.structs[i]
@@ -171,8 +194,10 @@ class EncoderStackFn(torch.autograd.Function):
         B, Lq, H = x.shape
         pk = [_bf16c(p) for p in params]
         seed = next_seed("encoder") if (training and (p_attn > 0 or p_hidden > 0)) else None
+        slots = kv_slots(Lq, Lq)
+        _check_mask_words(mask_bits, Lq)
         acts = _Acts(n_layers, B, Lq, H, heads, I, x.device, drop_bits=seed is not None)
-        shape = L.VlpkShape(B, Lq, Lq, H, heads, I)
+        shape = L.VlpkShape(B, Lq, Lq, H, heads, I, slots)
         ws = _weight_structs(pk, n_layers)
         drop = _drop(max(p_attn, p_hidden), seed)
         L.call("vlpk_encoder_fwd", C.byref(shape), n_layers, ws, x.data_ptr(), mask_bits.data_ptr(), mask_bits.shape[1], acts.structs,
@@ -223,7 +248,7 @@ class EncoderStackFn(torch.autograd.Function):
             setattr(ws_s, name, scratch[off:off + scr_sizes[name]].data_ptr())
             off += scr_sizes[name]
         dx0 = torch.empty_like(x)
-        shape = L.VlpkShape(B, Lq, Lq, H, heads, I)
+        shape = L.VlpkShape(B, Lq, Lq, H, heads, I, kv_slots(Lq, Lq))
         ws = _weight_structs(ctx.pk, n_layers)
         drop = _drop(max(p_attn, p_hidden), ctx.seed)
         L.call("vlpk_encoder_bwd", C.byref(shape), n_layers, ws, x.data_ptr(), ctx.mask_bits.data_ptr(), ctx.mask_bits.shape[1], acts.structs,
@@ -252,9 +277,11 @@ def layer_incremental_fwd(hidden, history, mask_bits, heads, I, params):
     xkv = _bf16c(torch.cat((history.to(x.dtype), x), dim=1))
     B, Lq, H = x.shape
     Lkv = xkv.shape[1]
+    slots = kv_slots(Lq, Lkv)
+    _check_mask_words(mask_bits, Lkv)
     pk = [_bf16c(p) for p in params]
     acts = _Acts(1, B, Lq, H, heads, I, x.device, Lkv=Lkv)
-    shape = L.VlpkShape(B, Lq, Lkv, H, heads, I)
+    shape = L.VlpkShape(B, Lq, Lkv, H, heads, I, slots)
     ws = _weight_structs(pk, 1)
     L.call("vlpk_layer_fwd", C.byref(shape), ws, x.data_ptr(), xkv.data_ptr(), mask_bits.data_ptr(), mask_bits.shape[1], acts.structs, 0.0, 0.0,
            None, 0, L.stream())
@@ -455,9 +482,11 @@ def layer_cached_fwd(hidden, kv_cache, pos, mask_bits, heads, I, params):
     B, Lq, H = x.shape
     if not (kv_cache.dtype == BF16 and kv_cache.is_contiguous() and kv_cache.shape[0] == B and kv_cache.shape[2] == 2 * H):
         raise RuntimeError("vlp_b200: kv_cache must be a contiguous bf16 [B, rows, 2H] tensor")
+    slots = kv_slots(Lq, pos + Lq)
+    _check_mask_words(mask_bits, pos + Lq)
     pk = [_bf16c(p) for p in params]
     acts = _Acts(1, B, Lq, H, heads, I, x.device, Lkv=Lq)            # acts.kv: scratch for the new rows' K | V
-    shape = L.VlpkShape(B, Lq, pos + Lq, H, heads, I)
+    shape = L.VlpkShape(B, Lq, pos + Lq, H, heads, I, slots)
     ws = _weight_structs(pk, 1)
     L.call("vlpk_layer_cached_fwd", C.byref(shape), ws, x.data_ptr(), kv_cache.data_ptr(), kv_cache.shape[1], int(pos), mask_bits.data_ptr(),
            mask_bits.shape[1], acts.structs, 0, L.stream())

@@ -6,7 +6,7 @@ fp32 region features [B,100,2048] + [B,100,1607] and an int64 [B,123,123] self-a
 quarter of the PCIe budget and the int64 mask is pure redundancy.  This module provides the H100-first replacement:
 
   * `mask_descriptor` / `PackedAttentionMask.synthesize`: the mask travels as three integers per sample (len_a, len_b, mode) and
-    is synthesised on the device, directly in the 128-bit-per-row packed form the attention kernels consume (`vlpk_mask_synth`,
+    is synthesised on the device, directly in the packed form (S = 128 * ceil(L / 128) bits per row) the attention kernels consume (`vlpk_mask_synth`,
     bit-identical to packing the loader's matrix — tests/test_staging_gpu.py);
   * features are staged as bf16 (the dtype the region projections read; feature files / loader workers should emit bf16 — a
     one-time dataset conversion — fp32 host tensors are accepted and converted on the host as a fallback);
@@ -19,6 +19,7 @@ The staged batch feeds the unchanged module surface: `model(img, vis_pe, input_i
 import torch
 
 from . import _lib as L
+from . import ops
 
 BF16 = torch.bfloat16
 FIELDS = ("input_ids", "segment_ids", "input_mask", "masked_ids", "masked_pos", "masked_weights", "is_next", "task_idx", "img",
@@ -76,7 +77,10 @@ class PackedAttentionMask:
         if not (len_b.is_cuda and mode.is_cuda and len_b.dtype == torch.int32 and mode.dtype == torch.int32):
             raise RuntimeError("vlp_b200.staging: len_b / mode must be int32 CUDA tensors")
         B = len_b.shape[0]
-        bits = out if out is not None else torch.empty(B, L_, 4, device=len_b.device, dtype=torch.int32)
+        shape = (B, int(L_), ops.key_slots(int(L_)) // 32)
+        if out is not None and not (tuple(out.shape) == shape and out.dtype == torch.int32 and out.is_cuda and out.is_contiguous()):
+            raise ValueError(f"vlp_b200.staging: out must be a contiguous int32 CUDA tensor of shape {shape}")
+        bits = out if out is not None else torch.empty(shape, device=len_b.device, dtype=torch.int32)
         L.call("vlpk_mask_synth", len_b.data_ptr(), mode.data_ptr(), int(len_a), B, int(L_), bits.data_ptr(), L.stream())
         return cls(bits, L_)
 

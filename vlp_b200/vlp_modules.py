@@ -124,6 +124,15 @@ class BertLayerNorm(nn.Module):
         return F.layer_norm(x, (x.shape[-1],), self.weight, self.bias, self.variance_epsilon)
 
 
+def _check_seq_len(config, L):
+    """Sequence lengths the model takes, checked before anything is launched: the attention kernels stop at ops.MAX_SEQ (512) and
+    the position table at max_position_embeddings (the reference fails there with an index error)."""
+    if L > ops.MAX_SEQ:
+        raise ValueError(f"vlp_b200: sequence length {L} exceeds {ops.MAX_SEQ}, the longest the attention kernels take")
+    if L > config.max_position_embeddings:
+        raise ValueError(f"vlp_b200: sequence length {L} exceeds max_position_embeddings {config.max_position_embeddings}")
+
+
 class BertEmbeddings(nn.Module):
     """modeling.py:195-241."""
 
@@ -540,7 +549,7 @@ class BertModel(PreTrainedBertModel):
 
     def get_extended_attention_mask(self, input_ids, token_type_ids, attention_mask):
         """Additive (1-m)*-10000 mask in the parameter dtype, [B,1,1,L] or [B,1,L,L] (modeling.py:807-833).  The packed
-        128-bit-per-row form the attention kernel consumes is attached to the returned tensor."""
+        per-row bitmask the attention kernel consumes (ops.pack_mask) is attached to the returned tensor."""
         if attention_mask is None:
             attention_mask = torch.ones_like(input_ids)
         if hasattr(attention_mask, "_vlpk_bits") and not torch.is_tensor(attention_mask):
@@ -559,6 +568,7 @@ class BertModel(PreTrainedBertModel):
         return ext
 
     def forward(self, vis_feats, vis_pe, input_ids, token_type_ids=None, attention_mask=None, output_all_encoded_layers=True, len_vis_input=49):
+        _check_seq_len(self.config, input_ids.size(1))
         ext = self.get_extended_attention_mask(input_ids, token_type_ids, attention_mask)
         embedding_output = self.embeddings(vis_feats, vis_pe, input_ids, token_type_ids, len_vis_input=len_vis_input)
         encoded_layers = self.encoder(embedding_output, ext, output_all_encoded_layers=output_all_encoded_layers)
@@ -576,6 +586,8 @@ class BertModelIncr(BertModel):
                 output_all_encoded_layers=True, len_vis_input=49, kv_caches=None, cache_pos=0):
         """Reference signature (modeling.py:856) plus `kv_caches` / `cache_pos`: decode against per-layer K/V caches instead of
         re-encoding `prev_embedding` / `prev_encoded_layers` (regions enter at cache_pos == 0 only)."""
+        prefix = cache_pos if kv_caches is not None else (0 if prev_embedding is None else prev_embedding.size(1))
+        _check_seq_len(self.config, prefix + input_ids.size(1))
         ext = self.get_extended_attention_mask(input_ids, token_type_ids, attention_mask)
         first = (prev_encoded_layers is None) if kv_caches is None else (cache_pos == 0)
         embedding_output = self.embeddings(vis_feats, vis_pe, input_ids, token_type_ids, position_ids, vis_input=first,
@@ -704,6 +716,7 @@ class BertForPreTrainingLossMask(PreTrainedBertModel, _RegionProjections):
                 drop_worst_ratio=0.2, vqa_inference=False):
         if not vqa_inference and masked_pos is not None and masked_pos.numel() > 0:
             self.cls.predictions.check_task_idx(task_idx)      # before anything is launched
+        _check_seq_len(self.config, input_ids.size(1))
         vis_feats, vis_pe = self.project_regions(vis_feats, vis_pe)
 
         if vqa_inference:                                    # modeling.py:1039-1047
@@ -800,12 +813,13 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         self._build_region_projections(config, enable_butd)
 
     def new_kv_caches(self, batch, device, rows=128):
-        """One [batch, rows, 2H] bf16 K|V cache per encoder layer."""
+        """One [batch, rows, 2H] bf16 K|V cache per encoder layer; decode passes its output length (token_type_ids.size(1))."""
         H = self.config.hidden_size
         return [torch.empty(batch, rows, 2 * H, device=device, dtype=torch.bfloat16) for _ in self.bert.encoder.layer]
 
     def forward(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, sample_mode="greedy"):
         self.cls.predictions.check_task_idx(task_idx)          # before anything is launched
+        _check_seq_len(self.config, token_type_ids.size(1))
         with torch.no_grad():
             vis_feats, vis_pe = self.project_regions(vis_feats, vis_pe)
             if self.search_beam_size > 1:
@@ -815,7 +829,7 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
             output_length = token_type_ids.size(1)
             output_ids, output_probs = [], []
             prev_embedding, prev_encoded_layers = None, None
-            caches = self.new_kv_caches(input_ids.size(0), input_ids.device) if self.use_kv_cache else None
+            caches = self.new_kv_caches(input_ids.size(0), input_ids.device, output_length) if self.use_kv_cache else None
             curr_ids = input_ids
             mask_ids = input_ids[:, :1] * 0 + self.mask_word_id
             next_pos = input_length
