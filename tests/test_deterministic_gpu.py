@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from tools import determinism_check as dc
+from tools import kernel_check as kc
 from vlp_b200 import _lib as L
 from vlp_b200 import graph, ops, synth
 from vlp_b200 import vlp_modules as vm
@@ -127,9 +128,7 @@ def test_embedding_backward_is_ordered(B, L_, R, H, V, vis):
         return [dz, dg, db, d_word, d_pos, d_type]
     dz, dg, db, d_word, d_pos, d_type = repeated(run)
     # LayerNorm dγ / dβ from the forward's statistics
-    z = word[ids].double() + posw[torch.arange(L_, device=DEV)].unsqueeze(0).double() + typew[tt].double()
-    if vis:
-        z = torch.cat((z[:, :1], visf.double() + vpef.double() + typew[tt[:, 1:R + 1]].double(), z[:, R + 1:]), dim=1)
+    z = kc.embed_z(ids, word, posw, typew, tt=tt, vis=visf if vis else None, vpe=vpef if vis else None, R=R)
     st = stats.double().view(B, L_, 2)
     xh = (z - st[..., :1]) * st[..., 1:]
     for got, terms in ((dg, (dy.double() * xh).reshape(-1, H)), (db, dy.double().reshape(-1, H))):

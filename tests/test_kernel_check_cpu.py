@@ -145,6 +145,202 @@ def test_attention_accepts_and_rejects_wrong_half_block():
         kc.check_attn_block("ctx", bad, f["ctx"], f["E"], kc.ATTN_FWD_BLOCK)
 
 
+# ---- row kernels -------------------------------------------------------------------------------------------------------------
+F64 = torch.float64
+
+
+def test_ln_refs_match_autograd():
+    gen = torch.Generator().manual_seed(11)
+    Mr, H, p = 6, 24, 0.25
+    t, res, dy = (torch.randn(Mr, H, generator=gen, dtype=F64) for _ in range(3))
+    g, b = torch.randn(H, generator=gen, dtype=F64), torch.randn(H, generator=gen, dtype=F64)
+    keep = (torch.rand(Mr, H, generator=gen) >= p).to(torch.uint8)
+    for kp, pp, r_ in ((keep, p, res), (None, 0.0, None)):
+        ta, ga, ba = t.clone().requires_grad_(True), g.clone().requires_grad_(True), b.clone().requires_grad_(True)
+        z = ta * (1.0 if kp is None else kp.to(F64) / (1 - pp)) + (0.0 if r_ is None else r_)
+        y = torch.nn.functional.layer_norm(z, (H,), ga, ba, kc.LN_EPS)
+        y.backward(dy)
+        ref = kc.ln_ref(t, r_, g, b, kp, pp)
+        torch.testing.assert_close(ref["y"][0], y.detach(), rtol=1e-12, atol=1e-12)
+        stats = torch.stack((ref["mean"], ref["rstd"]), -1)
+        r = kc.ln_bwd_ref(t, r_, g, stats, dy, kp, pp)
+        torch.testing.assert_close(r["dt"][0], ta.grad, rtol=1e-10, atol=1e-12)
+        torch.testing.assert_close(r["dgamma"].sum(0), ga.grad, rtol=1e-10, atol=1e-12)
+        torch.testing.assert_close(r["dbeta"].sum(0), ba.grad, rtol=1e-10, atol=1e-12)
+        torch.testing.assert_close(r["dbias"].sum(0), ta.grad.sum(0), rtol=1e-10, atol=1e-12)
+
+
+def test_embed_refs_match_autograd():
+    gen = torch.Generator().manual_seed(12)
+    B, Lq, H, R, V, P, T, p = 3, 7, 16, 2, 11, 9, 3, 0.2
+    word, posw, typew = (torch.randn(n, H, generator=gen, dtype=F64) for n in (V, P, T))
+    vis, vpe = torch.randn(B, R, H, generator=gen, dtype=F64), torch.randn(B, R, H, generator=gen, dtype=F64)
+    g, b = torch.randn(H, generator=gen, dtype=F64), torch.randn(H, generator=gen, dtype=F64)
+    ids, tt = torch.randint(0, V, (B, Lq), generator=gen), torch.randint(0, T, (B, Lq), generator=gen)
+    pos = torch.stack([torch.randperm(Lq, generator=gen) for _ in range(B)])
+    keep = (torch.rand(B, Lq, H, generator=gen) >= p).to(torch.uint8)
+    dy = torch.randn(B, Lq, H, generator=gen, dtype=F64)
+    z = kc.embed_z(ids, word, posw, typew, tt=tt, pos=pos, vis=vis, vpe=vpe, R=R)
+    for bb in range(B):
+        for l in range(Lq):
+            src = vis[bb, l - 1] + vpe[bb, l - 1] if 1 <= l <= R else word[ids[bb, l]] + posw[pos[bb, l]]
+            torch.testing.assert_close(z[bb, l], src + typew[tt[bb, l]], rtol=0, atol=0)
+    za, ga, ba = z.clone().requires_grad_(True), g.clone().requires_grad_(True), b.clone().requires_grad_(True)
+    y = torch.nn.functional.layer_norm(za, (H,), ga, ba, kc.LN_EPS) * keep.to(F64) / (1 - p)
+    y.backward(dy)
+    ref = kc.embed_ref(z, g, b, keep, p)
+    torch.testing.assert_close(ref["y"][0], y.detach(), rtol=1e-12, atol=1e-12)
+    r = kc.embed_bwd_ref(z, g, torch.stack((ref["mean"], ref["rstd"]), -1), dy, keep, p)
+    torch.testing.assert_close(r["dz"][0], za.grad, rtol=1e-10, atol=1e-12)
+    torch.testing.assert_close(r["dgamma"].reshape(-1, H).sum(0), ga.grad, rtol=1e-10, atol=1e-12)
+    torch.testing.assert_close(r["dbeta"].reshape(-1, H).sum(0), ba.grad, rtol=1e-10, atol=1e-12)
+
+
+def test_ce_ref_matches_autograd():
+    gen = torch.Generator().manual_seed(13)
+    R, V = 8, 37
+    x = (torch.randn(R, V, generator=gen, dtype=F64) * 3).requires_grad_(True)
+    labels = torch.tensor([0, V - 1, -1, -100, V, 5, 17, 36])
+    dloss = torch.rand(R, generator=gen, dtype=F64) + 0.5
+    live = (labels >= 0) & (labels < V)
+    loss = torch.nn.functional.cross_entropy(x, torch.where(live, labels, torch.zeros_like(labels)), reduction="none") * live
+    (loss * dloss).sum().backward()
+    ref = kc.ce_ref(x.detach(), labels, dloss)
+    torch.testing.assert_close(ref["loss"], loss.detach(), rtol=1e-12, atol=1e-12)
+    torch.testing.assert_close(ref["lse"], torch.logsumexp(x.detach(), -1), rtol=1e-12, atol=1e-12)
+    torch.testing.assert_close(ref["dlogits"], x.grad, rtol=1e-12, atol=1e-12)
+    assert bool((ref["dlogits"][~live] == 0).all()) and bool((ref["E"][~live] == 0).all())
+
+
+def _kernel_like_ln(t, res, g, b, dy, keep, p, two_pass=True):
+    """What a correct row kernel returns: fp32 arithmetic on the bf16 inputs, bf16 outputs, fp32 statistics and column sums."""
+    z = t.float() * (1.0 if keep is None else keep.float() * torch.tensor(1 / (1 - p), dtype=torch.float32)) + res.float()
+    mean = z.mean(-1, keepdim=True)
+    var = (z - mean).pow(2).mean(-1, keepdim=True) if two_pass else z.pow(2).mean(-1, keepdim=True) - mean * mean
+    rstd = torch.rsqrt(var + kc.LN_EPS)
+    xh = (z - mean) * rstd
+    y = xh * g.float() + b.float()
+    gy = dy.float() * g.float()
+    dz = rstd * (gy - gy.mean(-1, keepdim=True) - xh * (gy * xh).mean(-1, keepdim=True))
+    dt = dz * (1.0 if keep is None else keep.float() / (1 - p))
+    return {"y": y.to(BF), "stats": torch.cat((mean, rstd), -1), "dz": dz.to(BF), "dt": dt.to(BF), "dt32": dt,
+            "dgamma": (dy.float() * xh).sum(0), "dbeta": dy.float().sum(0), "dbias": dt.sum(0)}
+
+
+@pytest.fixture(scope="module")
+def ln_prod():
+    """LayerNorm + residual + dropout at the production shape (B 64 x L 123 rows, H 768); dy rows of varied magnitude."""
+    gen = torch.Generator().manual_seed(14)
+    Mr, H, p = 7872, 768, 0.1
+    t, res = torch.randn(Mr, H, generator=gen).to(BF), torch.randn(Mr, H, generator=gen).to(BF)
+    g, b = (1 + 0.1 * torch.randn(H, generator=gen)).to(BF), (0.1 * torch.randn(H, generator=gen)).to(BF)
+    scale = 0.5 + torch.rand(Mr, 1, generator=gen)
+    scale[-1] = 0.5
+    dy = (torch.randn(Mr, H, generator=gen) * scale).to(BF)
+    keep = (torch.rand(Mr, H, generator=gen) >= p).to(torch.uint8)
+    got = _kernel_like_ln(t, res, g, b, dy, keep, p)
+    ref = kc.ln_ref(t, res, g, b, keep, p)
+    bwd = kc.ln_bwd_ref(t, res, g, got["stats"], dy, keep, p)
+    return dict(t=t, res=res, g=g, b=b, dy=dy, keep=keep, p=p, got=got, ref=ref, bwd=bwd)
+
+
+def test_row_checks_accept_correctly_rounded_result(ln_prod):
+    got, ref, bwd = ln_prod["got"], ln_prod["ref"], ln_prod["bwd"]
+    assert kc.check_rows("y", got["y"], *ref["y"]) <= 1.0
+    assert kc.check_ln_stats("ln", got["stats"], ref["mean"], ref["rstd"], ref["z"]) <= 1.0
+    for o in ("dz", "dt"):
+        assert kc.check_rows(o, got[o], *bwd[o]) <= 1.0
+    prior = torch.randn(768, generator=torch.Generator().manual_seed(1))
+    for o in ("dgamma", "dbeta", "dbias"):
+        assert kc.check_sum_onto(o, prior + got[o], prior, bwd[o]) <= 1.0
+
+
+def test_row_check_rejects_one_zeroed_row(ln_prod):
+    bad = ln_prod["got"]["dz"].clone()
+    bad[-1] = 0                                           # the last row never written
+    assert bringup.rel(bad, ln_prod["bwd"]["dz"][0]) < 1e-2
+    with pytest.raises(kc.CheckError, match=r"row 7871 "):
+        kc.check_rows("dz", bad, *ln_prod["bwd"]["dz"])
+
+
+def test_row_check_rejects_dt_without_dropout_scale():
+    gen = torch.Generator().manual_seed(15)
+    Mr, H, p = 7872, 768, 0.008
+    t, res, dy = (torch.randn(Mr, H, generator=gen).to(BF) for _ in range(3))
+    g, b = (1 + 0.1 * torch.randn(H, generator=gen)).to(BF), (0.1 * torch.randn(H, generator=gen)).to(BF)
+    keep = (torch.rand(Mr, H, generator=gen) >= p).to(torch.uint8)
+    got = _kernel_like_ln(t, res, g, b, dy, keep, p)
+    bwd = kc.ln_bwd_ref(t, res, g, got["stats"], dy, keep, p)
+    kc.check_rows("dt", got["dt"], *bwd["dt"])
+    bad = (got["dz"].float() * keep.float()).to(BF)       # keep * dz: the 1 / (1 - p) forgotten
+    assert bringup.rel(bad, bwd["dt"][0]) < 1e-2
+    with pytest.raises(kc.CheckError, match="dt"):
+        kc.check_rows("dt", bad, *bwd["dt"])
+
+
+def test_stats_check_rejects_single_pass_variance():
+    gen = torch.Generator().manual_seed(16)
+    Mr, H = 7872, 768
+    t = torch.randn(Mr, H, generator=gen).to(BF)
+    sign = torch.randint(0, 2, (Mr, 1), generator=gen) * 2 - 1
+    res = (torch.randn(Mr, H, generator=gen) + 64 * 2 ** 0.5 * sign).to(BF)        # |mean| ~ 64 sigma
+    g, b = (1 + 0.1 * torch.randn(H, generator=gen)).to(BF), (0.1 * torch.randn(H, generator=gen)).to(BF)
+    dy = torch.randn(Mr, H, generator=gen).to(BF)
+    ref = kc.ln_ref(t, res, g, b)
+    good = _kernel_like_ln(t, res, g, b, dy, None, 0.0)
+    kc.check_ln_stats("two-pass", good["stats"], ref["mean"], ref["rstd"], ref["z"])
+    bad = _kernel_like_ln(t, res, g, b, dy, None, 0.0, two_pass=False)
+    assert bringup.rel(bad["y"], ref["y"][0]) < 1e-2
+    with pytest.raises(kc.CheckError, match="rstd"):
+        kc.check_ln_stats("single-pass", bad["stats"], ref["mean"], ref["rstd"], ref["z"])
+
+
+def test_sum_check_rejects_column_off_by_one_lane_in_ragged_chunk():
+    """H = 1000: the last chunk holds 232 columns (lanes 0..28).  dgamma of column 996 (lane 28) taken from column 988 (lane 27)."""
+    gen = torch.Generator().manual_seed(17)
+    Mr, H = 7872, 1000
+    t, res = torch.randn(Mr, H, generator=gen).to(BF), torch.randn(Mr, H, generator=gen).to(BF)
+    g, b = torch.ones(H).to(BF), torch.zeros(H).to(BF)
+    ref = kc.ln_ref(t, res, g, b)
+    dy = (ref["xhat"] + 0.1 * torch.randn(Mr, H, generator=gen, dtype=F64)).to(BF)   # an upstream gradient correlated with the output
+    got = _kernel_like_ln(t, res, g, b, dy, None, 0.0)
+    bwd = kc.ln_bwd_ref(t, res, g, got["stats"], dy)
+    prior = torch.randn(H, generator=gen)
+    dg = prior + got["dgamma"]
+    kc.check_sum_onto("dgamma", dg, prior, bwd["dgamma"])
+    bad = dg.clone()
+    bad[996] = prior[996] + got["dgamma"][988]
+    assert bringup.rel(bad, prior.double() + bwd["dgamma"].sum(0)) < 1e-2
+    with pytest.raises(kc.CheckError, match=r"column 996 \(chunk 3, lane 28\)"):
+        kc.check_sum_onto("dgamma", bad, prior, bwd["dgamma"])
+
+
+def test_ce_check_accepts_rounded_rows_and_rejects_shifted_one_hot():
+    gen = torch.Generator().manual_seed(18)
+    R, V = 192, 28996
+    x = (torch.randn(R, V, generator=gen) * 1.4)
+    x[::4] *= 20                                          # peaky rows: |logit| ~ 30, a few columns decide lse
+    x = x.to(BF)
+    labels = torch.randint(0, V, (R,), generator=gen)
+    labels[:5] = torch.tensor([V - 1, 0, -1, -100, V])
+    labels[4::8] = x[4::8].float().argmax(-1)             # peaky rows whose label holds nearly all the probability
+    dloss = torch.rand(R, generator=gen) + 0.5
+    live = (labels >= 0) & (labels < V)
+    lse = torch.logsumexp(x.float(), -1)
+    t = torch.where(live, labels, torch.zeros_like(labels))
+    loss = torch.where(live, lse - x.float().gather(1, t[:, None])[:, 0], torch.zeros_like(lse))
+    onehot = torch.zeros(R, V)
+    onehot[torch.arange(R)[live], t[live]] = 1
+    d = (torch.exp(x.float() - lse[:, None]) - onehot) * (dloss * live)[:, None]
+    ref = kc.ce_ref(x, labels, dloss)
+    kc.check_ce_rows("ce", lse, loss, d.to(BF), ref, labels)
+    shifted = torch.zeros(R, V)
+    shifted[torch.arange(R)[live], (t[live] + 1) % V] = 1
+    bad = ((torch.exp(x.float() - lse[:, None]) - shifted) * (dloss * live)[:, None]).to(BF)
+    with pytest.raises(kc.CheckError, match="dlogits"):
+        kc.check_ce_rows("ce", lse, loss, bad, ref, labels)
+
+
 def test_bits_to_allow_ignores_bits_beyond_lkv_and_broadcasts():
     bits = torch.zeros(2, 1, 4, dtype=torch.int32)
     bits[:, 0, 0] = 0b1011

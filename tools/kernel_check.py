@@ -10,6 +10,10 @@ written, a missing k-block or a wrong 64-row half passes it at production sizes.
 where E is the magnitude the kernel's fp32 sums run over: |A| |B|^T for a GEMM (times the epilogue's Lipschitz factor), P |V| for
 the attention context and |P|^T |dO| for dV.  Failures name the worst block, its error and its bound.  Every function here runs on
 whatever device its tensors live on; nothing needs a GPU except the helpers that call the library (replayed dropout masks).
+
+The row kernels (LayerNorm + residual + dropout, embeddings, cross-entropy rows) are held to the same kind of elementwise bound,
+with E = |gamma| (|x-hat| + 1) for a LayerNorm output and the magnitude of the three terms of the LayerNorm gradient for dz; their
+statistics, lse and loss per row; their column sums (dgamma, dbeta, bias and table gradients) per column onto prior contents.
 """
 import math
 
@@ -29,6 +33,12 @@ ATTN_FWD_BLOCK = 6e-3         # rel-L2 of ctx per (sequence, head)
 ATTN_LSE = 2e-5               # |lse - ref| <= ATTN_LSE * (1 + |ref|)
 ATTN_BWD_BLOCK = 2e-2         # rel-L2 of dq / dk / dv per (sequence, head)
 SUM_REL = 1e-5                # fp32 column sums (bias gradients): |got - ref| <= SUM_REL * sum |x|
+# row kernels (csrc/rowops.cu, csrc/tables.cu, the row part of csrc/head.cu)
+LN_A = 2.0 ** -15             # LayerNorm y / dz / dt: fp32 row arithmetic, per unit of E
+LN_STATS = 2e-6               # |mean - mu| <= LN_STATS * mean |z| and |rstd / rho - 1| <= LN_STATS, per row
+CE_LSE = 5e-6                 # cross-entropy lse and loss: |got - ref| <= CE_LSE * (1 + |ref|)
+CE_A = 2.0 ** -23             # dlogits: |got - ref| <= 2^-8 |ref| + CE_A * E (ce_magnitude)
+LN_EPS = float(torch.tensor(1e-5, dtype=torch.float32))    # the kernels' fp32 LayerNorm eps
 
 TILE = 128
 
@@ -148,6 +158,107 @@ def bits_to_allow(bits, Lq, Lkv):
     return allow.expand(bits.shape[0], Lq, Lkv) if bits.shape[1] == 1 else allow[:, :Lq]
 
 
+def _ln64(z, gamma, beta, eps):
+    """fp64 LayerNorm of rows z [..., H] (two-pass statistics): y with E_y = |gamma| (|x-hat| + 1), mean, rstd, x-hat."""
+    mu = z.mean(-1, keepdim=True)
+    rho = 1.0 / torch.sqrt((z - mu).pow(2).mean(-1, keepdim=True) + eps)
+    xh = (z - mu) * rho
+    g = gamma.to(F64)
+    return {"y": (xh * g + beta.to(F64), g.abs() * (xh.abs() + 1.0)), "mean": mu[..., 0], "rstd": rho[..., 0], "xhat": xh, "z": z}
+
+
+def _ln_bwd64(z, gamma, stats, dout):
+    """Gradient of LayerNorm rows with respect to their input z, given the gradient `dout` of the LN output and the kernel's own
+    fp32 (mean, rstd) `stats` [..., 2] (isolates the backward from the forward's error).  Returns (dz, E_dz, x-hat)."""
+    st = stats.to(F64)
+    mean, rstd = st[..., :1], st[..., 1:]
+    xh = (z - mean) * rstd
+    gy = dout * gamma.to(F64)
+    dz = rstd * (gy - gy.mean(-1, keepdim=True) - xh * (gy * xh).mean(-1, keepdim=True))
+    E = rstd * (gy.abs() + gy.abs().mean(-1, keepdim=True) + xh.abs() * (gy * xh).abs().mean(-1, keepdim=True))
+    return dz, E, xh
+
+
+def _drop_scale(keep, p, like):
+    return torch.ones_like(like) if keep is None else keep.to(F64) / (1.0 - p)
+
+
+def ln_ref(t, res, gamma, beta, keep=None, p=0.0, eps=LN_EPS):
+    """fp64 y = LayerNorm(keep * t / (1 - p) + res) (vlpk_ln_res_drop_fwd); res and keep may be None.
+    Returns dict(y=(y, E_y), mean, rstd, xhat, z)."""
+    t64 = t.to(F64)
+    z = t64 * _drop_scale(keep, p, t64)
+    if res is not None:
+        z = z + res.to(F64)
+    return _ln64(z, gamma, beta, eps)
+
+
+def ln_bwd_ref(t, res, gamma, stats, dy, keep=None, p=0.0):
+    """fp64 gradients of ln_ref for upstream dy, from the kernel's `stats` [M, 2] (vlpk_ln_res_drop_bwd).  Returns dict(dz=(dz, E),
+    dt=(dt, E)) and the per-row terms of the column sums: dgamma (dy x-hat), dbeta (dy), dbias (the fp64 dt)."""
+    t64 = t.to(F64)
+    s = _drop_scale(keep, p, t64)
+    z = t64 * s + (0.0 if res is None else res.to(F64))
+    dy64 = dy.to(F64)
+    dz, E, xh = _ln_bwd64(z, gamma, stats, dy64)
+    return {"dz": (dz, E), "dt": (dz * s, E * s), "dgamma": dy64 * xh, "dbeta": dy64, "dbias": dz * s}
+
+
+def embed_z(ids, word, posw, typew, tt=None, pos=None, vis=None, vpe=None, R=0):
+    """fp64 pre-LayerNorm embedding sum [B, L, H] as embed_row_z forms it: word[id] + posw[pos] + typew[type], and with regions
+    (vis / vpe [B, R, H] given) rows 1..R of every sample replaced by vis + vpe + typew[type].  pos None: position l; tt None: type 0."""
+    B, L = ids.shape
+    if pos is None:
+        pos = torch.arange(L, device=ids.device).expand(B, L)
+    if tt is None:
+        tt = torch.zeros_like(ids)
+    z = word[ids].to(F64) + posw[pos].to(F64) + typew[tt].to(F64)
+    if vis is not None:
+        z[:, 1:R + 1] = vis.to(F64) + vpe.to(F64) + typew[tt[:, 1:R + 1]].to(F64)
+    return z
+
+
+def embed_ref(z, gamma, beta, keep=None, p=0.0, eps=LN_EPS):
+    """fp64 y = dropout(LayerNorm(z)) of vlpk_embed_fwd on embed_z's rows.  Returns the dict of ln_ref with y = (y, E_y) after dropout."""
+    out = _ln64(z, gamma, beta, eps)
+    y, E = out["y"]
+    s = _drop_scale(keep, p, y)
+    out["y"] = (y * s, E * s)
+    return out
+
+
+def embed_bwd_ref(z, gamma, stats, dy, keep=None, p=0.0):
+    """fp64 gradient of embed_ref for upstream dy from the kernel's `stats`: dict(dz=(dz, E)) and the column-sum terms of dgamma
+    and dbeta (dropout applied to dy first)."""
+    d = dy.to(F64) * _drop_scale(keep, p, z)
+    dz, E, xh = _ln_bwd64(z, gamma, stats, d)
+    return {"dz": (dz, E), "dgamma": d * xh, "dbeta": d}
+
+
+def ce_ref(logits, labels, dloss):
+    """fp64 cross-entropy rows of vlpk_decoder_ce_fwd/bwd on the kernel's own bf16 logits [R, V]: dict(lse, loss, dlogits, live).
+    Labels outside [0, V) are ignored: loss 0, dlogits row 0."""
+    x = logits.to(F64)
+    R, V = x.shape
+    lse = torch.logsumexp(x, -1)
+    live = (labels >= 0) & (labels < V)
+    t = torch.where(live, labels, torch.zeros_like(labels))
+    loss = torch.where(live, lse - x.gather(1, t[:, None])[:, 0], torch.zeros_like(lse))
+    d = torch.exp(x - lse[:, None])
+    rows = torch.arange(R, device=x.device)[live]
+    d[rows, t[live]] -= 1.0
+    d = d * (dloss.to(F64) * live)[:, None]
+    return {"lse": lse, "loss": loss, "dlogits": d, "live": live, "E": ce_magnitude(x, lse, d, dloss.to(F64) * live)}
+
+
+def ce_magnitude(x, lse, d, g):
+    """E of dlogits = (exp(x - lse) - q) g: the largest |d| of its row, plus |g| exp(x - lse) (|x| + |lse|) for the fp32 rounding of
+    the exponent's argument (a row whose label holds nearly all the probability has dlogits far below that rounding)."""
+    x = x.to(F64)
+    p = torch.exp(x - lse[:, None])
+    return d.abs().amax(1, keepdim=True) + g.abs()[:, None] * p * (x.abs() + lse.abs()[:, None])
+
+
 # ---- bounds ------------------------------------------------------------------------------------------------------------------
 def _fmt_ratio(err, bound):
     return err / bound if bound > 0 else (0.0 if err == 0 else math.inf)
@@ -263,3 +374,45 @@ def check_colsum(name, got, x):
     x64 = x.to(F64)
     ref, mag = x64.sum(0), x64.abs().sum(0)
     return check_elementwise(name, got.to(F64), ref, mag, 0.0, SUM_REL, where=lambda j: f"column {j}")
+
+
+# ---- row kernels ---------------------------------------------------------------------------------------------------------------
+def row_where(i, j):
+    """An element of a row kernel's [M, H] output: a row is 32 lanes x 8 columns per 256-column chunk."""
+    return f"row {i} col {j} (chunk {j // 256}, lane {(j % 256) // 8})"
+
+
+def check_rows(name, got, ref, E, a=LN_A):
+    """A bf16 [M, H] row-kernel output (y, dz, dt) against its fp64 reference: |got - ref| <= 2^-8 |ref| + a E."""
+    assert got.shape == ref.shape, (got.shape, ref.shape)
+    return check_elementwise(name, got, ref, E, R_BF16, a, where=row_where)
+
+
+def check_ln_stats(name, stats, mean, rstd, z):
+    """The kernel's fp32 (mean, rstd) [M, 2]: |mean - mu| <= LN_STATS mean |z| and |rstd - rho| <= LN_STATS rho, per row."""
+    m = check_elementwise(f"{name} mean", stats[:, 0], mean, z.abs().mean(-1), 0.0, LN_STATS, where=lambda i: f"row {i}")
+    r = check_elementwise(f"{name} rstd", stats[:, 1], rstd, rstd, 0.0, LN_STATS, where=lambda i: f"row {i}")
+    return max(m, r)
+
+
+def check_sum_onto(name, got, prior, terms):
+    """fp32 column sums of terms [..., N] added onto prior contents [N] (dgamma / dbeta / bias / table gradients):
+    |got - (prior + sum)| <= SUM_REL (|prior| + sum |terms|) per column."""
+    t = terms.to(F64).reshape(-1, terms.shape[-1])
+    p = prior.to(F64)
+    return check_elementwise(name, got.to(F64), p + t.sum(0), p.abs() + t.abs().sum(0), 0.0, SUM_REL,
+                             where=lambda j: f"column {j} (chunk {j // 256}, lane {(j % 256) // 8})")
+
+
+def check_ce_rows(name, lse, loss, dlogits, ref, labels, lse_tol=CE_LSE, a=CE_A):
+    """lse / loss [R] to lse_tol (1 + |ref|) and dlogits [R, V] elementwise to 2^-8 |ref| + a E with E of ce_magnitude (0 in
+    ignored rows, which must be exactly 0).  `ref`: dict(lse, loss, dlogits, E) of ce_ref or of the smoothed loss.  Returns
+    dict(lse, loss, dlogits) of the worst shares of the bounds."""
+    def at(i):
+        return f"row {i} (label {int(labels[i])})"
+    out = {"lse": check_elementwise(f"{name} lse", lse, ref["lse"], 1.0 + ref["lse"].abs(), 0.0, lse_tol, where=at),
+           "loss": check_elementwise(f"{name} loss", loss, ref["loss"], 1.0 + ref["loss"].abs(), 0.0, lse_tol, where=at)}
+    d = ref["dlogits"]
+    out["dlogits"] = check_elementwise(f"{name} dlogits", dlogits, d, ref["E"].expand_as(d), R_BF16, a,
+                                       where=lambda i, j: f"row {i} col {j} (label {int(labels[i])})")
+    return out
