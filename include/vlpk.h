@@ -313,6 +313,21 @@ void vlpk_profile_reset(void);
 int vlpk_profile_get(int cat, double* ms, double* work, int64_t* launches);
 int64_t vlpk_launch_count(void);
 
+/* Beam search: duplicate-n-gram blocking (the reference's forbid_duplicate_ngrams / get_dup_ngram_candidates, modeling.py:1375-1428)
+ * for frame f >= 1 of a beam search over rows = B*K hypotheses (row i = b*K + k).  One launch:
+ *   hist_out[i, :f-1] = hist_in[b*K + ptr[i], :f-1];  hist_out[i, f-1] = wid[i]
+ *     hist_*: int32 [rows, T_cap] (two different buffers, used in turn); ptr / wid: int64 [rows] back pointers and word ids of
+ *     frame f-1.  At f = 1 hist_in and ptr are not read (may be NULL).
+ *   if f >= n: seq = hist_out[i, :f]; tail = seq[-(n-1):] (all of seq when n = 1); if no tail word is in ignore[0:n_ignore], then
+ *     for every s <= f-n with seq[s:s+n-1] == tail the word w = seq[s+n-1] (unless ignored, and only if 0 <= w < V) is blocked:
+ *     logp[i*ld + w] += -10000.0f, once per distinct w.  Rows without candidates and columns >= V are not touched.
+ *     logp: fp32 [rows, ld], frame f's log-probabilities, before the min_len [EOS] fill.  ignore: int32 device array, NULL if
+ *     n_ignore == 0.  Deterministic (no floating-point atomics).
+ * Returns < 0 without launching for n < 1, f < 1, f > T_cap, ld < V, hist_in == hist_out, rows not a multiple of K, a NULL
+ * pointer that is needed, or (T_cap + V/32) * 4 bytes above 48 KB of shared memory. */
+int vlpk_beam_ngram_block(int rows, int K, int f, int T_cap, int n, const int32_t* hist_in, int32_t* hist_out, const int64_t* ptr,
+                          const int64_t* wid, const int32_t* ignore, int n_ignore, float* logp, int64_t ld, int V, void* stream);
+
 /* utilities */
 int vlpk_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 int vlpk_colsum(const void* x, int64_t ld, int64_t M, int N, float* out, void* stream);

@@ -1,6 +1,7 @@
 """Decode throughput of BertForSeq2SeqDecoder at BERT-base size (100 regions + 20 generated tokens): per-layer K/V caches
 (`use_kv_cache`, vlpk_layer_cached_fwd) vs the reference's data flow (K, V of the whole prefix re-projected at every step), greedy
-and beam (K = 3).  python tools/decode_bench.py [batch]"""
+and beam (K = 3); then beam search with duplicate-trigram blocking (`forbid_duplicate_ngrams`, n = 3; on-device, vlpk_beam_ngram_block)
+at each K in BLOCKED_K, Python-driven and replayed as one CUDA graph.  python tools/decode_bench.py [batch] [blocked K ...]"""
 import os
 import sys
 
@@ -68,6 +69,31 @@ def main():
               f"{g.launches_per_replay} library launches per decode)")
         print(f"{name:10s}: K/V cache {res[True]:8.1f} ms ({B * steps / res[True] * 1e3:8.0f} tokens/s, {steps / res[True] * 1e3:6.1f} steps/s) | "
               f"re-projection {res[False]:8.1f} ms ({B * steps / res[False] * 1e3:8.0f} tokens/s) | speed-up {res[False] / res[True]:.2f}x")
+    blocked_k = [int(k) for k in sys.argv[2:]] or [3]
+    for K in blocked_k:
+        torch.manual_seed(0)
+        model = vm.BertForSeq2SeqDecoder(cfg, mask_word_id=103, eos_id=102, search_beam_size=K, enable_butd=True, len_vis_input=R,
+                                         forbid_duplicate_ngrams=True, ngram_size=3).cuda().bfloat16().eval()
+        from vlp_b200.graph import GraphedCall
+        g = GraphedCall(lambda *a: model(*a, task_idx=None), (vis, pe, input_ids, tt, pos, mask))
+        res = {}
+        for mode, fn in (("python", lambda: model(vis, pe, input_ids, tt, pos, mask, task_idx=None)),
+                         ("graph", lambda: g(vis, pe, input_ids, tt, pos, mask))):
+            for _ in range(2):
+                fn()
+            torch.cuda.synchronize()
+            ts = []
+            for _ in range(5):
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                fn()
+                e1.record()
+                torch.cuda.synchronize()
+                ts.append(e0.elapsed_time(e1))
+            res[mode] = sorted(ts)[2]
+        name = f"beam K={K} trigram-blocked"
+        print(f"{name}: K/V cache {res['python']:8.1f} ms ({B * steps / res['python'] * 1e3:8.0f} tokens/s) | "
+              f"+ graph replay {res['graph']:8.1f} ms ({B * steps / res['graph'] * 1e3:8.0f} tokens/s, {g.launches_per_replay} library launches per decode)")
 
 
 if __name__ == "__main__":

@@ -3,8 +3,9 @@
 Same algorithm and return format (a `traces` dict of padded tensors: pred_seq, scores, wids, ptrs), with ALL beam
 bookkeeping on the device — top-k, back pointers (integer floor division: the reference's `torch.div(k_ids, K)`, :1317, yields
 floats on torch >= 1.6 and breaks `gather`, SURVEY.md §2 #7), the per-layer K/V caches reordered by the back pointers, and the final
-best-hypothesis selection + back-tracking (:1431-1472) as vectorised tensor ops: no host synchronisation inside or after the loop
-(the optional duplicate-n-gram filter is the one host-side piece, as in the reference).
+best-hypothesis selection + back-tracking (:1431-1472) as vectorised tensor ops, and the optional duplicate-n-gram blocking
+(`forbid_duplicate_ngrams`, :1375-1428) as one vlpk_beam_ngram_block launch per frame over per-hypothesis word histories held on the
+device: no host synchronisation inside or after the loop, so a blocked decode can be captured as a CUDA graph too.
 Per-sample `task_idx` (the relaxed MLM head, relax_projection > 1) is expanded to the B*K beam rows with the other inputs; the
 reference does not expand it (:1297 vs :1325-1373), so its relaxed beam search only runs at B = 1.
 Every step runs the fused layers on the two new rows (token, [MASK]) against the K/V caches (`dec.use_kv_cache`), or — reference
@@ -14,6 +15,8 @@ import math
 
 import torch
 import torch.nn.functional as F
+
+from . import ops
 
 
 def _expand_beams(x, K):
@@ -29,7 +32,9 @@ def _reorder(x, back_ptrs, B, K):
 
 
 def _dup_ngram_candidates(seq, n, ignore):
-    """Words that would complete an n-gram already present in seq (reference get_dup_ngram_candidates, :1390-1406)."""
+    """Words that would complete an n-gram already present in seq (reference get_dup_ngram_candidates, :1390-1406).  The rule the
+    vlpk_beam_ngram_block kernel implements, kept as the host statement the tests compare against.  As in the reference, the ignore
+    test looks at seq[-(n-1):] — all of seq when n = 1 — while each match compares n - 1 words (none when n = 1)."""
     if len(seq) < n:
         return []
     tail = seq[-(n - 1):]
@@ -37,9 +42,26 @@ def _dup_ngram_candidates(seq, n, ignore):
         return []
     out = set()
     for i in range(len(seq) - (n - 1)):
-        if seq[i:i + n - 1] == tail and not (ignore and seq[i + n - 1] in ignore):
+        if seq[i:i + n - 1] == seq[len(seq) - (n - 1):] and not (ignore and seq[i + n - 1] in ignore):
             out.add(seq[i + n - 1])
     return sorted(out)
+
+
+def _ignore_tensor(dec, dev):
+    """The decoder's forbid_ignore_set as an int32 device tensor (None when empty), built once per distinct set and device and kept on
+    the decoder for its lifetime: the first call (a CUDA graph's warm-up) makes the host-to-device copy, so a capture never does, and
+    a graph captured with one set keeps reading a live tensor after decodes with other sets."""
+    key = (tuple(sorted(int(w) for w in dec.forbid_ignore_set or ())), str(dev))
+    cache = dec.__dict__.setdefault("_ngram_ignore_cache", {})
+    if key not in cache:
+        cache[key] = torch.tensor(key[0], dtype=torch.int32, device=dev) if key[0] else None
+    return cache[key]
+
+
+def check_ngram_args(dec):
+    """Raises before any launch for an n-gram size the blocking rule does not define."""
+    if dec.forbid_duplicate_ngrams and dec.search_beam_size > 1 and int(dec.ngram_size) < 1:
+        raise ValueError(f"vlp_b200: forbid_duplicate_ngrams needs ngram_size >= 1 (got {dec.ngram_size})")
 
 
 def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None):
@@ -52,7 +74,10 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
     curr_ids = input_ids
     mask_ids = input_ids[:, :1] * 0 + dec.mask_word_id
     total_scores, beam_eos, step_ids, step_ptrs = [], [], [], []
-    partial, forbid = None, None
+    if dec.forbid_duplicate_ngrams:
+        check_ngram_args(dec)
+        ngram, ignore = int(dec.ngram_size), _ignore_tensor(dec, dev)
+        hist = [torch.empty(B * K, out_len - in_len, dtype=torch.int32, device=dev) for _ in range(2)]    # word histories, in turn
     next_pos = in_len
     while next_pos < out_len:
         cl = curr_ids.shape[1]
@@ -69,8 +94,10 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
                                               prev_encoded_layers=prev_layers, output_all_encoded_layers=True, len_vis_input=dec.len_vis_input)
         scores, _ = dec.cls(new_layers[-1][:, -1:, :], None, task_idx=task_idx)
         logp = F.log_softmax(scores.float(), dim=-1)                      # [B or B*K, 1, V]
-        if forbid is not None:
-            logp = logp + forbid * -10000.0
+        frame = next_pos - in_len
+        if dec.forbid_duplicate_ngrams and frame >= 1:
+            # history of frame `frame` from the previous frame's words and back pointers; blocks in place once it holds n words
+            ops.beam_ngram_block(hist[(frame - 1) % 2], hist[frame % 2], step_ptrs[-1], step_ids[-1], frame, ngram, ignore, logp)
         if dec.min_len and (next_pos - in_len + 1 <= dec.min_len):
             logp[:, :, dec.eos_id] = -10000.0
         kk_scores, kk_ids = torch.topk(logp, k=K)                          # [*, 1, K]
@@ -105,20 +132,6 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
             prev_emb = _reorder(torch.cat((prev_emb, new_emb[:, :-1, :]), dim=1), back, B, K)
             prev_layers = [_reorder(torch.cat((a, b[:, :-1, :]), dim=1), back, B, K) for a, b in zip(prev_layers, new_layers)]
         curr_ids = k_ids.reshape(B * K, 1)
-        if dec.forbid_duplicate_ngrams:
-            wids, ptrs = k_ids.tolist(), back.tolist()
-            if first:
-                partial = [[wids[b][k]] for b in range(B) for k in range(K)]
-            else:
-                partial = [partial[ptrs[b][k] + b * K] + [wids[b][k]] for b in range(B) for k in range(K)]
-            forbid = None
-            if len(partial[0]) >= dec.ngram_size:
-                cands = [_dup_ngram_candidates(s, dec.ngram_size, dec.forbid_ignore_set) for s in partial]
-                if any(cands):
-                    forbid = torch.zeros(B * K, 1, logp.shape[-1], device=dev)
-                    for i, c in enumerate(cands):
-                        if c:
-                            forbid[i, 0, c] = 1.0
         next_pos += 1
 
     out = {"pred_seq": backtrack(torch.stack(total_scores), torch.stack(step_ids), torch.stack(step_ptrs), dec.eos_id, dec.length_penalty, out_len)}

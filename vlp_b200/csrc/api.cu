@@ -10,6 +10,7 @@
 #include <cstring>
 
 #include "attn.cuh"
+#include "decode.cuh"
 #include "gemm.cuh"
 #include "head.cuh"
 #include "host.cuh"
@@ -781,6 +782,17 @@ int vlpk_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream) { ret
 int vlpk_debug_dropout_mask(const VlpkDropout* drop, uint64_t site, int64_t n, unsigned char* out, void* stream) {
   VLPK_CHECK_ARG(drop != nullptr && out != nullptr, "dropout_mask: null pointer");
   return launch_dropout_mask(mk_drop(drop, drop->p, site), n, out, S(stream));
+}
+
+int vlpk_beam_ngram_block(int rows, int K, int f, int T_cap, int n, const int32_t* hist_in, int32_t* hist_out, const int64_t* ptr,
+                          const int64_t* wid, const int32_t* ignore, int n_ignore, float* logp, int64_t ld, int V, void* stream) {
+  NgramBlockArgs a;
+  a.rows = rows; a.K = K; a.f = f; a.T_cap = T_cap; a.n = n;
+  a.hist_in = hist_in; a.hist_out = hist_out;
+  a.ptr = reinterpret_cast<const long long*>(ptr); a.wid = reinterpret_cast<const long long*>(wid);
+  a.ignore = ignore; a.n_ignore = n_ignore;
+  a.logp = logp; a.ld = ld; a.V = V;
+  return launch_beam_ngram_block(a, S(stream));
 }
 
 int vlpk_colsum(const void* x, int64_t ld, int64_t M, int N, float* out, void* stream) {

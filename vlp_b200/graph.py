@@ -103,7 +103,8 @@ class GraphedCall:
     decode step touches 2 new rows per sequence and is launch-bound (12 layers x 6 launches + head per step, 21 steps); every step has its
     own shapes but the sequence of steps is fixed for a given (batch, lengths), so the whole loop — region projections, 21 cached decode
     steps, greedy arg-max or beam bookkeeping and back-tracking, all on the device — is one graph.  The returned tensors are overwritten by
-    the next call; clone what must survive.  Not for `forbid_duplicate_ngrams` (host-side n-gram bookkeeping)."""
+    the next call; clone what must survive.  Duplicate-n-gram blocking (`forbid_duplicate_ngrams`) runs on the device and is captured
+    too; its ignore set is copied to the device by the warm-up, before the capture."""
 
     def __init__(self, fn, example_args, warmup=2):
         self.static = tuple(a.clone() if torch.is_tensor(a) else a for a in example_args)

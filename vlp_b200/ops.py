@@ -491,3 +491,32 @@ def layer_cached_fwd(hidden, kv_cache, pos, mask_bits, heads, I, params):
     L.call("vlpk_layer_cached_fwd", C.byref(shape), ws, x.data_ptr(), kv_cache.data_ptr(), kv_cache.shape[1], int(pos), mask_bits.data_ptr(),
            mask_bits.shape[1], acts.structs, 0, L.stream())
     return acts.y[0]
+
+
+# ------------------------------------------------------------------------------------------------
+# beam search
+# ------------------------------------------------------------------------------------------------
+def beam_ngram_block(hist_in, hist_out, ptr, wid, f, n, ignore, logp):
+    """Duplicate-n-gram blocking of beam frame f >= 1 (vlpk_beam_ngram_block): hist_out [B*K, T_cap] int32 receives the history
+    hist_in[parent] + wid of every hypothesis (ptr / wid: int64 [B, K] back pointers and word ids of frame f-1); if f >= n, logp
+    (fp32, [B*K, ..., V] with unit stride in V) gets -10000 added in place at each hypothesis' repeated-n-gram completions.
+    ignore: int32 device tensor of exempt word ids, or None."""
+    for t, what in ((hist_in, "n-gram history"), (hist_out, "n-gram history"), (ptr, "beam back pointers"), (wid, "beam word ids"),
+                    (logp, "beam log-probabilities")) + (() if ignore is None else ((ignore, "n-gram ignore set"),)):
+        _require_cuda(t, what)
+    B, K = wid.shape
+    rows, T_cap = hist_out.shape
+    V = logp.shape[-1]
+    if rows != B * K or hist_out.dtype != torch.int32 or not hist_out.is_contiguous() or hist_in.shape != hist_out.shape \
+            or hist_in.dtype != torch.int32 or not hist_in.is_contiguous():
+        raise RuntimeError("vlp_b200: n-gram histories must be two contiguous int32 [B*K, T_cap] tensors")
+    if ptr.dtype != torch.int64 or wid.dtype != torch.int64 or not (ptr.is_contiguous() and wid.is_contiguous()) or ptr.shape != wid.shape:
+        raise RuntimeError("vlp_b200: back pointers and word ids must be contiguous int64 [B, K] tensors")
+    lp = logp.view(rows, -1) if logp.dim() != 2 else logp
+    if logp.dtype != torch.float32 or lp.stride(1) != 1 or lp.shape[0] != rows:
+        raise RuntimeError("vlp_b200: beam log-probabilities must be fp32 [B*K, V] rows with unit column stride")
+    if ignore is not None and (ignore.dtype != torch.int32 or ignore.dim() != 1 or not ignore.is_contiguous()):
+        raise RuntimeError("vlp_b200: the n-gram ignore set must be a contiguous 1-D int32 tensor of word ids")
+    n_ign = 0 if ignore is None else ignore.numel()
+    L.call("vlpk_beam_ngram_block", rows, K, int(f), T_cap, int(n), hist_in.data_ptr(), hist_out.data_ptr(), ptr.data_ptr(),
+           wid.data_ptr(), ignore.data_ptr() if n_ign else None, n_ign, lp.data_ptr(), lp.stride(0), V, L.stream())

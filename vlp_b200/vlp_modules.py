@@ -820,6 +820,8 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
     def forward(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, sample_mode="greedy"):
         self.cls.predictions.check_task_idx(task_idx)          # before anything is launched
         _check_seq_len(self.config, token_type_ids.size(1))
+        from .beam import check_ngram_args
+        check_ngram_args(self)
         with torch.no_grad():
             vis_feats, vis_pe = self.project_regions(vis_feats, vis_pe)
             if self.search_beam_size > 1:
