@@ -21,6 +21,10 @@
 // tile it belongs to (one set of full barriers per consumer), so each consumer waits only on phases of its own k-blocks and
 // can never mistake a phase of the other consumer's k-blocks for one of its own.  A consumer steps its ring position over
 // the k-blocks of the other consumer's tiles.
+// Aux epilogues (ADD / MUL / DRELU): while a tile's first wgmma group runs, the consumer's store thread loads the tile's
+// [128 x 128] aux block by TMA into the consumer's four staging boxes, in the swizzled layout of the output boxes.  Each
+// thread then reads its aux pair from the very place it writes its output pair, so the epilogue has no global loads to wait
+// on; per-thread 4-byte loads from global memory left the dgrad through GELU at about half the rate of a plain store.
 // Registers: a 12-warp block is capped at 168 per thread, too few for a 128-register accumulator plus an epilogue.  The
 // producer warpgroup gives registers back (setmaxnreg 24) and the consumers take them (setmaxnreg 240):
 // 128 x 24 + 256 x 240 = 64 512 of the 65 536-register file.  ptxas allocates the consumer code under the 240 only if
@@ -50,6 +54,7 @@ struct GemmTmaps {
   CUtensorMap b[3];
   CUtensorMap d0;
   CUtensorMap d1;
+  CUtensorMap aux;  // EPI_ADD / EPI_MUL / EPI_DRELU: the [M,N] side input, read in the output's 64 x 64 boxes
 };
 
 struct GemmArgs {
@@ -58,8 +63,6 @@ struct GemmArgs {
   int splits;
   int split_slices;  // EPI_REDUCE_F32: split s reduce-adds into slice s of the 3-D output map (else all into slice 0)
   const __nv_bfloat16* bias[3];
-  const __nv_bfloat16* aux;
-  long long ld_aux;
   float relu_scale;
   DropoutCfg drop;
   float* colsum;  // optional [N] fp32: += column sums of the (bf16-rounded) output tile, i.e. the bias gradient of a dgrad output
@@ -72,7 +75,7 @@ struct SmemLayout {
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int OFF_STG = STAGES * STAGE_BYTES;  // STG_PER_CONSUMER staging boxes per consumer warpgroup
   static constexpr int OFF_BAR = OFF_STG + 2 * STG_PER_CONSUMER * STG_BYTES;
-  static constexpr int NUM_BARS = 3 * STAGES;  // full (one set per consumer) + empty
+  static constexpr int NUM_BARS = 3 * STAGES + 2;  // full (one set per consumer) + empty + one aux-tile barrier per consumer
   static constexpr int TOTAL = OFF_BAR + NUM_BARS * 8;
   static constexpr int DYN_BYTES = TOTAL + 1024;  // slack for manual 1024-byte alignment
   static_assert(DYN_BYTES <= SMEM_MAX, "shared memory budget exceeded");
@@ -98,6 +101,8 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::OFF_BAR);
   uint64_t* full_bar = bars;                // TMA -> consumer c: full_bar[c * STAGES + stage]
   uint64_t* empty_bar = bars + 2 * STAGES;  // consumer -> TMA (one arrival per warp of the consuming warpgroup)
+  uint64_t* aux_bar = bars + 3 * STAGES;    // aux tile -> consumer c: aux_bar[c]
+  constexpr bool HAS_AUX = (EPI == EPI_ADD || EPI == EPI_MUL || EPI == EPI_DRELU);
 
   pdl_launch_dependents();  // the next kernel may be scheduled as SMs free up; it blocks in its own pdl_wait()
   const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);  // warp-uniform as far as the compiler can tell
@@ -113,8 +118,10 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
     tma_prefetch_desc(&tm.a);
     tma_prefetch_desc(&tm.b[0]);
     tma_prefetch_desc(&tm.d0);
+    if (HAS_AUX) tma_prefetch_desc(&tm.aux);
     for (int i = 0; i < 2 * STAGES; ++i) mbar_init(&full_bar[i], 1);
     for (int i = 0; i < STAGES; ++i) mbar_init(&empty_bar[i], 4);
+    for (int i = 0; i < 2; ++i) mbar_init(&aux_bar[i], 1);
     fence_mbar_init();
   }
   __syncthreads();
@@ -187,6 +194,7 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
     int stage = 0;        // ring stage of the next k-block, counted over both consumers' k-blocks
     uint32_t phases = 0;  // bit s: parity of this consumer's next wait on fb[s]
     uint32_t box_seq = 0;
+    uint32_t aux_phase = 0;  // parity of this consumer's next wait on aux_bar[cw]
     bool timed_out = false;  // a full-barrier wait gave up: trap after the loop (see mbar_wait_flag)
     float acc[2][BN / 2];  // rows 0-63 and 64-127 of the tile
     // Defined here so that the accumulator is live only in the consumer branch (reg_fence reads it before the first wgmma,
@@ -229,6 +237,20 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
           }
         }
         wgmma_commit();
+        if (HAS_AUX && kb == kb0) {
+          // The epilogue's aux tile goes into this consumer's four staging boxes, in the swizzled layout of the output boxes, while
+          // the tile's first wgmma group runs: the epilogue then reads it from shared memory instead of from global memory.
+          static_assert(STG_PER_CONSUMER == 2 * (BN / 64), "one staging box per aux box of a tile");
+          wg_bar_sync(cw);  // every thread of this consumer is done with the previous tile's staging boxes (colsum reads)
+          if (store_thread) {
+            tma_store_wait_read<0>();
+            fence_proxy_async_smem();
+            mbar_arrive_expect_tx(&aux_bar[cw], STG_PER_CONSUMER * STG_BYTES);
+#pragma unroll
+            for (int b = 0; b < STG_PER_CONSUMER; ++b)
+              tma_load_2d(stg_base + b * STG_BYTES, &tm.aux, &aux_bar[cw], n0 + (b & 1) * 64, m_blk * BM + (b >> 1) * 64);
+          }
+        }
         wgmma_wait<1>();
         reg_fence(acc[0]);
         reg_fence(acc[1]);
@@ -273,6 +295,10 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
         // bf16 staging: 64 columns = 128 bytes per row; one TMA store box per 64 rows x 64 columns.  GELU stores two outputs
         // per box position, from a pair of staging boxes; its two pairs alternate like the single boxes of the other epilogues.
         constexpr int NBOX = BN / 64;
+        if (HAS_AUX) {
+          mbar_wait_flag(&aux_bar[cw], aux_phase, timed_out);
+          aux_phase ^= 1u;
+        }
         const __nv_bfloat16* bp = nullptr;
         int bias_off = 0;
         if (HAS_BIAS) {
@@ -303,6 +329,7 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
               const int r = fr + 8 * (j & 1), col = 8 * (j >> 1) + fc;
               const int n = nh + c * 64 + col;
               const long long m = m0 + r;
+              const int so = r * 128 + (((col >> 3) ^ (r & 7)) << 4) + (col & 7) * 2;
               float v0 = acc[h][i], v1 = acc[h][i + 1];
               if (HAS_BIAS) {
                 if (bph != nullptr && n < args.N) {
@@ -311,7 +338,6 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
                   v1 += bb.y;
                 }
               }
-              const int so = r * 128 + (((col >> 3) ^ (r & 7)) << 4) + (col & 7) * 2;
               if (EPI == EPI_GELU) {
                 float g0, d0, g1, d1;
                 gelu_and_grad(v0, g0, d0);
@@ -329,8 +355,8 @@ gemm_kernel(const __grid_constant__ GemmTmaps tm, const GemmArgs args) {
                 v0 = ((keep >> fc) & 1u) ? v0 * args.drop.scale : 0.f;
                 v1 = ((keep >> (fc + 1)) & 1u) ? v1 * args.drop.scale : 0.f;
               } else if (EPI == EPI_ADD || EPI == EPI_MUL || EPI == EPI_DRELU) {
-                float2 x = make_float2(0.f, 0.f);
-                if (m < args.M && n < args.N) x = unpack_bf16x2(__ldg(reinterpret_cast<const unsigned int*>(args.aux + m * args.ld_aux + n)));
+                // this thread's aux pair, at the place its output pair goes (TMA zero-filled it beyond M and N)
+                const float2 x = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(stg + so));
                 if (EPI == EPI_ADD) {
                   v0 += x.x;
                   v1 += x.y;
@@ -520,6 +546,9 @@ int launch_gemm(const GemmDesc& g, cudaStream_t stream) {
   if (g.epi == EPI_ADD || g.epi == EPI_MUL || g.epi == EPI_DRELU) {
     VLPK_CHECK_ARG(g.aux != nullptr && (g.ld_aux % 8) == 0 && (reinterpret_cast<uintptr_t>(g.aux) & 15u) == 0,
                    "gemm: aux must be 16-byte aligned with ld %% 8 == 0");
+    VLPK_TRY(make_tmap_2d(&tm.aux, TM_BF16, g.aux, g.N, g.M, g.ld_aux, 64, 64));
+  } else {
+    tm.aux = tm.d0;
   }
 
   GemmArgs a;
@@ -530,8 +559,6 @@ int launch_gemm(const GemmDesc& g, cudaStream_t stream) {
   a.splits = splits;
   a.split_slices = (reduce && g.split_stride > 0) ? 1 : 0;
   for (int s = 0; s < 3; ++s) a.bias[s] = (s < g.nseg) ? g.bias[s] : nullptr;
-  a.aux = g.aux;
-  a.ld_aux = g.ld_aux;
   a.relu_scale = g.relu_scale;
   a.colsum = g.colsum;
   a.drop = g.drop;
