@@ -10,6 +10,8 @@ import ctypes as C
 
 import torch
 
+from tools import kernel_check as kc
+from tools import layer_check as lc
 from vlp_b200 import _lib as L
 from vlp_b200 import ops
 
@@ -142,3 +144,151 @@ def incremental_case(dev, B=2, Lq=2, Lkv=50, H=128, heads=2, I=512):
             L.call(entry, C.byref(shape), ws, x.data_ptr(), x_kv.data_ptr(), bits.data_ptr(), bits.shape[1], acts.structs, 0, L.stream())
         outs.append((act_view(acts, 0, "y1", B * Lq, H), acts))
     return {"y1_mha": outs[0][0], "y1_incr": outs[1][0], "_keep": (outs, params, bits, x_kv)}
+
+
+# ---- encoder stack and cached decode layer (tests/test_encoder_stack_gpu.py) ------------------------------------------------------
+def guarded_acts(n_layers, B, Lq, H, heads, I, dev, drop_bits=False, decode=False):
+    """Per-layer VlpkLayerActs whose every buffer is a NaN-guarded view (tools/kernel_check.guarded).  decode: the layout of
+    vlpk_layer_cached_fwd (qkv holds Q [B*Lq, H], kv the new rows' K | V [B*Lq, 2H]).  drop_bits: attention keep-bits followed by 64
+    guard bytes of 0xA5.  Returns (structs, [dict of views per layer], keep-bit buffer or None)."""
+    M = B * Lq
+    structs = (L.VlpkLayerActs * n_layers)()
+    nb = B * heads * Lq * ops.key_slots(Lq) // 8
+    bits = torch.full((n_layers, nb + 64), 0xA5, dtype=torch.uint8, device=dev) if drop_bits else None
+    views = []
+    widths = [("qkv", H if decode else 3 * H), ("ctx", H), ("t1", H), ("y1", H), ("u", I), ("hmid", I), ("t2", H), ("y", H)]
+    if decode:
+        widths.append(("kv", 2 * H))
+    for i in range(n_layers):
+        v = {n: kc.guarded(M, c, device=dev) for n, c in widths}
+        v["lse"] = kc.guarded(1, B * heads * Lq, dtype=torch.float32, device=dev)
+        v["stats1"] = kc.guarded(M, 2, dtype=torch.float32, device=dev)
+        v["stats2"] = kc.guarded(M, 2, dtype=torch.float32, device=dev)
+        for n, t in v.items():
+            setattr(structs[i], n, t.data_ptr())
+        if not decode:
+            structs[i].kv = None
+        structs[i].drop_attn = None if bits is None else bits[i].data_ptr()
+        views.append(v)
+    return structs, views, bits
+
+
+def guarded_scratch(M, H, I, dev):
+    """VlpkBwdScratch of NaN-guarded views: (struct, dict of views)."""
+    widths = {"dz2": H, "dt2": H, "du": I, "dy1": H, "dz1": H, "dt1": H, "dctx": H, "dqkv": 3 * H, "dx": H}
+    st, v = L.VlpkBwdScratch(), {}
+    for n in L.SCRATCH_FIELDS:
+        v[n] = kc.guarded(M, widths[n], device=dev)
+        setattr(st, n, v[n].data_ptr())
+    return st, v
+
+
+def guarded_grads(priors, H, I, dev):
+    """Per-layer VlpkLayerGrads of NaN-guarded fp32 views holding the given prior contents ([{name: tensor}] per layer, shapes of
+    layer_check.grad_shapes).  Returns (structs, [dict of 2-D guarded views per layer])."""
+    structs = (L.VlpkLayerGrads * len(priors))()
+    views = []
+    for i, pr in enumerate(priors):
+        v = {}
+        for n in L.GRAD_FIELDS:
+            t = pr[n] if pr[n].dim() == 2 else pr[n][None]
+            v[n] = kc.guard_fill(kc.guarded(t.shape[0], t.shape[1], dtype=torch.float32, device=dev), t)
+            setattr(structs[i], n, v[n].data_ptr())
+        views.append(v)
+    return structs, views
+
+
+def stack_inputs(dev, B, Lq, H, I, n_layers, p, mask="s2s", dys_mid=False, seed=0):
+    """Inputs of one encoder-stack case: parameters, x, the packed mask, the upstream gradients (dys[n-1], and dys[0] when
+    dys_mid), the arena's prior contents and the dropout seed."""
+    gen = torch.Generator().manual_seed(seed)
+    heads = H // 64
+    params = [t for _ in range(n_layers) for t in layer_params(gen, dev, H, I)]
+    x = _rn(gen, dev, B * Lq, H)
+    if mask == "s2s":
+        m = s2s_mask(B, Lq, max(1, Lq - Lq // 5), dev)
+    else:
+        m = (torch.rand(B, Lq, Lq, generator=gen) < 0.6).long().to(dev)
+    bits = ops.pack_mask(m, mode="zero_one")
+    dys = [None] * n_layers
+    dys[-1] = _rn(gen, dev, B * Lq, H, scale=0.1)
+    if dys_mid:
+        dys[0] = _rn(gen, dev, B * Lq, H, scale=0.05)
+    priors = [{n: torch.randn(s, generator=gen).to(dev) for n, s in lc.grad_shapes(H, I).items()} for _ in range(n_layers)]
+    shape = L.VlpkShape(B, Lq, Lq, H, heads, I, ops.kv_slots(Lq, Lq))
+    return dict(B=B, Lq=Lq, H=H, I=I, heads=heads, n_layers=n_layers, p=p, params=params, x=x, mask=m, bits=bits, dys=dys,
+                priors=priors, shape=shape, ws=ops._weight_structs(params, n_layers), seed=4242 + seed, dev=dev)
+
+
+def stack_run(c):
+    """One encoder step four ways: vlpk_encoder_fwd and a chain of vlpk_layer_fwd(layer_id = i); vlpk_encoder_bwd and a chain of
+    vlpk_layer_bwd(layer_id = i), each layer with its own scratch and arena, dy of layer i = dx of layer i + 1 (+ dys[i] rounded to
+    bf16).  Both backward runs read the encoder forward's activations.  Every output buffer is NaN-guarded."""
+    B, Lq, H, I, heads, n, p, dev = (c[k] for k in ("B", "Lq", "H", "I", "heads", "n_layers", "p", "dev"))
+    M = B * Lq
+    drop = L.VlpkDropout(p, c["seed"], None) if p > 0 else None
+    shape, ws, bits, x = c["shape"], c["ws"], c["bits"], c["x"]
+    out = {}
+    structs, acts, kbits = guarded_acts(n, B, Lq, H, heads, I, dev, drop_bits=p > 0)
+    L.call("vlpk_encoder_fwd", C.byref(shape), n, ws, x.data_ptr(), bits.data_ptr(), bits.shape[1], structs, p, p, drop, L.stream())
+    out.update(acts=acts, acts_structs=structs, keep_bits=kbits)
+    cstructs, cacts, cbits = guarded_acts(n, B, Lq, H, heads, I, dev, drop_bits=p > 0)
+    xin = x
+    for i in range(n):
+        L.call("vlpk_layer_fwd", C.byref(shape), C.byref(ws[i]), xin.data_ptr(), None, bits.data_ptr(), bits.shape[1], C.byref(cstructs[i]), p,
+               p, drop, i, L.stream())
+        xin = cacts[i]["y"]
+    out.update(chain_acts=cacts, chain_keep_bits=cbits)
+    # backward: the encoder
+    scr_st, scr = guarded_scratch(M, H, I, dev)
+    g_st, grads = guarded_grads(c["priors"], H, I, dev)
+    dx0 = kc.guarded(M, H, device=dev)
+    dys = (C.c_void_p * n)(*[None if d is None else d.data_ptr() for d in c["dys"]])
+    L.call("vlpk_encoder_bwd", C.byref(shape), n, ws, x.data_ptr(), bits.data_ptr(), bits.shape[1], structs, dys, dx0.data_ptr(), g_st,
+           C.byref(scr_st), p, p, drop, L.stream())
+    out.update(scratch=scr, grads=grads, dx0=dx0)
+    # backward: the chain
+    cscr, cgrads, cdx, cdy = [None] * n, [None] * n, [None] * n, [None] * n
+    dy = c["dys"][n - 1]
+    for i in reversed(range(n)):
+        st, cscr[i] = guarded_scratch(M, H, I, dev)
+        gs, g = guarded_grads([c["priors"][i]], H, I, dev)
+        cgrads[i] = g[0]
+        cdx[i] = kc.guarded(M, H, device=dev)
+        cdy[i] = dy
+        xi = x if i == 0 else acts[i - 1]["y"]
+        L.call("vlpk_layer_bwd", C.byref(shape), C.byref(ws[i]), xi.data_ptr(), bits.data_ptr(), bits.shape[1], C.byref(structs[i]),
+               dy.data_ptr(), cdx[i].data_ptr(), C.byref(gs[0]), C.byref(st), p, p, drop, i, L.stream())
+        dy = cdx[i]
+        if i > 0 and c["dys"][i - 1] is not None:
+            dy = (cdx[i].float() + c["dys"][i - 1].float()).to(BF16)
+    out.update(chain_scratch=cscr, chain_grads=cgrads, chain_dx=cdx, chain_dy=cdy)
+    return out
+
+
+def cached_decode_calls(dev, H, B, src, n_steps, cache_rows, seed=0):
+    """vlpk_layer_cached_fwd through a decode schedule: a prefix call at pos 0 with Lq = src (its last row the [MASK] row), then
+    n_steps calls with Lq = 2 ([word, MASK]) at pos = src - 1, src, ..., each overwriting the previous call's [MASK] row.  The
+    cache [B, cache_rows, 2H] starts NaN-filled.  Yields one record per call (taken right after it is enqueued) with the cache
+    contents before the call."""
+    gen = torch.Generator().manual_seed(seed)
+    I, heads = 4 * H, H // 64
+    params = layer_params(gen, dev, H, I)
+    ws = ops._weight_structs(params, 1)
+    cache = torch.empty(B, cache_rows, 2 * H, dtype=BF16, device=dev)
+    cache.view(torch.int16).fill_(0x7FA5)
+    for pos, Lq in [(0, src)] + [(src - 1 + k, 2) for k in range(n_steps)]:
+        Lkv = pos + Lq
+        x = _rn(gen, dev, B * Lq, H)
+        if pos == 0:
+            m = s2s_mask(B, Lq, Lq - 1, dev)
+        else:      # row r is position pos + r: it sees every earlier position and itself
+            m = torch.tril(torch.ones(Lq, Lkv, dtype=torch.long), diagonal=pos).expand(B, Lq, Lkv).contiguous().to(dev)
+        bits = ops.pack_mask(m, mode="zero_one")
+        structs, views, _ = guarded_acts(1, B, Lq, H, heads, I, dev, decode=True)
+        shape = L.VlpkShape(B, Lq, Lkv, H, heads, I, ops.kv_slots(Lq, Lkv))
+        before = cache.clone()
+        L.call("vlpk_layer_cached_fwd", C.byref(shape), ws, x.data_ptr(), cache.data_ptr(), cache_rows, pos, bits.data_ptr(), bits.shape[1],
+               structs, 0, L.stream())
+        yield dict(pos=pos, Lq=Lq, Lkv=Lkv, B=B, H=H, I=I, heads=heads, x=x, mask=m, bits=bits, acts=views[0], before=before, cache=cache,
+                   params=params)
