@@ -76,3 +76,56 @@ def case(seed=4321):
             gs[2].zero_()
         grads.append(gs)
     return params, wds, grads
+
+
+# Per-parameter schedule (tests/golden/bertadam_skip.pt): three groups, and two tensors that miss gradients on some steps, so their
+# own state['step'] falls behind their group's (:164-172 evaluates the schedule at each parameter's own count).
+SKIP_SHAPES = [(16, 33), (257,), (7,), (2, 100), (96,), (5,), (30, 5), (33,)]     # small: the golden stores every step in full
+SKIP_DEFAULTS = dict(lr=3e-3, warmup=0.3, t_total=10, schedule="warmup_linear", b1=0.9, b2=0.999, e=1e-6, weight_decay=0.01,
+                     max_grad_norm=1.0)
+SKIP_GROUPS = [((0, 1, 2, 3), {}),                                                             # warmup_linear, decay
+               ((4, 5), {"lr": 1e-3, "weight_decay": 0.0}),                                      # another lr, no decay
+               ((6, 7), {"schedule": "warmup_cosine", "lr": 2e-3, "warmup": 0.2, "t_total": 8})]
+SKIP_MISSING = {1: (0, 1), 2: (2,)}      # tensor -> steps on which it has no gradient
+SKIP_STEPS = 5
+
+
+def skip_hyper(i):
+    """The hyper-parameters tensor i sees: the defaults overridden by its group's entries."""
+    for idx, over in SKIP_GROUPS:
+        if i in idx:
+            return {**SKIP_DEFAULTS, **over}
+    raise KeyError(i)
+
+
+def skip_case(seed=8765):
+    """-> params [fp32], grads[step][tensor] (None on the steps in SKIP_MISSING).  Gradient scales straddle the clip threshold."""
+    gen = torch.Generator().manual_seed(seed)
+    params = [torch.randn(*s, generator=gen) * 0.05 for s in SKIP_SHAPES]
+    grads = []
+    for t in range(SKIP_STEPS):
+        gs = []
+        for i, s in enumerate(SKIP_SHAPES):
+            g = torch.randn(*s, generator=gen) * [2e-3, 0.3, 2.0, 1e-3, 0.5, 1e-4, 5e-3, 1.0][i] * (1.0 + t)
+            gs.append(None if t in SKIP_MISSING.get(i, ()) else g)
+        grads.append(gs)
+    return params, grads
+
+
+def run_skip(params, grads):
+    """The oracle over skip_case(): each tensor steps with its own count.  Returns per step dict(p, m, v, step) (m / v None and
+    step 0 before a tensor's first gradient)."""
+    ps = [p.clone() for p in params]
+    ms, vs, steps = [None] * len(ps), [None] * len(ps), [0] * len(ps)
+    out = []
+    for gs in grads:
+        for i, g in enumerate(gs):
+            if g is None:
+                continue
+            if ms[i] is None:
+                ms[i], vs[i] = torch.zeros_like(ps[i]), torch.zeros_like(ps[i])
+            step(ps[i], g.clone(), ms[i], vs[i], steps[i], **skip_hyper(i))
+            steps[i] += 1
+        out.append({"p": [p.clone() for p in ps], "m": [None if m is None else m.clone() for m in ms],
+                    "v": [None if v is None else v.clone() for v in vs], "step": list(steps)})
+    return out

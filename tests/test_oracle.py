@@ -135,6 +135,30 @@ def test_bertadam_oracle_matches_reference_golden(golden_dir):
     assert any(scaled) and not all(scaled)
 
 
+def test_bertadam_oracle_per_parameter_schedule_matches_reference_golden(golden_dir):
+    """oracle/bertadam_oracle.run_skip vs the reference's BertAdam on skip_case(): three groups (two schedules, two lrs, with and
+    without decay) and two tensors that miss gradients, whose own step counts — and so learning rates — lag their group's."""
+    from oracle import bertadam_oracle as bo
+    gold = torch.load(os.path.join(golden_dir, "bertadam_skip.pt"))
+    params, grads = bo.skip_case()
+    mine = bo.run_skip(params, grads)
+    assert len(gold["steps"]) == bo.SKIP_STEPS
+    for t, (a, b) in enumerate(zip(mine, gold["steps"])):
+        assert a["step"] == b["step"], t
+        for key in ("p", "m", "v"):
+            for i, (x, y) in enumerate(zip(a[key], b[key])):
+                if y is None:
+                    assert x is None, (t, key, i)
+                    continue
+                err, scale = float((x - y).abs().max()), float(y.abs().max())
+                assert err <= 1e-6 * scale, (t, key, i, err, scale)
+    # the lagging tensors are what the case is about: tensor 1 has no state before step 2 and sits at its own step 0 (lr 0 under
+    # warmup) on that step, while its group has moved on
+    assert gold["steps"][2]["step"][1] == 1 and gold["steps"][2]["step"][0] == 3
+    assert torch.equal(gold["steps"][2]["p"][1], params[1])
+    assert gold["steps"][2]["step"][2] == 2 and gold["steps"][4]["step"][2] == 4
+
+
 def test_bertadam_schedules():
     from oracle import bertadam_oracle as bo
     assert bo.schedule_value("warmup_linear", 0.05, 0.1) == 0.5

@@ -7,6 +7,7 @@ nothing: buffers keep whatever torch.empty returned.
 """
 import contextlib
 import ctypes as C
+import math
 
 import torch
 
@@ -292,3 +293,136 @@ def cached_decode_calls(dev, H, B, src, n_steps, cache_rows, seed=0):
                structs, 0, L.stream())
         yield dict(pos=pos, Lq=Lq, Lkv=Lkv, B=B, H=H, I=I, heads=heads, x=x, mask=m, bits=bits, acts=views[0], before=before, cache=cache,
                    params=params)
+
+
+# ---- fused BertAdam step (tests/test_adam_kernel_gpu.py) ----------------------------------------------------------------------------
+ADAM_ROLES = ("param", "grad", "master", "m", "v")
+ADAM_HYPER = (1e-3, 0.9, 0.999, 1e-6, 1.0)               # lr, b1, b2, e, max_grad_norm
+ADAM_SIZES = (1, 7, 8, 9, 4095, 4096, 4097, 32 * 4096, 33 * 4096 + 5, 2 * 4096 + 3)
+ADAM_WDS = (0.0, 0.01, 0.1)                              # per-tensor weight decay, cycled through every table
+ADAM_DT = {"bf16": BF16, "fp32": torch.float32}
+_ESZ = {BF16: 2, torch.float32: 4}
+ADAM_CASES = ([f"sizes-{p}-{g}" for p in ADAM_DT for g in ADAM_DT]
+              + [f"align-{r}-bf16-bf16" for r in ADAM_ROLES] + ["align-param-fp32-bf16", "align-grad-bf16-fp32"]
+              + ["bert-base", "many-small", "single", "clip", "no-clip", "nonfinite"])
+
+
+def adam_tensor(gen, dev, n, p_dt=BF16, g_dt=BF16, wd=0.01, g_scale=1e-2, g_norm=None, off=None, bad=None):
+    """One tensor of a vlpk_bertadam_step table, each of its buffers a NaN-guarded 1-D view with 16 guard elements behind it.
+    `off` {role: element offset of the view in its buffer}; the default is 16 bytes, so the pointer is 16-byte aligned behind a
+    front guard.  Gradient, m and v magnitudes spread over three decades inside the tensor, so an error in a small element is not
+    hidden by a large one.  g_norm: the gradient is rescaled to that 2-norm (0: all zero); bad: (element, value) written into
+    the gradient (inf / NaN)."""
+    off = off or {}
+    dts = dict(param=p_dt, grad=g_dt, master=torch.float32, m=torch.float32, v=torch.float32)
+    t = dict(n=n, p_dt=p_dt, g_dt=g_dt, wd=wd)
+    for role in ADAM_ROLES:
+        if role == "master" and p_dt != BF16:
+            t[role] = None
+            continue
+        o = off.get(role, 16 // _ESZ[dts[role]])
+        t[role] = kc.guarded(1, n, ld=o + n + 16, dtype=dts[role], extra_rows=0, col0=o, device=dev)
+    spread = torch.pow(10.0, -3.0 * torch.rand(n, generator=gen, device=dev))
+    g = torch.randn(n, generator=gen, device=dev) * spread * g_scale
+    if g_norm is not None:
+        g = g * (g_norm / g.double().norm().clamp_min(1e-300)).float()
+    g = g.to(g_dt)
+    if bad is not None:
+        g[bad[0]] = bad[1]
+    w = torch.randn(n, generator=gen, device=dev) * 0.05
+    m = torch.randn(n, generator=gen, device=dev) * 1e-3 * spread
+    v = (torch.randn(n, generator=gen, device=dev) * 1e-3).square() * spread
+    t["init"] = dict(w=w, g=g, m=m, v=v)
+    return t
+
+
+def adam_case(name, dev, bert_dims=None):
+    """(tensors, hyper) of one named case of ADAM_CASES.  bert_dims: the model whose parameter set "bert-base" uses (BERT-base)."""
+    import zlib
+
+    from vlp_b200 import synth
+    gen = torch.Generator(device=dev).manual_seed(zlib.crc32(name.encode()))
+    hyper = ADAM_HYPER
+    f32 = torch.float32
+
+    def T(i, n, **kw):
+        kw.setdefault("wd", ADAM_WDS[i % 3])
+        return adam_tensor(gen, dev, n, **kw)
+    kind = name.split("-")
+    if kind[0] == "sizes":
+        p, g = ADAM_DT[kind[1]], ADAM_DT[kind[2]]
+        ts = [T(i, n, p_dt=p, g_dt=g) for i, n in enumerate(ADAM_SIZES)]
+    elif kind[0] == "align":         # one role misaligned at a time: each condition of the update kernel's `vec` on its own
+        role, p, g = kind[1], ADAM_DT[kind[2]], ADAM_DT[kind[3]]
+        fp32_role = role in ("master", "m", "v") or (role == "param" and p == f32) or (role == "grad" and g == f32)
+        offs = (1, 2, 3, 1) if fp32_role else (1, 3, 7, 5)
+        ts = [T(i, n, p_dt=p, g_dt=g, off={role: o}) for i, (n, o) in enumerate(zip((9, 4097, 2 * 4096 + 3, 33 * 4096 + 5), offs))]
+    elif name == "bert-base":        # every parameter of the model, word embedding (5 437 chunks) included: CTAs loop many times
+        keys = synth.state_dict_keys(bert_dims or synth.BERT_BASE)
+        ts = [T(i, math.prod(shape), wd=0.0 if k in ("b", "g") else 0.01) for i, (_, shape, k) in enumerate(keys)]
+    elif name == "many-small":       # 500 tensors of 1-9 elements around 3 large ones: the chunk search crosses many boundaries
+        ts, dts = [], [(BF16, BF16), (BF16, f32), (f32, BF16), (f32, f32)]
+        for i in range(503):
+            n = (5 * 4096 + 77, 3 * 4096, 7 * 4096 + 1)[(i - 100) // 150] if i in (100, 250, 400) else 1 + i % 9
+            ts.append(T(i, n, p_dt=dts[i % 4][0], g_dt=dts[i % 4][1]))
+    elif name == "single":
+        ts = [T(0, 100003, p_dt=BF16, g_dt=f32)]
+    elif name in ("clip", "no-clip"):  # 2-norms just above and below max_norm, zero, far above, far below
+        mx = hyper[4]
+        norms = (mx * (1 + 1e-4), mx * (1 - 1e-4), 0.0, 37.0, 1e-3, mx * (1 + 1e-4), mx * (1 - 1e-4))
+        sizes = (4097, 33 * 4096 + 5, 9, 2 * 4096 + 3, 4095, 7, 1)
+        ts = [T(i, n, p_dt=(BF16, f32)[i % 2], g_dt=f32, g_norm=gn) for i, (n, gn) in enumerate(zip(sizes, norms))]
+        if name == "no-clip":
+            hyper = hyper[:4] + (-1.0,)
+    elif kind[0] == "nonfinite":     # "nonfinite" and the same table without its inf / NaN ("nonfinite-clean")
+        gen.manual_seed(zlib.crc32(b"nonfinite"))
+        clean = name == "nonfinite-clean"
+        ts = [T(0, 4096, g_scale=10.0), T(1, 5000, g_dt=f32, bad=None if clean else (3000, math.inf)), T(2, 3001, p_dt=f32),
+              T(3, 4097, bad=None if clean else (4096, math.nan)), T(4, 777, g_dt=f32, g_scale=1.0)]
+    else:
+        raise KeyError(name)
+    return ts, hyper
+
+
+def adam_reset(tensors):
+    """Put every tensor's initial values back into its buffers (guards untouched)."""
+    for t in tensors:
+        i = t["init"]
+        if t["master"] is not None:
+            t["master"][0].copy_(i["w"])
+        t["param"][0].copy_(i["w"].to(t["p_dt"]))
+        t["grad"][0].copy_(i["g"])
+        t["m"][0].copy_(i["m"])
+        t["v"][0].copy_(i["v"])
+
+
+def adam_table(tensors, dev):
+    """Host and device descriptor tables (the _TENSOR_DTYPE layout), chunk prefix and a NaN-guarded sums-of-squares buffer."""
+    import numpy as np
+
+    from vlp_b200 import optimization as opt_mod
+    tab = np.zeros(len(tensors), dtype=opt_mod._TENSOR_DTYPE)
+    for i, t in enumerate(tensors):
+        tab[i] = (t["param"].data_ptr(), t["grad"].data_ptr(), 0 if t["master"] is None else t["master"].data_ptr(), t["m"].data_ptr(),
+                  t["v"].data_ptr(), t["n"], t["wd"], opt_mod._DT[t["p_dt"]], opt_mod._DT[t["g_dt"]], 0)
+    prefix = np.zeros(len(tensors) + 1, dtype=np.int32)
+    np.cumsum((tab["n"] + kc.ADAM_CHUNK - 1) // kc.ADAM_CHUNK, out=prefix[1:])
+    return dict(tab=tab, prefix=prefix, tab_dev=torch.from_numpy(tab.view(np.uint8).copy()).to(dev),
+                prefix_dev=torch.from_numpy(prefix.copy()).to(dev),
+                sq=kc.guarded(1, len(tensors), ld=len(tensors) + 16, dtype=torch.float32, extra_rows=0, device=dev))
+
+
+def adam_run(tensors, table, hyper, det=False, reserved_sms=0):
+    """Reset the buffers and launch vlpk_bertadam_step once, in the default or the deterministic mode."""
+    adam_reset(tensors)
+    before = torch.are_deterministic_algorithms_enabled()
+    torch.use_deterministic_algorithms(det)
+    if reserved_sms:
+        L.invoke("vlpk_set_reserved_sms", reserved_sms)
+    try:
+        L.call("vlpk_bertadam_step", table["tab"].ctypes.data, table["tab_dev"].data_ptr(), table["prefix"].ctypes.data,
+               table["prefix_dev"].data_ptr(), len(tensors), table["sq"].data_ptr(), *(float(x) for x in hyper), L.stream())
+    finally:
+        if reserved_sms:
+            L.invoke("vlpk_set_reserved_sms", 0)
+        torch.use_deterministic_algorithms(before)

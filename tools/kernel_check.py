@@ -39,6 +39,10 @@ LN_STATS = 2e-6               # |mean - mu| <= LN_STATS * mean |z| and |rstd / r
 CE_LSE = 5e-6                 # cross-entropy lse and loss: |got - ref| <= CE_LSE * (1 + |ref|)
 CE_A = 2.0 ** -23             # dlogits: |got - ref| <= 2^-8 |ref| + CE_A * E (ce_magnitude)
 LN_EPS = float(torch.tensor(1e-5, dtype=torch.float32))    # the kernels' fp32 LayerNorm eps
+# fused BertAdam step (csrc/optim.cu)
+U32 = 2.0 ** -24              # fp32 unit roundoff
+ADAM_A = 2.0 ** -20           # m', v' and the updated fp32 weight, per unit of the magnitude of their terms
+ADAM_CHUNK = 4096             # elements per chunk (vlpk_bertadam_chunk)
 
 TILE = 128
 
@@ -416,3 +420,131 @@ def check_ce_rows(name, lse, loss, dlogits, ref, labels, lse_tol=CE_LSE, a=CE_A)
     out["dlogits"] = check_elementwise(f"{name} dlogits", dlogits, d, ref["E"].expand_as(d), R_BF16, a,
                                        where=lambda i, j: f"row {i} col {j} (label {int(labels[i])})")
     return out
+
+
+# ---- fused BertAdam step (csrc/optim.cu) ------------------------------------------------------------------------------------------
+# A table's tensors are checked as one flat concatenation: seg[i] is the tensor of flat element i.  Each stage is held to fp64
+# arithmetic on the kernel's own inputs to it: the sums of squares on the gradients, m' and v' on the clip factor of the kernel's own
+# sums, the updated fp32 weight on the kernel's own m' and v'.
+def f32(x):
+    return float(torch.tensor(x, dtype=torch.float32))
+
+
+def adam_hyper(lr, b1, b2, e, max_norm):
+    """The fp32 hyper-parameters vlpk_bertadam_step hands the kernels: each rounded from double, 1 - b formed in double first,
+    and the clip term's fp32 1e-6."""
+    return dict(lr=f32(lr), b1=f32(b1), omb1=f32(1.0 - b1), b2=f32(b2), omb2=f32(1.0 - b2), e=f32(e), max_norm=f32(max_norm),
+                tiny=f32(1e-6))
+
+
+def adam_sq_bound(n, ordered):
+    """Relative bound of the kernel's fp32 sum of squares of one n-element tensor: all terms are >= 0, so k roundings in a row
+    err by at most gamma_k = k u / (1 - k u) of the exact sum.  Within a chunk a thread chains at most 4096 / 256 = 16 fmaf, then
+    the warp and block butterflies add 5 + 3 levels; the nc chunk sums are then added by nc atomics in any order (default), or by
+    ceil(nc / 32) sequential adds per lane and a 5-level butterfly (deterministic mode)."""
+    nc = -(-n // ADAM_CHUNK)
+    k = 16 + 8 + (-(-nc // 32) + 5 if ordered else nc)
+    return k * U32 / (1.0 - k * U32)
+
+
+def adam_segments(ns, device):
+    return torch.repeat_interleave(torch.arange(len(ns), device=device), torch.tensor(ns, device=device))
+
+
+def adam_where(ns):
+    """Flat index -> 'tensor t element i (chunk c)'."""
+    import bisect
+    starts = [0]
+    for n in ns:
+        starts.append(starts[-1] + n)
+
+    def where(i):
+        t = bisect.bisect_right(starts, i) - 1
+        e = i - starts[t]
+        return f"tensor {t} (n={ns[t]}) element {e} (chunk {e // ADAM_CHUNK})"
+    return where
+
+
+def adam_sq_ref(g, seg, n_tensors):
+    """fp64 sum of squares of each tensor's gradient (as stored: bf16 or fp32)."""
+    g64 = g.to(F64)
+    return torch.zeros(n_tensors, dtype=F64, device=g.device).index_add_(0, seg, g64 * g64)
+
+
+def adam_clip_ref(sq, h):
+    """Per-tensor clip factor from the kernel's own sums: torch clip_grad_norm_ on each tensor, applied only when below 1, so a
+    NaN sum leaves the gradient unscaled and an infinite one scales it by 0.  No clipping when max_grad_norm <= 0."""
+    s = sq.to(F64)
+    if h["max_norm"] <= 0:
+        return torch.ones_like(s)
+    cc = h["max_norm"] / (s.sqrt() + h["tiny"])
+    return torch.where(cc < 1.0, cc, torch.ones_like(cc))
+
+
+def adam_moments_ref(g, m, v, c, h):
+    """fp64 m' = b1 m + (1 - b1) c g and v' = b2 v + (1 - b2) (c g)^2 with c per element: ((m', E_m), (v', E_v)), E the sum of the
+    magnitudes of the two terms."""
+    cg = c * g.to(F64)
+    tm, tv = h["b1"] * m.to(F64), h["b2"] * v.to(F64)
+    um, uv = h["omb1"] * cg, h["omb2"] * cg * cg
+    return (tm + um, tm.abs() + um.abs()), (tv + uv, tv.abs() + uv.abs())
+
+
+def adam_weight_ref(w, m1, v1, wd, h):
+    """fp64 w' = w - lr (m' / (sqrt(v') + e) + wd w) from the kernel's own m' and v' (w: the fp32 weight the kernel reads, the
+    master copy of a bf16 parameter), wd per element: (w', E)."""
+    w64 = w.to(F64)
+    q = m1.to(F64) / (v1.to(F64).sqrt() + h["e"])
+    d = wd.to(F64) * w64
+    return w64 - h["lr"] * (q + d), w64.abs() + h["lr"] * (q.abs() + d.abs())
+
+
+def check_adam_elem(name, got, ref, E, a=ADAM_A, where=None):
+    """|got - ref| <= a E elementwise, and got non-finite exactly where ref is, with the same value (a non-finite gradient under
+    clip_grad_norm_ semantics).  Returns the largest share of the bound used."""
+    fin = torch.isfinite(ref)
+    g64 = got.to(F64)
+    same = torch.where(fin, torch.isfinite(g64), (g64 == ref) | (torch.isnan(g64) & torch.isnan(ref)))
+    if not bool(same.all()):
+        i = int((~same).nonzero()[0, 0])
+        raise CheckError(f"{name}: non-finite pattern differs from the reference at {where(i) if where else i}: got {float(g64[i]):.6g} "
+                         f"ref {float(ref[i]):.6g}")
+    z = torch.zeros_like(ref)
+    return check_elementwise(name, torch.where(fin, g64, z), torch.where(fin, ref, z), torch.where(fin, E, z), 0.0, a, where=where)
+
+
+def check_adam(name, inp, out, sq, ns, wd, h, ordered):
+    """One vlpk_bertadam_step launch.  inp: flat initial g (as stored), m, v and w (the fp32 weight the kernel reads); out: flat
+    kernel m', v', w'; sq [T]: the kernel's sums of squares; ns: tensor sizes; wd [T]: weight decay per tensor.
+    Returns dict(sq, m, v, w) of the worst share of each bound."""
+    dev = inp["g"].device
+    seg = adam_segments(ns, dev)
+    where = adam_where(ns)
+    sq_ref = adam_sq_ref(inp["g"], seg, len(ns))
+    if h["max_norm"] > 0:
+        gam = torch.tensor([adam_sq_bound(n, ordered) for n in ns], dtype=F64, device=dev)
+        s_sq = check_adam_elem(f"{name} sq", sq, sq_ref, sq_ref.abs() * gam, a=1.0, where=lambda t: f"tensor {t} (n={ns[t]})")
+    else:
+        if not bool((sq == 0).all()):
+            raise CheckError(f"{name} sq: not zero with clipping off ({sq[sq != 0][:4].tolist()})")
+        s_sq = 0.0
+    c = adam_clip_ref(sq, h)[seg]
+    (mr, Em), (vr, Ev) = adam_moments_ref(inp["g"], inp["m"], inp["v"], c, h)
+    out_share = {"sq": s_sq,
+                 "m": check_adam_elem(f"{name} m'", out["m"], mr, Em, where=where),
+                 "v": check_adam_elem(f"{name} v'", out["v"], vr, Ev, where=where)}
+    del mr, Em, vr, Ev, c
+    wr, Ew = adam_weight_ref(inp["w"], out["m"], out["v"], wd.to(dev)[seg], h)
+    out_share["w"] = check_adam_elem(f"{name} w'", out["w"], wr, Ew, where=where)
+    return out_share
+
+
+def check_bf16_of_master(name, param, master):
+    """A bf16 parameter is its fp32 master copy rounded to nearest even, bit for bit (NaN where the master is NaN)."""
+    nan = torch.isnan(master)
+    want = master.to(BF)
+    same = (param.view(torch.int16) == want.view(torch.int16)) | (nan & torch.isnan(param))
+    if not bool(same.all()):
+        i = int((~same).nonzero()[0, 0])
+        raise CheckError(f"{name}: bf16 parameter is not the rounding of its master copy at element {i}: {float(param[i]):.8g} vs "
+                         f"{float(master[i]):.8g} -> {float(want[i]):.8g}")

@@ -150,7 +150,8 @@ class BertAdam(Optimizer):
         # pointers, sizes, weight decay, dtype tags, chunk prefix, validation) is cached in a plan, rebuilt when the set of parameters
         # that carry a gradient changes or state is (re)loaded.  One launch pair per distinct (device, scheduled lr, b1, b2, e,
         # max_grad_norm); in practice a single one: the two weight-decay groups of run_img2txt_dist.py:394-401 differ only in the
-        # per-tensor weight_decay field.
+        # per-tensor weight_decay field.  The schedule is evaluated at each tensor's own state['step'] (optimization.py:164-172): a
+        # tensor that had no gradient on some steps keeps a smaller count than its group and gets its own learning rate.
         sig = tuple((id(p), p.grad is None) for group in self.param_groups for p in group['params'])
         if self._plan is not None and self._plan_sig == sig:
             # state tensors replaced behind the plan's back (a hand-rolled state load, dtype casts): re-validate
@@ -175,8 +176,15 @@ class BertAdam(Optimizer):
                 grads.append(g)
             tab["grad"] = [g.data_ptr() for g in grads]
             tab["grad_dtype"] = [_DT[g.dtype] for g in grads]
-            key = (ps[0].device, self._scheduled_lr(group, states[0]['step']), group['b1'], group['b2'], group['e'], group['max_grad_norm'])
-            buckets.setdefault(key, []).append((tab, grads, states))
+            rest = (group['b1'], group['b2'], group['e'], group['max_grad_norm'])
+            steps = [st['step'] for st in states]
+            if steps.count(steps[0]) == len(steps):
+                buckets.setdefault((ps[0].device, self._scheduled_lr(group, steps[0])) + rest, []).append((tab, grads, states))
+            else:
+                lrs = [self._scheduled_lr(group, s) for s in steps]
+                for lr_s in dict.fromkeys(lrs):
+                    idx = [i for i, l in enumerate(lrs) if l == lr_s]
+                    buckets.setdefault((ps[0].device, lr_s) + rest, []).append((tab[idx], [grads[i] for i in idx], [states[i] for i in idx]))
         keep = []
         for (device, lr_s, b1, b2, e, max_norm), parts in buckets.items():
             tab = parts[0][0] if len(parts) == 1 else np.concatenate([t for t, _, _ in parts])
@@ -223,9 +231,13 @@ class BertAdam(Optimizer):
         chunk = L.lib().vlpk_bertadam_chunk()
         # The descriptor table travels through PINNED host memory: an asynchronous copy from pageable memory synchronises the host
         # with the stream, i.e. with the whole backward that is still in flight — a pipeline bubble every step.
-        # Three rotating slots: a slot is rewritten two steps after its copy was enqueued (the copy has long completed by then).
-        slot = self._pinned.setdefault((device, n), {"i": 0, "bufs": [None, None, None]})
+        # Three rotating slots.  The host may run ahead of the device (a GPU-bound step, a graph replay followed by step()), so a slot
+        # is only rewritten once the event recorded after its copies has completed: this waits only when the device is three
+        # launches behind, and otherwise costs an event query.
+        slot = self._pinned.setdefault((device, n), {"i": 0, "bufs": [None, None, None], "copied": [None, None, None]})
         k = slot["i"] = (slot["i"] + 1) % 3
+        if slot["copied"][k] is not None:
+            slot["copied"][k].synchronize()
         if slot["bufs"][k] is None:
             pin = (lambda t: t.pin_memory()) if torch.cuda.is_available() else (lambda t: t)     # (CPU dry-run tests marshal without a GPU)
             slot["bufs"][k] = (pin(torch.empty(n * _TENSOR_DTYPE.itemsize, dtype=torch.uint8)), pin(torch.empty(n + 1, dtype=torch.int32)))
@@ -237,6 +249,10 @@ class BertAdam(Optimizer):
         np.cumsum((tab["n"] + chunk - 1) // chunk, out=prefix[1:])
         tab_dev = tab_pin.to(device, non_blocking=True)
         prefix_dev = prefix_pin.to(device, non_blocking=True)
+        if device.type == "cuda":
+            if slot["copied"][k] is None:
+                slot["copied"][k] = torch.cuda.Event()
+            slot["copied"][k].record()
         sqnorm = torch.empty(n, dtype=torch.float32, device=device)
         L.call("vlpk_bertadam_step", tab_np.ctypes.data, tab_dev.data_ptr(), prefix.ctypes.data, prefix_dev.data_ptr(), n, sqnorm.data_ptr(),
                float(lr_s), float(b1), float(b2), float(e), float(max_norm), L.stream())
