@@ -328,6 +328,22 @@ int64_t vlpk_launch_count(void);
 int vlpk_beam_ngram_block(int rows, int K, int f, int T_cap, int n, const int32_t* hist_in, int32_t* hist_out, const int64_t* ptr,
                           const int64_t* wid, const int32_t* ignore, int n_ignore, float* logp, int64_t ld, int V, void* stream);
 
+/* Top-k / top-p sampling of decode frame f (0 <= f < T_cap) over rows sequences, one launch per frame, no host synchronisation:
+ *   x[v] = logits[row*ld + v] + bias[v], rounded to the logits' dtype (fp32 = 0: bf16, 1: fp32; bias may be NULL); then, as beam
+ *     search does, -10000 is added at the words the duplicate-n-gram rule of vlpk_beam_ngram_block blocks for the row's history
+ *     seq[row, :f] (n > 0 and f >= n; ignore / n_ignore as there), and x[eos_id] = -10000 if block_eos (frames below min_len).
+ *   Words are ranked by (x descending, index ascending).  mode 0 (top-k, 1 <= topk <= 64) keeps the first topk; mode 1 (top-p,
+ *     0 < topp <= 1) keeps the shortest prefix whose probability reaches topp (at least the first argmax).  One draw from the kept
+ *     words, renormalised, with a uniform from Philox keyed by (seed; f, row): reproducible for a seed whatever the batch.
+ *   seq: int64 [rows, T_cap] receives the word at [row, f]; score: fp32 [rows, T_cap] (or NULL) its log-probability under the
+ *     full softmax of x.  finished: int32 [rows]; a finished row writes pad_id (score 0); a row that draws eos_id is marked
+ *     finished and decrements live[0] (the host may poll live[0] == 0 to stop a decode early).
+ * Returns < 0 without launching for a mode, topk or topp outside its range, ld < V, V < 1, f outside [0, T_cap), a NULL pointer
+ * that is needed, or (V + V/32 + T_cap) * 4 bytes above 200 KB of shared memory. */
+int vlpk_sample_tokens(int rows, int V, const void* logits, int64_t ld, const void* bias, int fp32, int mode, int topk, float topp,
+                       uint64_t seed, int f, int64_t* seq, int T_cap, float* score, int32_t* finished, int32_t* live, int eos_id, int pad_id,
+                       int block_eos, int n, const int32_t* ignore, int n_ignore, void* stream);
+
 /* utilities */
 int vlpk_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 int vlpk_colsum(const void* x, int64_t ld, int64_t M, int N, float* out, void* stream);

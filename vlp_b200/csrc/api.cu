@@ -795,6 +795,18 @@ int vlpk_beam_ngram_block(int rows, int K, int f, int T_cap, int n, const int32_
   return launch_beam_ngram_block(a, S(stream));
 }
 
+int vlpk_sample_tokens(int rows, int V, const void* logits, int64_t ld, const void* bias, int fp32, int mode, int topk, float topp,
+                       uint64_t seed, int f, int64_t* seq, int T_cap, float* score, int32_t* finished, int32_t* live, int eos_id, int pad_id,
+                       int block_eos, int n, const int32_t* ignore, int n_ignore, void* stream) {
+  SampleArgs a;
+  a.rows = rows; a.V = V; a.logits = logits; a.ld = ld; a.bias = bias; a.fp32 = fp32;
+  a.mode = mode; a.topk = topk; a.topp = topp; a.seed = seed;
+  a.f = f; a.seq = reinterpret_cast<long long*>(seq); a.T_cap = T_cap; a.score = score;
+  a.finished = finished; a.live = live; a.eos_id = eos_id; a.pad_id = pad_id; a.block_eos = block_eos;
+  a.n = n; a.ignore = ignore; a.n_ignore = n_ignore;
+  return launch_sample(a, S(stream));
+}
+
 int vlpk_colsum(const void* x, int64_t ld, int64_t M, int N, float* out, void* stream) {
   VLPK_CHECK_ARG(x && out, "colsum: null pointer");
   return launch_colsum(x, ld, M, N, out, S(stream));

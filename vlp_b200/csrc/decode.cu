@@ -30,6 +30,35 @@ __device__ __forceinline__ bool is_ignored(int w, const int* ignore, int n_ignor
   return false;
 }
 
+// The candidates of history seq[0:f], f >= n, as set bits of `bits` ([ceil(V/32)] words, cleared here).  seq must be complete in
+// shared memory before the call (the first barrier here orders it).  Returns, uniformly across the CTA, whether any bit was set.
+__device__ bool ngram_candidates(const int* seq, int f, int n, int V, const int* ignore, int n_ignore, unsigned* bits) {
+  const int tid = threadIdx.x;
+  const int nwords = (V + 31) >> 5;
+  for (int j = tid; j < nwords; j += blockDim.x) bits[j] = 0u;
+  __syncthreads();
+
+  const int m = n - 1;                                             // words matched before a candidate
+  const int t0 = f - m;                                            // start of the tail
+  if (n_ignore > 0) {
+    int hit = 0;
+    for (int t = (m == 0 ? 0 : t0) + tid; t < f; t += blockDim.x) hit |= is_ignored(seq[t], ignore, n_ignore);
+    if (__syncthreads_or(hit)) return false;
+  }
+  int found = 0;
+  for (int s = tid; s < t0; s += blockDim.x) {                     // s <= f - n
+    bool match = true;
+    for (int j = 0; j < m && match; ++j) match = seq[s + j] == seq[t0 + j];
+    if (!match) continue;
+    const int w = seq[s + m];
+    if (w < 0 || w >= V) continue;
+    if (n_ignore > 0 && is_ignored(w, ignore, n_ignore)) continue;
+    atomicOr(bits + (w >> 5), 1u << (w & 31));
+    found = 1;
+  }
+  return __syncthreads_or(found) != 0;
+}
+
 __global__ void __launch_bounds__(NGRAM_THREADS) beam_ngram_block_kernel(NgramBlockArgs a) {
   extern __shared__ int smem[];
   int* seq = smem;                                                 // [T_cap] this row's history
@@ -56,31 +85,10 @@ __global__ void __launch_bounds__(NGRAM_THREADS) beam_ngram_block_kernel(NgramBl
   }
   if (f < a.n) return;                                             // uniform: too short for an n-gram
 
-  const int nwords = (a.V + 31) >> 5;
-  for (int j = tid; j < nwords; j += blockDim.x) bits[j] = 0u;
-  __syncthreads();
-
-  const int m = a.n - 1;                                           // words matched before a candidate
-  const int t0 = f - m;                                            // start of the tail
-  if (a.n_ignore > 0) {
-    int hit = 0;
-    for (int t = (m == 0 ? 0 : t0) + tid; t < f; t += blockDim.x) hit |= is_ignored(seq[t], a.ignore, a.n_ignore);
-    if (__syncthreads_or(hit)) return;
-  }
-  int found = 0;
-  for (int s = tid; s < t0; s += blockDim.x) {                     // s <= f - n
-    bool match = true;
-    for (int j = 0; j < m && match; ++j) match = seq[s + j] == seq[t0 + j];
-    if (!match) continue;
-    const int w = seq[s + m];
-    if (w < 0 || w >= a.V) continue;
-    if (a.n_ignore > 0 && is_ignored(w, a.ignore, a.n_ignore)) continue;
-    atomicOr(bits + (w >> 5), 1u << (w & 31));
-    found = 1;
-  }
-  if (!__syncthreads_or(found)) return;                            // no candidate: the row is not touched
+  if (!ngram_candidates(seq, f, a.n, a.V, a.ignore, a.n_ignore, bits)) return;      // no candidate: the row is not touched
 
   float* row = a.logp + static_cast<size_t>(i) * a.ld;
+  const int nwords = (a.V + 31) >> 5;
   for (int j = tid; j < nwords; j += blockDim.x) {
     unsigned w = bits[j];
     while (w) {
@@ -91,7 +99,250 @@ __global__ void __launch_bounds__(NGRAM_THREADS) beam_ngram_block_kernel(NgramBl
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Top-k / top-p sampling of one decode frame f, one CTA of SAMPLE_THREADS per row:
+//   x[v]   = logits[row, v] + bias[v], rounded to the logits' dtype (bit for bit the head's `decoder(h) + bias`), plus -10000 at
+//            the words the duplicate-n-gram rule above blocks for history seq[row, :f] (n > 0, f >= n), and x[eos] = -10000 while
+//            block_eos is set (beam search's order and values); e[v] = exp(x[v] - max x), Z = sum e.
+//   order  words ranked by (x descending, index ascending).  top-k keeps the first k; top-p keeps the shortest prefix whose e
+//            sum reaches topp * Z (always at least the first argmax, so topp -> 0 is greedy).  The cut is found as a threshold on
+//            an order-preserving 32-bit key (x for top-k, e for top-p) by binary search over the key's bits — no sort — and words
+//            tied at the threshold are taken lowest index first, as many as needed.
+//   draw   u = Philox(seed; frame f, row) in [0, 1); the chosen word is the first kept word, in index order, whose running e sum
+//          exceeds u * (kept e sum).  seq[row, f] = word, score[row, f] = log(e[word] / Z).
+// Each thread owns one contiguous chunk of the row in shared memory and every sum is taken in a fixed order (chunk, then a
+// fixed shuffle tree), so the result depends on (seed, f, row, logits) only: not on the batch, the grid or the run.
+// Finished rows write pad_id and score 0; a row that draws eos_id is marked finished and decrements *live.
+using bf16 = __nv_bfloat16;
+constexpr int SAMPLE_THREADS = 1024;                               // 32 warps: the block reductions below rely on it
+constexpr size_t SAMPLE_SMEM_MAX = 200 * 1024;
+
+__device__ __forceinline__ float head_logit(const bf16* l, const bf16* b, int v) {
+  const float x = __bfloat162float(l[v]);
+  return b ? __bfloat162float(__float2bfloat16_rn(x + __bfloat162float(b[v]))) : x;
+}
+__device__ __forceinline__ float head_logit(const float* l, const float* b, int v) { return b ? l[v] + b[v] : l[v]; }
+
+__device__ __forceinline__ unsigned order_key(float x) {           // unsigned order == float order
+  const unsigned u = __float_as_uint(x);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// Every thread gets op over the CTA's values; warp shuffle trees in a fixed order.  red: [33] shared.
+template <typename T, typename Op>
+__device__ __forceinline__ T block_reduce(T v, T* red, Op op) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = op(v, __shfl_down_sync(0xffffffffu, v, o));
+  __syncthreads();                                                  // red may still be read by the previous reduction
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  if (warp == 0) {
+    v = red[lane];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = op(v, __shfl_down_sync(0xffffffffu, v, o));
+    if (lane == 0) red[32] = v;
+  }
+  __syncthreads();
+  return red[32];
+}
+
+// pre[t] = sum of the values of threads < t, pre[SAMPLE_THREADS] = total.  red: [33] shared, pre: [SAMPLE_THREADS + 1] shared.
+template <typename T>
+__device__ __forceinline__ void block_exclusive_scan(T v, T* red, T* pre) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  T x = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const T y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  __syncthreads();
+  if (lane == 31) red[warp] = x;
+  __syncthreads();
+  if (warp == 0) {
+    T w = red[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const T y = __shfl_up_sync(0xffffffffu, w, o);
+      if (lane >= o) w += y;
+    }
+    const T before = __shfl_up_sync(0xffffffffu, w, 1);
+    red[lane] = lane == 0 ? T(0) : before;                         // warps before this one
+    if (lane == 31) pre[SAMPLE_THREADS] = w;
+  }
+  __syncthreads();
+  const T in_warp = __shfl_up_sync(0xffffffffu, x, 1);
+  pre[threadIdx.x] = red[warp] + (lane == 0 ? T(0) : in_warp);
+  __syncthreads();
+}
+
+template <typename T>
+__global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
+  extern __shared__ float sample_smem[];
+  __shared__ float redf[33], pref[SAMPLE_THREADS + 1];
+  __shared__ int redi[33], prei[SAMPLE_THREADS + 1];
+  const int V = a.V, tid = threadIdx.x, row = blockIdx.x;
+  const int nwords = (V + 31) >> 5;
+  float* val = sample_smem;                                          // [V] x (top-k) or e (top-p)
+  unsigned* bits = reinterpret_cast<unsigned*>(val + V);             // [nwords] blocked words
+  int* hist = reinterpret_cast<int*>(bits + nwords);                 // [T_cap] history
+  long long* out = a.seq + static_cast<size_t>(row) * a.T_cap;
+  if (a.finished[row]) {                                             // uniform
+    if (tid == 0) {
+      out[a.f] = a.pad_id;
+      if (a.score) a.score[static_cast<size_t>(row) * a.T_cap + a.f] = 0.f;
+    }
+    return;
+  }
+
+  bool blocked = false;
+  if (a.n > 0 && a.f >= a.n) {
+    for (int t = tid; t < a.f; t += SAMPLE_THREADS) {
+      const long long w = out[t];
+      hist[t] = (w >= INT_MIN && w <= INT_MAX) ? static_cast<int>(w) : -1;
+    }
+    blocked = ngram_candidates(hist, a.f, a.n, V, a.ignore, a.n_ignore, bits);
+  }
+
+  // x, coalesced, and its maximum (order-free)
+  const T* lrow = static_cast<const T*>(a.logits) + static_cast<size_t>(row) * a.ld;
+  const T* bias = static_cast<const T*>(a.bias);
+  float mx = -INFINITY;
+  for (int v = tid; v < V; v += SAMPLE_THREADS) {
+    float x = head_logit(lrow, bias, v);
+    if (blocked && ((bits[v >> 5] >> (v & 31)) & 1u)) x += -10000.0f;
+    if (a.block_eos && v == a.eos_id) x = -10000.0f;
+    val[v] = x;
+    mx = fmaxf(mx, x);
+  }
+  mx = block_reduce(mx, redf, [](float p, float q) { return fmaxf(p, q); });
+
+  // from here on thread t owns words [lo, hi); an odd chunk length keeps the threads' strided reads in distinct banks
+  const int C = ((V + SAMPLE_THREADS - 1) / SAMPLE_THREADS) | 1;
+  const int lo = min(tid * C, V), hi = min(lo + C, V);
+  const bool topp = a.mode == SAMPLE_TOPP;
+  float z = 0.f;
+  for (int v = lo; v < hi; ++v) {
+    const float e = expf(val[v] - mx);
+    z += e;
+    if (topp) val[v] = e;
+  }
+  const float Z = block_reduce(z, redf, [](float p, float q) { return p + q; });
+
+  auto key = [&](int v) { return topp ? __float_as_uint(val[v]) : order_key(val[v]); };
+  auto weight = [&](int v) { return topp ? val[v] : expf(val[v] - mx); };
+  // mass(t): sum of the selection weights (1 for top-k, e for top-p) of the words whose key is >= t.  mass(0) sums in Z's order.
+  auto mass = [&](unsigned t) {
+    float s = 0.f;
+    for (int v = lo; v < hi; ++v) s += key(v) >= t ? (topp ? val[v] : 1.f) : 0.f;
+    return block_reduce(s, redf, [](float p, float q) { return p + q; });
+  };
+  const float target = topp ? a.topp * Z : static_cast<float>(min(a.topk, V));
+  // tau = the largest key with mass(tau) >= target; mass(0) >= target always holds
+  unsigned klo = 0, khi = topp ? __float_as_uint(1.0f) : order_key(mx);
+  if (mass(khi) >= target) {
+    klo = khi;
+  } else {
+    khi -= 1;
+    while (klo < khi) {                                              // uniform: every thread sees the same masses
+      const unsigned mid = klo + (khi - klo + 1) / 2;
+      if (mass(mid) >= target) klo = mid; else khi = mid - 1;
+    }
+  }
+  const unsigned tau = klo;
+  const float above = tau == 0xffffffffu ? 0.f : mass(tau + 1);
+  int take;                                                           // words tied at tau to keep, lowest index first
+  if (!topp) {
+    take = static_cast<int>(target - above);
+  } else {
+    const float w_tie = __uint_as_float(tau);
+    take = w_tie > 0.f ? static_cast<int>(fminf(ceilf((target - above) / w_tie), static_cast<float>(V))) : V;
+  }
+  take = max(take, 1);
+
+  // ties before this chunk, then the kept weight of this chunk
+  int ties = 0;
+  for (int v = lo; v < hi; ++v) ties += key(v) == tau;
+  block_exclusive_scan(ties, redi, prei);
+  int rank = prei[tid];
+  float kept = 0.f;
+  for (int v = lo; v < hi; ++v) {
+    const unsigned k = key(v);
+    if (k > tau || (k == tau && rank++ < take)) kept += weight(v);
+  }
+  block_exclusive_scan(kept, redf, pref);
+
+  const uint4 r = Philox::gen(a.seed, static_cast<unsigned long long>(a.f), static_cast<unsigned long long>(row));
+  const float u = static_cast<float>(r.x >> 8) * (1.0f / 16777216.0f);
+  const float goal = u * pref[SAMPLE_THREADS];
+  int found = INT_MAX;
+  if (pref[tid] <= goal && goal < pref[tid + 1]) {                  // this chunk holds the draw: walk it
+    float acc = pref[tid];
+    rank = prei[tid];
+    for (int v = lo; v < hi; ++v) {
+      const unsigned k = key(v);
+      if (!(k > tau || (k == tau && rank++ < take))) continue;
+      found = v;                                                     // the last kept word, should rounding leave goal above acc
+      acc += weight(v);
+      if (goal < acc) break;
+    }
+  }
+  int pick = block_reduce(found, redi, [](int p, int q) { return min(p, q); });
+  if (pick == INT_MAX) {                                              // goal fell outside every chunk (rounding): first argmax
+    int first = INT_MAX;
+    for (int v = lo; v < hi && first == INT_MAX; ++v) if (val[v] == (topp ? 1.0f : mx)) first = v;
+    pick = block_reduce(first, redi, [](int p, int q) { return min(p, q); });
+  }
+  if (tid == 0) {
+    out[a.f] = pick;
+    if (a.score) a.score[static_cast<size_t>(row) * a.T_cap + a.f] = logf(topp ? val[pick] : expf(val[pick] - mx)) - logf(Z);
+    if (pick == a.eos_id) {
+      a.finished[row] = 1;
+      atomicSub(a.live, 1);
+    }
+  }
+}
+
 }  // namespace
+
+size_t sample_smem_bytes(int T_cap, int V) {
+  return (static_cast<size_t>(V) + (static_cast<size_t>(V) + 31) / 32 + static_cast<size_t>(T_cap)) * 4;
+}
+
+int launch_sample(const SampleArgs& a, cudaStream_t s) {
+  VLPK_CHECK_ARG(a.rows >= 0 && a.V >= 1 && a.ld >= a.V, "sample: rows=%d V=%d ld=%lld (ld must be >= V >= 1)", a.rows, a.V, a.ld);
+  VLPK_CHECK_ARG(a.mode == SAMPLE_TOPK || a.mode == SAMPLE_TOPP, "sample: mode=%d (0 top-k, 1 top-p)", a.mode);
+  VLPK_CHECK_ARG(a.mode != SAMPLE_TOPK || (a.topk >= 1 && a.topk <= SAMPLE_MAX_TOPK), "sample: topk=%d outside [1, %d]", a.topk,
+                 SAMPLE_MAX_TOPK);
+  VLPK_CHECK_ARG(a.mode != SAMPLE_TOPP || (a.topp > 0.f && a.topp <= 1.f), "sample: topp=%g outside (0, 1]", static_cast<double>(a.topp));
+  VLPK_CHECK_ARG(a.fp32 == 0 || a.fp32 == 1, "sample: fp32=%d (0 bf16, 1 fp32)", a.fp32);
+  VLPK_CHECK_ARG(a.T_cap >= 1 && a.f >= 0 && a.f < a.T_cap, "sample: frame f=%d outside [0, T_cap=%d)", a.f, a.T_cap);
+  VLPK_CHECK_ARG(a.n >= 0 && a.n_ignore >= 0 && (a.n_ignore == 0 || a.ignore), "sample: n=%d, ignore set of %d words", a.n, a.n_ignore);
+  VLPK_CHECK_ARG(a.logits && a.seq && a.finished && a.live, "sample: null pointer (logits, seq, finished, live)");
+  const size_t smem = sample_smem_bytes(a.T_cap, a.V);
+  VLPK_CHECK_ARG(smem <= SAMPLE_SMEM_MAX, "sample: T_cap=%d V=%d need %zu bytes of shared memory (at most %zu)", a.T_cap, a.V, smem,
+                 SAMPLE_SMEM_MAX);
+  if (a.rows == 0) return 0;
+  LaunchScope scope(CAT_MISC, (a.fp32 ? 8.0 : 4.0) * a.rows * a.V, s);
+  if (a.fp32) {
+    static bool attr_set = false;
+    if (!attr_set) {
+      VLPK_CUDA(cudaFuncSetAttribute(sample_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(SAMPLE_SMEM_MAX)));
+      attr_set = true;
+    }
+    sample_kernel<float><<<a.rows, SAMPLE_THREADS, smem, s>>>(a);
+  } else {
+    static bool attr_set = false;
+    if (!attr_set) {
+      VLPK_CUDA(cudaFuncSetAttribute(sample_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(SAMPLE_SMEM_MAX)));
+      attr_set = true;
+    }
+    sample_kernel<bf16><<<a.rows, SAMPLE_THREADS, smem, s>>>(a);
+  }
+  VLPK_CUDA(cudaGetLastError());
+  return 0;
+}
 
 size_t ngram_block_smem_bytes(int T_cap, int V) {
   return (static_cast<size_t>(T_cap) + (static_cast<size_t>(V) + 31) / 32) * 4;

@@ -23,4 +23,34 @@ struct NgramBlockArgs {
 size_t ngram_block_smem_bytes(int T_cap, int V);
 int launch_beam_ngram_block(const NgramBlockArgs& a, cudaStream_t s);
 
+// Top-k / top-p sampling of one decode frame, one CTA per row (see decode.cu).
+enum SampleMode { SAMPLE_TOPK = 0, SAMPLE_TOPP = 1 };
+constexpr int SAMPLE_MAX_TOPK = 64;
+
+struct SampleArgs {
+  int rows = 0, V = 0;
+  const void* logits = nullptr;       // [rows, ld] bf16 or fp32 decoder outputs, without the bias
+  long long ld = 0;
+  const void* bias = nullptr;         // [V] same dtype, or null
+  int fp32 = 0;                       // dtype of logits and bias: 0 bf16, 1 fp32
+  int mode = SAMPLE_TOPK;
+  int topk = 1;                       // 1 <= topk <= SAMPLE_MAX_TOPK
+  float topp = 1.f;                   // 0 < topp <= 1
+  unsigned long long seed = 0;
+  int f = 0;                          // frame: the token goes to seq[row, f], seq[row, :f] is the row's history
+  long long* seq = nullptr;           // [rows, T_cap] int64 word ids
+  int T_cap = 0;
+  float* score = nullptr;             // [rows, T_cap] log-probability of the chosen token, or null
+  int* finished = nullptr;            // [rows] 0 / 1
+  int* live = nullptr;                // [1] rows not finished yet
+  int eos_id = -1, pad_id = 0;
+  int block_eos = 0;                  // 1: frame below min_len, [EOS] is set to -10000
+  int n = 0;                          // duplicate-n-gram blocking: n-gram size, 0 = off
+  const int* ignore = nullptr;
+  int n_ignore = 0;
+};
+
+size_t sample_smem_bytes(int T_cap, int V);
+int launch_sample(const SampleArgs& a, cudaStream_t s);
+
 }  // namespace vlpk

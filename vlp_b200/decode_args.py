@@ -1,0 +1,69 @@
+"""Command-line options of a decode script (the reference's decode_img2txt.py flags) for BertForSeq2SeqDecoder.
+
+    parser = argparse.ArgumentParser()
+    decode_args.add_decode_args(parser)                 # --beam_size ... --forbid_duplicate_ngrams ... --sampling_method --topk --topp --seed
+    args = decode_args.parse_decode_args(parser)        # argparse's usage error (exit 2) for a combination the decoder refuses
+    model = BertForSeq2SeqDecoder.from_pretrained(..., **decode_args.decoder_kwargs(args, tokenizer))
+
+A script that already defines one of these options (decode_img2txt.py has its own --seed, --beam_size, ...) keeps its definition.
+"""
+import argparse
+
+from . import ops
+from .sampling import SAMPLING_METHODS, check_sampling_args
+
+_OPTIONS = (
+    ("--beam_size", dict(type=int, default=1, help="beam size for beam search; 1 = greedy, and required when sampling")),
+    ("--length_penalty", dict(type=float, default=0, help="length penalty for beam search")),
+    ("--forbid_duplicate_ngrams", dict(action="store_true", help="never repeat an n-gram (beam search and sampling)")),
+    ("--forbid_ignore_word", dict(type=str, default=None, help="'|'-separated words exempt from --forbid_duplicate_ngrams")),
+    ("--min_len", dict(type=int, default=None, help="no [SEP] before this many words")),
+    ("--ngram_size", dict(type=int, default=3, help="n of --forbid_duplicate_ngrams")),
+    ("--sampling_method", dict(type=str, default="beam_search", choices=SAMPLING_METHODS,
+                               help="beam_search (greedy at --beam_size 1), or top-k / top-p (nucleus) sampling on the device")),
+    ("--topk", dict(type=int, default=1, help=f"--sampling_method topk: sample from the k most likely words, 1 <= k <= {ops.MAX_TOPK}")),
+    ("--topp", dict(type=float, default=1.0, help="--sampling_method topp: sample from the smallest set of words whose probability "
+                                                  "reaches p, 0 < p <= 1")),
+    ("--seed", dict(type=int, default=123, help="random seed (keys the sampling draws)")),
+)
+
+
+def add_decode_args(parser):
+    """Adds every decode option the parser does not define yet; returns the parser."""
+    for flag, kw in _OPTIONS:
+        try:
+            parser.add_argument(flag, **kw)
+        except argparse.ArgumentError:
+            pass                                               # the script's own definition stays
+    return parser
+
+
+def check_decode_args(args):
+    """ValueError for a combination BertForSeq2SeqDecoder refuses (raised before any model is built)."""
+    check_sampling_args(args.sampling_method, args.topk, args.topp, args.beam_size)
+    if args.forbid_duplicate_ngrams and args.ngram_size < 1:
+        raise ValueError(f"vlp_b200: forbid_duplicate_ngrams needs ngram_size >= 1 (got {args.ngram_size})")
+
+
+def parse_decode_args(parser, argv=None):
+    """parser.parse_args(argv), then check_decode_args: a refused combination is reported as an argparse usage error (exit 2)."""
+    args = parser.parse_args(argv)
+    try:
+        check_decode_args(args)
+    except ValueError as e:
+        parser.error(str(e))
+    return args
+
+
+def decoder_kwargs(args, tokenizer=None):
+    """BertForSeq2SeqDecoder keyword arguments of the parsed options.  tokenizer (convert_tokens_to_ids) maps --forbid_ignore_word
+    to word ids, as decode_img2txt.py does; without one the option must be empty."""
+    check_decode_args(args)
+    ignore = None
+    if args.forbid_ignore_word:
+        if tokenizer is None:
+            raise ValueError("vlp_b200: --forbid_ignore_word needs a tokenizer to map its words to ids")
+        ignore = set(tokenizer.convert_tokens_to_ids(args.forbid_ignore_word.split("|")))
+    return dict(search_beam_size=args.beam_size, length_penalty=args.length_penalty, forbid_duplicate_ngrams=args.forbid_duplicate_ngrams,
+                forbid_ignore_set=ignore, ngram_size=args.ngram_size, min_len=args.min_len or 0, sampling_method=args.sampling_method,
+                topk=args.topk, topp=args.topp, seed=args.seed)

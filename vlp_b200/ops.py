@@ -520,3 +520,45 @@ def beam_ngram_block(hist_in, hist_out, ptr, wid, f, n, ignore, logp):
     n_ign = 0 if ignore is None else ignore.numel()
     L.call("vlpk_beam_ngram_block", rows, K, int(f), T_cap, int(n), hist_in.data_ptr(), hist_out.data_ptr(), ptr.data_ptr(),
            wid.data_ptr(), ignore.data_ptr() if n_ign else None, n_ign, lp.data_ptr(), lp.stride(0), V, L.stream())
+
+
+# ------------------------------------------------------------------------------------------------
+# top-k / top-p sampling
+# ------------------------------------------------------------------------------------------------
+SAMPLE_MODES = {"topk": 0, "topp": 1}
+MAX_TOPK = 64
+
+
+def sample_tokens(logits, bias, mode, topk, topp, seed, f, seq, score, finished, live, eos_id, pad_id=0, block_eos=False, ngram=0,
+                  ignore=None):
+    """One frame of top-k / top-p sampling (vlpk_sample_tokens): for every row of logits ([rows, ..., V], unit stride in V, bf16 or
+    fp32, without the head's bias), adds bias ([V], same dtype, or None), blocks the duplicate n-grams of the row's history
+    seq[row, :f] when ngram > 0 and [EOS] when block_eos, keeps the top-k words or the top-p nucleus and draws one with the
+    Philox uniform keyed by (seed; f, row).  seq: int64 [rows, T] receives column f; score: fp32 [rows, T] or None; finished: int32
+    [rows]; live: int32 [1], decremented once per row that draws eos_id.  ignore: int32 device tensor of exempt word ids, or None."""
+    tensors = ((logits, "logits"), (seq, "sampled ids"), (finished, "finished flags"), (live, "live-row count"))
+    for t, what in tensors + tuple((t, w) for t, w in ((bias, "logit bias"), (score, "scores"), (ignore, "n-gram ignore set"))
+                                   if t is not None):
+        _require_cuda(t, what)
+    if mode not in SAMPLE_MODES:
+        raise ValueError(f"vlp_b200: sampling mode must be one of {sorted(SAMPLE_MODES)}, got {mode!r}")
+    V = logits.shape[-1]
+    lg = logits.reshape(-1, V) if logits.dim() != 2 else logits
+    rows = lg.shape[0]
+    if logits.dtype not in (BF16, torch.float32) or lg.stride(1) != 1:
+        raise RuntimeError("vlp_b200: sampling logits must be bf16 or fp32 [rows, V] with unit column stride")
+    if bias is not None and (bias.dtype != logits.dtype or bias.shape != (V,) or not bias.is_contiguous()):
+        raise RuntimeError("vlp_b200: the logit bias must be a contiguous [V] tensor of the logits' dtype")
+    if seq.dtype != torch.int64 or seq.dim() != 2 or seq.shape[0] != rows or not seq.is_contiguous():
+        raise RuntimeError("vlp_b200: sampled ids must be a contiguous int64 [rows, T] tensor")
+    if score is not None and (score.dtype != torch.float32 or score.shape != seq.shape or not score.is_contiguous()):
+        raise RuntimeError("vlp_b200: sampling scores must be a contiguous fp32 tensor shaped like the ids")
+    if finished.dtype != torch.int32 or finished.shape != (rows,) or live.dtype != torch.int32 or live.numel() != 1:
+        raise RuntimeError("vlp_b200: finished flags must be int32 [rows] and the live-row count an int32 [1] tensor")
+    if ignore is not None and (ignore.dtype != torch.int32 or ignore.dim() != 1 or not ignore.is_contiguous()):
+        raise RuntimeError("vlp_b200: the n-gram ignore set must be a contiguous 1-D int32 tensor of word ids")
+    n_ign = 0 if ignore is None else ignore.numel()
+    L.call("vlpk_sample_tokens", rows, V, lg.data_ptr(), lg.stride(0), L.ptr(bias), int(logits.dtype == torch.float32), SAMPLE_MODES[mode],
+           int(topk), float(topp), int(seed) & 0xFFFFFFFFFFFFFFFF, int(f), seq.data_ptr(), seq.shape[1], L.ptr(score), finished.data_ptr(),
+           live.data_ptr(), int(eos_id), int(pad_id), int(bool(block_eos)), int(ngram), ignore.data_ptr() if n_ign else None, n_ign,
+           L.stream())

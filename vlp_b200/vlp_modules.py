@@ -793,7 +793,8 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
     re-implemented on-device-friendly (floor division fixes the torch>=1.6 breakage noted in SURVEY.md §2 #7)."""
 
     def __init__(self, config, mask_word_id=0, num_labels=2, search_beam_size=1, length_penalty=1.0, eos_id=0, forbid_duplicate_ngrams=False,
-                 forbid_ignore_set=None, ngram_size=3, min_len=0, enable_butd=False, len_vis_input=49):
+                 forbid_ignore_set=None, ngram_size=3, min_len=0, enable_butd=False, len_vis_input=49, sampling_method="beam_search", topk=1,
+                 topp=1.0, seed=0):
         super().__init__(config)
         self.bert = BertModelIncr(config)
         self.cls = BertPreTrainingHeads(config, self.bert.embeddings.word_embeddings.weight, num_labels=num_labels)
@@ -809,6 +810,10 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         self.forbid_ignore_set = forbid_ignore_set
         self.ngram_size = ngram_size
         self.min_len = min_len
+        # "topk" / "topp": stochastic decode on the device (vlp_b200/sampling.py) instead of greedy / beam search; beam size 1
+        from .sampling import check_sampling_args
+        check_sampling_args(sampling_method, topk, topp, search_beam_size)
+        self.sampling_method, self.topk, self.topp, self.seed = sampling_method, topk, topp, seed
         self.use_kv_cache = True     # False: the reference's data flow (K, V of the whole prefix re-projected at every step, modeling.py:273-277)
         self._build_region_projections(config, enable_butd)
 
@@ -817,13 +822,22 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         H = self.config.hidden_size
         return [torch.empty(batch, rows, 2 * H, device=device, dtype=torch.bfloat16) for _ in self.bert.encoder.layer]
 
-    def forward(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, sample_mode="greedy"):
+    def forward(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, sample_mode="greedy",
+                seed=None):
+        """seed: the sampling seed of this call (sampling_method "topk" / "topp"); None uses self.seed."""
         self.cls.predictions.check_task_idx(task_idx)          # before anything is launched
         _check_seq_len(self.config, token_type_ids.size(1))
         from .beam import check_ngram_args
         check_ngram_args(self)
+        sampling = getattr(self, "sampling_method", "beam_search") != "beam_search"
+        if sampling:
+            from .sampling import check_sampling_args
+            check_sampling_args(self.sampling_method, self.topk, self.topp, self.search_beam_size)
         with torch.no_grad():
             vis_feats, vis_pe = self.project_regions(vis_feats, vis_pe)
+            if sampling:
+                from .sampling import sample_decode
+                return sample_decode(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx, seed)
             if self.search_beam_size > 1:
                 from .beam import beam_search
                 return beam_search(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx)
