@@ -105,6 +105,11 @@ class GradientAllReducer:
         if w is not None:
             if self._accumulating:
                 w.wait()                          # the reduced values must be in place before autograd's `p.grad += view`
+            elif arena.dtype != torch.bfloat16:
+                # a group with non-bf16 parameters hands over its fp32 arena, and EncoderStackFn.backward converts the views of the
+                # bf16 parameters right after this hook returns, on the current stream: that conversion must read reduced values,
+                # so the stream waits for the collective here (no overlap for such groups)
+                w.wait()
             else:
                 self._works.append(w)
         if self.reserved_sms > 0:
