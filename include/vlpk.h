@@ -170,12 +170,6 @@ int vlpk_embed_bwd(int B, int L, int H, int R, int vis_input, const int64_t* ids
 int vlpk_embed_tables_bwd(int B, int L, int H, int R, int vis_input, const int64_t* ids, const int64_t* token_type, const int64_t* pos,
                           const void* dz, int V, int P, int T, void* d_word, float* word_scratch, float* d_pos, float* d_type,
                           void* stream);
-/* Data parallelism: add explicit looked-up rows (ids[n], optional pos[n], rows[n,H] bf16 — typically all ranks' rows after an
- * all-gather), scaled by `scale`, INTO an existing bf16 word-table gradient d_word [V,H] and the fp32 position gradient d_pos [P,H]
- * (NULL: skip).  scratch [V,H] fp32 and owner [V] int32 are uninitialised work buffers.  vlpk_embed_tables_bwd with d_word = scratch =
- * d_pos = NULL computes the token-type gradient only. */
-int vlpk_table_rows_add(int64_t n, const int64_t* ids, const int64_t* pos, const void* rows, int H, int V, int P, float scale, void* d_word,
-                        float* scratch, int32_t* owner, float* d_pos, void* stream);
 
 /* y = LayerNorm(dropout(t) + res) (BertSelfOutput / BertOutput tail, modeling.py:315-316, 355-356; eps 1e-5). */
 int vlpk_ln_res_drop_fwd(int64_t M, int H, const void* t, const void* res, const void* gamma, const void* beta, void* y,

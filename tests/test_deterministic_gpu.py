@@ -146,39 +146,6 @@ def test_embedding_backward_is_ordered(B, L_, R, H, V, vis):
     assert float((d_type.double() - ref_t).abs().max()) <= budget
 
 
-def test_table_rows_add_is_ordered():
-    gen = torch.Generator().manual_seed(4)
-    n, H, V, P = 4 * 64 * 23, 768, 28996, 512
-    ids = torch.randint(0, V, (n,), generator=gen)
-    ids[::7] = 101
-    ids[3::11] = 102
-    ids[5::97] = V + 3                                              # out of range: skipped
-    pos = torch.randint(0, 123, (n,), generator=gen)
-    rows = (torch.randn(n, H, generator=gen) * 0.05).bfloat16()
-    base = (torch.randn(V, H, generator=gen) * 0.01).bfloat16()
-    pos0 = torch.randn(P, H, generator=gen) * 0.01
-    ids_d, pos_d, rows_d = ids.to(DEV), pos.to(DEV), rows.to(DEV)
-    scale = 0.25
-
-    def run():
-        d_word, d_pos = base.to(DEV), pos0.to(DEV)
-        scratch = torch.empty(V, H, device=DEV)
-        owner = torch.empty(V, device=DEV, dtype=torch.int32)
-        L.call("vlpk_table_rows_add", n, ids_d.data_ptr(), pos_d.data_ptr(), rows_d.data_ptr(), H, V, P, scale, d_word.data_ptr(),
-               scratch.data_ptr(), owner.data_ptr(), d_pos.data_ptr(), L.stream())
-        return [d_word, d_pos]
-    d_word, d_pos = repeated(run)
-    ok = ids < V
-    add = torch.zeros(V, H, dtype=torch.float64).index_add_(0, ids[ok], rows[ok].double() * scale)
-    ref_w = base.double() + add
-    touched = add.abs().sum(-1) > 0
-    err = (d_word.cpu().double() - ref_w)[touched].abs()
-    assert float((err / (ref_w[touched].abs() + 1e-3)).max()) < 8e-3          # one bf16 rounding of the sum
-    assert torch.equal(d_word.cpu()[~touched], base[~touched])
-    ref_p = pos0.double().index_add_(0, pos, rows.double() * scale)
-    assert float((d_pos.cpu().double() - ref_p).abs().max()) <= 1e-5 * float((rows.double() * scale).abs().sum(0).max() + 1)
-
-
 def test_bertadam_matches_golden_and_is_ordered(golden_dir):
     from oracle import bertadam_oracle as bo
     from vlp_b200 import optimization as opt_mod

@@ -2,14 +2,12 @@
 EncoderStackFn.backward turns into `.grad`.
 
  (1) World 1 over NCCL, in this process (file:// rendezvous, no sockets): a world-1 all-reduce leaves values unchanged, so the real
-     code path — asynchronous works, finish(), reserved SMs, the early decoder-weight reduction — must give every gradient bit for
-     bit as the step without the reducer, in deterministic mode: layer groups [1, 3], [2, 1, 1] and the default, the accumulation
-     branch (a second backward without zero_grad), a model with fp32 LayerNorm parameters (the fp32-arena branch; world 1 checks
-     values only, the ordering against the collective needs N >= 2), and a GraphedStep whose body ends in finish() against the eager
-     reducer step.  The opt-in sparse embedding path (VLP_DP_SPARSE_EMB=1) is held element by element to fp64 sums of the step's
-     decoder dW and looked-up rows.
- (2) Two gloo ranks sharing the GPU: each rank trains on its own shard through the reducer (dense, then sparse) and also computes both
-     shards' gradients without it; every reduced gradient must lie within a per-element bound of the fp64 mean of the two."""
+     code path — asynchronous works, finish(), reserved SMs — must give every gradient bit for bit as the step without the reducer,
+     in deterministic mode: layer groups [1, 3], [2, 1, 1] and the default, the accumulation branch (a second backward without
+     zero_grad), a model with fp32 LayerNorm parameters (the fp32-arena branch; world 1 checks values only, the ordering against the
+     collective needs N >= 2), and a GraphedStep whose body ends in finish() against the eager reducer step.
+ (2) Two gloo ranks sharing the GPU: each rank trains on its own shard through the reducer and also computes both shards'
+     gradients without it; every reduced gradient must lie within a per-element bound of the fp64 mean of the two."""
 import itertools
 import os
 
@@ -30,7 +28,7 @@ from test_parity_gpu import build
 
 pytestmark = pytest.mark.gpu
 D4 = synth.VlpDims(vocab=1000, hidden=128, layers=4, heads=2, inter=512, regions=100, text=20)      # SMALL_L123 with 4 layers
-U8, U24 = 2.0 ** -8, 2.0 ** -24          # unit roundoff of bf16 and fp32
+U8 = 2.0 ** -8                           # unit roundoff of bf16
 
 
 @pytest.fixture(scope="module")
@@ -113,51 +111,6 @@ def test_world1_graphed_reducer_step_equals_eager(nccl_world1):
     red.close()
 
 
-class _RowTap:
-    """Takes the reducer's place on the decoder / embedding hooks of a step without communication: records the decoder's dW and the
-    looked-up rows (the components of the word and position gradients) and leaves the word gradient to the decoder's dW alone."""
-
-    def __init__(self):
-        self.rec = {}
-
-    def on_decoder_weight_grad(self, dw):
-        self.rec["dw"] = dw.detach().clone()
-
-    def wants_embedding_rows(self):
-        return True
-
-    def on_embedding_rows(self, ids, pos, rows, V, P_):
-        self.rec.update(ids=ids.clone(), pos=pos.clone(), rows=rows.clone())
-        return None, torch.zeros(P_, rows.shape[1], device=rows.device)
-
-
-def table_refs(recs, V, P_):
-    """fp64 word / position gradients of the mean over shards from each shard's components, with their per-element error bounds:
-    one bf16 rounding of the result, (world > 1) one of the all-reduced decoder dW, and the fp32 summation of the rows, whose
-    depth is the number of rows that land on the element (+ the prior)."""
-    world = len(recs)
-    H = recs[0]["rows"].shape[1]
-    dev = recs[0]["rows"].device
-    f64 = dict(dtype=torch.float64, device=dev)
-    dw = sum(r["dw"].double() for r in recs) / world
-    dw_mag = sum(r["dw"].double().abs() for r in recs) / world
-    w_rows, w_mag, w_cnt = torch.zeros(V, H, **f64), torch.zeros(V, H, **f64), torch.zeros(V, **f64)
-    p_rows, p_mag, p_cnt = torch.zeros(P_, H, **f64), torch.zeros(P_, H, **f64), torch.zeros(P_, **f64)
-    for r in recs:
-        ok = r["ids"] < V
-        rows = r["rows"].double() / world
-        w_rows.index_add_(0, r["ids"][ok], rows[ok])
-        w_mag.index_add_(0, r["ids"][ok], rows[ok].abs())
-        w_cnt.index_add_(0, r["ids"][ok], torch.ones(int(ok.sum()), **f64))
-        p_rows.index_add_(0, r["pos"], rows)
-        p_mag.index_add_(0, r["pos"], rows.abs())
-        p_cnt.index_add_(0, r["pos"], torch.ones(rows.shape[0], **f64))
-    ref_w = dw + w_rows
-    tol_w = U8 * ref_w.abs() + (2 * U8 * dw_mag if world > 1 else 0.0) + (w_cnt[:, None] + 2) * U24 * (dw_mag + w_mag)
-    tol_p = U8 * p_rows.abs() + (p_cnt[:, None] + 1) * U24 * p_mag
-    return (ref_w, tol_w, w_cnt > 0), (p_rows, tol_p)
-
-
 def check_within(name, got, ref, tol):
     """|got - ref| <= tol elementwise; returns an error string naming the tensor, or None."""
     err = (got.double() - ref).abs()
@@ -167,59 +120,6 @@ def check_within(name, got, ref, tol):
     i = int(torch.argmax((err / (tol + 1e-300)).flatten()))
     return (f"{name}: {int(over.sum())} of {got.numel()} elements out of bound, worst at flat index {i}: got "
             f"{float(got.flatten()[i])}, ref {float(ref.flatten()[i])}, bound {float(tol.flatten()[i])}")
-
-
-def test_world1_sparse_embedding_rows_against_fp64(nccl_world1, monkeypatch):
-    monkeypatch.setattr(ops, "_seed_counter", ops._seed_counter)
-    monkeypatch.setenv("VLP_DP_SPARSE_EMB", "1")
-    model = build(D4, "img2txt", drop=P).train()
-    host = synth.make_batch(D4, 4, seed=9, mode="mix", ragged=True)
-    b = _dev(host)
-    red = GradientAllReducer(model)
-    assert red.sparse_embeddings and red.wants_embedding_rows()
-    rec = {}
-    on_dw, on_rows = red.on_decoder_weight_grad, red.on_embedding_rows
-
-    def tap_dw(dw):
-        rec["dw"] = dw.detach().clone()
-        return on_dw(dw)
-
-    def tap_rows(ids, pos, rows, V, P_):
-        rec.update(ids=ids.clone(), pos=pos.clone(), rows=rows.clone())
-        return on_rows(ids, pos, rows, V, P_)
-    monkeypatch.setattr(red, "on_decoder_weight_grad", tap_dw)
-    monkeypatch.setattr(red, "on_embedding_rows", tap_rows)
-    emb = model.bert.embeddings
-
-    def tap_vis(module, args):         # the region rows' pre-LayerNorm gradient arrives as the gradient of the projected regions
-        args[0].register_hook(lambda g: rec.__setitem__("dvis", g.detach().clone()))
-    h = emb.register_forward_pre_hook(tap_vis)
-    _, got = _run(model, b, make_step("img2txt", after=red.finish))
-    h.remove()
-    lpc = list(model.bert.encoder.layers_per_call)
-    red.close()
-    assert {"dw", "ids", "pos", "rows", "dvis"} <= rec.keys(), rec.keys()
-    V, P_ = emb.word_embeddings.weight.shape[0], emb.position_embeddings.weight.shape[0]
-    (ref_w, tol_w, touched), (ref_p, tol_p) = table_refs([rec], V, P_)
-    W, Pn, T = "bert.embeddings.word_embeddings.weight", "bert.embeddings.position_embeddings.weight", "bert.embeddings.token_type_embeddings.weight"
-    errs = [check_within(W, got[W], ref_w, tol_w), check_within(Pn, got[Pn], ref_p, tol_p)]
-    assert torch.equal(got[W][~touched], rec["dw"][~touched]), f"{W}: rows no sample looked up differ from the decoder's dW"
-    # token types: every row's pre-LayerNorm gradient — the looked-up rows ([CLS], text) and the region rows
-    B, L_, R, H = 4, D4.seq_len, D4.regions, D4.hidden
-    looked = rec["rows"].view(B, L_ - R, H).double()
-    dz = torch.cat((looked[:, :1], rec["dvis"].double().view(B, R, H), looked[:, 1:]), dim=1).view(-1, H)
-    tt = b["segment_ids"].reshape(-1)
-    ref_t = torch.zeros(emb.token_type_embeddings.weight.shape[0], H, dtype=torch.float64, device=dz.device).index_add_(0, tt, dz)
-    mag_t = torch.zeros_like(ref_t).index_add_(0, tt, dz.abs())
-    errs.append(check_within(T, got[T], ref_t, U8 * ref_t.abs() + 1e-5 * mag_t))        # bf16 rounding + the column-sum bound
-    errs = [e for e in errs if e]
-    assert not errs, errs
-    # everything else is the dense path: bit for bit the step without the reducer
-    assert model.bert.embeddings._vlpk_dp_hook is None and model._vlpk_dp_hook is None
-    model.bert.encoder.layers_per_call = lpc
-    plain = _run(model, b, make_step("img2txt"))[1]
-    assert_bitwise("sparse embedding path, non-table gradients", (torch.zeros(1), {k: v for k, v in got.items() if k not in (W, Pn)}),
-                   (torch.zeros(1), {k: v for k, v in plain.items() if k not in (W, Pn)}))
 
 
 # ---- (2) two gloo ranks on one GPU -------------------------------------------------------------------------------------------
@@ -247,43 +147,25 @@ def _gloo_checks(rank, world):
     model = build(D4, "img2txt", drop=P).train()
     step = make_step("img2txt")
     dev = [_dev(synth.make_batch(D4, GLOO_B, seed=900 + s, mode="mix", ragged=True)) for s in range(world)]
-    emb = model.bert.embeddings
-    V, P_ = emb.word_embeddings.weight.shape[0], emb.position_embeddings.weight.shape[0]
-    W, Pn = "bert.embeddings.word_embeddings.weight", "bert.embeddings.position_embeddings.weight"
-    # every shard's gradients without the reducer (same grouping, same dropout streams as the shard's own rank), and the components
-    # of its word / position gradients
+    # every shard's gradients without the reducer (same grouping, same dropout streams as the shard's own rank)
     model.bert.encoder.layers_per_call = list(GROUPS)
-    plain, recs = [], []
-    for s in range(world):
-        plain.append(_run(model, dev[s], step)[1])
-        tap = _RowTap()
-        model._vlpk_dp_hook = emb._vlpk_dp_hook = tap
-        _run(model, dev[s], step)
-        model._vlpk_dp_hook = emb._vlpk_dp_hook = None
-        recs.append(tap.rec)
+    plain = [_run(model, dev[s], step)[1] for s in range(world)]
     mean = {k: sum(p[k].double() for p in plain) / world for k in plain[0]}
+    red = GradientAllReducer(model, layer_groups=GROUPS)
+    red.broadcast_parameters(0)
+    got = _run(model, dev[rank], make_step("img2txt", after=red.finish))[1]
+    red.close()
+    tag = f"rank {rank}"
     errs = []
-    for sparse in (False, True):
-        os.environ["VLP_DP_SPARSE_EMB"] = "1" if sparse else "0"
-        red = GradientAllReducer(model, layer_groups=GROUPS)
-        red.broadcast_parameters(0)
-        got = _run(model, dev[rank], make_step("img2txt", after=red.finish))[1]
-        red.close()
-        tag = f"rank {rank} {'sparse' if sparse else 'dense'}"
-        if got.keys() != mean.keys():
-            errs.append(f"{tag}: gradients of {sorted(got.keys() ^ mean.keys())} on one side only")
-        for k in mean:
-            if sparse and k in (W, Pn):
-                continue
-            # one bf16 rounding of the sum of the two bf16 gradients and one of the quotient
-            errs.append(check_within(f"{tag} {k}", got[k], mean[k], 2 * U8 * mean[k].abs()))
-        if sparse:
-            (ref_w, tol_w, _), (ref_p, tol_p) = table_refs(recs, V, P_)
-            errs += [check_within(f"{tag} {W}", got[W], ref_w, tol_w), check_within(f"{tag} {Pn}", got[Pn], ref_p, tol_p)]
+    if got.keys() != mean.keys():
+        errs.append(f"{tag}: gradients of {sorted(got.keys() ^ mean.keys())} on one side only")
+    for k in mean:
+        # one bf16 rounding of the sum of the two bf16 gradients and one of the quotient
+        errs.append(check_within(f"{tag} {k}", got[k], mean[k], 2 * U8 * mean[k].abs()))
     return [e for e in errs if e]
 
 
-def test_two_gloo_ranks_reduce_to_the_fp64_mean(tmp_path):
+def test_two_gloo_ranks_reduce_every_gradient_to_the_fp64_mean(tmp_path):
     world = 2
     ctx = mp.get_context("spawn")
     q = ctx.Queue()

@@ -281,7 +281,7 @@ def test_embedding_rows(case, det):
 
 
 # ================================================================================================================================
-# Table scatter (vlpk_embed_tables_bwd, vlpk_table_rows_add)
+# Table scatter (vlpk_embed_tables_bwd)
 # ================================================================================================================================
 def _scatter_ref(n_rows, keys, rows, prior=None):
     """fp64 (prior + sum of rows per key, |prior| + sum of |rows| per key) over the keys in [0, n_rows); other keys are skipped."""
@@ -344,48 +344,6 @@ def test_embedding_table_scatter(case, det):
     _note("table sums", kc.check_elementwise(f"{tag} d_pos", d_pos, ref_p, mag_p, 0.0, kc.SUM_REL, where=kc.row_where))
     ref_t, mag_t = _scatter_ref(T, tt.reshape(-1), dz.reshape(-1, H), type0)
     _note("table sums", kc.check_elementwise(f"{tag} d_type", d_type, ref_t, mag_t, 0.0, kc.SUM_REL, where=kc.row_where))
-
-
-@MODES
-@pytest.mark.parametrize("variant", ["pos", "no_pos", "no_d_pos"])
-@pytest.mark.parametrize("n", [1, 7, 9, 300])
-def test_table_rows_add(n, variant, det):
-    H, V, P, scale = 136, 50, 20, 0.5
-    tag = f"table_rows_add n={n} {variant} {'deterministic' if det else 'default'}"
-    gen = _gen(n * 3 + len(variant))
-    ids = torch.randint(0, V, (n,), generator=gen, device=DEV)
-    ids[::4] = 7                                                      # repeated
-    if n > 1:
-        ids[1::5] = V                                                 # out of range: skipped
-        ids[2::6] = -1
-    pos = torch.randint(0, P, (n,), generator=gen, device=DEV)
-    if n > 1:
-        pos[1::3] = P + 2
-    rows = _rn(gen, n, H)
-    base = _rn(gen, V, H, scale=0.1)
-    d_word = kc.guarded(V, H)
-    kc.guard_fill(d_word, base)
-    d_pos = kc.guarded(P, H, dtype=F32)
-    pos0 = torch.randn(P, H, generator=gen, device=DEV)
-    kc.guard_fill(d_pos, pos0)
-    scratch = torch.full((V, H), float("nan"), device=DEV)
-    owner = torch.full((V,), -7, device=DEV, dtype=torch.int32)
-    use_pos = variant != "no_pos"
-    use_dpos = variant != "no_d_pos"
-    call(det, "vlpk_table_rows_add", n, ids.data_ptr(), pos.data_ptr() if use_pos else None, rows.data_ptr(), H, V, P, scale,
-         d_word.data_ptr(), scratch.data_ptr(), owner.data_ptr(), d_pos.data_ptr() if use_dpos else None, L.stream())
-    _intact((f"{tag} d_word", d_word), (f"{tag} d_pos", d_pos))
-    srows = rows.to(F64) * scale
-    ref_w, mag_w = _scatter_ref(V, ids, srows, base)
-    touched = torch.zeros(V, dtype=torch.bool, device=DEV)
-    touched[ids[(ids >= 0) & (ids < V)]] = True
-    assert torch.equal(d_word[~touched].view(torch.int16), base[~touched].view(torch.int16)), f"{tag}: untouched d_word rows changed"
-    _note("table sums", kc.check_elementwise(f"{tag} d_word", d_word[touched], ref_w[touched], mag_w[touched], kc.R_BF16, kc.SUM_REL))
-    if use_pos and use_dpos:
-        ref_p, mag_p = _scatter_ref(P, pos, srows, pos0)
-        _note("table sums", kc.check_elementwise(f"{tag} d_pos", d_pos, ref_p, mag_p, 0.0, kc.SUM_REL, where=kc.row_where))
-    else:
-        assert torch.equal(d_pos, pos0), f"{tag}: d_pos must be untouched"
 
 
 # ================================================================================================================================

@@ -45,34 +45,3 @@ def test_table_grads_match_fp32_autograd(B, L, R, H, V, vis):
         assert float(b.norm()) > 0 and float((a - b).norm() / b.norm()) < 1e-2, name
         untouched = (b.abs().sum(-1) == 0)
         assert float(a[untouched].abs().sum()) == 0.0, name       # rows never looked up get an exactly-zero gradient
-
-
-def test_table_rows_add_matches_index_add():
-    """vlpk_table_rows_add (data-parallel path: all ranks' looked-up rows added into an existing bf16 table gradient): duplicates summed in
-    fp32, scaled, added once per id; position rows into an fp32 table — vs torch index_add_ in fp32."""
-    from vlp_b200 import _lib as L
-    gen = torch.Generator().manual_seed(4)
-    n, H, V, P = 4 * 64 * 23, 768, 28996, 512
-    ids = torch.randint(0, V, (n,), generator=gen)
-    ids[::7] = 101                                               # heavy duplication ([CLS])
-    ids[3::11] = 102
-    pos = torch.randint(0, 123, (n,), generator=gen)
-    rows = (torch.randn(n, H, generator=gen) * 0.05).bfloat16()
-    base = (torch.randn(V, H, generator=gen) * 0.01).bfloat16()
-    d_word = base.clone().cuda()
-    scratch = torch.empty(V, H, device="cuda", dtype=torch.float32)
-    owner = torch.empty(V, device="cuda", dtype=torch.int32)
-    d_pos = torch.zeros(P, H, device="cuda", dtype=torch.float32)
-    scale = 0.25
-    ids_d, pos_d, rows_d = ids.cuda(), pos.cuda(), rows.cuda()
-    L.call("vlpk_table_rows_add", n, ids_d.data_ptr(), pos_d.data_ptr(), rows_d.data_ptr(), H, V, P, scale, d_word.data_ptr(),
-           scratch.data_ptr(), owner.data_ptr(), d_pos.data_ptr(), L.stream())
-    torch.cuda.synchronize()
-    add = torch.zeros(V, H).index_add_(0, ids, rows.float() * scale)
-    want = base.float() + add
-    touched = add.abs().sum(-1) > 0
-    assert torch.equal(d_word.cpu()[~touched], base[~touched])                      # untouched rows are bit-identical
-    err = (d_word.float().cpu()[touched] - want[touched]).abs().max()
-    assert float(err) <= 2 ** -8 * float(want[touched].abs().max()) + 1e-6              # one bf16 rounding of the sum
-    want_pos = torch.zeros(P, H).index_add_(0, pos, rows.float() * scale)
-    assert float((d_pos.cpu() - want_pos).abs().max()) < 1e-4 * float(want_pos.abs().max())

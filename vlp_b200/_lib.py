@@ -71,7 +71,6 @@ _SIGS = {
     "vlpk_embed_bwd": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                C.POINTER(VlpkDropout), c_u64, _P]),
     "vlpk_embed_tables_bwd": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
-    "vlpk_table_rows_add": (c_int, [c_i64, _P, _P, _P, c_int, c_int, c_int, c_float, _P, _P, _P, _P, _P]),
     "vlpk_ln_res_drop_fwd": (c_int, [c_i64, c_int, _P, _P, _P, _P, _P, _P, C.POINTER(VlpkDropout), c_u64, _P]),
     "vlpk_ln_res_drop_bwd": (c_int, [c_i64, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.POINTER(VlpkDropout), c_u64, _P]),
     "vlpk_attn_core_fwd": (c_int, [c_int, c_int, c_int, c_int, _P, c_i64, _P, _P, c_i64, _P, c_int, _P, c_i64, _P,

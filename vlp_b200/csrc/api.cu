@@ -507,18 +507,6 @@ int vlpk_embed_tables_bwd(int B, int L, int H, int R, int vis_input, const int64
   return launch_embed_tables_bwd(a, S(stream));
 }
 
-int vlpk_table_rows_add(int64_t n, const int64_t* ids, const int64_t* pos, const void* rows, int H, int V, int P, float scale, void* d_word,
-                        float* scratch, int32_t* owner, float* d_pos, void* stream) {
-  TableRowsArgs a;
-  a.n = n; a.H = H; a.V = V; a.P = P; a.scale = scale;
-  a.ids = reinterpret_cast<const long long*>(ids);
-  a.pos = reinterpret_cast<const long long*>(pos);
-  a.rows = static_cast<const bf16*>(rows);
-  a.d_word = static_cast<bf16*>(d_word);
-  a.scratch = scratch; a.owner = owner; a.d_pos = d_pos;
-  return launch_table_rows_add(a, S(stream));
-}
-
 int vlpk_ln_res_drop_fwd(int64_t M, int H, const void* t, const void* res, const void* gamma, const void* beta, void* y, float* stats,
                          const VlpkDropout* drop, uint64_t site, void* stream) {
   VLPK_CHECK_ARG(t && gamma && beta && y, "ln_res_drop_fwd: null pointer");

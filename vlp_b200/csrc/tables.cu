@@ -139,60 +139,6 @@ __global__ void __launch_bounds__(256) type_grad_kernel(TableGradArgs a, float* 
   }
 }
 
-// Explicit row lists (data parallelism, vlp_b200/dp.py): the looked-up rows of ALL ranks (all-gathered: 23 rows per sample instead of
-// all-reducing the dense [V,H] table gradient) are added, scaled by 1/world, INTO an existing bf16 word-table gradient — the tied
-// decoder weight's gradient, whose own all-reduce was issued as soon as the head's backward produced it — and into the fp32 position
-// gradient.  Duplicate ids (every [CLS] / [SEP]) are summed in fp32 first; one warp per id (elected through `owner`) does the bf16 update.
-template <int PHASE>
-__global__ void __launch_bounds__(256) table_rows_kernel(TableRowsArgs a) {
-  const long long e = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
-  if (e >= a.n) return;
-  const int lane = threadIdx.x & 31;
-  const long long id = a.ids[e];
-  const bool id_ok = (id >= 0 && id < a.V);
-  const long long p = (a.pos != nullptr) ? a.pos[e] : -1;
-  const bool p_ok = (a.d_pos != nullptr && p >= 0 && p < a.P);
-  bool won = false;
-  if (PHASE == 0) {
-    if (id_ok && lane == 0) a.owner[id] = 0;
-  } else if (PHASE == 2) {
-    int w = 0;
-    if (id_ok && lane == 0) w = (atomicExch(a.owner + id, 1) == 0) ? 1 : 0;
-    won = __shfl_sync(0xffffffffu, w, 0) != 0;
-    if (!won) return;
-  }
-  for (int c = lane * 8; c < a.H; c += 256) {
-    if (PHASE == 0) {
-      if (id_ok) {
-        float* d = a.scratch + id * a.H + c;
-        *reinterpret_cast<float4*>(d) = make_float4(0.f, 0.f, 0.f, 0.f);
-        *reinterpret_cast<float4*>(d + 4) = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    } else if (PHASE == 1) {
-      float v[8];
-      ld8(a.rows + e * a.H + c, v);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] *= a.scale;
-      if (id_ok) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) atomicAdd(a.scratch + id * a.H + c + j, v[j]);
-      }
-      if (p_ok) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) atomicAdd(a.d_pos + p * a.H + c + j, v[j]);
-      }
-    } else {
-      float cur[8];
-      ld8(a.d_word + id * a.H + c, cur);
-      const float* sp = a.scratch + id * a.H + c;
-      const float4 x = *reinterpret_cast<const float4*>(sp), y = *reinterpret_cast<const float4*>(sp + 4);
-      *reinterpret_cast<uint4*>(a.d_word + id * a.H + c) =
-          make_uint4(pack_bf16x2(cur[0] + x.x, cur[1] + x.y), pack_bf16x2(cur[2] + x.z, cur[3] + x.w), pack_bf16x2(cur[4] + y.x, cur[5] + y.y),
-                     pack_bf16x2(cur[6] + y.z, cur[7] + y.w));
-    }
-  }
-}
-
 // ---- deterministic mode: sorted segmented scatter ----------------------------------------------------------------------------
 // Sort inputs: word key, position key and source row of every entry.  Keys outside the table become V resp. P and sort last.
 __global__ void __launch_bounds__(256) table_keys_kernel(TableGradArgs a, long long n, int* __restrict__ wk, int* __restrict__ pk,
@@ -207,24 +153,14 @@ __global__ void __launch_bounds__(256) table_keys_kernel(TableGradArgs a, long l
   rows[e] = static_cast<int>(row);
 }
 
-__global__ void __launch_bounds__(256) rows_keys_kernel(TableRowsArgs a, int* __restrict__ wk, int* __restrict__ pk, int* __restrict__ rows) {
-  const long long e = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (e >= a.n) return;
-  const long long id = a.ids[e];
-  const long long p = (a.pos != nullptr) ? a.pos[e] : -1;
-  wk[e] = (id >= 0 && id < a.V) ? static_cast<int>(id) : a.V;
-  pk[e] = (p >= 0 && p < a.P) ? static_cast<int>(p) : a.P;
-  rows[e] = static_cast<int>(e);
-}
+enum { RUN_WORD_STORE = 0, RUN_F32_ADD = 2 };
 
-enum { RUN_WORD_STORE = 0, RUN_WORD_ADD = 1, RUN_F32_ADD = 2 };
-
-// One warp per sorted position that starts a run of equal keys: sums scale * src[row] over the run in sorted order (= ascending
+// One warp per sorted position that starts a run of equal keys: sums src[row] over the run in sorted order (= ascending
 // row order: the sort is stable and its input was in row order) and updates table row `key` once.
-//   RUN_WORD_STORE: bf16 dst[key] = sum        RUN_WORD_ADD: bf16 dst[key] = dst[key] + sum        RUN_F32_ADD: fp32 dst[key] += each row in turn
+//   RUN_WORD_STORE: bf16 dst[key] = sum        RUN_F32_ADD: fp32 dst[key] += each row in turn
 template <int MODE>
 __global__ void __launch_bounds__(256) sorted_run_sum_kernel(const int* __restrict__ keys, const int* __restrict__ rows, long long n, int n_keys,
-                                                               const __nv_bfloat16* __restrict__ src, int H, float scale, void* dst) {
+                                                               const __nv_bfloat16* __restrict__ src, int H, void* dst) {
   const long long i = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
   if (i >= n) return;
   const int key = keys[i];
@@ -241,19 +177,13 @@ __global__ void __launch_bounds__(256) sorted_run_sum_kernel(const int* __restri
       float v[8];
       ld8(src + static_cast<long long>(rows[r]) * H + c, v);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) acc[j] += v[j] * scale;
+      for (int j = 0; j < 8; ++j) acc[j] += v[j];
     }
     if (MODE == RUN_F32_ADD) {
 #pragma unroll
       for (int j = 0; j < 8; ++j) d32[j] = acc[j];
     } else {
       __nv_bfloat16* d16 = static_cast<__nv_bfloat16*>(dst) + static_cast<long long>(key) * H + c;
-      if (MODE == RUN_WORD_ADD) {
-        float cur[8];
-        ld8(d16, cur);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[j] += cur[j];
-      }
       *reinterpret_cast<uint4*>(d16) =
           make_uint4(pack_bf16x2(acc[0], acc[1]), pack_bf16x2(acc[2], acc[3]), pack_bf16x2(acc[4], acc[5]), pack_bf16x2(acc[6], acc[7]));
     }
@@ -291,88 +221,47 @@ int sort_bufs(long long n, int V, int P, cudaStream_t s, SortBufs* b) {
   return 0;
 }
 
-// Sort by word key (and by position key when d_pos is given) and apply the runs.
-int sorted_scatter(const SortBufs& b, long long n, int H, int V, int P, const __nv_bfloat16* src, float scale, __nv_bfloat16* d_word,
-                   bool word_add, float* d_pos, cudaStream_t s) {
+// Sort by word key and by position key and apply the runs.
+int sorted_scatter(const SortBufs& b, long long n, int H, int V, int P, const __nv_bfloat16* src, __nv_bfloat16* d_word, float* d_pos,
+                   cudaStream_t s) {
   size_t tb = b.temp_bytes;
   VLPK_CUDA(cub::DeviceRadixSort::SortPairs(b.temp, tb, b.wk, b.wk_s, b.rows, b.wrow_s, static_cast<int>(n), 0, key_bits(V), s));
   const unsigned grid = static_cast<unsigned>((n + 7) / 8);
   {
     LaunchScope scope(CAT_EMBED, 0.0, s);
-    if (word_add)
-      sorted_run_sum_kernel<RUN_WORD_ADD><<<grid, 256, 0, s>>>(b.wk_s, b.wrow_s, n, V, src, H, scale, d_word);
-    else
-      sorted_run_sum_kernel<RUN_WORD_STORE><<<grid, 256, 0, s>>>(b.wk_s, b.wrow_s, n, V, src, H, scale, d_word);
+    sorted_run_sum_kernel<RUN_WORD_STORE><<<grid, 256, 0, s>>>(b.wk_s, b.wrow_s, n, V, src, H, d_word);
     VLPK_CUDA(cudaGetLastError());
   }
-  if (d_pos == nullptr) return 0;
   tb = b.temp_bytes;
   VLPK_CUDA(cub::DeviceRadixSort::SortPairs(b.temp, tb, b.pk, b.pk_s, b.rows, b.prow_s, static_cast<int>(n), 0, key_bits(P), s));
   LaunchScope scope(CAT_EMBED, 0.0, s);
-  sorted_run_sum_kernel<RUN_F32_ADD><<<grid, 256, 0, s>>>(b.pk_s, b.prow_s, n, P, src, H, scale, d_pos);
+  sorted_run_sum_kernel<RUN_F32_ADD><<<grid, 256, 0, s>>>(b.pk_s, b.prow_s, n, P, src, H, d_pos);
   VLPK_CUDA(cudaGetLastError());
   return 0;
 }
 
 }  // namespace
 
-int launch_table_rows_add(const TableRowsArgs& a, cudaStream_t s) {
-  VLPK_CHECK_ARG(a.n > 0 && a.H > 0 && a.H % 8 == 0 && a.V > 0, "table_rows_add: n=%lld H=%d V=%d", a.n, a.H, a.V);
-  VLPK_CHECK_ARG(a.ids && a.rows && a.d_word && a.scratch && a.owner, "table_rows_add: null pointer");
-  VLPK_CHECK_ARG(((reinterpret_cast<uintptr_t>(a.rows) | reinterpret_cast<uintptr_t>(a.d_word) | reinterpret_cast<uintptr_t>(a.scratch)) & 15u) == 0,
-                 "table_rows_add: rows / d_word / scratch must be 16-byte aligned");
-  if (deterministic()) {
-    SortBufs b;
-    VLPK_TRY(sort_bufs(a.n, a.V, a.P, s, &b));
-    {
-      LaunchScope scope(CAT_EMBED, 0.0, s);
-      rows_keys_kernel<<<static_cast<unsigned>((a.n + 255) / 256), 256, 0, s>>>(a, b.wk, b.pk, b.rows);
-      VLPK_CUDA(cudaGetLastError());
-    }
-    return sorted_scatter(b, a.n, a.H, a.V, a.P, a.rows, a.scale, a.d_word, true, a.d_pos, s);
-  }
-  const unsigned grid = static_cast<unsigned>((a.n + 7) / 8);
-  {
-    LaunchScope scope(CAT_EMBED, 0.0, s);
-    table_rows_kernel<0><<<grid, 256, 0, s>>>(a);
-    VLPK_CUDA(cudaGetLastError());
-  }
-  {
-    LaunchScope scope(CAT_EMBED, 0.0, s);
-    table_rows_kernel<1><<<grid, 256, 0, s>>>(a);
-    VLPK_CUDA(cudaGetLastError());
-  }
-  LaunchScope scope(CAT_EMBED, 0.0, s);
-  table_rows_kernel<2><<<grid, 256, 0, s>>>(a);
-  VLPK_CUDA(cudaGetLastError());
-  return 0;
-}
-
 int launch_embed_tables_bwd(const TableGradArgs& a, cudaStream_t s) {
   VLPK_CHECK_ARG(a.B > 0 && a.L > 0 && a.H > 0 && a.H % 8 == 0, "embed_tables_bwd: B=%d L=%d H=%d (H must be a multiple of 8)", a.B, a.L, a.H);
   VLPK_CHECK_ARG(a.V > 0 && a.P > 0 && a.T > 0 && a.T <= TT_MAX, "embed_tables_bwd: V=%d P=%d T=%d (at most %d token types)", a.V, a.P, a.T, TT_MAX);
   VLPK_CHECK_ARG(!a.vis_input || (a.R > 0 && a.R < a.L), "embed_tables_bwd: R=%d regions do not fit L=%d", a.R, a.L);
-  const bool type_only = (a.d_word == nullptr && a.scratch == nullptr && a.d_pos == nullptr);   // word / position rows handled elsewhere
-  VLPK_CHECK_ARG(a.ids && a.dz && a.d_type && (type_only || (a.d_word && a.scratch && a.d_pos)), "embed_tables_bwd: null pointer");
+  VLPK_CHECK_ARG(a.ids && a.dz && a.d_type && a.d_word && a.scratch && a.d_pos, "embed_tables_bwd: null pointer");
   VLPK_CHECK_ARG(((reinterpret_cast<uintptr_t>(a.dz) | reinterpret_cast<uintptr_t>(a.d_word) | reinterpret_cast<uintptr_t>(a.scratch)) & 15u) == 0,
                  "embed_tables_bwd: dz / d_word / scratch must be 16-byte aligned");
   const long long M = static_cast<long long>(a.B) * a.L;
   const long long n_entries = static_cast<long long>(a.B) * (a.vis_input ? a.L - a.R : a.L);
   const unsigned grid = static_cast<unsigned>((n_entries + 7) / 8);
-  if (!type_only) {
-    VLPK_CUDA(cudaMemsetAsync(a.d_word, 0, static_cast<size_t>(a.V) * a.H * 2, s));
-  }
+  VLPK_CUDA(cudaMemsetAsync(a.d_word, 0, static_cast<size_t>(a.V) * a.H * 2, s));
   if (deterministic()) {
-    if (!type_only) {
-      SortBufs b;
-      VLPK_TRY(sort_bufs(n_entries, a.V, a.P, s, &b));
-      {
-        LaunchScope scope(CAT_EMBED, 0.0, s);
-        table_keys_kernel<<<static_cast<unsigned>((n_entries + 255) / 256), 256, 0, s>>>(a, n_entries, b.wk, b.pk, b.rows);
-        VLPK_CUDA(cudaGetLastError());
-      }
-      VLPK_TRY(sorted_scatter(b, n_entries, a.H, a.V, a.P, a.dz, 1.f, a.d_word, false, a.d_pos, s));
+    SortBufs b;
+    VLPK_TRY(sort_bufs(n_entries, a.V, a.P, s, &b));
+    {
+      LaunchScope scope(CAT_EMBED, 0.0, s);
+      table_keys_kernel<<<static_cast<unsigned>((n_entries + 255) / 256), 256, 0, s>>>(a, n_entries, b.wk, b.pk, b.rows);
+      VLPK_CUDA(cudaGetLastError());
     }
+    VLPK_TRY(sorted_scatter(b, n_entries, a.H, a.V, a.P, a.dz, a.d_word, a.d_pos, s));
     const unsigned slabs = static_cast<unsigned>((M + SLAB - 1) / SLAB);
     float* part = scratch_f32(SCRATCH_ORDERED, static_cast<size_t>(slabs) * a.T * a.H, s);
     if (part == nullptr) return -1;
@@ -383,17 +272,17 @@ int launch_embed_tables_bwd(const TableGradArgs& a, cudaStream_t s) {
     }
     return launch_sum_parts(part, static_cast<int>(slabs), static_cast<long long>(a.T) * a.H, a.d_type, s);
   }
-  if (!type_only) {
+  {
     LaunchScope scope(CAT_EMBED, 0.0, s);
     word_pos_kernel<0><<<grid, 256, 0, s>>>(a, n_entries);
     VLPK_CUDA(cudaGetLastError());
   }
-  if (!type_only) {
+  {
     LaunchScope scope(CAT_EMBED, 0.0, s);
     word_pos_kernel<1><<<grid, 256, 0, s>>>(a, n_entries);
     VLPK_CUDA(cudaGetLastError());
   }
-  if (!type_only) {
+  {
     LaunchScope scope(CAT_EMBED, 2.0 * a.V * a.H, s);
     word_pos_kernel<2><<<grid, 256, 0, s>>>(a, n_entries);
     VLPK_CUDA(cudaGetLastError());

@@ -17,20 +17,6 @@ struct TableGradArgs {
   float* d_type = nullptr;            // [T,H] fp32, zeroed by the caller
 };
 
-int launch_embed_tables_bwd(const TableGradArgs& a, cudaStream_t s);   // d_word = scratch = d_pos = null: token-type gradient only
-
-struct TableRowsArgs {
-  long long n = 0;                    // entries
-  const long long* ids = nullptr;     // [n] word ids
-  const long long* pos = nullptr;     // [n] position ids (may be null)
-  const __nv_bfloat16* rows = nullptr;  // [n,H] pre-LayerNorm gradient rows
-  int H = 0, V = 0, P = 0;
-  float scale = 1.f;
-  __nv_bfloat16* d_word = nullptr;    // [V,H] bf16, += (in place)
-  float* scratch = nullptr;           // [V,H] fp32, uninitialised
-  int* owner = nullptr;               // [V] int32, uninitialised
-  float* d_pos = nullptr;             // [P,H] fp32, += (may be null)
-};
-int launch_table_rows_add(const TableRowsArgs& a, cudaStream_t s);
+int launch_embed_tables_bwd(const TableGradArgs& a, cudaStream_t s);
 
 }  // namespace vlpk

@@ -338,7 +338,7 @@ class EmbedFn(torch.autograd.Function):
     """BertEmbeddings.forward (modeling.py:217-241)."""
 
     @staticmethod
-    def forward(ctx, vis, vpe, word_w, pos_w, type_w, ln_g, ln_b, ids, tt, pos, vis_input, R, p, training, dp_hook=None):
+    def forward(ctx, vis, vpe, word_w, pos_w, type_w, ln_g, ln_b, ids, tt, pos, vis_input, R, p, training):
         _require_cuda(ids, "input_ids")
         B, Lq = ids.shape
         H = word_w.shape[1]
@@ -355,7 +355,6 @@ class EmbedFn(torch.autograd.Function):
                tabs[2].data_ptr(), L.ptr(visc), L.ptr(vpec), tabs[3].data_ptr(), tabs[4].data_ptr(), y.data_ptr(), stats.data_ptr(), drop, 1 << 20,
                L.stream())
         ctx.saved = (visc, vpec, tabs, ids, tt, pos, stats)
-        ctx.dp_hook = dp_hook
         ctx.meta = (vis_input, R, p if seed is not None else 0.0, seed, [t.dtype for t in (vis, vpe, word_w, pos_w, type_w, ln_g, ln_b)] if vis_input
                     else [None, None] + [t.dtype for t in (word_w, pos_w, type_w, ln_g, ln_b)])
         return y
@@ -379,26 +378,6 @@ class EmbedFn(torch.autograd.Function):
         # pre-LN gradient -> tables: region rows feed the projections, the B x (L - R) looked-up rows are scattered by
         # vlpk_embed_tables_bwd (csrc/tables.cu: touched-rows-only word/position scatter, segmented token-type sums)
         V, P, T = tabs[0].shape[0], tabs[1].shape[0], tabs[2].shape[0]
-        hook = ctx.dp_hook
-        if hook is not None and hook.wants_embedding_rows():
-            # data parallelism: hand the looked-up rows (23 per sample) to the reducer, which all-gathers them and adds every rank's rows
-            # to the word / position gradients itself — instead of all-reducing two dense tables after backward (vlp_b200/dp.py)
-            if vis_input:
-                keep = torch.cat((torch.zeros(1, dtype=torch.long, device=dev), torch.arange(R + 1, Lq, device=dev)))
-                rows = dz[:, keep].reshape(-1, H)
-                ids_tab = ids[:, keep].reshape(-1)
-                pos_tab = (pos[:, keep] if pos is not None else keep.unsqueeze(0).expand(B, -1)).reshape(-1)
-            else:
-                rows, ids_tab = dz.reshape(-1, H), ids.reshape(-1)
-                pos_tab = (pos if pos is not None else torch.arange(Lq, device=dev).unsqueeze(0).expand(B, -1)).reshape(-1)
-            d_word, d_pos = hook.on_embedding_rows(ids_tab.contiguous(), pos_tab.contiguous(), rows.contiguous(), V, P)
-            d_type = torch.zeros(T, H, device=dev, dtype=torch.float32)
-            L.call("vlpk_embed_tables_bwd", B, Lq, H, R, 1 if vis_input else 0, ids.data_ptr(), L.ptr(tt), L.ptr(pos), dz.data_ptr(), V, P, T,
-                   None, None, None, d_type.data_ptr(), L.stream())
-            out = [None if d_vis is None else d_vis.to(dts[0]), None if d_vis is None else d_vis.to(dts[1]),
-                   None if d_word is None else d_word.to(dts[2]), None if d_pos is None else d_pos.to(dts[3]), d_type.to(dts[4]), dg.to(dts[5]),
-                   db.to(dts[6])]
-            return tuple(out) + (None,) * 8
         d_word = torch.empty(V, H, device=dev, dtype=BF16)
         scratch = torch.empty(V, H, device=dev, dtype=torch.float32)
         d_pos = torch.zeros(P, H, device=dev, dtype=torch.float32)
@@ -407,7 +386,7 @@ class EmbedFn(torch.autograd.Function):
                d_word.data_ptr(), scratch.data_ptr(), d_pos.data_ptr(), d_type.data_ptr(), L.stream())
         out = [None if d_vis is None else d_vis.to(dts[0]), None if d_vis is None else d_vis.to(dts[1]), d_word.to(dts[2]), d_pos.to(dts[3]),
                d_type.to(dts[4]), dg.to(dts[5]), db.to(dts[6])]
-        return tuple(out) + (None,) * 8
+        return tuple(out) + (None,) * 7
 
 
 # ------------------------------------------------------------------------------------------------
@@ -422,9 +401,8 @@ class DecoderCEFn(torch.autograd.Function):
     (vlpk_decoder_ce_ls_fwd/bwd).  0 keeps the cross-entropy calls."""
 
     @staticmethod
-    def forward(ctx, h, w, bias, labels, dp_hook=None, label_smoothing=0.0):
+    def forward(ctx, h, w, bias, labels, label_smoothing=0.0):
         _require_cuda(h, "decoder input")
-        ctx.dp_hook = dp_hook
         eps = float(label_smoothing)
         ctx.eps = eps
         R, H = h.shape
@@ -468,10 +446,7 @@ class DecoderCEFn(torch.autograd.Function):
         else:
             L.call("vlpk_decoder_ce_bwd", R, V, H, hc.data_ptr(), wc.data_ptr(), labels.data_ptr(), logits.data_ptr(), lse.data_ptr(),
                    dl.data_ptr(), dlogits.data_ptr(), dh.data_ptr(), dw.data_ptr(), dbias.data_ptr(), L.stream())
-        dwp = dw.to(wdt)
-        if ctx.dp_hook is not None:
-            ctx.dp_hook.on_decoder_weight_grad(dwp)      # data parallelism: this (tied) gradient is complete FIRST — reduce it now
-        return dh.to(hdt), dwp, dbias[:V].to(bdt), None, None, None
+        return dh.to(hdt), dw.to(wdt), dbias[:V].to(bdt), None, None
 
 
 def layer_cached_fwd(hidden, kv_cache, pos, mask_bits, heads, I, params):

@@ -144,7 +144,6 @@ class BertEmbeddings(nn.Module):
         self.fp32_embedding = getattr(config, "fp32_embedding", False)
         self.LayerNorm = BertLayerNorm(config.hidden_size, eps=1e-5)
         self.dropout = nn.Dropout(config.hidden_dropout_prob)
-        self._vlpk_dp_hook = None      # data parallelism (vlp_b200/dp.py): receives the looked-up rows' gradients in backward
 
     def forward(self, vis_feats, vis_pe, input_ids, token_type_ids=None, position_ids=None, vis_input=True, len_vis_input=49):
         if vis_input and input_ids.size(1) < len_vis_input + 1:
@@ -152,7 +151,7 @@ class BertEmbeddings(nn.Module):
         return ops.EmbedFn.apply(vis_feats if vis_input else None, vis_pe if vis_input else None, self.word_embeddings.weight,
                                  self.position_embeddings.weight, self.token_type_embeddings.weight, self.LayerNorm.weight, self.LayerNorm.bias,
                                  input_ids, token_type_ids, position_ids, bool(vis_input), int(len_vis_input), float(self.dropout.p),
-                                 self.training, self._vlpk_dp_hook)
+                                 self.training)
 
 
 class BertSelfAttention(nn.Module):
@@ -697,7 +696,6 @@ class BertForPreTrainingLossMask(PreTrainedBertModel, _RegionProjections):
         # vlpk_decoder_ce_ls_fwd/bwd.  False selects the torch evaluation of the same ops, kept only as the comparison arm of
         # tests/test_fused_head_gpu.py and tests/test_label_smoothing_gpu.py.
         self.fused_mlm_head = os.environ.get("VLP_FUSED_HEAD", "1") != "0"
-        self._vlpk_dp_hook = None      # data parallelism (vlp_b200/dp.py): receives the tied decoder weight's gradient as soon as it exists
         if tasks == "vqa2":
             self.ans_classifier = nn.Sequential(nn.Linear(config.hidden_size, config.hidden_size * 2), nn.ReLU(),
                                                 nn.Linear(config.hidden_size * 2, 3129))
@@ -753,7 +751,7 @@ class BertForPreTrainingLossMask(PreTrainedBertModel, _RegionProjections):
                 hid = pred.select_task(pred.transform(gathered.to(pred.decoder.weight.dtype)), task_idx)
                 eps = self.crit_mask_lm_smoothed.label_smoothing if self.crit_mask_lm_smoothed is not None else 0.0
                 loss_flat, scores = ops.DecoderCEFn.apply(hid.reshape(-1, hid.size(-1)), pred.decoder.weight, pred.bias,
-                                                          masked_lm_labels.reshape(-1), self._vlpk_dp_hook, eps)
+                                                          masked_lm_labels.reshape(-1), eps)
                 self.last_prediction_scores = scores.view(*masked_lm_labels.shape, -1)
                 masked_lm_loss = loss_flat.view_as(masked_lm_labels)
             else:
