@@ -194,6 +194,24 @@ int vlpk_attn_core_bwd_wide(int B, int heads, int L, const void* q, const void* 
                             const uint32_t* mask_bits, int mask_rows, const void* ctx, const void* dctx, int64_t ld_ctx, const float* lse,
                             void* dq, void* dk, void* dv, int64_t ld_dqkv, const VlpkDropout* drop, uint64_t site, int kv_slots,
                             void* stream);
+/* Attention probabilities of one layer (opt-in: the forward kernels never store them).  Recomputed from the layer's bf16 q, k and the
+ * logsumexp its forward attention saved (VlpkLayerActs.lse):
+ *   P[b, h, i - row0, j] = exp(s_ij - lse[b, h, i]),  s_ij = q_i . k_j / 8 + (mask bit (i, j) ? 0 : -10000)   (fp32)
+ * for query rows i in [row0, Lq) and keys j in [0, Lkv): the reference's attention_probs before dropout (modeling.py:283-295); a
+ * fully masked row is the softmax of the unmasked scores (every score is shifted by the same -10000), never zero or NaN.
+ *   q: Lq rows per sequence, ld_q elements apart, sequences q_bstride apart (0: Lq * ld_q); head h at columns [64 h, 64 h + 64).
+ *      In place in VlpkLayerActs.qkv (ld 3H; decode layouts: ld H).
+ *   k: Lkv rows, ld_k apart, sequences k_bstride apart (0: Lkv * ld_k): qkv + H (ld 3H), VlpkLayerActs.kv (ld 2H) or a K/V cache
+ *      [B, rows, 2H] (ld 2H, k_bstride = rows * 2H).
+ *   mask_bits / mask_rows (1 or Lq) / kv_slots: as for vlpk_attn_core_fwd_wide.  lse: [B, heads, Lq].
+ *   p: fp32, [Lq - row0, ld_p] per (sequence, head), heads (Lq - row0) * ld_p floats apart, sequences p_bstride apart (0: heads *
+ *      (Lq - row0) * ld_p).  Columns [Lkv, ld_p) are not written.
+ * One launch, no allocation, no host synchronisation.  < 0 without launching for: Lq, Lkv or kv_slots outside the attention kernels'
+ * range (Lkv <= 512), mask_rows neither 1 nor Lq, row0 outside [0, Lq), ld_p < Lkv, p_bstride below one sequence's block, a NULL
+ * pointer, or q / k pointers and strides that are not multiples of 16 bytes (TMA). */
+int vlpk_attn_probs(int B, int heads, int Lq, int Lkv, int row0, const void* q, int64_t ld_q, int64_t q_bstride, const void* k, int64_t ld_k,
+                    int64_t k_bstride, const uint32_t* mask_bits, int mask_rows, int kv_slots, const float* lse, float* p, int64_t ld_p,
+                    int64_t p_bstride, void* stream);
 
 /* BertAttention.forward (modeling.py:326-330): QKV projection + attention core + output projection + LN.
  * x_kv == NULL or == x: self-attention over x (training / encoder path).

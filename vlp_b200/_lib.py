@@ -81,6 +81,8 @@ _SIGS = {
                                         C.POINTER(VlpkDropout), c_u64, c_int, _P]),
     "vlpk_attn_core_bwd_wide": (c_int, [c_int, c_int, c_int, _P, _P, _P, c_i64, _P, c_int, _P, _P, c_i64, _P, _P, _P, _P, c_i64,
                                         C.POINTER(VlpkDropout), c_u64, c_int, _P]),
+    "vlpk_attn_probs": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, c_i64, c_i64, _P, c_i64, c_i64, _P, c_int, c_int, _P, _P, c_i64,
+                                c_i64, _P]),
     "vlpk_mha_fwd": (c_int, [C.POINTER(VlpkShape), C.POINTER(VlpkLayerWeights), _P, _P, _P, c_int, C.POINTER(VlpkLayerActs),
                              c_float, c_float, C.POINTER(VlpkDropout), c_u64, _P]),
     "vlpk_ffn_fwd": (c_int, [C.POINTER(VlpkShape), C.POINTER(VlpkLayerWeights), C.POINTER(VlpkLayerActs), c_float,

@@ -64,7 +64,9 @@ def check_ngram_args(dec):
         raise ValueError(f"vlp_b200: forbid_duplicate_ngrams needs ngram_size >= 1 (got {dec.ngram_size})")
 
 
-def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None):
+def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, output_attentions=False):
+    """output_attentions: out["attentions"] [B, out_len - in_len, layers, heads, out_len] holds, for frame t of pred_seq, the [MASK]-row
+    maps of step t taken from the row its hypothesis continued (beam_maps)."""
     K = dec.search_beam_size
     B, in_len = input_ids.shape
     out_len = token_type_ids.shape[1]
@@ -78,20 +80,28 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
         check_ngram_args(dec)
         ngram, ignore = int(dec.ngram_size), _ignore_tensor(dec, dev)
         hist = [torch.empty(B * K, out_len - in_len, dtype=torch.int32, device=dev) for _ in range(2)]    # word histories, in turn
+    # per step t, the [MASK]-row maps of its B*K input rows (step 0: B rows, written at rows b*K)
+    maps = dec.new_attention_maps(out_len - in_len, B * K, out_len, dev) if output_attentions else None
     next_pos = in_len
     while next_pos < out_len:
         cl = curr_ids.shape[1]
         st = next_pos - cl
         x_ids = torch.cat((curr_ids, mask_ids), dim=1)
+        extra = {}
+        if maps is not None:
+            buf = maps[next_pos - in_len]
+            buf = buf.view(B, K, *buf.shape[1:])[:, 0] if next_pos == in_len else buf
+            extra["output_attentions"] = dec.step_maps(buf, cl, next_pos + 1)
         if caches is not None:
-            new_emb, last, _ = dec.bert(vis_feats, vis_pe, x_ids, token_type_ids[:, st:next_pos + 1], position_ids[:, st:next_pos + 1],
-                                        attention_mask[:, st:next_pos + 1, :next_pos + 1], output_all_encoded_layers=False,
-                                        len_vis_input=dec.len_vis_input, kv_caches=caches, cache_pos=st)
+            new_emb, last = dec.bert(vis_feats, vis_pe, x_ids, token_type_ids[:, st:next_pos + 1], position_ids[:, st:next_pos + 1],
+                                     attention_mask[:, st:next_pos + 1, :next_pos + 1], output_all_encoded_layers=False,
+                                     len_vis_input=dec.len_vis_input, kv_caches=caches, cache_pos=st, **extra)[:2]
             new_layers = [last]
         else:
-            new_emb, new_layers, _ = dec.bert(vis_feats, vis_pe, x_ids, token_type_ids[:, st:next_pos + 1], position_ids[:, st:next_pos + 1],
-                                              attention_mask[:, st:next_pos + 1, :next_pos + 1], prev_embedding=prev_emb,
-                                              prev_encoded_layers=prev_layers, output_all_encoded_layers=True, len_vis_input=dec.len_vis_input)
+            new_emb, new_layers = dec.bert(vis_feats, vis_pe, x_ids, token_type_ids[:, st:next_pos + 1], position_ids[:, st:next_pos + 1],
+                                           attention_mask[:, st:next_pos + 1, :next_pos + 1], prev_embedding=prev_emb,
+                                           prev_encoded_layers=prev_layers, output_all_encoded_layers=True, len_vis_input=dec.len_vis_input,
+                                           **extra)[:2]
         scores, _ = dec.cls(new_layers[-1][:, -1:, :], None, task_idx=task_idx)
         logp = F.log_softmax(scores.float(), dim=-1)                      # [B or B*K, 1, V]
         frame = next_pos - in_len
@@ -134,7 +144,10 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
         curr_ids = k_ids.reshape(B * K, 1)
         next_pos += 1
 
-    out = {"pred_seq": backtrack(torch.stack(total_scores), torch.stack(step_ids), torch.stack(step_ptrs), dec.eos_id, dec.length_penalty, out_len)}
+    sc, wi, pt = torch.stack(total_scores), torch.stack(step_ids), torch.stack(step_ptrs)
+    out = {"pred_seq": backtrack(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len)}
+    if maps is not None:
+        out["attentions"] = beam_maps(maps, *best_path(sc, wi, pt, dec.eos_id, dec.length_penalty), pt)
     T = len(total_scores)
     for k, t in (("scores", torch.stack(total_scores)), ("wids", torch.stack(step_ids)), ("ptrs", torch.stack(step_ptrs))):
         padded = t.new_zeros((B, out_len, K))
@@ -149,6 +162,28 @@ def backtrack(sc, wi, pt, eos_id, length_penalty, out_len):
       candidate = (word is [EOS], or frame == last[b]) within frames <= last[b]; score + length_penalty * (frame + 1); FIRST maximum wins
     sc [T,B,K] float scores, wi [T,B,K] word ids, pt [T,B,K] back pointers -> pred_seq [B, out_len] (zero padded)."""
     T, B, K = sc.shape
+    active, pos = best_path(sc, wi, pt, eos_id, length_penalty)
+    pred = torch.zeros(B, out_len, dtype=torch.long, device=sc.device)
+    tok = wi.gather(2, pos.unsqueeze(-1)).squeeze(-1)                    # [T,B]
+    pred[:, :T] = torch.where(active, tok, torch.zeros_like(tok)).t()
+    return pred
+
+
+def beam_maps(maps, active, pos, pt):
+    """Attention maps of the chosen hypotheses: frame t of sample b takes row b*K + pt[t, b, pos[t, b]] of step t — the hypothesis
+    that the frame-t word continued, whose [MASK] row predicted it.  maps [T, B*K, ...] per-step maps, active / pos [T,B] of
+    best_path, pt [T,B,K] back pointers -> [B, T, ...], zero at frames past the hypothesis' end."""
+    T, B, K = pt.shape
+    rows = pt.gather(2, pos.unsqueeze(-1)).squeeze(-1) + torch.arange(B, device=pt.device) * K        # [T,B]
+    got = maps[torch.arange(T, device=pt.device).unsqueeze(1), rows]                                  # [T,B,...]
+    keep = active.view(T, B, *([1] * (got.dim() - 2)))
+    return torch.where(keep, got, torch.zeros_like(got)).transpose(0, 1)
+
+
+def best_path(sc, wi, pt, eos_id, length_penalty):
+    """The hypothesis backtrack() selects, frame by frame: (active [T,B] — frame t belongs to it —, pos [T,B] — its beam index at
+    frame t)."""
+    T, B, K = sc.shape
     dev = sc.device
     frames = torch.arange(T, device=dev).view(T, 1)
     all_eos = (wi == eos_id).all(-1)                                      # [T,B]
@@ -159,11 +194,10 @@ def backtrack(sc, wi, pt, eos_id, length_penalty, out_len):
     best = flat.argmax(-1)                                                # first maximal value
     frame, pos = torch.div(best, K, rounding_mode="floor"), best % K
     found = torch.isfinite(flat.gather(1, best.unsqueeze(1)).squeeze(1))
-    pred = torch.zeros(B, out_len, dtype=torch.long, device=dev)
     bidx = torch.arange(B, device=dev)
+    actives, poss = [None] * T, [None] * T
     for fid in range(T - 1, -1, -1):                                      # walk the back pointers from `frame` down to 0
         active = found & (fid <= frame)
-        tok = wi[fid, bidx, pos]
-        pred[:, fid] = torch.where(active, tok, pred[:, fid])
+        actives[fid], poss[fid] = active, pos
         pos = torch.where(active & (fid > 0), pt[fid, bidx, pos], pos)
-    return pred
+    return torch.stack(actives), torch.stack(poss)

@@ -554,6 +554,18 @@ int vlpk_attn_core_fwd(int B, int heads, int Lq, int Lkv, const void* q, int64_t
   return vlpk_attn_core_fwd_wide(B, heads, Lq, Lkv, q, ld_q, k, v, ld_kv, mask_bits, mask_rows, ctx, ld_ctx, lse, drop, site, 0, stream);
 }
 
+int vlpk_attn_probs(int B, int heads, int Lq, int Lkv, int row0, const void* q, int64_t ld_q, int64_t q_bstride, const void* k, int64_t ld_k,
+                    int64_t k_bstride, const uint32_t* mask_bits, int mask_rows, int kv_slots, const float* lse, float* p, int64_t ld_p,
+                    int64_t p_bstride, void* stream) {
+  AttnDesc d;
+  d.B = B; d.heads = heads; d.Lq = Lq; d.Lkv = Lkv; d.kv_slots = kv_slots;
+  d.q = q; d.ld_q = ld_q;
+  d.k = k; d.ld_kv = ld_k; d.kv_batch_stride = k_bstride;
+  d.mask_bits = mask_bits; d.mask_rows = mask_rows;
+  d.lse = const_cast<float*>(lse);
+  return launch_attn_probs(d, q_bstride, row0, p, ld_p, p_bstride, S(stream));
+}
+
 int vlpk_attn_core_bwd_wide(int B, int heads, int L, const void* q, const void* k, const void* v, int64_t ld_qkv, const uint32_t* mask_bits,
                             int mask_rows, const void* ctx, const void* dctx, int64_t ld_ctx, const float* lse, void* dq, void* dk, void* dv,
                             int64_t ld_dqkv, const VlpkDropout* drop, uint64_t site, int kv_slots, void* stream) {

@@ -906,6 +906,111 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_bwd_dkv_tiled_kernel(cons
 }
 
 // ------------------------------------------------------------------------------------------------
+// attention probabilities (opt-in, vlpk_attn_probs): P[b, h, i, j] = exp(s_ij - lse_i), recomputed from Q, K and the logsumexp the
+// forward kernels save, so that those kernels stay as they are and one kernel serves every forward path (single-tile, tiled,
+// re-projected prefix, K/V cache).  CTA per (head, sequence, 128-row query tile from row0); K tiles stream through a two-stage TMA
+// ring; S = QK^T as in the forward, the same score() (scale, additive -10000 mask, key slots), then exp2(s - lse2) stored as fp32
+// straight from the accumulator registers: a quad of threads writes 8 consecutive columns (32 bytes) of a row.
+// ------------------------------------------------------------------------------------------------
+struct ProbsArgs {
+  AttnTiledArgs t;      // B, heads, Lq, Lkv, slots, mask_bits, mask_rows, lse (the mask loader's view)
+  int row0;             // first query row written
+  float* p;             // [B, heads, Lq - row0, ld_p], sequences p_bstride floats apart
+  long long ld_p, p_bstride;
+  int vec2;             // p and ld_p allow 8-byte stores
+};
+
+struct ProbsSmem {
+  static constexpr int OFF_Q = 0;
+  static constexpr int OFF_K = TILE_B;  // 2 stages of K
+  static constexpr int OFF_BAR = 3 * TILE_B;
+  static constexpr int TOTAL = OFF_BAR + 24;
+  static constexpr int DYN = TOTAL + 1024;
+};
+
+__global__ void __launch_bounds__(ATT_THREADS, 2) attn_probs_kernel(const __grid_constant__ AttnTmaps tm, const ProbsArgs a) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem + ProbsSmem::OFF_Q;
+  uint8_t* sK = smem + ProbsSmem::OFF_K;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + ProbsSmem::OFF_BAR);  // [0] Q, [1 + s] K stage s
+
+  pdl_launch_dependents();
+  const int h = blockIdx.x, b = blockIdx.y, q0 = a.row0 + blockIdx.z * TL;
+  const int tid = threadIdx.x, wg = tid >> 7;
+  const Frag f;
+  const int nkt = (a.t.Lkv + TL - 1) / TL;
+
+  if (tid == 0) {
+    tma_prefetch_desc(&tm.q);
+    tma_prefetch_desc(&tm.k);
+    for (int i = 0; i < 3; ++i) mbar_init(&bars[i], 1);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  pdl_wait();
+  if (tid == 0) {
+    mbar_arrive_expect_tx(&bars[0], TILE_B);
+    tma_load_3d(sQ, &tm.q, &bars[0], h * HD, q0, b);
+    for (int kt = 0; kt < 2 && kt < nkt; ++kt) {
+      mbar_arrive_expect_tx(&bars[1 + kt], TILE_B);
+      tma_load_3d(sK + kt * TILE_B, &tm.k, &bars[1 + kt], h * HD, kt * TL, b);
+    }
+  }
+
+  const int row[2] = {q0 + wg * 64 + f.fr, q0 + wg * 64 + f.fr + 8};
+  float lse2[2];
+  bool row_ok[2];
+  float* prow[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    row_ok[hh] = row[hh] < a.t.Lq;
+    lse2[hh] = row_ok[hh] ? a.t.lse[(static_cast<size_t>(b) * a.t.heads + h) * a.t.Lq + row[hh]] * LOG2E : 0.f;
+    prow[hh] = a.p + b * a.p_bstride + (static_cast<long long>(h) * (a.t.Lq - a.row0) + (row[hh] - a.row0)) * a.ld_p;
+  }
+  mbar_wait(&bars[0], 0);
+  for (int kt = 0; kt < nkt; ++kt) {
+    const int st = kt & 1;
+    uint8_t* sKs = sK + st * TILE_B;
+    uint32_t mw[2][4];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) load_mask_tile(a.t, b, row[hh], kt, mw[hh]);
+    float s[64];
+    mbar_wait(&bars[1 + st], (kt >> 1) & 1);
+    {
+      const uint32_t qa = smem_u32(sQ) + wg * 8192, k0 = smem_u32(sKs);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < HD / 16; ++k)
+        wgmma_m64n128k16_ss<0, 0>(s, wgmma_desc_sw128(qa + k * 32, 16, 1024), wgmma_desc_sw128(k0 + k * 32, 16, 1024), k > 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(s);
+    }
+    __syncthreads();  // both warpgroups are done with stage st
+    if (tid == 0 && kt + 2 < nkt) {
+      mbar_arrive_expect_tx(&bars[1 + st], TILE_B);
+      tma_load_3d(sKs, &tm.k, &bars[1 + st], h * HD, (kt + 2) * TL, b);
+    }
+    const int lkv = a.t.Lkv - kt * TL;
+#pragma unroll
+    for (int i = 0; i < 64; i += 2) {
+      const int hh = (i >> 1) & 1, col = 8 * (i >> 2) + f.fc;
+      if (!row_ok[hh] || col >= lkv) continue;
+      const float p0 = fast_ex2(score(s[i], mw[hh], col, lkv) - lse2[hh]);
+      const float p1 = fast_ex2(score(s[i + 1], mw[hh], col + 1, lkv) - lse2[hh]);
+      float* dst = prow[hh] + kt * TL + col;
+      if (col + 1 < lkv && a.vec2) {
+        *reinterpret_cast<float2*>(dst) = make_float2(p0, p1);
+      } else {
+        dst[0] = p0;
+        if (col + 1 < lkv) dst[1] = p1;
+      }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
 static int make_seq_tmap(CUtensorMap* out, const void* base, int width, int L, int B, int64_t ld, int64_t batch_stride = 0) {
@@ -1057,6 +1162,49 @@ int launch_attn_bwd(const AttnDesc& d, cudaStream_t stream) {
     VLPK_CUDA(launch_ex(attn_bwd_kernel, dim3(d.heads, d.B), dim3(ATT_THREADS), BwdSmem::DYN, stream, 1, tm, a));
   }
   if (d.dbias != nullptr) VLPK_TRY(launch_sum_parts(a.dbias_part, d.B, nbias, d.dbias, stream));
+  return 0;
+}
+
+int launch_attn_probs(const AttnDesc& d, int64_t q_batch_stride, int row0, float* p, int64_t ld_p, int64_t p_batch_stride,
+                      cudaStream_t stream) {
+  VLPK_TRY(check_common(d));
+  VLPK_CHECK_ARG(d.q != nullptr && d.k != nullptr && d.lse != nullptr && p != nullptr, "attn_probs: null pointer");
+  VLPK_CHECK_ARG(row0 >= 0 && row0 < d.Lq, "attn_probs: row0=%d outside [0, Lq=%d)", row0, d.Lq);
+  VLPK_CHECK_ARG(ld_p >= d.Lkv, "attn_probs: ld_p=%lld < Lkv=%d", static_cast<long long>(ld_p), d.Lkv);
+  const int64_t rows = d.Lq - row0;
+  const int64_t pbs = p_batch_stride != 0 ? p_batch_stride : d.heads * rows * ld_p;
+  VLPK_CHECK_ARG(pbs >= d.heads * rows * ld_p || d.B == 1, "attn_probs: p batch stride %lld overlaps the %d x %lld x %lld block of a sequence",
+                 static_cast<long long>(pbs), d.heads, static_cast<long long>(rows), static_cast<long long>(ld_p));
+  // TMA: 16-byte aligned bases and row / sequence strides; checked here so that a bad stride is an argument error on any machine
+  const auto a16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15u) == 0; };
+  VLPK_CHECK_ARG(a16(d.q) && a16(d.k) && d.ld_q % 8 == 0 && d.ld_kv % 8 == 0 && q_batch_stride % 8 == 0 && d.kv_batch_stride % 8 == 0,
+                 "attn_probs: q / k pointers and strides must be 16-byte multiples (ld_q=%lld ld_k=%lld q_bstride=%lld k_bstride=%lld)",
+                 static_cast<long long>(d.ld_q), static_cast<long long>(d.ld_kv), static_cast<long long>(q_batch_stride),
+                 static_cast<long long>(d.kv_batch_stride));
+  const int width = d.heads * HD;
+  VLPK_CHECK_ARG(d.ld_q >= width && d.ld_kv >= width, "attn_probs: ld_q=%lld / ld_k=%lld below heads * 64 = %d",
+                 static_cast<long long>(d.ld_q), static_cast<long long>(d.ld_kv), width);
+  AttnTmaps tm;
+  memset(&tm, 0, sizeof(tm));
+  VLPK_TRY(make_seq_tmap(&tm.q, d.q, width, d.Lq, d.B, d.ld_q, q_batch_stride));
+  VLPK_TRY(make_seq_tmap(&tm.k, d.k, width, d.Lkv, d.B, d.ld_kv, d.kv_batch_stride));
+  tm.v = tm.o = tm.dq = tm.dk = tm.dv = tm.q;
+  ProbsArgs a;
+  a.t = tiled_args(d);
+  a.row0 = row0;
+  a.p = p;
+  a.ld_p = ld_p;
+  a.p_bstride = pbs;
+  a.vec2 = (reinterpret_cast<uintptr_t>(p) & 7u) == 0 && ld_p % 2 == 0 && pbs % 2 == 0;
+  static bool attr_set = false;
+  if (!attr_set) {
+    VLPK_CUDA(cudaFuncSetAttribute(attn_probs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ProbsSmem::DYN));
+    attr_set = true;
+  }
+  // bandwidth kernel: fp32 P written, Q / K / lse read
+  const double bytes = 4.0 * d.B * d.heads * rows * d.Lkv + 2.0 * d.B * width * (rows + d.Lkv) + 4.0 * d.B * d.heads * rows;
+  LaunchScope scope(CAT_MISC, bytes, stream);
+  VLPK_CUDA(launch_ex(attn_probs_kernel, dim3(d.heads, d.B, (rows + TL - 1) / TL), dim3(ATT_THREADS), ProbsSmem::DYN, stream, 1, tm, a));
   return 0;
 }
 

@@ -34,5 +34,9 @@ struct AttnDesc {
 int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream);
 int launch_attn_bwd(const AttnDesc& d, cudaStream_t stream);
 void set_attn_tiled(bool on);
+// Attention probabilities exp(s - lse) of query rows [row0, Lq) into p [B, heads, Lq - row0, ld_p] (sequences p_batch_stride floats
+// apart, 0 = heads * (Lq - row0) * ld_p) from d.q / d.k / d.mask_bits / d.lse; q_batch_stride as d.kv_batch_stride for Q.
+int launch_attn_probs(const AttnDesc& d, int64_t q_batch_stride, int row0, float* p, int64_t ld_p, int64_t p_batch_stride,
+                      cudaStream_t stream);
 
 }  // namespace vlpk

@@ -183,7 +183,10 @@ def _weight_structs(params, n_layers):
 
 
 class EncoderStackFn(torch.autograd.Function):
-    """n_layers x BertLayer (modeling.py:367-402) in one C call each way.  Returns every layer's output."""
+    """n_layers x BertLayer (modeling.py:367-402) in one C call each way.  Returns every layer's output.
+    cfg = (n_layers, heads, I, p_attn, p_hidden, training[, grad_hook[, maps]]): maps, when not None, is (row0, views, sink): the forward
+    appends every layer's attention probabilities of query rows [row0, L) (attn_probs over the saved qkv and lse; into views[i] when
+    views is not None) to the list sink."""
 
     @staticmethod
     def forward(ctx, hidden, mask_bits, cfg, *params):
@@ -202,6 +205,10 @@ class EncoderStackFn(torch.autograd.Function):
         drop = _drop(max(p_attn, p_hidden), seed)
         L.call("vlpk_encoder_fwd", C.byref(shape), n_layers, ws, x.data_ptr(), mask_bits.data_ptr(), mask_bits.shape[1], acts.structs,
                float(p_attn if training else 0.0), float(p_hidden if training else 0.0), drop, L.stream())
+        maps = cfg[7] if len(cfg) > 7 else None     # output_attentions: (row0, per-layer output views or None, list receiving the maps)
+        if maps is not None:
+            row0, views, sink = maps
+            sink.extend(_acts_maps(acts, i, B, Lq, H, heads, mask_bits, row0, None if views is None else views[i]) for i in range(n_layers))
         ctx.cfg = cfg
         ctx.seed = seed
         ctx.acts = acts
@@ -270,9 +277,59 @@ class EncoderStackFn(torch.autograd.Function):
         return (dx0, None, None) + tuple(grads)
 
 
-def layer_incremental_fwd(hidden, history, mask_bits, heads, I, params):
+def attn_probs(q, k, lse, mask_bits, row0=0, out=None):
+    """Attention probabilities of one layer (vlpk_attn_probs): P[b, h, i - row0, j] = exp(q_i . k_j / 8 + mask_add - lse[b, h, i]) for
+    query rows [row0, Lq), fp32, not differentiable — the reference's attention_probs before dropout.
+    q: bf16 [B, Lq, heads * 64] and k: bf16 [B, Lkv, heads * 64] views with unit column stride (e.g. slices of the packed qkv
+    buffer or of a K/V cache); lse: fp32 [B, heads, Lq] contiguous; mask_bits: the packed mask of the layer's forward.
+    out: None (a new [B, heads, Lq - row0, Lkv] tensor) or an fp32 view of that shape with unit column stride, row stride
+    ld_p >= Lkv and head stride (Lq - row0) * ld_p; any sequence stride.  Returns out."""
+    for t, what in ((q, "attention-map queries"), (k, "attention-map keys"), (lse, "attention logsumexp"), (mask_bits, "attention mask")):
+        _require_cuda(t, what)
+    if q.dim() != 3 or k.dim() != 3 or q.dtype != BF16 or k.dtype != BF16 or q.stride(2) != 1 or k.stride(2) != 1:
+        raise RuntimeError("vlp_b200: attention maps take bf16 [B, L, heads * 64] q / k views with unit column stride")
+    B, Lq, H = q.shape
+    Lkv = k.shape[1]
+    if lse.dim() != 3 or lse.shape[0] != B or lse.shape[2] != Lq or lse.dtype != torch.float32 or not lse.is_contiguous():
+        raise RuntimeError("vlp_b200: the attention logsumexp must be a contiguous fp32 [B, heads, Lq] tensor")
+    heads = lse.shape[1]
+    if k.shape[0] != B or H != heads * 64 or k.shape[2] != H:
+        raise RuntimeError(f"vlp_b200: attention-map q {tuple(q.shape)} / k {tuple(k.shape)} do not match {heads} heads of 64")
+    if not 0 <= row0 < Lq:
+        raise ValueError(f"vlp_b200: attention-map row0={row0} outside [0, {Lq})")
+    slots = kv_slots(Lq, Lkv)
+    _check_mask_words(mask_bits, Lkv)
+    if mask_bits.shape[0] != B or mask_bits.shape[1] not in (1, Lq):
+        raise ValueError(f"vlp_b200: packed mask {tuple(mask_bits.shape)} does not fit B={B}, Lq={Lq}")
+    rows = Lq - row0
+    if out is None:
+        out = torch.empty(B, heads, rows, Lkv, device=q.device, dtype=torch.float32)
+    elif (out.dtype != torch.float32 or out.shape != (B, heads, rows, Lkv) or out.stride(3) != 1 or out.stride(2) < Lkv
+          or out.stride(1) != rows * out.stride(2)):
+        raise RuntimeError(f"vlp_b200: attention-map output must be an fp32 [{B}, {heads}, {rows}, {Lkv}] view with unit column "
+                           "stride, row stride >= Lkv and head stride rows * row stride")
+    L.call("vlpk_attn_probs", B, heads, Lq, Lkv, int(row0), q.data_ptr(), q.stride(1), q.stride(0), k.data_ptr(), k.stride(1), k.stride(0),
+           mask_bits.data_ptr(), mask_bits.shape[1], slots, lse.data_ptr(), out.data_ptr(), out.stride(2), out.stride(0) if B > 1 else 0,
+           L.stream())
+    return out
+
+
+def _acts_maps(acts, i, B, Lq, H, heads, mask_bits, row0=0, out=None, k=None):
+    """attn_probs of layer i of an _Acts: q in place in its qkv buffer (ld 3H, or ld H in the decode layouts that pass k)."""
+    qkv = acts.bf[i][:B * Lq * 3 * H]
+    lse = acts.f32[i][:B * heads * Lq].view(B, heads, Lq)
+    if k is None:
+        v = qkv.view(B, Lq, 3 * H)
+        q, k = v[..., :H], v[..., H:2 * H]
+    else:
+        q = qkv[:B * Lq * H].view(B, Lq, H)
+    return attn_probs(q, k, lse, mask_bits, row0, out)
+
+
+def layer_incremental_fwd(hidden, history, mask_bits, heads, I, params, maps=None):
     """BertLayer.forward with history_states (modeling.py:273-277, 389-390): inference only, q rows = hidden,
-    kv rows = cat(history, hidden)."""
+    kv rows = cat(history, hidden).  maps: None, or (row0, out) — the layer's attention probabilities of query rows [row0, Lq) are
+    written into out (None: a new tensor) and (y, probs) is returned."""
     x = _bf16c(hidden)
     xkv = _bf16c(torch.cat((history.to(x.dtype), x), dim=1))
     B, Lq, H = x.shape
@@ -285,7 +342,20 @@ def layer_incremental_fwd(hidden, history, mask_bits, heads, I, params):
     ws = _weight_structs(pk, 1)
     L.call("vlpk_layer_fwd", C.byref(shape), ws, x.data_ptr(), xkv.data_ptr(), mask_bits.data_ptr(), mask_bits.shape[1], acts.structs, 0.0, 0.0,
            None, 0, L.stream())
-    return acts.y[0]
+    if maps is None:
+        return acts.y[0]
+    k = _acts_region(acts, 0, "kv").view(B, Lkv, 2 * H)[..., :H]
+    return acts.y[0], _acts_maps(acts, 0, B, Lq, H, heads, mask_bits, maps[0], maps[1], k=k)
+
+
+def _acts_region(acts, i, name):
+    """Layer i's flat bf16 buffer `name` of an _Acts."""
+    off = 0
+    for n, sz in acts.bf_sizes:
+        if n == name:
+            return acts.bf[i][off:off + sz]
+        off += sz
+    raise KeyError(name)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -449,10 +519,10 @@ class DecoderCEFn(torch.autograd.Function):
         return dh.to(hdt), dw.to(wdt), dbias[:V].to(bdt), None, None
 
 
-def layer_cached_fwd(hidden, kv_cache, pos, mask_bits, heads, I, params):
+def layer_cached_fwd(hidden, kv_cache, pos, mask_bits, heads, I, params, maps=None):
     """BertLayer.forward for decode with a persistent K/V cache (vlpk_layer_cached_fwd): `hidden` [B, Lq, H] are the new rows, `kv_cache`
     [B, rows, 2H] bf16 holds this layer's key | value projections of the `pos` rows already seen; the new rows' K | V are appended at
-    [pos, pos + Lq).  Inference only."""
+    [pos, pos + Lq).  Inference only.  maps: as for layer_incremental_fwd (keys read from the cache)."""
     x = _bf16c(hidden)
     B, Lq, H = x.shape
     if not (kv_cache.dtype == BF16 and kv_cache.is_contiguous() and kv_cache.shape[0] == B and kv_cache.shape[2] == 2 * H):
@@ -465,7 +535,9 @@ def layer_cached_fwd(hidden, kv_cache, pos, mask_bits, heads, I, params):
     ws = _weight_structs(pk, 1)
     L.call("vlpk_layer_cached_fwd", C.byref(shape), ws, x.data_ptr(), kv_cache.data_ptr(), kv_cache.shape[1], int(pos), mask_bits.data_ptr(),
            mask_bits.shape[1], acts.structs, 0, L.stream())
-    return acts.y[0]
+    if maps is None:
+        return acts.y[0]
+    return acts.y[0], _acts_maps(acts, 0, B, Lq, H, heads, mask_bits, maps[0], maps[1], k=kv_cache[:, :pos + Lq, :H])
 
 
 # ------------------------------------------------------------------------------------------------

@@ -12,7 +12,8 @@ greedy arg-max.  The uniform of row r at step t comes from a Philox counter keye
 seed whatever the batch around the row, and the same seed gives the same uniforms to every batch — pass another seed (the `seed`
 argument of forward, or `dec.seed`) for independent draws.
 
-Output: (ids, scores), int64 / fp32 [B, out_len - in_len]: the sampled words and their log-probabilities under the full softmax.
+Output: (ids, scores), int64 / fp32 [B, out_len - in_len]: the sampled words and their log-probabilities under the full softmax
+(and the per-frame attention maps with output_attentions).
 A row that draws [EOS] is finished; its later positions hold PAD_ID with score 0.  Outside CUDA-graph capture the loop also stops
 once every row is finished: each step copies the device's count of live rows to pinned host memory and the loop reads it once
 the copy's event has completed (a non-blocking query, never a synchronisation), so it stops a step or two after the last [EOS].
@@ -41,7 +42,10 @@ def check_sampling_args(sampling_method, topk, topp, search_beam_size):
         raise ValueError(f"vlp_b200: topp must lie in (0, 1], got {topp!r}")
 
 
-def sample_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, seed=None):
+def sample_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, seed=None,
+                  output_attentions=False):
+    """output_attentions: (ids, scores, attentions), attentions as for greedy decode (BertForSeq2SeqDecoder.forward); frames after an
+    early stop stay 0."""
     check_sampling_args(dec.sampling_method, dec.topk, dec.topp, dec.search_beam_size)
     if dec.forbid_duplicate_ngrams and int(dec.ngram_size) < 1:
         raise ValueError(f"vlp_b200: forbid_duplicate_ngrams needs ngram_size >= 1 (got {dec.ngram_size})")
@@ -61,6 +65,7 @@ def sample_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_id
     if dev.type == "cuda" and not torch.cuda.is_current_stream_capturing():
         poll, polled = torch.empty(1, dtype=torch.int32, pin_memory=True), None
     caches = dec.new_kv_caches(B, dev, out_len) if dec.use_kv_cache else None
+    maps = dec.new_attention_maps(B, T, out_len, dev) if output_attentions else None
     prev_emb, prev_layers = None, None
     curr_ids = input_ids
     mask_ids = input_ids[:, :1] * 0 + dec.mask_word_id
@@ -74,15 +79,17 @@ def sample_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_id
         cl = curr_ids.shape[1]
         st = next_pos - cl
         x_ids = torch.cat((curr_ids, mask_ids), dim=1)
+        extra = {} if maps is None else {"output_attentions": dec.step_maps(maps[:, next_pos - in_len], cl, next_pos + 1)}
         if caches is not None:
-            new_emb, last, _ = dec.bert(vis_feats, vis_pe, x_ids, token_type_ids[:, st:next_pos + 1], position_ids[:, st:next_pos + 1],
-                                        attention_mask[:, st:next_pos + 1, :next_pos + 1], output_all_encoded_layers=False,
-                                        len_vis_input=dec.len_vis_input, kv_caches=caches, cache_pos=st)
+            new_emb, last = dec.bert(vis_feats, vis_pe, x_ids, token_type_ids[:, st:next_pos + 1], position_ids[:, st:next_pos + 1],
+                                     attention_mask[:, st:next_pos + 1, :next_pos + 1], output_all_encoded_layers=False,
+                                     len_vis_input=dec.len_vis_input, kv_caches=caches, cache_pos=st, **extra)[:2]
             new_layers = [last]
         else:
-            new_emb, new_layers, _ = dec.bert(vis_feats, vis_pe, x_ids, token_type_ids[:, st:next_pos + 1], position_ids[:, st:next_pos + 1],
-                                              attention_mask[:, st:next_pos + 1, :next_pos + 1], prev_embedding=prev_emb,
-                                              prev_encoded_layers=prev_layers, output_all_encoded_layers=True, len_vis_input=dec.len_vis_input)
+            new_emb, new_layers = dec.bert(vis_feats, vis_pe, x_ids, token_type_ids[:, st:next_pos + 1], position_ids[:, st:next_pos + 1],
+                                           attention_mask[:, st:next_pos + 1, :next_pos + 1], prev_embedding=prev_emb,
+                                           prev_encoded_layers=prev_layers, output_all_encoded_layers=True, len_vis_input=dec.len_vis_input,
+                                           **extra)[:2]
         h = pred.select_task(pred.transform(new_layers[-1][:, -1:, :].to(pred.decoder.weight.dtype)), task_idx)
         logits = pred.decoder(h)                                       # [B, 1, V]; the bias is added inside the sampling kernel
         frame = next_pos - in_len
@@ -101,4 +108,4 @@ def sample_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_id
         curr_ids = ids[:, frame:frame + 1]
         next_pos += 1
         dec.last_decode_steps += 1
-    return ids, scores
+    return (ids, scores) if maps is None else (ids, scores, maps)

@@ -249,21 +249,35 @@ class BertLayer(nn.Module):
     def _cfg(self, n_layers):
         return (n_layers, self._heads, self._inter, float(self.attention.self.dropout.p), float(self.output.dropout.p), self.training)
 
-    def forward(self, hidden_states, attention_mask, history_states=None, kv_cache=None, cache_pos=0):
+    def forward(self, hidden_states, attention_mask, history_states=None, kv_cache=None, cache_pos=0, output_attentions=False):
         """Reference signature (modeling.py:367) plus an optional decode extension: `kv_cache` [B, rows, 2H] (this layer's key | value
-        projections of the `cache_pos` rows already decoded) replaces `history_states` — K and V of the prefix are not re-projected."""
+        projections of the `cache_pos` rows already decoded) replaces `history_states` — K and V of the prefix are not re-projected.
+
+        output_attentions=True returns (layer_output, attention_probs): fp32 [B, heads, Lq, Lkv], the reference's attention_probs before
+        dropout (modeling.py:283-295), recomputed by ops.attn_probs from the layer's saved q, k and logsumexp; not differentiable.  It may
+        instead be (row0, out): only query rows [row0, Lq) are computed, into the fp32 view `out` [B, heads, Lq - row0, Lkv] (None: a
+        new tensor; see ops.attn_probs), which is returned as attention_probs."""
         bits = _mask_bits(attention_mask)
+        spec = None if output_attentions is False or output_attentions is None else (
+            (0, None) if output_attentions is True else tuple(output_attentions))
+        probs = None
         if kv_cache is not None:
             if torch.is_grad_enabled() and (hidden_states.requires_grad or any(p.requires_grad for p in self.flat_params())):
                 raise RuntimeError("vlp_b200: BertLayer with kv_cache is an inference-only path (decode); wrap in torch.no_grad()")
-            out = ops.layer_cached_fwd(hidden_states, kv_cache, cache_pos, bits, self._heads, self._inter, self.flat_params())
+            out = ops.layer_cached_fwd(hidden_states, kv_cache, cache_pos, bits, self._heads, self._inter, self.flat_params(), maps=spec)
         elif history_states is None:
-            out = ops.EncoderStackFn.apply(hidden_states, bits, self._cfg(1), *self.flat_params())[0]
+            sink = []
+            maps = () if spec is None else ((spec[0], None if spec[1] is None else [spec[1]], sink),)
+            out = ops.EncoderStackFn.apply(hidden_states, bits, self._cfg(1) + (None,) + maps, *self.flat_params())[0]
+            probs = sink[0] if sink else None
         else:
             if torch.is_grad_enabled() and (hidden_states.requires_grad or any(p.requires_grad for p in self.flat_params())):
                 raise RuntimeError("vlp_b200: BertLayer with history_states is an inference-only path (decode); wrap in torch.no_grad()")
-            out = ops.layer_incremental_fwd(hidden_states, history_states, bits, self._heads, self._inter, self.flat_params())
-        return out.to(hidden_states.dtype) if out.dtype != hidden_states.dtype else out
+            out = ops.layer_incremental_fwd(hidden_states, history_states, bits, self._heads, self._inter, self.flat_params(), maps=spec)
+        if isinstance(out, tuple):
+            out, probs = out
+        out = out.to(hidden_states.dtype) if out.dtype != hidden_states.dtype else out
+        return out if spec is None else (out, probs)
 
 
 class BertEncoder(nn.Module):
@@ -282,29 +296,34 @@ class BertEncoder(nn.Module):
         self._vlpk_grad_hook = None
 
     def forward(self, hidden_states, attention_mask, prev_embedding=None, prev_encoded_layers=None, output_all_encoded_layers=True,
-                kv_caches=None, cache_pos=0):
+                kv_caches=None, cache_pos=0, output_attentions=False):
+        """output_attentions=True returns (encoded_layers, attentions), attentions a list of one fp32 [B, heads, Lq, Lkv] map per layer
+        (BertLayer.forward).  It may instead be (row0, outs): layer i writes query rows [row0, Lq) into the view outs[i]."""
         assert (prev_embedding is None) == (prev_encoded_layers is None), \
             "history embedding and encoded layer must be simultanously given."
-        if kv_caches is not None:                            # decode with per-layer K/V caches (SURVEY.md §8f-2)
-            all_layers = []
-            for layer_module, cache in zip(self.layer, kv_caches):
-                hidden_states = layer_module(hidden_states, attention_mask, kv_cache=cache, cache_pos=cache_pos)
-                if output_all_encoded_layers:
-                    all_layers.append(hidden_states)
-            if not output_all_encoded_layers:
-                all_layers.append(hidden_states)
-            return all_layers
-        if prev_embedding is not None:
-            all_layers = []
+        want = not (output_attentions is False or output_attentions is None)
+        per_layer = [True] * len(self.layer) if output_attentions is True else (
+            [(output_attentions[0], o) for o in output_attentions[1]] if want else [False] * len(self.layer))
+        if kv_caches is not None or prev_embedding is not None:
+            all_layers, attentions = [], []
             history_states = prev_embedding
             for i, layer_module in enumerate(self.layer):
-                hidden_states = layer_module(hidden_states, attention_mask, history_states=history_states)
+                if kv_caches is not None:                    # decode with per-layer K/V caches (SURVEY.md §8f-2)
+                    hidden_states = layer_module(hidden_states, attention_mask, kv_cache=kv_caches[i], cache_pos=cache_pos,
+                                                 output_attentions=per_layer[i])
+                else:
+                    hidden_states = layer_module(hidden_states, attention_mask, history_states=history_states, output_attentions=per_layer[i])
+                    history_states = prev_encoded_layers[i]
+                if want:
+                    hidden_states, probs = hidden_states
+                    attentions.append(probs)
                 if output_all_encoded_layers:
                     all_layers.append(hidden_states)
-                history_states = prev_encoded_layers[i]
             if not output_all_encoded_layers:
                 all_layers.append(hidden_states)
-            return all_layers
+            return (all_layers, attentions) if want else all_layers
+        attentions = [] if want else None
+        row0, views = (0, None) if output_attentions is True or not want else output_attentions
         # whole stack in one call each way — or, under data parallelism, in groups of `layers_per_call` layers so that the
         # gradients of the last group are complete (and their all-reduce bucket can start) while earlier layers still run backward
         bits = _mask_bits(attention_mask)
@@ -325,11 +344,13 @@ class BertEncoder(nn.Module):
             params = []
             for l in group:
                 params.extend(l.flat_params())
-            g_outs = ops.EncoderStackFn.apply(cur, bits, self.layer[0]._cfg(len(group)) + (self._vlpk_grad_hook,), *params)
+            maps = ((row0, None if views is None else views[s - size:s], attentions),) if want else ()
+            g_outs = ops.EncoderStackFn.apply(cur, bits, self.layer[0]._cfg(len(group)) + (self._vlpk_grad_hook,) + maps, *params)
             outs.extend(g_outs)
             cur = g_outs[-1]
         outs = [o if o.dtype == dt else o.to(dt) for o in outs]
-        return list(outs) if output_all_encoded_layers else [outs[-1]]
+        layers = list(outs) if output_all_encoded_layers else [outs[-1]]
+        return (layers, attentions) if want else layers
 
 
 class BertPooler(nn.Module):
@@ -566,38 +587,49 @@ class BertModel(PreTrainedBertModel):
             ext._vlpk_bits_version = _tensor_version(ext)
         return ext
 
-    def forward(self, vis_feats, vis_pe, input_ids, token_type_ids=None, attention_mask=None, output_all_encoded_layers=True, len_vis_input=49):
+    def forward(self, vis_feats, vis_pe, input_ids, token_type_ids=None, attention_mask=None, output_all_encoded_layers=True, len_vis_input=49,
+                output_attentions=False):
+        """output_attentions=True returns (encoded_layers, pooled_output, attentions): one fp32 [B, heads, L, L] map per layer, the
+        reference's attention_probs before dropout (what a forward hook on its attention.self.dropout receives)."""
         _check_seq_len(self.config, input_ids.size(1))
         ext = self.get_extended_attention_mask(input_ids, token_type_ids, attention_mask)
         embedding_output = self.embeddings(vis_feats, vis_pe, input_ids, token_type_ids, len_vis_input=len_vis_input)
-        encoded_layers = self.encoder(embedding_output, ext, output_all_encoded_layers=output_all_encoded_layers)
+        encoded_layers = self.encoder(embedding_output, ext, output_all_encoded_layers=output_all_encoded_layers,
+                                      output_attentions=bool(output_attentions))
+        if output_attentions:
+            encoded_layers, attentions = encoded_layers
         sequence_output = encoded_layers[-1]
         pooled_output = self.pooler(sequence_output)
         if not output_all_encoded_layers:
             encoded_layers = encoded_layers[-1]
-        return encoded_layers, pooled_output
+        return (encoded_layers, pooled_output, attentions) if output_attentions else (encoded_layers, pooled_output)
 
 
 class BertModelIncr(BertModel):
     """modeling.py:852-875."""
 
     def forward(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, prev_embedding=None, prev_encoded_layers=None,
-                output_all_encoded_layers=True, len_vis_input=49, kv_caches=None, cache_pos=0):
+                output_all_encoded_layers=True, len_vis_input=49, kv_caches=None, cache_pos=0, output_attentions=False):
         """Reference signature (modeling.py:856) plus `kv_caches` / `cache_pos`: decode against per-layer K/V caches instead of
-        re-encoding `prev_embedding` / `prev_encoded_layers` (regions enter at cache_pos == 0 only)."""
+        re-encoding `prev_embedding` / `prev_encoded_layers` (regions enter at cache_pos == 0 only).  output_attentions (True, or
+        (row0, outs) as for BertEncoder.forward) appends the list of per-layer maps to the returned tuple."""
         prefix = cache_pos if kv_caches is not None else (0 if prev_embedding is None else prev_embedding.size(1))
         _check_seq_len(self.config, prefix + input_ids.size(1))
         ext = self.get_extended_attention_mask(input_ids, token_type_ids, attention_mask)
         first = (prev_encoded_layers is None) if kv_caches is None else (cache_pos == 0)
         embedding_output = self.embeddings(vis_feats, vis_pe, input_ids, token_type_ids, position_ids, vis_input=first,
                                            len_vis_input=len_vis_input)
+        want = not (output_attentions is False or output_attentions is None)
         encoded_layers = self.encoder(embedding_output, ext, prev_embedding=prev_embedding, prev_encoded_layers=prev_encoded_layers,
-                                      output_all_encoded_layers=output_all_encoded_layers, kv_caches=kv_caches, cache_pos=cache_pos)
+                                      output_all_encoded_layers=output_all_encoded_layers, kv_caches=kv_caches, cache_pos=cache_pos,
+                                      output_attentions=output_attentions)
+        if want:
+            encoded_layers, attentions = encoded_layers
         sequence_output = encoded_layers[-1]
         pooled_output = self.pooler(sequence_output)
         if not output_all_encoded_layers:
             encoded_layers = encoded_layers[-1]
-        return embedding_output, encoded_layers, pooled_output
+        return (embedding_output, encoded_layers, pooled_output, attentions) if want else (embedding_output, encoded_layers, pooled_output)
 
 
 class _RegionProjections:
@@ -820,9 +852,24 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         H = self.config.hidden_size
         return [torch.empty(batch, rows, 2 * H, device=device, dtype=torch.bfloat16) for _ in self.bert.encoder.layer]
 
+    def new_attention_maps(self, n0, n1, out_len, device):
+        """Zeroed fp32 [n0, n1, layers, heads, out_len] buffer for the [MASK]-row attention maps of a decode: [B, frames, ...] for greedy
+        and sampling, [frames, B*K, ...] (per step, its input rows) for beam search."""
+        cfg = self.config
+        return torch.zeros(n0, n1, cfg.num_hidden_layers, cfg.num_attention_heads, out_len, device=device, dtype=torch.float32)
+
+    @staticmethod
+    def step_maps(buf, row0, n_keys):
+        """BertModelIncr's output_attentions for one decode step: buf [rows, layers, heads, out_len] (a frame of new_attention_maps,
+        any row stride) receives, per layer, query row row0 (the step's [MASK] row) over keys [0, n_keys)."""
+        return row0, [buf[:, l].unsqueeze(2)[..., :n_keys] for l in range(buf.shape[1])]
+
     def forward(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, sample_mode="greedy",
-                seed=None):
-        """seed: the sampling seed of this call (sampling_method "topk" / "topp"); None uses self.seed."""
+                seed=None, output_attentions=False):
+        """seed: the sampling seed of this call (sampling_method "topk" / "topp"); None uses self.seed.
+        output_attentions: greedy / sample / top-k / top-p decode return (ids, scores, attentions) and beam search adds
+        out["attentions"]: fp32 [B, out_len - in_len, layers, heads, out_len], for every output word the attention probabilities of the
+        [MASK] query row that predicted it, over keys [0, out_len) (keys not yet visible, and frames not decoded, are 0)."""
         self.cls.predictions.check_task_idx(task_idx)          # before anything is launched
         _check_seq_len(self.config, token_type_ids.size(1))
         from .beam import check_ngram_args
@@ -835,15 +882,19 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
             vis_feats, vis_pe = self.project_regions(vis_feats, vis_pe)
             if sampling:
                 from .sampling import sample_decode
-                return sample_decode(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx, seed)
+                return sample_decode(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx, seed,
+                                     output_attentions=output_attentions)
             if self.search_beam_size > 1:
                 from .beam import beam_search
-                return beam_search(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx)
+                return beam_search(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx,
+                                   output_attentions=output_attentions)
             input_length = input_ids.size(1)
             output_length = token_type_ids.size(1)
             output_ids, output_probs = [], []
             prev_embedding, prev_encoded_layers = None, None
             caches = self.new_kv_caches(input_ids.size(0), input_ids.device, output_length) if self.use_kv_cache else None
+            maps = self.new_attention_maps(input_ids.size(0), output_length - input_length, output_length, input_ids.device) \
+                if output_attentions else None
             curr_ids = input_ids
             mask_ids = input_ids[:, :1] * 0 + self.mask_word_id
             next_pos = input_length
@@ -851,19 +902,20 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
                 curr_length = curr_ids.size(1)
                 start_pos = next_pos - curr_length
                 x_input_ids = torch.cat((curr_ids, mask_ids), dim=1)
+                extra = {} if maps is None else {"output_attentions": self.step_maps(maps[:, next_pos - input_length], curr_length, next_pos + 1)}
                 if caches is not None:
                     # rows [0, start_pos) of every layer's cache hold K|V of the real tokens decoded so far; this step appends
                     # (new token, [MASK]) at [start_pos, next_pos] — the [MASK] row is overwritten by the next step's token
-                    new_embedding, new_encoded_layers, _ = self.bert(
+                    new_embedding, new_encoded_layers = self.bert(
                         vis_feats, vis_pe, x_input_ids, token_type_ids[:, start_pos:next_pos + 1], position_ids[:, start_pos:next_pos + 1],
                         attention_mask[:, start_pos:next_pos + 1, :next_pos + 1], output_all_encoded_layers=False,
-                        len_vis_input=self.len_vis_input, kv_caches=caches, cache_pos=start_pos)
+                        len_vis_input=self.len_vis_input, kv_caches=caches, cache_pos=start_pos, **extra)[:2]
                     new_encoded_layers = [new_encoded_layers]
                 else:
-                    new_embedding, new_encoded_layers, _ = self.bert(
+                    new_embedding, new_encoded_layers = self.bert(
                         vis_feats, vis_pe, x_input_ids, token_type_ids[:, start_pos:next_pos + 1], position_ids[:, start_pos:next_pos + 1],
                         attention_mask[:, start_pos:next_pos + 1, :next_pos + 1], prev_embedding=prev_embedding,
-                        prev_encoded_layers=prev_encoded_layers, output_all_encoded_layers=True, len_vis_input=self.len_vis_input)
+                        prev_encoded_layers=prev_encoded_layers, output_all_encoded_layers=True, len_vis_input=self.len_vis_input, **extra)[:2]
                 last_hidden = new_encoded_layers[-1][:, -1:, :]
                 prediction_scores, _ = self.cls(last_hidden, None, task_idx=task_idx)
                 if sample_mode == "greedy":
@@ -886,4 +938,6 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
                     prev_encoded_layers = [torch.cat((a, b[:, :-1, :]), dim=1) for a, b in zip(prev_encoded_layers, new_encoded_layers)]
                 curr_ids = max_ids
                 next_pos += 1
+            if maps is not None:
+                return torch.cat(output_ids, dim=1), torch.cat(output_probs, dim=1), maps
             return torch.cat(output_ids, dim=1), torch.cat(output_probs, dim=1)
