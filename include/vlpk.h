@@ -253,6 +253,20 @@ int vlpk_mha_incr_fwd(const VlpkShape* s, const VlpkLayerWeights* w, const void*
  * the rows of real tokens: the [MASK] row written at pos + Lq - 1 is overwritten by the next step). */
 int vlpk_layer_cached_fwd(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, void* kv_cache, int cache_rows, int pos,
                           const uint32_t* mask_bits, int mask_rows, VlpkLayerActs* a, uint64_t layer_id, void* stream);
+/* vlpk_layer_cached_fwd for s->B hypotheses in groups of G per image that share one image prefix (several captions per image: beam
+ * n-best lists, N samples).  K/V come from two caches instead of one contiguous cache per hypothesis:
+ *   prefix [B / G, prefix_rows, 2H] bf16: keys 0 .. P-1 of image b / G (written once, e.g. by vlpk_layer_cached_fwd at B / G rows);
+ *   text   [B, T, 2H] bf16: the K | V of the Lq new rows x [B*Lq, H] of hypothesis i go to text[i, pos .. pos + Lq);
+ *   slots  [B, T] int32, one table for all layers: key P + j (j < pos) of hypothesis i is the flat text row slots[i * T + j] (a beam
+ *          reorder moves table entries, not K/V rows).  Entries outside [0, B * T) are clamped: wrong numbers, never a bad read.
+ * Keys P + pos .. P + pos + Lq - 1 are the hypothesis' own new rows; s->Lkv must equal P + pos + Lq (<= 512).  mask_bits: one
+ * sequence per image, [B / G, mask_rows, S / 32].  Output, a->qkv / a->kv and the rest as vlpk_layer_cached_fwd: the layer is
+ * bitwise what vlpk_layer_cached_fwd computes on each hypothesis' materialised contiguous cache.  < 0 with nothing launched for:
+ * B % G != 0, P outside [1, prefix_rows], pos < 0 or pos + Lq > T, Lkv != P + pos + Lq, a bad shape, mask_rows neither 1 nor Lq,
+ * a NULL pointer, or x / prefix / text / mask_bits not 16-byte aligned (slots: 4-byte). */
+int vlpk_layer_cached_group_fwd(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, const void* prefix, int prefix_rows, int P,
+                                void* text, int T, const int32_t* slots, int G, int pos, const uint32_t* mask_bits, int mask_rows,
+                                VlpkLayerActs* a, uint64_t layer_id, void* stream);
 /* Host-only: bytes the caller must provide for a shape.  out3 = { all VlpkLayerActs buffers of ONE layer (without the optional
  * drop_attn keep-bytes: B*heads*Lq*S/8),
  * all VlpkBwdScratch buffers (shared by the layers), the fp32 VlpkLayerGrads accumulators of ONE layer }. */

@@ -101,6 +101,8 @@ _SIGS = {
                                   C.POINTER(VlpkLayerActs), c_u64, _P]),
     "vlpk_layer_cached_fwd": (c_int, [C.POINTER(VlpkShape), C.POINTER(VlpkLayerWeights), _P, _P, c_int, c_int, _P, c_int,
                                       C.POINTER(VlpkLayerActs), c_u64, _P]),
+    "vlpk_layer_cached_group_fwd": (c_int, [C.POINTER(VlpkShape), C.POINTER(VlpkLayerWeights), _P, _P, c_int, c_int, _P, c_int, _P, c_int,
+                                            c_int, _P, c_int, C.POINTER(VlpkLayerActs), c_u64, _P]),
     "vlpk_workspace_bytes": (c_int, [C.POINTER(VlpkShape), C.POINTER(C.c_size_t)]),
     "vlpk_encoder_fwd": (c_int, [C.POINTER(VlpkShape), c_int, C.POINTER(VlpkLayerWeights), _P, _P, c_int,
                                  C.POINTER(VlpkLayerActs), c_float, c_float, C.POINTER(VlpkDropout), _P]),

@@ -17,6 +17,7 @@ import torch
 import torch.nn.functional as F
 
 from . import ops
+from .shared_prefix import SharedPrefixCache
 
 
 def _expand_beams(x, K):
@@ -72,7 +73,12 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
     out_len = token_type_ids.shape[1]
     dev = input_ids.device
     prev_emb, prev_layers = None, None
-    caches = dec.new_kv_caches(B, dev, out_len) if getattr(dec, "use_kv_cache", False) else None
+    N = getattr(dec, "num_return_sequences", 1)
+    shared = None
+    if N > 1:           # the K hypotheses of an image share its prefix K/V; a reorder moves slot-table entries, not cache rows
+        caches = shared = SharedPrefixCache(len(dec.bert.encoder.layer), B, K, in_len, out_len - in_len, dec.config.hidden_size, dev)
+    else:
+        caches = dec.new_kv_caches(B, dev, out_len) if getattr(dec, "use_kv_cache", False) else None
     curr_ids = input_ids
     mask_ids = input_ids[:, :1] * 0 + dec.mask_word_id
     total_scores, beam_eos, step_ids, step_ptrs = [], [], [], []
@@ -126,15 +132,20 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
         beam_eos.append((k_ids == dec.eos_id).float())
         total_scores.append(k_scores)
         if first:
-            if caches is not None:
+            if shared is not None:
+                pass                                                       # the attention mask stays per image, as the shared cache reads it
+            elif caches is not None:
                 caches = [_expand_beams(c, K).contiguous() for c in caches]
             else:
                 prev_emb = _expand_beams(new_emb[:, :-1, :], K)
                 prev_layers = [_expand_beams(x[:, :-1, :], K) for x in new_layers]
             token_type_ids, position_ids = _expand_beams(token_type_ids, K), _expand_beams(position_ids, K)
-            attention_mask, mask_ids = _expand_beams(attention_mask, K), _expand_beams(mask_ids, K)
+            attention_mask = attention_mask if shared is not None else _expand_beams(attention_mask, K)
+            mask_ids = _expand_beams(mask_ids, K)
             if torch.is_tensor(task_idx) and task_idx.dim() == 1 and task_idx.shape[0] == B:
                 task_idx = _expand_beams(task_idx, K)                      # per-sample ids follow their beams (relaxed head)
+        elif shared is not None:
+            shared.reorder((back + torch.arange(B, device=dev).unsqueeze(1) * K).reshape(-1), frame - 1)
         elif caches is not None:
             parent = (back + torch.arange(B, device=dev).unsqueeze(1) * K).reshape(-1)      # beam i continues hypothesis parent[i]
             caches = [c.index_select(0, parent) for c in caches]
@@ -153,6 +164,8 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
         padded = t.new_zeros((B, out_len, K))
         padded[:, :T] = t.permute(1, 0, 2)
         out[k] = padded
+    if N > 1:
+        out["nbest_seq"], out["nbest_scores"] = nbest(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len, N)
     return out
 
 
@@ -180,9 +193,9 @@ def beam_maps(maps, active, pos, pt):
     return torch.where(keep, got, torch.zeros_like(got)).transpose(0, 1)
 
 
-def best_path(sc, wi, pt, eos_id, length_penalty):
-    """The hypothesis backtrack() selects, frame by frame: (active [T,B] — frame t belongs to it —, pos [T,B] — its beam index at
-    frame t)."""
+def candidate_values(sc, wi, eos_id, length_penalty):
+    """The final-selection rule's value of every (frame, beam), [B, T*K] in (frame, beam) order — the reference's loop order: score +
+    length_penalty * (frame + 1) for a candidate ([EOS] word, or the last frame, within frames <= last[b]), -inf otherwise."""
     T, B, K = sc.shape
     dev = sc.device
     frames = torch.arange(T, device=dev).view(T, 1)
@@ -190,7 +203,36 @@ def best_path(sc, wi, pt, eos_id, length_penalty):
     last = torch.where(all_eos.any(0), all_eos.float().argmax(0), torch.full((B,), T - 1, device=dev))      # [B]
     cand = (frames <= last.unsqueeze(0)).unsqueeze(-1) & ((wi == eos_id) | (frames == last.unsqueeze(0)).unsqueeze(-1))
     val = torch.where(cand, sc + length_penalty * (frames + 1).unsqueeze(-1).to(sc.dtype), torch.full_like(sc, -math.inf))
-    flat = val.permute(1, 0, 2).reshape(B, T * K)                          # (frame, beam) order = the reference's loop order
+    return val.permute(1, 0, 2).reshape(B, T * K)
+
+
+def nbest(sc, wi, pt, eos_id, length_penalty, out_len, n):
+    """The n highest-ranked candidates of the final-selection rule, each back-tracked as backtrack() does its best one: (nbest_seq
+    int64 [B, n, out_len] zero padded, nbest_scores [B, n] — the rule's values).  Equal values keep (frame, beam) order, so entry 0
+    is backtrack()'s hypothesis; the list is not deduplicated.  Every beam of the last frame is a candidate, so n <= K always fills."""
+    T, B, K = sc.shape
+    dev = sc.device
+    flat = candidate_values(sc, wi, eos_id, length_penalty)
+    val, idx = torch.sort(flat, dim=1, descending=True, stable=True)
+    val, idx = val[:, :n], idx[:, :n]                                     # [B, n]
+    frame, pos = torch.div(idx, K, rounding_mode="floor"), idx % K
+    found = torch.isfinite(val)
+    toks = [None] * T
+    for fid in range(T - 1, -1, -1):                                      # walk the back pointers from `frame` down to 0
+        active = found & (fid <= frame)
+        toks[fid] = torch.where(active, wi[fid].gather(1, pos), torch.zeros_like(pos))
+        pos = torch.where(active & (fid > 0), pt[fid].gather(1, pos), pos)
+    seq = torch.zeros(B, n, out_len, dtype=torch.long, device=dev)
+    seq[:, :, :T] = torch.stack(toks, dim=-1)
+    return seq, val
+
+
+def best_path(sc, wi, pt, eos_id, length_penalty):
+    """The hypothesis backtrack() selects, frame by frame: (active [T,B] — frame t belongs to it —, pos [T,B] — its beam index at
+    frame t)."""
+    T, B, K = sc.shape
+    dev = sc.device
+    flat = candidate_values(sc, wi, eos_id, length_penalty)
     best = flat.argmax(-1)                                                # first maximal value
     frame, pos = torch.div(best, K, rounding_mode="floor"), best % K
     found = torch.isfinite(flat.gather(1, best.unsqueeze(1)).squeeze(1))

@@ -158,7 +158,23 @@ struct KvCache {       // incremental decode with a persistent K/V cache (vlpk_l
   void* base = nullptr;  // [B, rows, 2H] bf16: key | value projections of the rows this layer has seen
   int rows = 0;          // allocated rows per sequence
   int pos = 0;           // rows already valid; the call appends the Lq new rows at [pos, pos + Lq)
+  const AttnGroupKv* group = nullptr;  // vlpk_layer_cached_group_fwd: base / rows / pos are the text cache, keys from the group loader
 };
+
+// BertSelfOutput after the attention core: output projection of a->ctx, residual x, dropout, LayerNorm -> a->y1
+int attn_out_ln(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, VlpkLayerActs* a, float p_hidden, const VlpkDropout* drop,
+                uint64_t layer_id, cudaStream_t st) {
+  const int H = s->H, Mq = s->B * s->Lq;
+  const DropoutCfg none = make_dropout(0.f, 0, 0);
+  VLPK_TRY(fwd_linear(Mq, H, H, a->ctx, H, w->wo, H, w->bo, a->t1, H, EPI_STORE, nullptr, 0, none, st));
+  LnArgs ln;
+  ln.M = Mq; ln.H = H;
+  ln.t = static_cast<const bf16*>(a->t1); ln.res = static_cast<const bf16*>(x);
+  ln.gamma = static_cast<const bf16*>(w->ln1_g); ln.beta = static_cast<const bf16*>(w->ln1_b);
+  ln.y = static_cast<bf16*>(a->y1); ln.stats = reinterpret_cast<float2*>(a->stats1);
+  ln.drop = mk_drop(drop, p_hidden, site_of(layer_id, SITE_HID1));
+  return launch_ln_res_drop_fwd(ln, st);
+}
 
 int mha_fwd_impl(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, const void* x_kv, const uint32_t* bits, int mask_rows,
                  VlpkLayerActs* a, float p_attn, float p_hidden, const VlpkDropout* drop, uint64_t layer_id, cudaStream_t st,
@@ -174,8 +190,9 @@ int mha_fwd_impl(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, c
   ad.keep_out = (ad.drop.p > 0.f) ? a->drop_attn : nullptr;   // forward stores its keep-decisions for backward
   if (cache != nullptr) {
     // Q and K|V of the NEW rows only; K|V are appended to the cache (rows [pos, pos + Lq) of every sequence), attention reads the cache
-    VLPK_CHECK_ARG(a->kv != nullptr && cache->base != nullptr && cache->pos >= 0 && cache->pos + s->Lq == s->Lkv && s->Lkv <= cache->rows,
-                   "mha_cached_fwd: pos=%d + Lq=%d must equal Lkv=%d <= cache rows %d", cache->pos, s->Lq, s->Lkv, cache->rows);
+    if (cache->group == nullptr)
+      VLPK_CHECK_ARG(a->kv != nullptr && cache->base != nullptr && cache->pos >= 0 && cache->pos + s->Lq == s->Lkv && s->Lkv <= cache->rows,
+                     "mha_cached_fwd: pos=%d + Lq=%d must equal Lkv=%d <= cache rows %d", cache->pos, s->Lq, s->Lkv, cache->rows);
     VLPK_TRY(fwd_linear(Mq, H, H, x, H, w->wq, H, w->bq, a->qkv, H, EPI_STORE, nullptr, 0, none, st));
     GemmDesc g;
     g.M = Mq; g.N = 2 * H; g.K = H;
@@ -195,6 +212,10 @@ int mha_fwd_impl(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, c
     ad.v = static_cast<const bf16*>(cache->base) + H;
     ad.ld_kv = 2 * H;
     ad.kv_batch_stride = static_cast<int64_t>(cache->rows) * 2 * H;
+    if (cache->group != nullptr) {
+      VLPK_TRY(launch_attn_fwd_group(ad, *cache->group, st));
+      return attn_out_ln(s, w, x, a, p_hidden, drop, layer_id, st);
+    }
   } else if (!incr) {
     VLPK_CHECK_ARG(s->Lq == s->Lkv, "mha_fwd: Lq != Lkv requires x_kv");
     GemmDesc g;  // packed QKV projection: three [H,H] weights read in place as N-segments
@@ -231,14 +252,7 @@ int mha_fwd_impl(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, c
     ad.ld_kv = 2 * H;
   }
   VLPK_TRY(launch_attn_fwd(ad, st));
-  VLPK_TRY(fwd_linear(Mq, H, H, a->ctx, H, w->wo, H, w->bo, a->t1, H, EPI_STORE, nullptr, 0, none, st));
-  LnArgs ln;
-  ln.M = Mq; ln.H = H;
-  ln.t = static_cast<const bf16*>(a->t1); ln.res = static_cast<const bf16*>(x);
-  ln.gamma = static_cast<const bf16*>(w->ln1_g); ln.beta = static_cast<const bf16*>(w->ln1_b);
-  ln.y = static_cast<bf16*>(a->y1); ln.stats = reinterpret_cast<float2*>(a->stats1);
-  ln.drop = mk_drop(drop, p_hidden, site_of(layer_id, SITE_HID1));
-  return launch_ln_res_drop_fwd(ln, st);
+  return attn_out_ln(s, w, x, a, p_hidden, drop, layer_id, st);
 }
 
 int ffn_fwd_impl(const VlpkShape* s, const VlpkLayerWeights* w, VlpkLayerActs* a, float p_hidden, const VlpkDropout* drop,
@@ -647,6 +661,29 @@ int vlpk_layer_cached_fwd(const VlpkShape* s, const VlpkLayerWeights* w, const v
   VLPK_CHECK_ARG(w && x && kv_cache && mask_bits && a, "layer_cached_fwd: null pointer");
   KvCache c;
   c.base = kv_cache; c.rows = cache_rows; c.pos = pos;
+  VLPK_TRY(mha_fwd_impl(s, w, x, nullptr, mask_bits, mask_rows, a, 0.f, 0.f, nullptr, layer_id, S(stream), &c));
+  return ffn_fwd_impl(s, w, a, 0.f, nullptr, layer_id, S(stream));
+}
+
+int vlpk_layer_cached_group_fwd(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, const void* prefix, int prefix_rows, int P,
+                                void* text, int T, const int32_t* slots, int G, int pos, const uint32_t* mask_bits, int mask_rows,
+                                VlpkLayerActs* a, uint64_t layer_id, void* stream) {
+  VLPK_TRY(check_shape(s));
+  VLPK_CHECK_ARG(w && x && prefix && text && slots && mask_bits && a && a->qkv && a->kv && a->ctx && a->lse,
+                 "layer_cached_group_fwd: null pointer");
+  VLPK_CHECK_ARG(G >= 1 && s->B % G == 0, "layer_cached_group_fwd: B=%d hypotheses are not whole groups of G=%d", s->B, G);
+  VLPK_CHECK_ARG(P >= 1 && P <= prefix_rows, "layer_cached_group_fwd: P=%d must be in [1, prefix rows %d]", P, prefix_rows);
+  VLPK_CHECK_ARG(pos >= 0 && pos + s->Lq <= T, "layer_cached_group_fwd: pos=%d + Lq=%d exceeds the T=%d text rows", pos, s->Lq, T);
+  VLPK_CHECK_ARG(P + pos + s->Lq == s->Lkv, "layer_cached_group_fwd: Lkv=%d must equal P=%d + pos=%d + Lq=%d", s->Lkv, P, pos, s->Lq);
+  VLPK_CHECK_ARG(mask_rows == 1 || mask_rows == s->Lq, "layer_cached_group_fwd: mask rows %d (1 or Lq=%d)", mask_rows, s->Lq);
+  const auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; };
+  VLPK_CHECK_ARG(a16(x) && a16(prefix) && a16(text) && a16(mask_bits) && (reinterpret_cast<uintptr_t>(slots) & 3u) == 0,
+                 "layer_cached_group_fwd: x, prefix, text and mask_bits must be 16-byte aligned, slots 4-byte aligned");
+  AttnGroupKv g;
+  g.prefix = prefix; g.prefix_rows = prefix_rows; g.P = P;
+  g.text = text; g.slots = slots; g.T = T; g.G = G; g.pos = pos;
+  KvCache c;
+  c.base = text; c.rows = T; c.pos = pos; c.group = &g;
   VLPK_TRY(mha_fwd_impl(s, w, x, nullptr, mask_bits, mask_rows, a, 0.f, 0.f, nullptr, layer_id, S(stream), &c));
   return ffn_fwd_impl(s, w, a, 0.f, nullptr, layer_id, S(stream));
 }

@@ -105,6 +105,42 @@ __device__ __forceinline__ void load_mask_words(const AttnArgs& a, int b, int ro
 }
 
 // ------------------------------------------------------------------------------------------------
+// shared-prefix K/V (vlpk_layer_cached_group_fwd): hypothesis b of image b / G reads key r < P from the image's prefix cache (a
+// TMA box, like a contiguous cache), key r = P + j from text row slots[b, j] when j < pos and from its own row b * T + j otherwise.
+// The text rows are gathered into the same 128B-swizzled tile slots a TMA box of the contiguous cache fills, and slots past Lkv
+// are zeroed as TMA's out-of-bounds fill zeroes them: the tiles, and so every instruction after the load, are those of
+// the contiguous cache.  A slot entry outside the text tensor is clamped into it (wrong numbers, never an out-of-bounds read).
+// ------------------------------------------------------------------------------------------------
+struct GroupKv {
+  const __nv_bfloat16* text;  // [B, T, ld]: K | V rows, V at column H
+  const int* slots;           // [B, T]
+  long long ld;
+  int H, G, P, pos, T;
+  long long text_rows;        // B * T
+};
+
+// Key rows [max(P, k0), k0 + 128) of a K tile and its V tile, for hypothesis b and head h.  Called by all threads after the tile's
+// TMA box (if any) has landed; the caller fences and synchronises before the tiles are read.
+__device__ __forceinline__ void group_fill(uint8_t* sK, uint8_t* sV, const GroupKv& g, int b, int h, int k0, int Lkv) {
+  for (int i = threadIdx.x; i < TL * 8; i += ATT_THREADS) {
+    const int r = i >> 3, c = i & 7, key = k0 + r;
+    if (key < g.P) continue;
+    uint4 kx = make_uint4(0u, 0u, 0u, 0u), vx = kx;
+    if (key < Lkv) {
+      const int j = key - g.P;
+      long long row = static_cast<long long>(b) * g.T + j;
+      if (j < g.pos) row = min(max(static_cast<long long>(__ldg(g.slots + static_cast<long long>(b) * g.T + j)), 0ll), g.text_rows - 1);
+      const __nv_bfloat16* src = g.text + row * g.ld + h * HD + c * 8;
+      kx = __ldg(reinterpret_cast<const uint4*>(src));
+      vx = __ldg(reinterpret_cast<const uint4*>(src + g.H));
+    }
+    const int off = r * 128 + ((c ^ (r & 7)) << 4);
+    *reinterpret_cast<uint4*>(sK + off) = kx;
+    *reinterpret_cast<uint4*>(sV + off) = vx;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // forward  (256 threads, 48 KB smem: Q | K | V; the Q tile is reused as output staging)
 // ------------------------------------------------------------------------------------------------
 struct FwdSmem {
@@ -116,7 +152,10 @@ struct FwdSmem {
   static constexpr int DYN = TOTAL + 1024;
 };
 
-__global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a) {
+// GROUP: K/V from a shared prefix + text rows (GroupKv); grid (G * heads, images), so the G hypotheses of an image and head run
+// next to each other and read its prefix box from L2.  Otherwise grid (heads, B) and K/V from tm.k / tm.v.
+template <bool GROUP>
+__device__ __forceinline__ void attn_fwd_body(const AttnTmaps& tm, const AttnArgs a, const GroupKv g) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem + FwdSmem::OFF_Q;
@@ -127,7 +166,9 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_kernel(const __grid_c
   uint64_t* bar_v = &bars[1];
 
   pdl_launch_dependents();
-  const int h = blockIdx.x, b = blockIdx.y;
+  const int h = GROUP ? blockIdx.x / g.G : blockIdx.x;
+  const int b = GROUP ? blockIdx.y * g.G + blockIdx.x % g.G : blockIdx.y;
+  const int kb = GROUP ? blockIdx.y : b;  // sequence of the K/V boxes and of the mask rows
   const int tid = threadIdx.x, wg = tid >> 7;
   const Frag f;
   const int qi = tid & 3;
@@ -146,9 +187,9 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_kernel(const __grid_c
   if (tid == 0) {
     mbar_arrive_expect_tx(bar_qk, 2 * TILE_B);
     tma_load_3d(sQ, &tm.q, bar_qk, h * HD, 0, b);
-    tma_load_3d(sK, &tm.k, bar_qk, h * HD, 0, b);
+    tma_load_3d(sK, &tm.k, bar_qk, h * HD, 0, kb);
     mbar_arrive_expect_tx(bar_v, TILE_B);
-    tma_load_3d(sV, &tm.v, bar_v, h * HD, 0, b);
+    tma_load_3d(sV, &tm.v, bar_v, h * HD, 0, kb);
   }
 
   const int row[2] = {wg * 64 + f.fr, wg * 64 + f.fr + 8};
@@ -156,8 +197,15 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_kernel(const __grid_c
   uint64_t row_elem0[2];
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
-    load_mask_words(a, b, row[hh], mw[hh]);
+    load_mask_words(a, kb, row[hh], mw[hh]);
     row_elem0[hh] = ((static_cast<uint64_t>(b) * a.heads + h) * a.Lq + min(row[hh], a.Lq - 1)) * TL;
+  }
+  if constexpr (GROUP) {  // text rows over the prefix box's out-of-bounds rows
+    mbar_wait(bar_qk, 0);
+    mbar_wait(bar_v, 0);
+    group_fill(sK, sV, g, b, h, 0, a.Lkv);
+    fence_proxy_async_smem();
+    __syncthreads();
   }
 
   // S = Q K^T for this warpgroup's 64 query rows
@@ -238,6 +286,15 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_kernel(const __grid_c
     tma_store_commit();
     tma_store_wait<0>();
   }
+}
+
+__global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a) {
+  attn_fwd_body<false>(tm, a, GroupKv{});
+}
+
+__global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_group_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a,
+                                                                         const GroupKv g) {
+  attn_fwd_body<true>(tm, a, g);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -476,8 +533,10 @@ struct FwdTiledSmem {
   static constexpr int DYN = TOTAL + 1024;
 };
 
-// One CTA per SM: the running O (32 registers) stays live beside S and P, which does not fit the 128 registers of two CTAs
-__global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_tiled_kernel(const __grid_constant__ AttnTmaps tm, const AttnTiledArgs a) {
+// One CTA per SM: the running O (32 registers) stays live beside S and P, which does not fit the 128 registers of two CTAs.
+// GROUP: as attn_fwd_body; a key tile that starts at or past the prefix gets no TMA box (its barrier is arrived on without bytes).
+template <bool GROUP>
+__device__ __forceinline__ void attn_fwd_tiled_body(const AttnTmaps& tm, const AttnTiledArgs a, const GroupKv g) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem + FwdTiledSmem::OFF_Q;
@@ -485,7 +544,10 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_tiled_kernel(const __
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + FwdTiledSmem::OFF_BAR);  // [0] Q, [1 + s] K|V stage s
 
   pdl_launch_dependents();
-  const int h = blockIdx.x, b = blockIdx.y, q0 = blockIdx.z * TL;
+  const int h = GROUP ? blockIdx.x / g.G : blockIdx.x;
+  const int b = GROUP ? blockIdx.y * g.G + blockIdx.x % g.G : blockIdx.y;
+  const int kb = GROUP ? blockIdx.y : b;  // sequence of the K/V boxes and of the mask rows
+  const int q0 = blockIdx.z * TL;
   const int tid = threadIdx.x, wg = tid >> 7;
   const Frag f;
   const int qi = tid & 3;
@@ -505,9 +567,13 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_tiled_kernel(const __
     mbar_arrive_expect_tx(&bars[0], TILE_B);
     tma_load_3d(sQ, &tm.q, &bars[0], h * HD, q0, b);
     for (int kt = 0; kt < 2 && kt < nkt; ++kt) {
+      if (GROUP && kt * TL >= g.P) {
+        mbar_arrive(&bars[1 + kt]);
+        continue;
+      }
       mbar_arrive_expect_tx(&bars[1 + kt], 2 * TILE_B);
-      tma_load_3d(sKV + kt * 2 * TILE_B, &tm.k, &bars[1 + kt], h * HD, kt * TL, b);
-      tma_load_3d(sKV + kt * 2 * TILE_B + TILE_B, &tm.v, &bars[1 + kt], h * HD, kt * TL, b);
+      tma_load_3d(sKV + kt * 2 * TILE_B, &tm.k, &bars[1 + kt], h * HD, kt * TL, kb);
+      tma_load_3d(sKV + kt * 2 * TILE_B + TILE_B, &tm.v, &bars[1 + kt], h * HD, kt * TL, kb);
     }
   }
 
@@ -528,9 +594,14 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_tiled_kernel(const __
     uint8_t* sV = sK + TILE_B;
     uint32_t mw[2][4];
 #pragma unroll
-    for (int hh = 0; hh < 2; ++hh) load_mask_tile(a, b, row[hh], kt, mw[hh]);
+    for (int hh = 0; hh < 2; ++hh) load_mask_tile(a, kb, row[hh], kt, mw[hh]);
     float s[64];
     mbar_wait(&bars[1 + st], (kt >> 1) & 1);
+    if constexpr (GROUP) {
+      group_fill(sK, sV, g, b, h, kt * TL, a.Lkv);
+      fence_proxy_async_smem();
+      __syncthreads();
+    }
     {
       const uint32_t qa = smem_u32(sQ) + wg * 8192, k0 = smem_u32(sK);
       wgmma_fence();
@@ -592,9 +663,13 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_tiled_kernel(const __
     }
     __syncthreads();  // both warpgroups are done with stage st
     if (tid == 0 && kt + 2 < nkt) {
-      mbar_arrive_expect_tx(&bars[1 + st], 2 * TILE_B);
-      tma_load_3d(sK, &tm.k, &bars[1 + st], h * HD, (kt + 2) * TL, b);
-      tma_load_3d(sV, &tm.v, &bars[1 + st], h * HD, (kt + 2) * TL, b);
+      if (GROUP && (kt + 2) * TL >= g.P) {
+        mbar_arrive(&bars[1 + st]);
+      } else {
+        mbar_arrive_expect_tx(&bars[1 + st], 2 * TILE_B);
+        tma_load_3d(sK, &tm.k, &bars[1 + st], h * HD, (kt + 2) * TL, kb);
+        tma_load_3d(sV, &tm.v, &bars[1 + st], h * HD, (kt + 2) * TL, kb);
+      }
     }
   }
 #pragma unroll
@@ -618,6 +693,15 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_tiled_kernel(const __
     tma_store_commit();
     tma_store_wait<0>();
   }
+}
+
+__global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_tiled_kernel(const __grid_constant__ AttnTmaps tm, const AttnTiledArgs a) {
+  attn_fwd_tiled_body<false>(tm, a, GroupKv{});
+}
+
+__global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_group_tiled_kernel(const __grid_constant__ AttnTmaps tm, const AttnTiledArgs a,
+                                                                               const GroupKv g) {
+  attn_fwd_tiled_body<true>(tm, a, g);
 }
 
 // P (recomputed from the logsumexp; 0 for keys >= Lkv and rows >= Lq) and the dropout-masked dP of one 64 x 128 (q, key) block,
@@ -1119,6 +1203,55 @@ int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream) {
   }
   LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * d.Lkv * HD, stream);
   VLPK_CUDA(launch_ex(attn_fwd_kernel, dim3(d.heads, d.B), dim3(ATT_THREADS), FwdSmem::DYN, stream, 1, tm, a));
+  return 0;
+}
+
+int launch_attn_fwd_group(const AttnDesc& d, const AttnGroupKv& gd, cudaStream_t stream) {
+  VLPK_TRY(check_common(d));
+  VLPK_CHECK_ARG(gd.G >= 1 && d.B % gd.G == 0, "attention group: %d hypotheses are not whole groups of G=%d", d.B, gd.G);
+  VLPK_CHECK_ARG(gd.P >= 1 && gd.P <= gd.prefix_rows && gd.pos >= 0 && gd.pos + d.Lq <= gd.T && gd.P + gd.pos + d.Lq == d.Lkv,
+                 "attention group: P=%d (prefix rows %d) pos=%d Lq=%d T=%d Lkv=%d", gd.P, gd.prefix_rows, gd.pos, d.Lq, gd.T, d.Lkv);
+  VLPK_CHECK_ARG(gd.prefix != nullptr && gd.text != nullptr && gd.slots != nullptr, "attention group: null pointer");
+  const int width = d.heads * HD, images = d.B / gd.G;
+  AttnTmaps tm;
+  memset(&tm, 0, sizeof(tm));
+  VLPK_TRY(make_seq_tmap(&tm.q, d.q, width, d.Lq, d.B, d.ld_q));
+  VLPK_TRY(make_seq_tmap(&tm.k, gd.prefix, width, gd.P, images, d.ld_kv, static_cast<int64_t>(gd.prefix_rows) * d.ld_kv));
+  VLPK_TRY(make_seq_tmap(&tm.v, static_cast<const __nv_bfloat16*>(gd.prefix) + width, width, gd.P, images, d.ld_kv,
+                         static_cast<int64_t>(gd.prefix_rows) * d.ld_kv));
+  VLPK_TRY(make_seq_tmap(&tm.o, d.o, width, d.Lq, d.B, d.ld_o));
+  tm.dq = tm.dk = tm.dv = tm.o;
+  GroupKv g;
+  g.text = static_cast<const __nv_bfloat16*>(gd.text);
+  g.slots = gd.slots;
+  g.ld = d.ld_kv;
+  g.H = width; g.G = gd.G; g.P = gd.P; g.pos = gd.pos; g.T = gd.T;
+  g.text_rows = static_cast<long long>(d.B) * gd.T;
+  const dim3 grid(gd.G * d.heads, images, (d.Lq + TL - 1) / TL);
+  LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * d.Lkv * HD, stream);
+  if (use_tiled(d)) {
+    AttnTiledArgs a = tiled_args(d);
+    static bool attr_set = false;
+    if (!attr_set) {
+      VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_group_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdTiledSmem::DYN));
+      attr_set = true;
+    }
+    VLPK_CUDA(launch_ex(attn_fwd_group_tiled_kernel, grid, dim3(ATT_THREADS), FwdTiledSmem::DYN, stream, 1, tm, a, g));
+    return 0;
+  }
+  AttnArgs a;
+  a.B = d.B; a.heads = d.heads; a.Lq = d.Lq; a.Lkv = d.Lkv;
+  a.mask_bits = d.mask_bits; a.mask_rows = d.mask_rows;
+  a.lse = d.lse; a.o_ptr = nullptr; a.do_ptr = nullptr; a.ld_o = d.ld_o;
+  a.drop = d.drop;
+  a.keep_out = nullptr;
+  a.dbias_part = nullptr;
+  static bool attr_set = false;
+  if (!attr_set) {
+    VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem::DYN));
+    attr_set = true;
+  }
+  VLPK_CUDA(launch_ex(attn_fwd_group_kernel, dim3(grid.x, grid.y), dim3(ATT_THREADS), FwdSmem::DYN, stream, 1, tm, a, g));
   return 0;
 }
 

@@ -30,8 +30,21 @@ struct AttnDesc {
   float* dbias = nullptr;  // optional [3 * heads * 64] fp32: += column sums of dQ | dK | dV, summed over sequences in a fixed order
 };
 
+// Keys of d.B hypotheses in groups of G per image (vlpk_layer_cached_group_fwd): hypothesis b reads key r < P from row r of image
+// b / G's prefix [images, prefix_rows, ld_kv], key P + j from text row slots[b * T + j] (j < pos) or b * T + j (its own new rows) of
+// text [B * T, ld_kv]; K at column 0, V at column heads * 64 of both.  mask_bits has one sequence per image.
+struct AttnGroupKv {
+  const void* prefix = nullptr;
+  int prefix_rows = 0, P = 0;
+  const void* text = nullptr;
+  const int32_t* slots = nullptr;
+  int T = 0, G = 1, pos = 0;
+};
+
 // Lq, Lkv <= 128: the single-tile kernels; longer sequences (or the "attn_tiled" test option): the KV-tiled kernels.
 int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream);
+// Forward only, no dropout: d.k / d.v / d.kv_batch_stride unused, d.ld_kv is the row stride of prefix and text.
+int launch_attn_fwd_group(const AttnDesc& d, const AttnGroupKv& g, cudaStream_t stream);
 int launch_attn_bwd(const AttnDesc& d, cudaStream_t stream);
 void set_attn_tiled(bool on);
 // Attention probabilities exp(s - lse) of query rows [row0, Lq) into p [B, heads, Lq - row0, ld_p] (sequences p_batch_stride floats

@@ -11,6 +11,7 @@ import argparse
 
 from . import ops
 from .sampling import SAMPLING_METHODS, check_sampling_args
+from .shared_prefix import check_num_return_sequences
 
 _OPTIONS = (
     ("--beam_size", dict(type=int, default=1, help="beam size for beam search; 1 = greedy, and required when sampling")),
@@ -25,6 +26,8 @@ _OPTIONS = (
     ("--topp", dict(type=float, default=1.0, help="--sampling_method topp: sample from the smallest set of words whose probability "
                                                   "reaches p, 0 < p <= 1")),
     ("--seed", dict(type=int, default=123, help="random seed (keys the sampling draws)")),
+    ("--num_return_sequences", dict(type=int, default=1, help="captions per image: the N best of beam search (N <= --beam_size) or N "
+                                                              "top-k / top-p samples, over one K/V cache of the image prefix")),
 )
 
 
@@ -43,6 +46,7 @@ def check_decode_args(args):
     check_sampling_args(args.sampling_method, args.topk, args.topp, args.beam_size)
     if args.forbid_duplicate_ngrams and args.ngram_size < 1:
         raise ValueError(f"vlp_b200: forbid_duplicate_ngrams needs ngram_size >= 1 (got {args.ngram_size})")
+    check_num_return_sequences(args.num_return_sequences, args.sampling_method, args.beam_size)
 
 
 def parse_decode_args(parser, argv=None):
@@ -64,6 +68,9 @@ def decoder_kwargs(args, tokenizer=None):
         if tokenizer is None:
             raise ValueError("vlp_b200: --forbid_ignore_word needs a tokenizer to map its words to ids")
         ignore = set(tokenizer.convert_tokens_to_ids(args.forbid_ignore_word.split("|")))
-    return dict(search_beam_size=args.beam_size, length_penalty=args.length_penalty, forbid_duplicate_ngrams=args.forbid_duplicate_ngrams,
-                forbid_ignore_set=ignore, ngram_size=args.ngram_size, min_len=args.min_len or 0, sampling_method=args.sampling_method,
-                topk=args.topk, topp=args.topp, seed=args.seed)
+    kw = dict(search_beam_size=args.beam_size, length_penalty=args.length_penalty, forbid_duplicate_ngrams=args.forbid_duplicate_ngrams,
+              forbid_ignore_set=ignore, ngram_size=args.ngram_size, min_len=args.min_len or 0, sampling_method=args.sampling_method,
+              topk=args.topk, topp=args.topp, seed=args.seed)
+    if args.num_return_sequences != 1:
+        kw["num_return_sequences"] = args.num_return_sequences       # the decoder's default otherwise
+    return kw

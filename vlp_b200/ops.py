@@ -540,6 +540,33 @@ def layer_cached_fwd(hidden, kv_cache, pos, mask_bits, heads, I, params, maps=No
     return acts.y[0], _acts_maps(acts, 0, B, Lq, H, heads, mask_bits, maps[0], maps[1], k=kv_cache[:, :pos + Lq, :H])
 
 
+def layer_cached_group_fwd(hidden, prefix, P, text, slots, G, pos, mask_bits, heads, I, params):
+    """vlpk_layer_cached_group_fwd: layer_cached_fwd for the B*G hypotheses `hidden` [B*G, Lq, H] that share, per group of G, one
+    image prefix.  Keys [0, P) come from prefix [B, rows >= P, 2H]; key P + j (j < pos) of hypothesis i from text row
+    slots[i, j] of text [B*G, T, 2H]; the new rows' K | V are written to text[:, pos:pos + Lq) and are the last keys.  mask_bits:
+    one sequence per image.  Inference only."""
+    x = _bf16c(hidden)
+    BG, Lq, H = x.shape
+    if G < 1 or BG % G or prefix.shape[0] * G != BG:
+        raise ValueError(f"vlp_b200: {BG} hypotheses are not {prefix.shape[0]} groups of G={G}")
+    for t, what in ((prefix, "prefix cache"), (text, "text cache")):
+        if not (t.dtype == BF16 and t.is_contiguous() and t.dim() == 3 and t.shape[2] == 2 * H):
+            raise RuntimeError(f"vlp_b200: the {what} must be a contiguous bf16 [*, rows, 2H] tensor")
+    T = text.shape[1]
+    if text.shape[0] != BG or slots.dtype != torch.int32 or not slots.is_contiguous() or tuple(slots.shape) != (BG, T):
+        raise RuntimeError("vlp_b200: text cache [B*G, T, 2H] and an int32 slot table [B*G, T] are needed")
+    Lkv = P + pos + Lq
+    slots_kv = kv_slots(Lq, Lkv)
+    _check_mask_words(mask_bits, Lkv)
+    pk = [_bf16c(p) for p in params]
+    acts = _Acts(1, BG, Lq, H, heads, I, x.device, Lkv=Lq)           # acts.kv: scratch for the new rows' K | V
+    shape = L.VlpkShape(BG, Lq, Lkv, H, heads, I, slots_kv)
+    ws = _weight_structs(pk, 1)
+    L.call("vlpk_layer_cached_group_fwd", C.byref(shape), ws, x.data_ptr(), prefix.data_ptr(), prefix.shape[1], int(P), text.data_ptr(), T,
+           slots.data_ptr(), int(G), int(pos), mask_bits.data_ptr(), mask_bits.shape[1], acts.structs, 0, L.stream())
+    return acts.y[0]
+
+
 # ------------------------------------------------------------------------------------------------
 # beam search
 # ------------------------------------------------------------------------------------------------

@@ -13,7 +13,8 @@ seed whatever the batch around the row, and the same seed gives the same uniform
 argument of forward, or `dec.seed`) for independent draws.
 
 Output: (ids, scores), int64 / fp32 [B, out_len - in_len]: the sampled words and their log-probabilities under the full softmax
-(and the per-frame attention maps with output_attentions).
+(and the per-frame attention maps with output_attentions).  With num_return_sequences N > 1: [B, N, out_len - in_len], sample j of
+image b drawn as row b * N + j of the batch repeated N times, over one K/V cache of each image's prefix (shared_prefix.py).
 A row that draws [EOS] is finished; its later positions hold PAD_ID with score 0.  Outside CUDA-graph capture the loop also stops
 once every row is finished: each step copies the device's count of live rows to pinned host memory and the loop reads it once
 the copy's event has completed (a non-blocking query, never a synchronisation), so it stops a step or two after the last [EOS].
@@ -22,6 +23,7 @@ import torch
 
 from . import ops
 from .beam import _ignore_tensor
+from .shared_prefix import SharedPrefixCache
 
 SAMPLING_METHODS = ("beam_search", "topk", "topp")
 PAD_ID = 0
@@ -57,14 +59,22 @@ def sample_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_id
     ngram = int(dec.ngram_size) if dec.forbid_duplicate_ngrams else 0
     ignore = _ignore_tensor(dec, dev) if ngram else None
     pred = dec.cls.predictions
-    ids = torch.full((B, T), PAD_ID, dtype=torch.int64, device=dev)
-    scores = torch.zeros(B, T, dtype=torch.float32, device=dev)
-    finished = torch.zeros(B, dtype=torch.int32, device=dev)
-    live = torch.full((1,), B, dtype=torch.int32, device=dev)
+    # N > 1: row b * N + j is sample j of image b, drawn exactly as row b * N + j of the batch repeated with repeat_interleave(N)
+    N = getattr(dec, "num_return_sequences", 1)
+    R = B * N
+    ids = torch.full((R, T), PAD_ID, dtype=torch.int64, device=dev)
+    scores = torch.zeros(R, T, dtype=torch.float32, device=dev)
+    finished = torch.zeros(R, dtype=torch.int32, device=dev)
+    live = torch.full((1,), R, dtype=torch.int32, device=dev)
     poll = None
     if dev.type == "cuda" and not torch.cuda.is_current_stream_capturing():
         poll, polled = torch.empty(1, dtype=torch.int32, pin_memory=True), None
-    caches = dec.new_kv_caches(B, dev, out_len) if dec.use_kv_cache else None
+    if N > 1:
+        caches = SharedPrefixCache(len(dec.bert.encoder.layer), B, N, in_len, T, dec.config.hidden_size, dev)
+        if torch.is_tensor(task_idx) and task_idx.dim() == 1 and task_idx.shape[0] == B:
+            task_idx = task_idx.repeat_interleave(N)                  # per-sample ids follow their samples (relaxed head)
+    else:
+        caches = dec.new_kv_caches(B, dev, out_len) if dec.use_kv_cache else None
     maps = dec.new_attention_maps(B, T, out_len, dev) if output_attentions else None
     prev_emb, prev_layers = None, None
     curr_ids = input_ids
@@ -90,8 +100,19 @@ def sample_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_id
                                            attention_mask[:, st:next_pos + 1, :next_pos + 1], prev_embedding=prev_emb,
                                            prev_encoded_layers=prev_layers, output_all_encoded_layers=True, len_vis_input=dec.len_vis_input,
                                            **extra)[:2]
-        h = pred.select_task(pred.transform(new_layers[-1][:, -1:, :].to(pred.decoder.weight.dtype)), task_idx)
-        logits = pred.decoder(h)                                       # [B, 1, V]; the bias is added inside the sampling kernel
+        last = new_layers[-1][:, -1:, :]
+        if N > 1 and next_pos == in_len:
+            # the prefill ran at B images: its [MASK] row feeds the head at B*N rows, the row count of the repeated batch, and from
+            # here on every input is per sample (the attention mask stays per image: the shared cache reads it so).  The rows keep
+            # the prefill output's row stride too, as a slice of the repeated batch's output would: the head's GEMMs pick their
+            # kernels by shape and strides, and a contiguous copy rounds differently at BERT-base sizes.
+            full = last.new_empty(R, in_len + 1, last.shape[2])
+            full[:, -1:] = last.repeat_interleave(N, 0)
+            last = full[:, -1:]
+            token_type_ids, position_ids = token_type_ids.repeat_interleave(N, 0), position_ids.repeat_interleave(N, 0)
+            mask_ids = mask_ids.repeat_interleave(N, 0)
+        h = pred.select_task(pred.transform(last.to(pred.decoder.weight.dtype)), task_idx)
+        logits = pred.decoder(h)                                       # [R, 1, V]; the bias is added inside the sampling kernel
         frame = next_pos - in_len
         ops.sample_tokens(logits, pred.bias.to(logits.dtype), dec.sampling_method, dec.topk, dec.topp, seed, frame, ids, scores, finished,
                           live, dec.eos_id, PAD_ID, block_eos=bool(dec.min_len) and frame + 1 <= dec.min_len, ngram=ngram, ignore=ignore)
@@ -108,4 +129,6 @@ def sample_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_id
         curr_ids = ids[:, frame:frame + 1]
         next_pos += 1
         dec.last_decode_steps += 1
+    if N > 1:
+        return ids.view(B, N, T), scores.view(B, N, T)
     return (ids, scores) if maps is None else (ids, scores, maps)

@@ -264,7 +264,12 @@ class BertLayer(nn.Module):
         if kv_cache is not None:
             if torch.is_grad_enabled() and (hidden_states.requires_grad or any(p.requires_grad for p in self.flat_params())):
                 raise RuntimeError("vlp_b200: BertLayer with kv_cache is an inference-only path (decode); wrap in torch.no_grad()")
-            out = ops.layer_cached_fwd(hidden_states, kv_cache, cache_pos, bits, self._heads, self._inter, self.flat_params(), maps=spec)
+            if not torch.is_tensor(kv_cache):                # a layer of shared_prefix.SharedPrefixCache (num_return_sequences > 1)
+                if spec is not None:
+                    raise ValueError("vlp_b200: output_attentions is not available with a shared-prefix K/V cache")
+                out = kv_cache.layer_fwd(hidden_states, cache_pos, bits, self._heads, self._inter, self.flat_params())
+            else:
+                out = ops.layer_cached_fwd(hidden_states, kv_cache, cache_pos, bits, self._heads, self._inter, self.flat_params(), maps=spec)
         elif history_states is None:
             sink = []
             maps = () if spec is None else ((spec[0], None if spec[1] is None else [spec[1]], sink),)
@@ -824,7 +829,7 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
 
     def __init__(self, config, mask_word_id=0, num_labels=2, search_beam_size=1, length_penalty=1.0, eos_id=0, forbid_duplicate_ngrams=False,
                  forbid_ignore_set=None, ngram_size=3, min_len=0, enable_butd=False, len_vis_input=49, sampling_method="beam_search", topk=1,
-                 topp=1.0, seed=0):
+                 topp=1.0, seed=0, num_return_sequences=1):
         super().__init__(config)
         self.bert = BertModelIncr(config)
         self.cls = BertPreTrainingHeads(config, self.bert.embeddings.word_embeddings.weight, num_labels=num_labels)
@@ -844,6 +849,10 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         from .sampling import check_sampling_args
         check_sampling_args(sampling_method, topk, topp, search_beam_size)
         self.sampling_method, self.topk, self.topp, self.seed = sampling_method, topk, topp, seed
+        # N > 1: N captions per image — beam search's N best hypotheses, or N samples — over one K/V cache of the image prefix
+        from .shared_prefix import check_num_return_sequences
+        check_num_return_sequences(num_return_sequences, sampling_method, search_beam_size)
+        self.num_return_sequences = num_return_sequences
         self.use_kv_cache = True     # False: the reference's data flow (K, V of the whole prefix re-projected at every step, modeling.py:273-277)
         self._build_region_projections(config, enable_butd)
 
@@ -869,7 +878,9 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         """seed: the sampling seed of this call (sampling_method "topk" / "topp"); None uses self.seed.
         output_attentions: greedy / sample / top-k / top-p decode return (ids, scores, attentions) and beam search adds
         out["attentions"]: fp32 [B, out_len - in_len, layers, heads, out_len], for every output word the attention probabilities of the
-        [MASK] query row that predicted it, over keys [0, out_len) (keys not yet visible, and frames not decoded, are 0)."""
+        [MASK] query row that predicted it, over keys [0, out_len) (keys not yet visible, and frames not decoded, are 0).
+        num_return_sequences N > 1: beam search adds out["nbest_seq"] int64 [B, N, out_len] and out["nbest_scores"] fp32 [B, N];
+        top-k / top-p sampling returns ids and scores [B, N, out_len - in_len]."""
         self.cls.predictions.check_task_idx(task_idx)          # before anything is launched
         _check_seq_len(self.config, token_type_ids.size(1))
         from .beam import check_ngram_args
@@ -878,6 +889,9 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         if sampling:
             from .sampling import check_sampling_args
             check_sampling_args(self.sampling_method, self.topk, self.topp, self.search_beam_size)
+        from .shared_prefix import check_num_return_sequences
+        check_num_return_sequences(getattr(self, "num_return_sequences", 1), getattr(self, "sampling_method", "beam_search"),
+                                   self.search_beam_size, self.use_kv_cache, output_attentions)
         with torch.no_grad():
             vis_feats, vis_pe = self.project_regions(vis_feats, vis_pe)
             if sampling:
