@@ -1,25 +1,9 @@
-"""Host-side pieces of the beam search (vlp_b200/beam.py, semantics of the reference's modeling.py:1326-1350, 1390-1406) that need
-no GPU: beam expansion / re-ordering by back pointers and the duplicate-n-gram candidate rule."""
+"""Host-side pieces of the beam search (vlp_b200/beam.py, semantics of the reference's modeling.py:1390-1406, 1431-1472) that need
+no GPU: the duplicate-n-gram candidate rule, integer back pointers and the back-tracking.  Expansion to the beams and re-ordering by
+back pointers: test_decode_state_cpu.py."""
 import torch
 
 from vlp_b200 import beam
-
-
-def test_expand_beams_repeats_each_item_consecutively():
-    x = torch.arange(6).view(3, 2)
-    y = beam._expand_beams(x, 2)
-    assert y.tolist() == [[0, 1], [0, 1], [2, 3], [2, 3], [4, 5], [4, 5]]
-
-
-def test_reorder_follows_back_pointers_per_batch_item():
-    B, K = 2, 3
-    x = torch.arange(B * K * 4, dtype=torch.float32).view(B * K, 2, 2)
-    back = torch.tensor([[2, 0, 0], [1, 1, 2]])
-    y = beam._reorder(x, back, B, K)
-    xs = x.view(B, K, 2, 2)
-    for b in range(B):
-        for k in range(K):
-            assert torch.equal(y.view(B, K, 2, 2)[b, k], xs[b, back[b, k]])
 
 
 def test_dup_ngram_candidates_match_reference_rule():

@@ -1,4 +1,4 @@
-"""Top-k / top-p sampling decode (vlp_b200/sampling.py, vlpk_sample_tokens in csrc/decode.cu), host side: argument validation at the
+"""Top-k / top-p sampling decode (vlp_b200/decode.py, vlpk_sample_tokens in csrc/decode.cu), host side: argument validation at the
 C ABI, the Python API and the command line (nothing is launched for a refused combination), and the launches of a sampling decode
 under the dry-run."""
 import argparse

@@ -1,4 +1,4 @@
-"""GPU: top-k / top-p sampling (vlpk_sample_tokens, vlp_b200/sampling.py).
+"""GPU: top-k / top-p sampling (vlpk_sample_tokens, vlp_b200/decode.py).
  (1) the kernel: topk = 1 and topp -> 0 are the first arg-max of the head's logits (bias added in the logits' dtype), ties included, at
      ragged vocabularies up to 30 522; every draw lies in the torch-computed top-k set / nucleus (words ranked by logit, then id) and its
      score is the full log-softmax; 2^16 draws per case pass a chi-square test against the renormalised torch distribution at

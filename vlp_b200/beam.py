@@ -8,8 +8,8 @@ best-hypothesis selection + back-tracking (:1431-1472) as vectorised tensor ops,
 device: no host synchronisation inside or after the loop, so a blocked decode can be captured as a CUDA graph too.
 Per-sample `task_idx` (the relaxed MLM head, relax_projection > 1) is expanded to the B*K beam rows with the other inputs; the
 reference does not expand it (:1297 vs :1325-1373), so its relaxed beam search only runs at B = 1.
-Every step runs the fused layers on the two new rows (token, [MASK]) against the K/V caches (`dec.use_kv_cache`), or — reference
-data flow — against the re-encoded prefix.
+Every step runs the fused layers on the two new rows (token, [MASK]) through decode.DecodeState, which also expands the history to the
+beams after the first step and reorders it by the back pointers after every later one.
 """
 import math
 
@@ -17,19 +17,7 @@ import torch
 import torch.nn.functional as F
 
 from . import ops
-from .shared_prefix import SharedPrefixCache
-
-
-def _expand_beams(x, K):
-    """[B, ...] -> [B*K, ...], each item repeated K times consecutively (reference first_expand, :1326-1333)."""
-    return x.unsqueeze(1).expand(x.shape[0], K, *x.shape[1:]).reshape(x.shape[0] * K, *x.shape[1:])
-
-
-def _reorder(x, back_ptrs, B, K):
-    """Select, per batch item, the K parent beams named by back_ptrs [B,K] (reference select_beam_items, :1335-1350)."""
-    xs = x.view(B, K, *x.shape[1:])
-    idx = back_ptrs.view(B, K, *([1] * (x.dim() - 1))).expand(B, K, *x.shape[1:])
-    return torch.gather(xs, 1, idx).reshape(x.shape)
+from .decode import DecodeState, _ignore_tensor, expand_task_idx, new_attention_maps
 
 
 def _dup_ngram_candidates(seq, n, ignore):
@@ -48,23 +36,6 @@ def _dup_ngram_candidates(seq, n, ignore):
     return sorted(out)
 
 
-def _ignore_tensor(dec, dev):
-    """The decoder's forbid_ignore_set as an int32 device tensor (None when empty), built once per distinct set and device and kept on
-    the decoder for its lifetime: the first call (a CUDA graph's warm-up) makes the host-to-device copy, so a capture never does, and
-    a graph captured with one set keeps reading a live tensor after decodes with other sets."""
-    key = (tuple(sorted(int(w) for w in dec.forbid_ignore_set or ())), str(dev))
-    cache = dec.__dict__.setdefault("_ngram_ignore_cache", {})
-    if key not in cache:
-        cache[key] = torch.tensor(key[0], dtype=torch.int32, device=dev) if key[0] else None
-    return cache[key]
-
-
-def check_ngram_args(dec):
-    """Raises before any launch for an n-gram size the blocking rule does not define."""
-    if dec.forbid_duplicate_ngrams and dec.search_beam_size > 1 and int(dec.ngram_size) < 1:
-        raise ValueError(f"vlp_b200: forbid_duplicate_ngrams needs ngram_size >= 1 (got {dec.ngram_size})")
-
-
 def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, output_attentions=False):
     """output_attentions: out["attentions"] [B, out_len - in_len, layers, heads, out_len] holds, for frame t of pred_seq, the [MASK]-row
     maps of step t taken from the row its hypothesis continued (beam_maps)."""
@@ -72,53 +43,29 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
     B, in_len = input_ids.shape
     out_len = token_type_ids.shape[1]
     dev = input_ids.device
-    prev_emb, prev_layers = None, None
-    N = getattr(dec, "num_return_sequences", 1)
-    shared = None
-    if N > 1:           # the K hypotheses of an image share its prefix K/V; a reorder moves slot-table entries, not cache rows
-        caches = shared = SharedPrefixCache(len(dec.bert.encoder.layer), B, K, in_len, out_len - in_len, dec.config.hidden_size, dev)
-    else:
-        caches = dec.new_kv_caches(B, dev, out_len) if getattr(dec, "use_kv_cache", False) else None
-    curr_ids = input_ids
-    mask_ids = input_ids[:, :1] * 0 + dec.mask_word_id
+    N = dec.num_return_sequences
+    # N > 1: the K hypotheses of an image share its prefix K/V; a reorder moves slot-table entries, not cache rows
+    state = DecodeState(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, K if N > 1 else None)
     total_scores, beam_eos, step_ids, step_ptrs = [], [], [], []
     if dec.forbid_duplicate_ngrams:
-        check_ngram_args(dec)
         ngram, ignore = int(dec.ngram_size), _ignore_tensor(dec, dev)
         hist = [torch.empty(B * K, out_len - in_len, dtype=torch.int32, device=dev) for _ in range(2)]    # word histories, in turn
     # per step t, the [MASK]-row maps of its B*K input rows (step 0: B rows, written at rows b*K)
-    maps = dec.new_attention_maps(out_len - in_len, B * K, out_len, dev) if output_attentions else None
-    next_pos = in_len
-    while next_pos < out_len:
-        cl = curr_ids.shape[1]
-        st = next_pos - cl
-        x_ids = torch.cat((curr_ids, mask_ids), dim=1)
-        extra = {}
+    maps = new_attention_maps(dec, out_len - in_len, B * K, out_len, dev) if output_attentions else None
+    curr_ids = input_ids
+    for frame in range(out_len - in_len):
+        buf = None
         if maps is not None:
-            buf = maps[next_pos - in_len]
-            buf = buf.view(B, K, *buf.shape[1:])[:, 0] if next_pos == in_len else buf
-            extra["output_attentions"] = dec.step_maps(buf, cl, next_pos + 1)
-        if caches is not None:
-            new_emb, last = dec.bert(vis_feats, vis_pe, x_ids, token_type_ids[:, st:next_pos + 1], position_ids[:, st:next_pos + 1],
-                                     attention_mask[:, st:next_pos + 1, :next_pos + 1], output_all_encoded_layers=False,
-                                     len_vis_input=dec.len_vis_input, kv_caches=caches, cache_pos=st, **extra)[:2]
-            new_layers = [last]
-        else:
-            new_emb, new_layers = dec.bert(vis_feats, vis_pe, x_ids, token_type_ids[:, st:next_pos + 1], position_ids[:, st:next_pos + 1],
-                                           attention_mask[:, st:next_pos + 1, :next_pos + 1], prev_embedding=prev_emb,
-                                           prev_encoded_layers=prev_layers, output_all_encoded_layers=True, len_vis_input=dec.len_vis_input,
-                                           **extra)[:2]
-        scores, _ = dec.cls(new_layers[-1][:, -1:, :], None, task_idx=task_idx)
+            buf = maps[frame] if frame else maps[0].view(B, K, *maps.shape[2:])[:, 0]
+        scores, _ = dec.cls(state.step(curr_ids, buf), None, task_idx=task_idx)
         logp = F.log_softmax(scores.float(), dim=-1)                      # [B or B*K, 1, V]
-        frame = next_pos - in_len
         if dec.forbid_duplicate_ngrams and frame >= 1:
             # history of frame `frame` from the previous frame's words and back pointers; blocks in place once it holds n words
             ops.beam_ngram_block(hist[(frame - 1) % 2], hist[frame % 2], step_ptrs[-1], step_ids[-1], frame, ngram, ignore, logp)
-        if dec.min_len and (next_pos - in_len + 1 <= dec.min_len):
+        if dec.min_len and (frame + 1 <= dec.min_len):
             logp[:, :, dec.eos_id] = -10000.0
         kk_scores, kk_ids = torch.topk(logp, k=K)                          # [*, 1, K]
-        first = (next_pos == in_len)
-        if first:
+        if frame == 0:
             k_ids = kk_ids.reshape(B, K)
             back = torch.zeros(B, K, dtype=torch.long, device=dev)
             k_scores = kk_scores.reshape(B, K)
@@ -131,29 +78,12 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
         step_ids.append(k_ids)
         beam_eos.append((k_ids == dec.eos_id).float())
         total_scores.append(k_scores)
-        if first:
-            if shared is not None:
-                pass                                                       # the attention mask stays per image, as the shared cache reads it
-            elif caches is not None:
-                caches = [_expand_beams(c, K).contiguous() for c in caches]
-            else:
-                prev_emb = _expand_beams(new_emb[:, :-1, :], K)
-                prev_layers = [_expand_beams(x[:, :-1, :], K) for x in new_layers]
-            token_type_ids, position_ids = _expand_beams(token_type_ids, K), _expand_beams(position_ids, K)
-            attention_mask = attention_mask if shared is not None else _expand_beams(attention_mask, K)
-            mask_ids = _expand_beams(mask_ids, K)
-            if torch.is_tensor(task_idx) and task_idx.dim() == 1 and task_idx.shape[0] == B:
-                task_idx = _expand_beams(task_idx, K)                      # per-sample ids follow their beams (relaxed head)
-        elif shared is not None:
-            shared.reorder((back + torch.arange(B, device=dev).unsqueeze(1) * K).reshape(-1), frame - 1)
-        elif caches is not None:
-            parent = (back + torch.arange(B, device=dev).unsqueeze(1) * K).reshape(-1)      # beam i continues hypothesis parent[i]
-            caches = [c.index_select(0, parent) for c in caches]
+        if frame == 0:
+            state.expand(K)
+            task_idx = expand_task_idx(task_idx, B, K)                     # per-sample ids follow their beams (relaxed head)
         else:
-            prev_emb = _reorder(torch.cat((prev_emb, new_emb[:, :-1, :]), dim=1), back, B, K)
-            prev_layers = [_reorder(torch.cat((a, b[:, :-1, :]), dim=1), back, B, K) for a, b in zip(prev_layers, new_layers)]
+            state.reorder((back + torch.arange(B, device=dev).unsqueeze(1) * K).reshape(-1))      # beam i continues hypothesis parent[i]
         curr_ids = k_ids.reshape(B * K, 1)
-        next_pos += 1
 
     sc, wi, pt = torch.stack(total_scores), torch.stack(step_ids), torch.stack(step_ptrs)
     out = {"pred_seq": backtrack(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len)}

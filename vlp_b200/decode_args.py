@@ -10,8 +10,7 @@ A script that already defines one of these options (decode_img2txt.py has its ow
 import argparse
 
 from . import ops
-from .sampling import SAMPLING_METHODS, check_sampling_args
-from .shared_prefix import check_num_return_sequences
+from .decode import SAMPLING_METHODS, check_decode
 
 _OPTIONS = (
     ("--beam_size", dict(type=int, default=1, help="beam size for beam search; 1 = greedy, and required when sampling")),
@@ -42,11 +41,10 @@ def add_decode_args(parser):
 
 
 def check_decode_args(args):
-    """ValueError for a combination BertForSeq2SeqDecoder refuses (raised before any model is built)."""
-    check_sampling_args(args.sampling_method, args.topk, args.topp, args.beam_size)
-    if args.forbid_duplicate_ngrams and args.ngram_size < 1:
-        raise ValueError(f"vlp_b200: forbid_duplicate_ngrams needs ngram_size >= 1 (got {args.ngram_size})")
-    check_num_return_sequences(args.num_return_sequences, args.sampling_method, args.beam_size)
+    """ValueError for a combination BertForSeq2SeqDecoder refuses (raised before any model is built); --ngram_size is checked with
+    --forbid_duplicate_ngrams in every mode, greedy included."""
+    check_decode(args.sampling_method, args.topk, args.topp, args.beam_size, args.num_return_sequences, args.forbid_duplicate_ngrams,
+                 args.ngram_size, ngram_in_greedy=True)
 
 
 def parse_decode_args(parser, argv=None):

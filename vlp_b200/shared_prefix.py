@@ -21,24 +21,6 @@ import torch
 from . import ops
 
 
-def check_num_return_sequences(n, sampling_method, beam_size, use_kv_cache=True, output_attentions=False):
-    """Raises ValueError, before anything is launched, for a number of captions per image the decode does not provide."""
-    if isinstance(n, bool) or not isinstance(n, int) or n < 1:
-        raise ValueError(f"vlp_b200: num_return_sequences must be an integer >= 1, got {n!r}")
-    if n == 1:
-        return
-    if sampling_method == "beam_search":
-        if int(beam_size) <= 1:
-            raise ValueError("vlp_b200: num_return_sequences > 1 needs beam search (beam size > 1) or top-k / top-p sampling; "
-                             "greedy decode and sample_mode='sample' return one caption per image")
-        if n > int(beam_size):
-            raise ValueError(f"vlp_b200: num_return_sequences={n} exceeds the beam size {beam_size}")
-    if not use_kv_cache:
-        raise ValueError("vlp_b200: num_return_sequences > 1 needs use_kv_cache (the shared image-prefix cache)")
-    if output_attentions:
-        raise ValueError("vlp_b200: output_attentions is not available with num_return_sequences > 1")
-
-
 class SharedPrefixCache:
     """Per-layer prefix / text caches and the shared slot table of B images x G hypotheses.  Indexing gives the per-layer views
     BertEncoder passes to each BertLayer as its kv_cache."""

@@ -22,6 +22,8 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import ops
+from .beam import beam_search
+from .decode import check_decode, greedy_decode, sample_decode
 
 logger = logging.getLogger(__name__)
 
@@ -845,13 +847,11 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         self.forbid_ignore_set = forbid_ignore_set
         self.ngram_size = ngram_size
         self.min_len = min_len
-        # "topk" / "topp": stochastic decode on the device (vlp_b200/sampling.py) instead of greedy / beam search; beam size 1
-        from .sampling import check_sampling_args
-        check_sampling_args(sampling_method, topk, topp, search_beam_size)
+        # "topk" / "topp": stochastic decode on the device (decode.sample_decode) instead of greedy / beam search; beam size 1.
+        # N > 1: N captions per image (beam search's N best hypotheses, or N samples) over one K/V cache of the image prefix.
+        # forward checks every decode setting again, the n-gram settings included, since callers may change these attributes.
+        check_decode(sampling_method, topk, topp, search_beam_size, num_return_sequences)
         self.sampling_method, self.topk, self.topp, self.seed = sampling_method, topk, topp, seed
-        # N > 1: N captions per image — beam search's N best hypotheses, or N samples — over one K/V cache of the image prefix
-        from .shared_prefix import check_num_return_sequences
-        check_num_return_sequences(num_return_sequences, sampling_method, search_beam_size)
         self.num_return_sequences = num_return_sequences
         self.use_kv_cache = True     # False: the reference's data flow (K, V of the whole prefix re-projected at every step, modeling.py:273-277)
         self._build_region_projections(config, enable_butd)
@@ -860,18 +860,6 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         """One [batch, rows, 2H] bf16 K|V cache per encoder layer; decode passes its output length (token_type_ids.size(1))."""
         H = self.config.hidden_size
         return [torch.empty(batch, rows, 2 * H, device=device, dtype=torch.bfloat16) for _ in self.bert.encoder.layer]
-
-    def new_attention_maps(self, n0, n1, out_len, device):
-        """Zeroed fp32 [n0, n1, layers, heads, out_len] buffer for the [MASK]-row attention maps of a decode: [B, frames, ...] for greedy
-        and sampling, [frames, B*K, ...] (per step, its input rows) for beam search."""
-        cfg = self.config
-        return torch.zeros(n0, n1, cfg.num_hidden_layers, cfg.num_attention_heads, out_len, device=device, dtype=torch.float32)
-
-    @staticmethod
-    def step_maps(buf, row0, n_keys):
-        """BertModelIncr's output_attentions for one decode step: buf [rows, layers, heads, out_len] (a frame of new_attention_maps,
-        any row stride) receives, per layer, query row row0 (the step's [MASK] row) over keys [0, n_keys)."""
-        return row0, [buf[:, l].unsqueeze(2)[..., :n_keys] for l in range(buf.shape[1])]
 
     def forward(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, sample_mode="greedy",
                 seed=None, output_attentions=False):
@@ -883,75 +871,13 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         top-k / top-p sampling returns ids and scores [B, N, out_len - in_len]."""
         self.cls.predictions.check_task_idx(task_idx)          # before anything is launched
         _check_seq_len(self.config, token_type_ids.size(1))
-        from .beam import check_ngram_args
-        check_ngram_args(self)
-        sampling = getattr(self, "sampling_method", "beam_search") != "beam_search"
-        if sampling:
-            from .sampling import check_sampling_args
-            check_sampling_args(self.sampling_method, self.topk, self.topp, self.search_beam_size)
-        from .shared_prefix import check_num_return_sequences
-        check_num_return_sequences(getattr(self, "num_return_sequences", 1), getattr(self, "sampling_method", "beam_search"),
-                                   self.search_beam_size, self.use_kv_cache, output_attentions)
+        check_decode(self.sampling_method, self.topk, self.topp, self.search_beam_size, self.num_return_sequences,
+                     self.forbid_duplicate_ngrams, self.ngram_size, self.use_kv_cache, output_attentions)
         with torch.no_grad():
             vis_feats, vis_pe = self.project_regions(vis_feats, vis_pe)
-            if sampling:
-                from .sampling import sample_decode
-                return sample_decode(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx, seed,
-                                     output_attentions=output_attentions)
+            inputs = (self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx)
+            if self.sampling_method != "beam_search":
+                return sample_decode(*inputs, seed, output_attentions=output_attentions)
             if self.search_beam_size > 1:
-                from .beam import beam_search
-                return beam_search(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx,
-                                   output_attentions=output_attentions)
-            input_length = input_ids.size(1)
-            output_length = token_type_ids.size(1)
-            output_ids, output_probs = [], []
-            prev_embedding, prev_encoded_layers = None, None
-            caches = self.new_kv_caches(input_ids.size(0), input_ids.device, output_length) if self.use_kv_cache else None
-            maps = self.new_attention_maps(input_ids.size(0), output_length - input_length, output_length, input_ids.device) \
-                if output_attentions else None
-            curr_ids = input_ids
-            mask_ids = input_ids[:, :1] * 0 + self.mask_word_id
-            next_pos = input_length
-            while next_pos < output_length:                  # modeling.py:1210-1252
-                curr_length = curr_ids.size(1)
-                start_pos = next_pos - curr_length
-                x_input_ids = torch.cat((curr_ids, mask_ids), dim=1)
-                extra = {} if maps is None else {"output_attentions": self.step_maps(maps[:, next_pos - input_length], curr_length, next_pos + 1)}
-                if caches is not None:
-                    # rows [0, start_pos) of every layer's cache hold K|V of the real tokens decoded so far; this step appends
-                    # (new token, [MASK]) at [start_pos, next_pos] — the [MASK] row is overwritten by the next step's token
-                    new_embedding, new_encoded_layers = self.bert(
-                        vis_feats, vis_pe, x_input_ids, token_type_ids[:, start_pos:next_pos + 1], position_ids[:, start_pos:next_pos + 1],
-                        attention_mask[:, start_pos:next_pos + 1, :next_pos + 1], output_all_encoded_layers=False,
-                        len_vis_input=self.len_vis_input, kv_caches=caches, cache_pos=start_pos, **extra)[:2]
-                    new_encoded_layers = [new_encoded_layers]
-                else:
-                    new_embedding, new_encoded_layers = self.bert(
-                        vis_feats, vis_pe, x_input_ids, token_type_ids[:, start_pos:next_pos + 1], position_ids[:, start_pos:next_pos + 1],
-                        attention_mask[:, start_pos:next_pos + 1, :next_pos + 1], prev_embedding=prev_embedding,
-                        prev_encoded_layers=prev_encoded_layers, output_all_encoded_layers=True, len_vis_input=self.len_vis_input, **extra)[:2]
-                last_hidden = new_encoded_layers[-1][:, -1:, :]
-                prediction_scores, _ = self.cls(last_hidden, None, task_idx=task_idx)
-                if sample_mode == "greedy":
-                    max_probs, max_ids = torch.max(prediction_scores, dim=-1)
-                elif sample_mode == "sample":
-                    ps = prediction_scores.squeeze(1).float()
-                    max_ids = torch.multinomial(F.softmax(ps, dim=-1), num_samples=1, replacement=True)
-                    max_probs = torch.gather(F.log_softmax(ps, dim=-1), 1, max_ids)
-                else:
-                    raise NotImplementedError
-                output_ids.append(max_ids)
-                output_probs.append(max_probs)
-                if caches is not None:
-                    pass
-                elif prev_embedding is None:
-                    prev_embedding = new_embedding[:, :-1, :]
-                    prev_encoded_layers = [x[:, :-1, :] for x in new_encoded_layers]
-                else:
-                    prev_embedding = torch.cat((prev_embedding, new_embedding[:, :-1, :]), dim=1)
-                    prev_encoded_layers = [torch.cat((a, b[:, :-1, :]), dim=1) for a, b in zip(prev_encoded_layers, new_encoded_layers)]
-                curr_ids = max_ids
-                next_pos += 1
-            if maps is not None:
-                return torch.cat(output_ids, dim=1), torch.cat(output_probs, dim=1), maps
-            return torch.cat(output_ids, dim=1), torch.cat(output_probs, dim=1)
+                return beam_search(*inputs, output_attentions=output_attentions)
+            return greedy_decode(*inputs, sample_mode, output_attentions=output_attentions)
