@@ -213,6 +213,18 @@ int vlpk_attn_probs(int B, int heads, int Lq, int Lkv, int row0, const void* q, 
                     int64_t k_bstride, const uint32_t* mask_bits, int mask_rows, int kv_slots, const float* lse, float* p, int64_t ld_p,
                     int64_t p_bstride, void* stream);
 
+/* Attention core with a per-row self key (forward only, eval: no dropout), for scoring given captions (vlpk_encoder_score_fwd):
+ *   ctx_i = softmax([ q_i . k_j / 8 + mask_add(i, j) for j < Lkv ] ++ [ q_i . k_self_i / 8 ]) [ v_0 .. v_{Lkv-1} ; v_self_i ]
+ * The self key of query row i is the row k_self + b * q_bstride + i * ld_q (v_self alike: the strides of q), and no mask bit hides
+ * it.  lse [B, heads, Lq] is the logsumexp over all Lkv + 1 scores.  q / ctx: Lq rows per sequence, sequences q_bstride / ctx_bstride
+ * apart (0: Lq * ld); k / v: Lkv rows, kv_bstride apart (0: Lkv * ld_kv).  mask_bits: [B, Lq, S / 32], one row per query row, with
+ * kv_slots as for vlpk_attn_core_fwd_wide, except that Lq need not be <= kv_slots.  Lq, Lkv in [1, 512]; both <= 128: the single-tile
+ * kernel, else the KV-tiled one.  < 0 with nothing launched on bad lengths or kv_slots, a NULL pointer, or self rows that are not
+ * 16-byte aligned. */
+int vlpk_attn_core_self_fwd(int B, int heads, int Lq, int Lkv, const void* q, int64_t ld_q, int64_t q_bstride, const void* k, const void* v,
+                            int64_t ld_kv, int64_t kv_bstride, const void* k_self, const void* v_self, const uint32_t* mask_bits, int kv_slots,
+                            void* ctx, int64_t ld_ctx, int64_t ctx_bstride, float* lse, void* stream);
+
 /* BertAttention.forward (modeling.py:326-330): QKV projection + attention core + output projection + LN.
  * x_kv == NULL or == x: self-attention over x (training / encoder path).
  * x_kv != x: incremental decode (modeling.py:273-277): keys/values projected from x_kv = cat(history, x), [B*Lkv,H]. */
@@ -275,6 +287,23 @@ int vlpk_workspace_bytes(const VlpkShape* s, size_t* out3);
 /* BertEncoder.forward (modeling.py:382-402): n_layers x BertLayer in one host call.  acts[i].y is layer i's output. */
 int vlpk_encoder_fwd(const VlpkShape* s, int n_layers, const VlpkLayerWeights* w, const void* x, const uint32_t* mask_bits,
                      int mask_rows, VlpkLayerActs* acts, float p_attn, float p_hidden, const VlpkDropout* drop, void* stream);
+/* Teacher-forced scoring pass of the seq2seq decoder (forward only, eval, no dropout): n_layers x BertLayer over B sequences of
+ * S + T rows, x [B, S + T, H].  Rows [0, S) are shared rows ([CLS] regions [SEP] and the caption words but the last); rows [S, S + T)
+ * are query rows ([MASK]).  Per layer: QKV projection, output projection, both LayerNorms and the FFN over all S + T rows; attention
+ * in two launches: shared rows against the shared rows under shared_bits [B, S, S' / 32], then query rows against the shared rows
+ * under query_bits [B, T, S' / 32] plus each query row's own key (vlpk_attn_core_self_fwd); S' = 128 * ceil(S / 128).
+ *   s: B, Lq = Lkv = S, H, heads, I, kv_slots (as for an S-row encoder);  T in [1, 512].
+ *   acts[i]: layer i's buffers sized for B * (S + T) rows (vlpk_encoder_score_workspace_bytes; kv and drop_attn unused); lse holds
+ *   [B, heads, S] of the shared rows, then [B, heads, T] of the query rows.  Layer i reads acts[i - 1].y, so two buffers used in turn
+ *   serve any depth.
+ * One host call, no allocation, no host synchronisation.  < 0 with nothing launched for: a bad shape, Lq != Lkv, T outside [1, 512],
+ * H not a multiple of 128, a NULL pointer, a layer's output aliasing its input, or x / mask bits / qkv / ctx not 16-byte aligned. */
+int vlpk_encoder_score_fwd(const VlpkShape* s, int T, int n_layers, const VlpkLayerWeights* w, const void* x, const uint32_t* shared_bits,
+                           const uint32_t* query_bits, VlpkLayerActs* acts, void* stream);
+/* Host-only: bytes of one layer's VlpkLayerActs buffers for vlpk_encoder_score_fwd (the layout of vlpk_workspace_bytes' out3[0] over
+ * B * (S + T) rows, without kv).  A separate entry point because a VlpkShape cannot describe the scoring stack: its rows per sequence
+ * (S + T, up to 1023) exceed the 512 vlpk_workspace_bytes' shape check allows, and the attention's key count S differs from them. */
+int vlpk_encoder_score_workspace_bytes(const VlpkShape* s, int T, size_t* out1);
 /* Backward of the stack.  dys[i] (may be NULL) is the gradient flowing into layer i's output from outside the stack
  * (output_all_encoded_layers consumers); dys[n_layers-1] is normally the only non-NULL entry.  dx0 receives d/dx. */
 int vlpk_encoder_bwd(const VlpkShape* s, int n_layers, const VlpkLayerWeights* w, const void* x, const uint32_t* mask_bits,

@@ -81,6 +81,8 @@ _SIGS = {
                                         C.POINTER(VlpkDropout), c_u64, c_int, _P]),
     "vlpk_attn_core_bwd_wide": (c_int, [c_int, c_int, c_int, _P, _P, _P, c_i64, _P, c_int, _P, _P, c_i64, _P, _P, _P, _P, c_i64,
                                         C.POINTER(VlpkDropout), c_u64, c_int, _P]),
+    "vlpk_attn_core_self_fwd": (c_int, [c_int, c_int, c_int, c_int, _P, c_i64, c_i64, _P, _P, c_i64, c_i64, _P, _P, _P, c_int, _P, c_i64,
+                                        c_i64, _P, _P]),
     "vlpk_attn_probs": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, c_i64, c_i64, _P, c_i64, c_i64, _P, c_int, c_int, _P, _P, c_i64,
                                 c_i64, _P]),
     "vlpk_mha_fwd": (c_int, [C.POINTER(VlpkShape), C.POINTER(VlpkLayerWeights), _P, _P, _P, c_int, C.POINTER(VlpkLayerActs),
@@ -106,6 +108,9 @@ _SIGS = {
     "vlpk_workspace_bytes": (c_int, [C.POINTER(VlpkShape), C.POINTER(C.c_size_t)]),
     "vlpk_encoder_fwd": (c_int, [C.POINTER(VlpkShape), c_int, C.POINTER(VlpkLayerWeights), _P, _P, c_int,
                                  C.POINTER(VlpkLayerActs), c_float, c_float, C.POINTER(VlpkDropout), _P]),
+    "vlpk_encoder_score_fwd": (c_int, [C.POINTER(VlpkShape), c_int, c_int, C.POINTER(VlpkLayerWeights), _P, _P, _P, C.POINTER(VlpkLayerActs),
+                                       _P]),
+    "vlpk_encoder_score_workspace_bytes": (c_int, [C.POINTER(VlpkShape), c_int, C.POINTER(C.c_size_t)]),
     "vlpk_encoder_bwd": (c_int, [C.POINTER(VlpkShape), c_int, C.POINTER(VlpkLayerWeights), _P, _P, c_int,
                                  C.POINTER(VlpkLayerActs), C.POINTER(c_void_p), _P, C.POINTER(VlpkLayerGrads),
                                  C.POINTER(VlpkBwdScratch), c_float, c_float, C.POINTER(VlpkDropout), _P]),

@@ -161,6 +161,21 @@ struct KvCache {       // incremental decode with a persistent K/V cache (vlpk_l
   const AttnGroupKv* group = nullptr;  // vlpk_layer_cached_group_fwd: base / rows / pos are the text cache, keys from the group loader
 };
 
+// Packed QKV projection of M rows x [M, H] -> qkv [M, 3H]: the three [H,H] weights read in place as N-segments.
+int qkv_fwd(int M, int H, const VlpkLayerWeights* w, const void* x, void* qkv, cudaStream_t st) {
+  if (H % 128 != 0) { set_error("mha_fwd: H=%d must be a multiple of 128 for the packed QKV projection", H); return -1; }
+  GemmDesc g;
+  g.M = M; g.N = 3 * H; g.K = H;
+  g.A = x; g.lda = H;
+  g.nseg = 3; g.b_seg_rows = H; g.ldb = H;
+  g.B[0] = w->wq; g.B[1] = w->wk; g.B[2] = w->wv;
+  g.bias[0] = static_cast<const bf16*>(w->bq); g.bias[1] = static_cast<const bf16*>(w->bk); g.bias[2] = static_cast<const bf16*>(w->bv);
+  g.D0 = qkv; g.ldd0 = 3 * H;
+  g.epi = EPI_STORE;
+  g.bn = (H % 256 == 0) ? 0 : 128;
+  return launch_gemm(g, st);
+}
+
 // BertSelfOutput after the attention core: output projection of a->ctx, residual x, dropout, LayerNorm -> a->y1
 int attn_out_ln(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, VlpkLayerActs* a, float p_hidden, const VlpkDropout* drop,
                 uint64_t layer_id, cudaStream_t st) {
@@ -218,17 +233,7 @@ int mha_fwd_impl(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, c
     }
   } else if (!incr) {
     VLPK_CHECK_ARG(s->Lq == s->Lkv, "mha_fwd: Lq != Lkv requires x_kv");
-    GemmDesc g;  // packed QKV projection: three [H,H] weights read in place as N-segments
-    g.M = Mq; g.N = 3 * H; g.K = H;
-    g.A = x; g.lda = H;
-    g.nseg = 3; g.b_seg_rows = H; g.ldb = H;
-    g.B[0] = w->wq; g.B[1] = w->wk; g.B[2] = w->wv;
-    g.bias[0] = static_cast<const bf16*>(w->bq); g.bias[1] = static_cast<const bf16*>(w->bk); g.bias[2] = static_cast<const bf16*>(w->bv);
-    g.D0 = a->qkv; g.ldd0 = 3 * H;
-    g.epi = EPI_STORE;
-    g.bn = (H % 256 == 0) ? 0 : 128;
-    if (H % 128 != 0) { set_error("mha_fwd: H=%d must be a multiple of 128 for the packed QKV projection", H); return -1; }
-    VLPK_TRY(launch_gemm(g, st));
+    VLPK_TRY(qkv_fwd(Mq, H, w, x, a->qkv, st));
     ad.q = a->qkv; ad.ld_q = 3 * H;
     ad.k = static_cast<const bf16*>(a->qkv) + H;
     ad.v = static_cast<const bf16*>(a->qkv) + 2 * H;
@@ -397,6 +402,42 @@ __global__ void relu_bwd_kernel(bf16* __restrict__ dpre, const bf16* __restrict_
     o[j] = pack_bf16x2(v.x > 0.f ? d.x * scale : 0.f, v.y > 0.f ? d.y * scale : 0.f);
   }
   *reinterpret_cast<uint4*>(dpre + i) = make_uint4(o[0], o[1], o[2], o[3]);
+}
+
+// One layer of vlpk_encoder_score_fwd over B sequences of S + T rows (S shared rows, then T query rows).  s: Lq = Lkv = S.
+int score_layer_fwd(const VlpkShape* s, int T, const VlpkLayerWeights* w, const void* x, const uint32_t* shared_bits,
+                    const uint32_t* query_bits, VlpkLayerActs* a, uint64_t layer_id, cudaStream_t st) {
+  const int H = s->H, S = s->Lq, R = S + T;
+  const DropoutCfg none = make_dropout(0.f, 0, 0);
+  VLPK_TRY(qkv_fwd(s->B * R, H, w, x, a->qkv, st));
+  const bf16* qkv = static_cast<const bf16*>(a->qkv);
+  // shared rows against the shared rows
+  AttnDesc ad;
+  ad.B = s->B; ad.heads = s->heads; ad.Lq = S; ad.Lkv = S; ad.kv_slots = s->kv_slots;
+  ad.q = qkv; ad.k = qkv + H; ad.v = qkv + 2 * H;
+  ad.ld_q = ad.ld_kv = 3 * H;
+  ad.q_batch_stride = ad.kv_batch_stride = static_cast<int64_t>(R) * 3 * H;
+  ad.o = a->ctx; ad.ld_o = H; ad.o_batch_stride = static_cast<int64_t>(R) * H;
+  ad.mask_bits = shared_bits; ad.mask_rows = S;
+  ad.lse = a->lse;
+  ad.drop = none;
+  VLPK_TRY(launch_attn_fwd(ad, st));
+  // query rows against the shared rows, each plus its own key
+  AttnDesc qd = ad;
+  qd.Lq = T;
+  qd.q = qkv + static_cast<size_t>(S) * 3 * H;
+  qd.o = static_cast<bf16*>(a->ctx) + static_cast<size_t>(S) * H;
+  qd.mask_bits = query_bits; qd.mask_rows = T;
+  qd.lse = a->lse + static_cast<size_t>(s->B) * s->heads * S;
+  AttnSelfKv sk;
+  sk.k = qkv + static_cast<size_t>(S) * 3 * H + H;
+  sk.v = qkv + static_cast<size_t>(S) * 3 * H + 2 * H;
+  sk.ld = 3 * H; sk.batch_stride = static_cast<int64_t>(R) * 3 * H;
+  VLPK_TRY(launch_attn_fwd_self(qd, sk, st));
+  VlpkShape rows = *s;  // the row-wise tail (output projection, LayerNorms, FFN) over all B * (S + T) rows
+  rows.Lq = rows.Lkv = R;
+  VLPK_TRY(attn_out_ln(&rows, w, x, a, 0.f, nullptr, layer_id, st));
+  return ffn_fwd_impl(&rows, w, a, 0.f, nullptr, layer_id, st);
 }
 
 }  // namespace
@@ -568,6 +609,20 @@ int vlpk_attn_core_fwd(int B, int heads, int Lq, int Lkv, const void* q, int64_t
   return vlpk_attn_core_fwd_wide(B, heads, Lq, Lkv, q, ld_q, k, v, ld_kv, mask_bits, mask_rows, ctx, ld_ctx, lse, drop, site, 0, stream);
 }
 
+int vlpk_attn_core_self_fwd(int B, int heads, int Lq, int Lkv, const void* q, int64_t ld_q, int64_t q_bstride, const void* k, const void* v,
+                            int64_t ld_kv, int64_t kv_bstride, const void* k_self, const void* v_self, const uint32_t* mask_bits, int kv_slots,
+                            void* ctx, int64_t ld_ctx, int64_t ctx_bstride, float* lse, void* stream) {
+  AttnDesc d;
+  d.B = B; d.heads = heads; d.Lq = Lq; d.Lkv = Lkv; d.kv_slots = kv_slots;
+  d.q = q; d.ld_q = ld_q; d.q_batch_stride = q_bstride;
+  d.k = k; d.v = v; d.ld_kv = ld_kv; d.kv_batch_stride = kv_bstride;
+  d.o = ctx; d.ld_o = ld_ctx; d.o_batch_stride = ctx_bstride;
+  d.mask_bits = mask_bits; d.mask_rows = Lq; d.lse = lse;
+  AttnSelfKv s;
+  s.k = k_self; s.v = v_self; s.ld = ld_q; s.batch_stride = q_bstride;
+  return launch_attn_fwd_self(d, s, S(stream));
+}
+
 int vlpk_attn_probs(int B, int heads, int Lq, int Lkv, int row0, const void* q, int64_t ld_q, int64_t q_bstride, const void* k, int64_t ld_k,
                     int64_t k_bstride, const uint32_t* mask_bits, int mask_rows, int kv_slots, const float* lse, float* p, int64_t ld_p,
                     int64_t p_bstride, void* stream) {
@@ -708,6 +763,41 @@ int vlpk_encoder_fwd(const VlpkShape* s, int n_layers, const VlpkLayerWeights* w
   for (int i = 0; i < n_layers; ++i) {
     VLPK_TRY(mha_fwd_impl(s, &w[i], cur, nullptr, mask_bits, mask_rows, &acts[i], p_attn, p_hidden, drop, i, S(stream)));
     VLPK_TRY(ffn_fwd_impl(s, &w[i], &acts[i], p_hidden, drop, i, S(stream)));
+    cur = acts[i].y;
+  }
+  return 0;
+}
+
+int vlpk_encoder_score_workspace_bytes(const VlpkShape* s, int T, size_t* out1) {
+  VLPK_TRY(check_shape(s));
+  VLPK_CHECK_ARG(out1 != nullptr, "encoder_score_workspace_bytes: null output");
+  VLPK_CHECK_ARG(s->Lq == s->Lkv && T >= 1 && T <= 512, "encoder_score: Lq=%d must equal Lkv=%d (the shared rows S), T=%d in [1,512]", s->Lq,
+                 s->Lkv, T);
+  const size_t H = s->H, I = s->I, M = static_cast<size_t>(s->B) * (s->Lq + T);
+  const size_t lse = (static_cast<size_t>(s->B) * s->heads * (s->Lq + T) + 3) / 4 * 4;
+  out1[0] = 2 * M * (3 * H + 5 * H + 2 * I) + 4 * (lse + 4 * M);
+  return 0;
+}
+
+int vlpk_encoder_score_fwd(const VlpkShape* s, int T, int n_layers, const VlpkLayerWeights* w, const void* x, const uint32_t* shared_bits,
+                           const uint32_t* query_bits, VlpkLayerActs* acts, void* stream) {
+  VLPK_TRY(check_shape(s));
+  VLPK_CHECK_ARG(s->Lq == s->Lkv && T >= 1 && T <= 512, "encoder_score: Lq=%d must equal Lkv=%d (the shared rows S), T=%d in [1,512]", s->Lq,
+                 s->Lkv, T);
+  VLPK_CHECK_ARG(s->H % 128 == 0, "encoder_score: H=%d must be a multiple of 128 for the packed QKV projection", s->H);
+  VLPK_CHECK_ARG(n_layers > 0 && w && x && shared_bits && query_bits && acts, "encoder_score: null pointer");
+  const auto al = [](const void* p, uintptr_t n) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & (n - 1)) == 0; };
+  VLPK_CHECK_ARG(al(x, 16) && al(shared_bits, 16) && al(query_bits, 16), "encoder_score: x and the mask bits must be 16-byte aligned");
+  for (int i = 0; i < n_layers; ++i) {  // every layer's buffers, so that no check fails after a launch
+    const VlpkLayerActs& a = acts[i];
+    VLPK_CHECK_ARG(al(a.qkv, 16) && al(a.ctx, 16) && al(a.t1, 16) && al(a.y1, 16) && al(a.u, 16) && al(a.hmid, 16) && al(a.t2, 16) &&
+                   al(a.y, 16) && al(a.lse, 4) && al(a.stats1, 8) && al(a.stats2, 8) && (i == 0 || a.y != acts[i - 1].y),
+                   "encoder_score: layer %d acts missing or misaligned (16-byte bf16 buffers, 4-byte lse, 8-byte statistics), or its output "
+                   "aliases its input", i);
+  }
+  const void* cur = x;
+  for (int i = 0; i < n_layers; ++i) {
+    VLPK_TRY(score_layer_fwd(s, T, &w[i], cur, shared_bits, query_bits, &acts[i], i, S(stream)));
     cur = acts[i].y;
   }
   return 0;

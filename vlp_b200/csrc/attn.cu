@@ -141,6 +141,66 @@ __device__ __forceinline__ void group_fill(uint8_t* sK, uint8_t* sV, const Group
 }
 
 // ------------------------------------------------------------------------------------------------
+// per-row self key (vlpk_encoder_score_fwd): query row i of sequence b also attends to one extra key, its own (k_i, v_i), which no
+// mask hides.  Its score q_i . k_i / 8 joins the row's maximum and sums after the shared keys (the O accumulator and sums rescaled to
+// the new maximum), and p_self v_i joins O, so the softmax runs over [shared keys | self] and the saved logsumexp includes the self
+// term.  Row i reads k / v at k + b * bstride + i * ld (the same for v); rows past Lq read row Lq - 1 (never stored).
+// ------------------------------------------------------------------------------------------------
+struct SelfKv {
+  const __nv_bfloat16* k;
+  const __nv_bfloat16* v;
+  long long ld, bstride;
+};
+
+// This thread's two rows' self scores in the log2 domain (scaled, unmasked): q_i . k_i with q from the swizzled Q tile (local rows
+// lr[hh]) and k from global memory; each thread of a quad takes 16 of the 64 dimensions.
+__device__ __forceinline__ void self_scores(const uint8_t* sQ, const SelfKv& sk, int b, int h, const int (&lr)[2], const int (&row)[2],
+                                            int Lq, float (&ss)[2]) {
+  const int qi = threadIdx.x & 3;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const __nv_bfloat16* kp = sk.k + b * sk.bstride + static_cast<long long>(min(row[hh], Lq - 1)) * sk.ld + h * HD;
+    float acc = 0.f;
+#pragma unroll
+    for (int c = 2 * qi; c < 2 * qi + 2; ++c) {
+      const uint4 q4 = *reinterpret_cast<const uint4*>(sQ + lr[hh] * 128 + ((c ^ (lr[hh] & 7)) << 4));
+      const uint4 k4 = __ldg(reinterpret_cast<const uint4*>(kp + c * 8));
+      const uint32_t qw[4] = {q4.x, q4.y, q4.z, q4.w}, kw[4] = {k4.x, k4.y, k4.z, k4.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 a = unpack_bf16x2(qw[j]), k2 = unpack_bf16x2(kw[j]);
+        acc = fmaf(a.x, k2.x, fmaf(a.y, k2.y, acc));
+      }
+    }
+    ss[hh] = quad_sum(acc) * (0.125f * LOG2E);
+  }
+}
+
+// Folds the self key into a finished row (quad-reduced mx / lsum / rsum, unnormalised o) as one more online-softmax step.
+__device__ __forceinline__ void fold_self(const SelfKv& sk, const Frag& f, int b, int h, const int (&row)[2], int Lq, const float (&ss)[2],
+                                          float (&mx)[2], float (&lsum)[2], float (&rsum)[2], float (&o)[32]) {
+  float alpha[2], es[2];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const float mnew = fmaxf(mx[hh], ss[hh]);
+    alpha[hh] = fast_ex2(mx[hh] - mnew);
+    const float x = fast_ex2(ss[hh] - mnew);
+    es[hh] = bf16_round(x);  // the self term enters O and the normalising sum as the bf16 value the shared keys' P would be
+    lsum[hh] = lsum[hh] * alpha[hh] + x;
+    rsum[hh] = rsum[hh] * alpha[hh] + es[hh];
+    mx[hh] = mnew;
+  }
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    const int hh = (i >> 1) & 1, col = 8 * (i >> 2) + f.fc;
+    const __nv_bfloat16* vp = sk.v + b * sk.bstride + static_cast<long long>(min(row[hh], Lq - 1)) * sk.ld + h * HD + col;
+    const float2 v2 = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(vp)));
+    o[i] = fmaf(es[hh], v2.x, o[i] * alpha[hh]);
+    o[i + 1] = fmaf(es[hh], v2.y, o[i + 1] * alpha[hh]);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // forward  (256 threads, 48 KB smem: Q | K | V; the Q tile is reused as output staging)
 // ------------------------------------------------------------------------------------------------
 struct FwdSmem {
@@ -154,8 +214,10 @@ struct FwdSmem {
 
 // GROUP: K/V from a shared prefix + text rows (GroupKv); grid (G * heads, images), so the G hypotheses of an image and head run
 // next to each other and read its prefix box from L2.  Otherwise grid (heads, B) and K/V from tm.k / tm.v.
-template <bool GROUP>
-__device__ __forceinline__ void attn_fwd_body(const AttnTmaps& tm, const AttnArgs a, const GroupKv g) {
+// SELF: every query row also attends to its own key (SelfKv), folded in after the shared keys; no dropout.
+template <bool GROUP, bool SELF>
+__device__ __forceinline__ void attn_fwd_body(const AttnTmaps& tm, const AttnArgs a, const GroupKv g, const SelfKv sk) {
+  static_assert(!(GROUP && SELF), "a per-row self key is not combined with the shared-prefix loader");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem + FwdSmem::OFF_Q;
@@ -256,7 +318,7 @@ __device__ __forceinline__ void attn_fwd_body(const AttnTmaps& tm, const AttnArg
   for (int hh = 0; hh < 2; ++hh) {
     rsum[hh] = quad_sum(rsum[hh]);
     lsum[hh] = quad_sum(lsum[hh]);
-    if (qi == 0 && a.lse != nullptr && row[hh] < a.Lq)
+    if (!SELF && qi == 0 && a.lse != nullptr && row[hh] < a.Lq)
       a.lse[(static_cast<size_t>(b) * a.heads + h) * a.Lq + row[hh]] = (mx[hh] + log2f(lsum[hh])) * LN2;
   }
   // O = P V
@@ -270,6 +332,15 @@ __device__ __forceinline__ void attn_fwd_body(const AttnTmaps& tm, const AttnArg
     wgmma_commit();
     wgmma_wait<0>();
     reg_fence(o);
+  }
+  if constexpr (SELF) {  // this warpgroup's Q rows are still in its half of the Q tile: staging below overwrites them
+    float ss[2];
+    self_scores(sQ, sk, b, h, row, row, a.Lq, ss);
+    fold_self(sk, f, b, h, row, a.Lq, ss, mx, lsum, rsum, o);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+      if (qi == 0 && a.lse != nullptr && row[hh] < a.Lq)
+        a.lse[(static_cast<size_t>(b) * a.heads + h) * a.Lq + row[hh]] = (mx[hh] + log2f(lsum[hh])) * LN2;
   }
   // O / rowsum -> bf16 -> this warpgroup's half of the (dead) Q tile -> one TMA store of the whole tile
   const float inv[2] = {1.0f / rsum[0], 1.0f / rsum[1]};
@@ -289,12 +360,17 @@ __device__ __forceinline__ void attn_fwd_body(const AttnTmaps& tm, const AttnArg
 }
 
 __global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a) {
-  attn_fwd_body<false>(tm, a, GroupKv{});
+  attn_fwd_body<false, false>(tm, a, GroupKv{}, SelfKv{});
 }
 
 __global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_group_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a,
                                                                          const GroupKv g) {
-  attn_fwd_body<true>(tm, a, g);
+  attn_fwd_body<true, false>(tm, a, g, SelfKv{});
+}
+
+__global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_self_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a,
+                                                                        const SelfKv sk) {
+  attn_fwd_body<false, true>(tm, a, GroupKv{}, sk);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -535,8 +611,10 @@ struct FwdTiledSmem {
 
 // One CTA per SM: the running O (32 registers) stays live beside S and P, which does not fit the 128 registers of two CTAs.
 // GROUP: as attn_fwd_body; a key tile that starts at or past the prefix gets no TMA box (its barrier is arrived on without bytes).
-template <bool GROUP>
-__device__ __forceinline__ void attn_fwd_tiled_body(const AttnTmaps& tm, const AttnTiledArgs a, const GroupKv g) {
+// SELF: as attn_fwd_body.
+template <bool GROUP, bool SELF>
+__device__ __forceinline__ void attn_fwd_tiled_body(const AttnTmaps& tm, const AttnTiledArgs a, const GroupKv g, const SelfKv sk) {
+  static_assert(!(GROUP && SELF), "a per-row self key is not combined with the shared-prefix loader");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem + FwdTiledSmem::OFF_Q;
@@ -676,8 +754,18 @@ __device__ __forceinline__ void attn_fwd_tiled_body(const AttnTmaps& tm, const A
   for (int hh = 0; hh < 2; ++hh) {
     rsum[hh] = quad_sum(rsum[hh]);
     lsum[hh] = quad_sum(lsum[hh]);
-    if (qi == 0 && a.lse != nullptr && row[hh] < a.Lq)
+    if (!SELF && qi == 0 && a.lse != nullptr && row[hh] < a.Lq)
       a.lse[(static_cast<size_t>(b) * a.heads + h) * a.Lq + row[hh]] = (mx[hh] + log2f(lsum[hh])) * LN2;
+  }
+  if constexpr (SELF) {
+    const int lr[2] = {wg * 64 + f.fr, wg * 64 + f.fr + 8};
+    float ss[2];
+    self_scores(sQ, sk, b, h, lr, row, a.Lq, ss);
+    fold_self(sk, f, b, h, row, a.Lq, ss, mx, lsum, rsum, o);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+      if (qi == 0 && a.lse != nullptr && row[hh] < a.Lq)
+        a.lse[(static_cast<size_t>(b) * a.heads + h) * a.Lq + row[hh]] = (mx[hh] + log2f(lsum[hh])) * LN2;
   }
   const float inv[2] = {1.0f / rsum[0], 1.0f / rsum[1]};
   uint8_t* stg = sQ + wg * 8192;  // this warpgroup's own Q rows: only its own S = QK^T read them
@@ -696,12 +784,17 @@ __device__ __forceinline__ void attn_fwd_tiled_body(const AttnTmaps& tm, const A
 }
 
 __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_tiled_kernel(const __grid_constant__ AttnTmaps tm, const AttnTiledArgs a) {
-  attn_fwd_tiled_body<false>(tm, a, GroupKv{});
+  attn_fwd_tiled_body<false, false>(tm, a, GroupKv{}, SelfKv{});
 }
 
 __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_group_tiled_kernel(const __grid_constant__ AttnTmaps tm, const AttnTiledArgs a,
                                                                                const GroupKv g) {
-  attn_fwd_tiled_body<true>(tm, a, g);
+  attn_fwd_tiled_body<true, false>(tm, a, g, SelfKv{});
+}
+
+__global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_self_tiled_kernel(const __grid_constant__ AttnTmaps tm, const AttnTiledArgs a,
+                                                                              const SelfKv sk) {
+  attn_fwd_tiled_body<false, true>(tm, a, GroupKv{}, sk);
 }
 
 // P (recomputed from the logsumexp; 0 for keys >= Lkv and rows >= Lq) and the dropout-masked dP of one 64 x 128 (q, key) block,
@@ -1178,17 +1271,20 @@ static int launch_attn_bwd_tiled(const AttnDesc& d, const AttnTmaps& tm, cudaStr
   return 0;
 }
 
-int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream) {
-  VLPK_TRY(check_common(d));
+// Tensor maps of a forward over contiguous K/V: Q / ctx and K / V with their row and sequence strides.
+static int fwd_tmaps(const AttnDesc& d, AttnTmaps* tm) {
   const int width = d.heads * HD;
-  AttnTmaps tm;
-  memset(&tm, 0, sizeof(tm));
-  VLPK_TRY(make_seq_tmap(&tm.q, d.q, width, d.Lq, d.B, d.ld_q));
-  VLPK_TRY(make_seq_tmap(&tm.k, d.k, width, d.Lkv, d.B, d.ld_kv, d.kv_batch_stride));
-  VLPK_TRY(make_seq_tmap(&tm.v, d.v, width, d.Lkv, d.B, d.ld_kv, d.kv_batch_stride));
-  VLPK_TRY(make_seq_tmap(&tm.o, d.o, width, d.Lq, d.B, d.ld_o));
-  tm.dq = tm.dk = tm.dv = tm.o;
-  if (use_tiled(d)) return launch_attn_fwd_tiled(d, tm, stream);
+  memset(tm, 0, sizeof(*tm));
+  VLPK_TRY(make_seq_tmap(&tm->q, d.q, width, d.Lq, d.B, d.ld_q, d.q_batch_stride));
+  VLPK_TRY(make_seq_tmap(&tm->k, d.k, width, d.Lkv, d.B, d.ld_kv, d.kv_batch_stride));
+  VLPK_TRY(make_seq_tmap(&tm->v, d.v, width, d.Lkv, d.B, d.ld_kv, d.kv_batch_stride));
+  VLPK_TRY(make_seq_tmap(&tm->o, d.o, width, d.Lq, d.B, d.ld_o, d.o_batch_stride));
+  tm->dq = tm->dk = tm->dv = tm->o;
+  return 0;
+}
+
+// Arguments of the single-tile forward kernels.
+static AttnArgs fwd_args(const AttnDesc& d) {
   AttnArgs a;
   a.B = d.B; a.heads = d.heads; a.Lq = d.Lq; a.Lkv = d.Lkv;
   a.mask_bits = d.mask_bits; a.mask_rows = d.mask_rows;
@@ -1196,6 +1292,15 @@ int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream) {
   a.drop = d.drop;
   a.keep_out = d.keep_out;
   a.dbias_part = nullptr;
+  return a;
+}
+
+int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream) {
+  VLPK_TRY(check_common(d));
+  AttnTmaps tm;
+  VLPK_TRY(fwd_tmaps(d, &tm));
+  if (use_tiled(d)) return launch_attn_fwd_tiled(d, tm, stream);
+  const AttnArgs a = fwd_args(d);
   static bool attr_set = false;
   if (!attr_set) {
     VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem::DYN));
@@ -1252,6 +1357,49 @@ int launch_attn_fwd_group(const AttnDesc& d, const AttnGroupKv& gd, cudaStream_t
     attr_set = true;
   }
   VLPK_CUDA(launch_ex(attn_fwd_group_kernel, dim3(grid.x, grid.y), dim3(ATT_THREADS), FwdSmem::DYN, stream, 1, tm, a, g));
+  return 0;
+}
+
+int launch_attn_fwd_self(const AttnDesc& d, const AttnSelfKv& sd, cudaStream_t stream) {
+  VLPK_CHECK_ARG(d.head_dim == HD, "attention self: head_dim %d unsupported (only 64)", d.head_dim);
+  VLPK_CHECK_ARG(d.B >= 1 && d.heads >= 1 && d.Lq >= 1 && d.Lq <= MAX_SLOTS && d.Lkv >= 1 && d.Lkv <= MAX_SLOTS,
+                 "attention self: B=%d heads=%d Lq=%d Lkv=%d (lengths in [1,512])", d.B, d.heads, d.Lq, d.Lkv);
+  VLPK_CHECK_ARG(d.kv_slots == 0 ? d.Lkv <= TL : d.kv_slots == (d.Lkv + TL - 1) / TL * TL,
+                 "attention self: kv_slots=%d for Lkv=%d (0 needs Lkv <= 128, else 128 * ceil(Lkv / 128))", d.kv_slots, d.Lkv);
+  VLPK_CHECK_ARG(d.mask_bits != nullptr && d.mask_rows == d.Lq, "attention self: one mask row per query row needed (%d for Lq=%d)",
+                 d.mask_rows, d.Lq);
+  VLPK_CHECK_ARG(d.q && d.k && d.v && d.o && sd.k && sd.v, "attention self: null pointer");
+  VLPK_CHECK_ARG(d.drop.p == 0.f && d.keep_out == nullptr, "attention self: forward only, without dropout");
+  const auto a16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15u) == 0; };
+  VLPK_CHECK_ARG(a16(sd.k) && a16(sd.v) && sd.ld % 8 == 0 && sd.batch_stride % 8 == 0 && sd.ld >= d.heads * HD,
+                 "attention self: self keys / values need 16-byte rows (ld=%lld, batch stride=%lld)", static_cast<long long>(sd.ld),
+                 static_cast<long long>(sd.batch_stride));
+  AttnTmaps tm;
+  VLPK_TRY(fwd_tmaps(d, &tm));
+  SelfKv sk;
+  sk.k = static_cast<const __nv_bfloat16*>(sd.k);
+  sk.v = static_cast<const __nv_bfloat16*>(sd.v);
+  sk.ld = sd.ld;
+  sk.bstride = sd.batch_stride != 0 ? sd.batch_stride : static_cast<int64_t>(d.Lq) * sd.ld;
+  LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * (d.Lkv + 1) * HD, stream);
+  if (use_tiled(d)) {
+    const AttnTiledArgs a = tiled_args(d);
+    static bool attr_set = false;
+    if (!attr_set) {
+      VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_self_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdTiledSmem::DYN));
+      attr_set = true;
+    }
+    VLPK_CUDA(launch_ex(attn_fwd_self_tiled_kernel, dim3(d.heads, d.B, (d.Lq + TL - 1) / TL), dim3(ATT_THREADS), FwdTiledSmem::DYN, stream,
+                        1, tm, a, sk));
+    return 0;
+  }
+  const AttnArgs a = fwd_args(d);  // keep_out is null: checked above
+  static bool attr_set = false;
+  if (!attr_set) {
+    VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_self_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem::DYN));
+    attr_set = true;
+  }
+  VLPK_CUDA(launch_ex(attn_fwd_self_kernel, dim3(d.heads, d.B), dim3(ATT_THREADS), FwdSmem::DYN, stream, 1, tm, a, sk));
   return 0;
 }
 

@@ -16,6 +16,7 @@ struct AttnDesc {
   int64_t kv_batch_stride = 0;  // elements between consecutive sequences of K / V (0 = Lkv * ld_kv); a K/V cache has cache_rows * ld_kv
   void* o = nullptr;  // ctx [B, Lq, ld_o]   (bwd: forward output, read for delta)
   int64_t ld_o = 0;
+  int64_t q_batch_stride = 0, o_batch_stride = 0;  // forward: as kv_batch_stride for Q and ctx (0 = Lq * ld_q / Lq * ld_o)
   const uint32_t* mask_bits = nullptr;  // [B, mask_rows, S / 32] packed by vlpk_mask_pack, S = kv_slots (128 when 0)
   int mask_rows = 0;                    // Lq or 1
   float* lse = nullptr;                 // [B, heads, Lq] (fwd: optional output ; bwd: input)
@@ -46,6 +47,15 @@ int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream);
 // Forward only, no dropout: d.k / d.v / d.kv_batch_stride unused, d.ld_kv is the row stride of prefix and text.
 int launch_attn_fwd_group(const AttnDesc& d, const AttnGroupKv& g, cudaStream_t stream);
 int launch_attn_bwd(const AttnDesc& d, cudaStream_t stream);
+// Query row i of sequence b also attends to one extra key, its own (k_self, v_self) row: k_self + b * self_batch_stride + i * ld_self
+// (v_self alike), never masked.  Forward only, no dropout; d.mask_rows must be d.Lq.  Lq, Lkv in [1, 512]: the single-tile kernel when
+// both are <= 128 (kv_slots 0), else the tiled one (kv_slots = 128 * ceil(Lkv / 128), or 0 for Lkv <= 128: the 128-slot layout).
+struct AttnSelfKv {
+  const void* k = nullptr;
+  const void* v = nullptr;
+  int64_t ld = 0, batch_stride = 0;
+};
+int launch_attn_fwd_self(const AttnDesc& d, const AttnSelfKv& s, cudaStream_t stream);
 void set_attn_tiled(bool on);
 // Attention probabilities exp(s - lse) of query rows [row0, Lq) into p [B, heads, Lq - row0, ld_p] (sequences p_batch_stride floats
 // apart, 0 = heads * (Lq - row0) * ld_p) from d.q / d.k / d.mask_bits / d.lse; q_batch_stride as d.kv_batch_stride for Q.

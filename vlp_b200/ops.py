@@ -277,6 +277,31 @@ class EncoderStackFn(torch.autograd.Function):
         return (dx0, None, None) + tuple(grads)
 
 
+def encoder_score_fwd(x, shared_bits, query_bits, T, heads, I, params):
+    """vlpk_encoder_score_fwd: the teacher-forced scoring pass of the decoder's layer stack, forward only.  x: [B, S + T, H] embeddings
+    of S shared rows then T query rows; shared_bits [B, S, S' / 32] / query_bits [B, T, S' / 32]: the packed masks of the shared rows
+    and of the query rows over the shared keys (each query row also sees its own key).  params: PARAMS_PER_LAYER per layer.  Returns
+    the last layer's output [B, S + T, H] and its _Acts (two buffers used in turn, whatever the depth)."""
+    xc = _bf16c(x)
+    B, R, H = xc.shape
+    S = R - T
+    n_layers = len(params) // PARAMS_PER_LAYER
+    if not 1 <= T < R:
+        raise ValueError(f"vlp_b200: scoring needs 1 <= T < rows, got T={T} of {R} rows")
+    slots = kv_slots(S, S)
+    for bits, rows in ((shared_bits, S), (query_bits, T)):
+        _check_mask_words(bits, S)
+        if tuple(bits.shape[:2]) != (B, rows) or bits.dtype != torch.int32 or not bits.is_contiguous():
+            raise ValueError(f"vlp_b200: packed scoring mask {tuple(bits.shape)} does not fit B={B}, {rows} rows")
+    pk = [_bf16c(p) for p in params]
+    acts = _Acts(min(n_layers, 2), B, R, H, heads, I, xc.device)
+    structs = (L.VlpkLayerActs * n_layers)(*[acts.structs[i % 2] for i in range(n_layers)])
+    shape = L.VlpkShape(B, S, S, H, heads, I, slots)
+    L.call("vlpk_encoder_score_fwd", C.byref(shape), int(T), n_layers, _weight_structs(pk, n_layers), xc.data_ptr(), shared_bits.data_ptr(),
+           query_bits.data_ptr(), structs, L.stream())
+    return acts.y[(n_layers - 1) % 2], acts
+
+
 def attn_probs(q, k, lse, mask_bits, row0=0, out=None):
     """Attention probabilities of one layer (vlpk_attn_probs): P[b, h, i - row0, j] = exp(q_i . k_j / 8 + mask_add - lse[b, h, i]) for
     query rows [row0, Lq), fp32, not differentiable — the reference's attention_probs before dropout.

@@ -24,6 +24,7 @@ from torch import nn
 from . import ops
 from .beam import beam_search
 from .decode import check_decode, greedy_decode, sample_decode
+from .score import score_captions
 
 logger = logging.getLogger(__name__)
 
@@ -881,3 +882,13 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
             if self.search_beam_size > 1:
                 return beam_search(*inputs, output_attentions=output_attentions)
             return greedy_decode(*inputs, sample_mode, output_attentions=output_attentions)
+
+    def score_captions(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, caption_ids, task_idx=None):
+        """log p(c_t | image, c_<t) of given captions in one teacher-forced pass (score.score_captions): the decoder's own input tuple,
+        as forward takes it, and int64 caption_ids [B, T] or [B, N, T] (N captions per image, 0-padded after the end), T <= out_len -
+        in_len.  Returns fp32 logp shaped like caption_ids, 0 at and after the first 0.  The same as frame t of the decode fed
+        c_0 .. c_{t-1} whenever the prefix rows see no text column and no text row a later one (the reference's decoder input).
+        Inference only: raises ValueError in grad mode with parameters that require grad, and for bad inputs, before any launch."""
+        if torch.is_tensor(token_type_ids):
+            _check_seq_len(self.config, token_type_ids.size(-1))
+        return score_captions(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, caption_ids, task_idx)
