@@ -224,6 +224,18 @@ int vlpk_attn_probs(int B, int heads, int Lq, int Lkv, int row0, const void* q, 
 int vlpk_attn_core_self_fwd(int B, int heads, int Lq, int Lkv, const void* q, int64_t ld_q, int64_t q_bstride, const void* k, const void* v,
                             int64_t ld_kv, int64_t kv_bstride, const void* k_self, const void* v_self, const uint32_t* mask_bits, int kv_slots,
                             void* ctx, int64_t ld_ctx, int64_t ctx_bstride, float* lse, void* stream);
+/* vlpk_attn_core_self_fwd with the keys of a shared image prefix (the caption matrix, vlpk_encoder_score_group_fwd): B hypotheses in
+ * groups of G per image.  Key j < P of hypothesis b is row j of image b / G's prefix [B / G, prefix_rows, ld_prefix] (K at column 0,
+ * V at column heads * 64); key P + j, j < Lkv - P, is its text row b * T + j of text [B * T rows, ld_text] (K at column 0, V at column
+ * heads * 64; e.g. a pair's word rows in place in a packed qkv: text = qkv + H, ld_text = 3H); then each query row's own key, as for
+ * vlpk_attn_core_self_fwd (k_self / v_self with the strides of q).  mask_bits: one sequence per image, [B / G, Lq, S / 32].  The
+ * result is bitwise vlpk_attn_core_self_fwd's on each hypothesis' materialised keys [prefix rows | text rows].  < 0 with nothing
+ * launched for the refusals of vlpk_attn_core_self_fwd, B % G != 0, P outside [1, prefix_rows], Lkv - P outside [0, T], or text rows
+ * that are not 16-byte aligned. */
+int vlpk_attn_core_group_self_fwd(int B, int G, int heads, int Lq, int Lkv, int P, const void* q, int64_t ld_q, int64_t q_bstride,
+                                  const void* prefix, int prefix_rows, int64_t ld_prefix, const void* text, int T, int64_t ld_text,
+                                  const void* k_self, const void* v_self, const uint32_t* mask_bits, int kv_slots, void* ctx, int64_t ld_ctx,
+                                  int64_t ctx_bstride, float* lse, void* stream);
 
 /* BertAttention.forward (modeling.py:326-330): QKV projection + attention core + output projection + LN.
  * x_kv == NULL or == x: self-attention over x (training / encoder path).
@@ -304,6 +316,28 @@ int vlpk_encoder_score_fwd(const VlpkShape* s, int T, int n_layers, const VlpkLa
  * B * (S + T) rows, without kv).  A separate entry point because a VlpkShape cannot describe the scoring stack: its rows per sequence
  * (S + T, up to 1023) exceed the 512 vlpk_workspace_bytes' shape check allows, and the attention's key count S differs from them. */
 int vlpk_encoder_score_workspace_bytes(const VlpkShape* s, int T, size_t* out1);
+/* The caption matrix: the scoring pass of vlpk_encoder_score_fwd for s->B (image, caption) pairs, G captions per image, against
+ * per-layer K/V caches of the images' prefixes, so that the P prefix rows run once per image instead of once per pair.  A pair has
+ * 2T - 1 rows, x [B, 2T - 1, H]: rows [0, T - 1) are its words c_0 .. c_{T-2}, rows [T - 1, 2T - 1) its T query rows ([MASK]).
+ *   s: B pairs (pair i of image i / G), Lq = Lkv = S = P + T - 1 (a pair's keys), H, heads, I, kv_slots (as for an S-row encoder).
+ *   prefix[l]: layer l's K | V of the prefix rows, [B / G, prefix_rows, 2H] bf16 (e.g. written by vlpk_layer_cached_fwd at pos 0).
+ *   word_bits [B / G, T - 1, S' / 32] (NULL allowed when T = 1) and query_bits [B / G, T, S' / 32]: one sequence per image, shared
+ *   by its G pairs; S' = 128 * ceil(S / 128).  Key j < P is prefix row j, key P + j the pair's word j.
+ * Per layer: the packed QKV projection over all pair rows; the word rows against [prefix | words] (vlpk_layer_cached_group_fwd's
+ * kernel, pos 0); the query rows against [prefix | words] plus each its own key (vlpk_attn_core_group_self_fwd); the output
+ * projection, both LayerNorms and the FFN over all rows.  Word K | V are read in place from the layer's qkv, nothing is copied.
+ *   acts[i]: layer i's buffers for B * (2T - 1) rows (vlpk_encoder_score_group_workspace_bytes; kv and drop_attn unused); lse holds
+ *   [B, heads, T - 1] of the word rows, then [B, heads, T] of the query rows.  Layer i reads acts[i - 1].y: two buffers used in turn
+ *   serve any depth.
+ * One host call, no allocation, no host synchronisation.  < 0 with nothing launched for: a bad shape, Lq != Lkv, T outside [1, 512],
+ * P outside [1, prefix_rows] or P + T - 1 != S, B % G != 0, H not a multiple of 128, a NULL pointer, a layer's output aliasing its
+ * input, or x / mask bits / prefix caches / acts misaligned. */
+int vlpk_encoder_score_group_fwd(const VlpkShape* s, int T, int G, int P, int n_layers, const VlpkLayerWeights* w, const void* x,
+                                 const void* const* prefix, int prefix_rows, const uint32_t* word_bits, const uint32_t* query_bits,
+                                 VlpkLayerActs* acts, void* stream);
+/* Host-only: bytes of one layer's VlpkLayerActs buffers for vlpk_encoder_score_group_fwd (vlpk_encoder_score_workspace_bytes' layout
+ * over B * (2T - 1) rows).  s as for vlpk_encoder_score_group_fwd; T in [1, S]. */
+int vlpk_encoder_score_group_workspace_bytes(const VlpkShape* s, int T, size_t* out1);
 /* Backward of the stack.  dys[i] (may be NULL) is the gradient flowing into layer i's output from outside the stack
  * (output_all_encoded_layers consumers); dys[n_layers-1] is normally the only non-NULL entry.  dx0 receives d/dx. */
 int vlpk_encoder_bwd(const VlpkShape* s, int n_layers, const VlpkLayerWeights* w, const void* x, const uint32_t* mask_bits,

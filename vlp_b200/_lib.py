@@ -83,6 +83,8 @@ _SIGS = {
                                         C.POINTER(VlpkDropout), c_u64, c_int, _P]),
     "vlpk_attn_core_self_fwd": (c_int, [c_int, c_int, c_int, c_int, _P, c_i64, c_i64, _P, _P, c_i64, c_i64, _P, _P, _P, c_int, _P, c_i64,
                                         c_i64, _P, _P]),
+    "vlpk_attn_core_group_self_fwd": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _P, c_i64, c_i64, _P, c_int, c_i64, _P, c_int,
+                                              c_i64, _P, _P, _P, c_int, _P, c_i64, c_i64, _P, _P]),
     "vlpk_attn_probs": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, c_i64, c_i64, _P, c_i64, c_i64, _P, c_int, c_int, _P, _P, c_i64,
                                 c_i64, _P]),
     "vlpk_mha_fwd": (c_int, [C.POINTER(VlpkShape), C.POINTER(VlpkLayerWeights), _P, _P, _P, c_int, C.POINTER(VlpkLayerActs),
@@ -111,6 +113,9 @@ _SIGS = {
     "vlpk_encoder_score_fwd": (c_int, [C.POINTER(VlpkShape), c_int, c_int, C.POINTER(VlpkLayerWeights), _P, _P, _P, C.POINTER(VlpkLayerActs),
                                        _P]),
     "vlpk_encoder_score_workspace_bytes": (c_int, [C.POINTER(VlpkShape), c_int, C.POINTER(C.c_size_t)]),
+    "vlpk_encoder_score_group_fwd": (c_int, [C.POINTER(VlpkShape), c_int, c_int, c_int, c_int, C.POINTER(VlpkLayerWeights), _P,
+                                             C.POINTER(c_void_p), c_int, _P, _P, C.POINTER(VlpkLayerActs), _P]),
+    "vlpk_encoder_score_group_workspace_bytes": (c_int, [C.POINTER(VlpkShape), c_int, C.POINTER(C.c_size_t)]),
     "vlpk_encoder_bwd": (c_int, [C.POINTER(VlpkShape), c_int, C.POINTER(VlpkLayerWeights), _P, _P, c_int,
                                  C.POINTER(VlpkLayerActs), C.POINTER(c_void_p), _P, C.POINTER(VlpkLayerGrads),
                                  C.POINTER(VlpkBwdScratch), c_float, c_float, C.POINTER(VlpkDropout), _P]),

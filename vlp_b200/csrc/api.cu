@@ -440,6 +440,46 @@ int score_layer_fwd(const VlpkShape* s, int T, const VlpkLayerWeights* w, const 
   return ffn_fwd_impl(&rows, w, a, 0.f, nullptr, layer_id, st);
 }
 
+// One layer of vlpk_encoder_score_group_fwd over s->B pairs (G per image) of 2T - 1 rows: T - 1 word rows, then T query rows.
+// s: Lq = Lkv = S = P + T - 1, the keys of a pair: P prefix rows of its image, then its words.
+int score_group_layer_fwd(const VlpkShape* s, int T, int G, int P, int prefix_rows, const VlpkLayerWeights* w, const void* x,
+                          const void* prefix, const uint32_t* word_bits, const uint32_t* query_bits, VlpkLayerActs* a, uint64_t layer_id,
+                          cudaStream_t st) {
+  const int H = s->H, W = T - 1, R = 2 * T - 1;
+  VLPK_TRY(qkv_fwd(s->B * R, H, w, x, a->qkv, st));
+  const bf16* qkv = static_cast<const bf16*>(a->qkv);
+  AttnGroupKv g;  // keys P + j: word j of the pair, read in place from its rows of the packed qkv
+  g.prefix = prefix; g.prefix_rows = prefix_rows; g.P = P;
+  g.text = qkv + H; g.ld_text = 3 * H; g.T = R; g.G = G; g.pos = 0;
+  AttnDesc ad;
+  ad.B = s->B; ad.heads = s->heads; ad.Lkv = s->Lkv; ad.kv_slots = s->kv_slots;
+  ad.ld_q = 3 * H; ad.q_batch_stride = static_cast<int64_t>(R) * 3 * H;
+  ad.ld_kv = 2 * H;
+  ad.ld_o = H; ad.o_batch_stride = static_cast<int64_t>(R) * H;
+  ad.drop = make_dropout(0.f, 0, 0);
+  if (W > 0) {  // word rows against the prefix and the words up to their own
+    AttnDesc wd = ad;
+    wd.Lq = W; wd.q = qkv; wd.o = a->ctx;
+    wd.mask_bits = word_bits; wd.mask_rows = W;
+    wd.lse = a->lse;
+    VLPK_TRY(launch_attn_fwd_group(wd, g, st));
+  }
+  // query rows against the prefix and the words, each plus its own key
+  AttnDesc qd = ad;
+  qd.Lq = T; qd.q = qkv + static_cast<size_t>(W) * 3 * H; qd.o = static_cast<bf16*>(a->ctx) + static_cast<size_t>(W) * H;
+  qd.mask_bits = query_bits; qd.mask_rows = T;
+  qd.lse = a->lse + static_cast<size_t>(s->B) * s->heads * W;
+  AttnSelfKv sk;
+  sk.k = qkv + static_cast<size_t>(W) * 3 * H + H;
+  sk.v = qkv + static_cast<size_t>(W) * 3 * H + 2 * H;
+  sk.ld = 3 * H; sk.batch_stride = static_cast<int64_t>(R) * 3 * H;
+  VLPK_TRY(launch_attn_fwd_group_self(qd, g, sk, st));
+  VlpkShape rows = *s;  // the row-wise tail over all B * (2T - 1) rows
+  rows.Lq = rows.Lkv = R;
+  VLPK_TRY(attn_out_ln(&rows, w, x, a, 0.f, nullptr, layer_id, st));
+  return ffn_fwd_impl(&rows, w, a, 0.f, nullptr, layer_id, st);
+}
+
 }  // namespace
 
 #pragma GCC visibility push(default)
@@ -623,6 +663,24 @@ int vlpk_attn_core_self_fwd(int B, int heads, int Lq, int Lkv, const void* q, in
   return launch_attn_fwd_self(d, s, S(stream));
 }
 
+int vlpk_attn_core_group_self_fwd(int B, int G, int heads, int Lq, int Lkv, int P, const void* q, int64_t ld_q, int64_t q_bstride,
+                                  const void* prefix, int prefix_rows, int64_t ld_prefix, const void* text, int T, int64_t ld_text,
+                                  const void* k_self, const void* v_self, const uint32_t* mask_bits, int kv_slots, void* ctx, int64_t ld_ctx,
+                                  int64_t ctx_bstride, float* lse, void* stream) {
+  AttnDesc d;
+  d.B = B; d.heads = heads; d.Lq = Lq; d.Lkv = Lkv; d.kv_slots = kv_slots;
+  d.q = q; d.ld_q = ld_q; d.q_batch_stride = q_bstride;
+  d.ld_kv = ld_prefix;
+  d.o = ctx; d.ld_o = ld_ctx; d.o_batch_stride = ctx_bstride;
+  d.mask_bits = mask_bits; d.mask_rows = Lq; d.lse = lse;
+  AttnGroupKv g;
+  g.prefix = prefix; g.prefix_rows = prefix_rows; g.P = P;
+  g.text = text; g.T = T; g.G = G; g.pos = 0; g.ld_text = ld_text;
+  AttnSelfKv s;
+  s.k = k_self; s.v = v_self; s.ld = ld_q; s.batch_stride = q_bstride;
+  return launch_attn_fwd_group_self(d, g, s, S(stream));
+}
+
 int vlpk_attn_probs(int B, int heads, int Lq, int Lkv, int row0, const void* q, int64_t ld_q, int64_t q_bstride, const void* k, int64_t ld_k,
                     int64_t k_bstride, const uint32_t* mask_bits, int mask_rows, int kv_slots, const float* lse, float* p, int64_t ld_p,
                     int64_t p_bstride, void* stream) {
@@ -798,6 +856,46 @@ int vlpk_encoder_score_fwd(const VlpkShape* s, int T, int n_layers, const VlpkLa
   const void* cur = x;
   for (int i = 0; i < n_layers; ++i) {
     VLPK_TRY(score_layer_fwd(s, T, &w[i], cur, shared_bits, query_bits, &acts[i], i, S(stream)));
+    cur = acts[i].y;
+  }
+  return 0;
+}
+
+int vlpk_encoder_score_group_workspace_bytes(const VlpkShape* s, int T, size_t* out1) {
+  VLPK_TRY(check_shape(s));
+  VLPK_CHECK_ARG(out1 != nullptr, "encoder_score_group_workspace_bytes: null output");
+  VLPK_CHECK_ARG(s->Lq == s->Lkv && T >= 1 && T <= s->Lkv, "encoder_score_group: Lq=%d must equal Lkv=%d (the keys S), T=%d in [1, S]", s->Lq,
+                 s->Lkv, T);
+  const size_t H = s->H, I = s->I, M = static_cast<size_t>(s->B) * (2 * T - 1);
+  const size_t lse = (static_cast<size_t>(s->B) * s->heads * (2 * T - 1) + 3) / 4 * 4;
+  out1[0] = 2 * M * (3 * H + 5 * H + 2 * I) + 4 * (lse + 4 * M);
+  return 0;
+}
+
+int vlpk_encoder_score_group_fwd(const VlpkShape* s, int T, int G, int P, int n_layers, const VlpkLayerWeights* w, const void* x,
+                                 const void* const* prefix, int prefix_rows, const uint32_t* word_bits, const uint32_t* query_bits,
+                                 VlpkLayerActs* acts, void* stream) {
+  VLPK_TRY(check_shape(s));
+  VLPK_CHECK_ARG(s->Lq == s->Lkv && T >= 1 && T <= 512, "encoder_score_group: Lq=%d must equal Lkv=%d (the keys S), T=%d in [1,512]", s->Lq,
+                 s->Lkv, T);
+  VLPK_CHECK_ARG(P >= 1 && P <= prefix_rows && P + T - 1 == s->Lkv, "encoder_score_group: P=%d must be in [1, prefix rows %d] with P + T - 1 "
+                 "= S=%d (T=%d)", P, prefix_rows, s->Lkv, T);
+  VLPK_CHECK_ARG(G >= 1 && s->B % G == 0, "encoder_score_group: B=%d pairs are not whole groups of G=%d", s->B, G);
+  VLPK_CHECK_ARG(s->H % 128 == 0, "encoder_score_group: H=%d must be a multiple of 128 for the packed QKV projection", s->H);
+  VLPK_CHECK_ARG(n_layers > 0 && w && x && prefix && (word_bits || T == 1) && query_bits && acts, "encoder_score_group: null pointer");
+  const auto al = [](const void* p, uintptr_t n) { return p != nullptr && (reinterpret_cast<uintptr_t>(p) & (n - 1)) == 0; };
+  VLPK_CHECK_ARG(al(x, 16) && (T == 1 || al(word_bits, 16)) && al(query_bits, 16), "encoder_score_group: x and the mask bits must be 16-byte "
+                 "aligned");
+  for (int i = 0; i < n_layers; ++i) {  // every layer's buffers, so that no check fails after a launch
+    const VlpkLayerActs& a = acts[i];
+    VLPK_CHECK_ARG(al(prefix[i], 16) && al(a.qkv, 16) && al(a.ctx, 16) && al(a.t1, 16) && al(a.y1, 16) && al(a.u, 16) && al(a.hmid, 16) &&
+                   al(a.t2, 16) && al(a.y, 16) && al(a.lse, 4) && al(a.stats1, 8) && al(a.stats2, 8) && a.y != (i == 0 ? x : acts[i - 1].y),
+                   "encoder_score_group: layer %d prefix cache or acts missing or misaligned (16-byte bf16 buffers, 4-byte lse, 8-byte "
+                   "statistics), or its output aliases its input", i);
+  }
+  const void* cur = x;
+  for (int i = 0; i < n_layers; ++i) {
+    VLPK_TRY(score_group_layer_fwd(s, T, G, P, prefix_rows, &w[i], cur, prefix[i], word_bits, query_bits, &acts[i], i, S(stream)));
     cur = acts[i].y;
   }
   return 0;

@@ -105,15 +105,17 @@ __device__ __forceinline__ void load_mask_words(const AttnArgs& a, int b, int ro
 }
 
 // ------------------------------------------------------------------------------------------------
-// shared-prefix K/V (vlpk_layer_cached_group_fwd): hypothesis b of image b / G reads key r < P from the image's prefix cache (a
-// TMA box, like a contiguous cache), key r = P + j from text row slots[b, j] when j < pos and from its own row b * T + j otherwise.
+// shared-prefix K/V (vlpk_layer_cached_group_fwd, vlpk_encoder_score_group_fwd): hypothesis b of image b / G reads key r < P from
+// the image's prefix cache (a TMA box, like a contiguous cache), key r = P + j from text row slots[b, j] when j < pos and from its
+// own row b * T + j otherwise.  T is the text rows per hypothesis: the decode's text cache rows, or, for the caption matrix (pos = 0),
+// the 2 t - 1 rows of a pair of a t-word caption in the layer's packed qkv.
 // The text rows are gathered into the same 128B-swizzled tile slots a TMA box of the contiguous cache fills, and slots past Lkv
 // are zeroed as TMA's out-of-bounds fill zeroes them: the tiles, and so every instruction after the load, are those of
 // the contiguous cache.  A slot entry outside the text tensor is clamped into it (wrong numbers, never an out-of-bounds read).
 // ------------------------------------------------------------------------------------------------
 struct GroupKv {
   const __nv_bfloat16* text;  // [B, T, ld]: K | V rows, V at column H
-  const int* slots;           // [B, T]
+  const int* slots;           // [B, T]; not read when pos = 0
   long long ld;
   int H, G, P, pos, T;
   long long text_rows;        // B * T
@@ -214,10 +216,10 @@ struct FwdSmem {
 
 // GROUP: K/V from a shared prefix + text rows (GroupKv); grid (G * heads, images), so the G hypotheses of an image and head run
 // next to each other and read its prefix box from L2.  Otherwise grid (heads, B) and K/V from tm.k / tm.v.
-// SELF: every query row also attends to its own key (SelfKv), folded in after the shared keys; no dropout.
+// SELF: every query row also attends to its own key (SelfKv), folded in after the shared keys; no dropout.  With GROUP, b (the
+// hypothesis) selects the query, output, lse and self rows, the image the prefix box and the mask rows.
 template <bool GROUP, bool SELF>
 __device__ __forceinline__ void attn_fwd_body(const AttnTmaps& tm, const AttnArgs a, const GroupKv g, const SelfKv sk) {
-  static_assert(!(GROUP && SELF), "a per-row self key is not combined with the shared-prefix loader");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem + FwdSmem::OFF_Q;
@@ -371,6 +373,11 @@ __global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_group_kernel(const __
 __global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_self_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a,
                                                                         const SelfKv sk) {
   attn_fwd_body<false, true>(tm, a, GroupKv{}, sk);
+}
+
+__global__ void __launch_bounds__(ATT_THREADS, 2) attn_fwd_group_self_kernel(const __grid_constant__ AttnTmaps tm, const AttnArgs a,
+                                                                              const GroupKv g, const SelfKv sk) {
+  attn_fwd_body<true, true>(tm, a, g, sk);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -614,7 +621,6 @@ struct FwdTiledSmem {
 // SELF: as attn_fwd_body.
 template <bool GROUP, bool SELF>
 __device__ __forceinline__ void attn_fwd_tiled_body(const AttnTmaps& tm, const AttnTiledArgs a, const GroupKv g, const SelfKv sk) {
-  static_assert(!(GROUP && SELF), "a per-row self key is not combined with the shared-prefix loader");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem + FwdTiledSmem::OFF_Q;
@@ -795,6 +801,11 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_group_tiled_kernel(co
 __global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_self_tiled_kernel(const __grid_constant__ AttnTmaps tm, const AttnTiledArgs a,
                                                                               const SelfKv sk) {
   attn_fwd_tiled_body<false, true>(tm, a, GroupKv{}, sk);
+}
+
+__global__ void __launch_bounds__(ATT_THREADS, 1) attn_fwd_group_self_tiled_kernel(const __grid_constant__ AttnTmaps tm, const AttnTiledArgs a,
+                                                                                    const GroupKv g, const SelfKv sk) {
+  attn_fwd_tiled_body<true, true>(tm, a, g, sk);
 }
 
 // P (recomputed from the logsumexp; 0 for keys >= Lkv and rows >= Lq) and the dropout-masked dP of one 64 x 128 (q, key) block,
@@ -1311,28 +1322,38 @@ int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream) {
   return 0;
 }
 
+// Tensor maps and loader arguments of a shared-prefix forward: Q / ctx of the d.B hypotheses with their strides, K / V boxes over
+// the P prefix rows of each image, text rows gd.ld_text (0: d.ld_kv) elements apart.
+static int group_setup(const AttnDesc& d, const AttnGroupKv& gd, AttnTmaps* tm, GroupKv* g) {
+  VLPK_CHECK_ARG(gd.G >= 1 && d.B % gd.G == 0, "attention group: %d hypotheses are not whole groups of G=%d", d.B, gd.G);
+  VLPK_CHECK_ARG(gd.prefix != nullptr && gd.text != nullptr && (gd.slots != nullptr || gd.pos == 0), "attention group: null pointer");
+  const int width = d.heads * HD, images = d.B / gd.G;
+  const int64_t ld_text = gd.ld_text != 0 ? gd.ld_text : d.ld_kv;
+  VLPK_CHECK_ARG((reinterpret_cast<uintptr_t>(gd.text) & 15u) == 0 && ld_text % 8 == 0 && ld_text >= 2 * width,
+                 "attention group: text rows need 16-byte alignment and K | V in each row (ld=%lld)", static_cast<long long>(ld_text));
+  memset(tm, 0, sizeof(*tm));
+  VLPK_TRY(make_seq_tmap(&tm->q, d.q, width, d.Lq, d.B, d.ld_q, d.q_batch_stride));
+  VLPK_TRY(make_seq_tmap(&tm->k, gd.prefix, width, gd.P, images, d.ld_kv, static_cast<int64_t>(gd.prefix_rows) * d.ld_kv));
+  VLPK_TRY(make_seq_tmap(&tm->v, static_cast<const __nv_bfloat16*>(gd.prefix) + width, width, gd.P, images, d.ld_kv,
+                         static_cast<int64_t>(gd.prefix_rows) * d.ld_kv));
+  VLPK_TRY(make_seq_tmap(&tm->o, d.o, width, d.Lq, d.B, d.ld_o, d.o_batch_stride));
+  tm->dq = tm->dk = tm->dv = tm->o;
+  g->text = static_cast<const __nv_bfloat16*>(gd.text);
+  g->slots = gd.slots;
+  g->ld = ld_text;
+  g->H = width; g->G = gd.G; g->P = gd.P; g->pos = gd.pos; g->T = gd.T;
+  g->text_rows = static_cast<long long>(d.B) * gd.T;
+  return 0;
+}
+
 int launch_attn_fwd_group(const AttnDesc& d, const AttnGroupKv& gd, cudaStream_t stream) {
   VLPK_TRY(check_common(d));
-  VLPK_CHECK_ARG(gd.G >= 1 && d.B % gd.G == 0, "attention group: %d hypotheses are not whole groups of G=%d", d.B, gd.G);
   VLPK_CHECK_ARG(gd.P >= 1 && gd.P <= gd.prefix_rows && gd.pos >= 0 && gd.pos + d.Lq <= gd.T && gd.P + gd.pos + d.Lq == d.Lkv,
                  "attention group: P=%d (prefix rows %d) pos=%d Lq=%d T=%d Lkv=%d", gd.P, gd.prefix_rows, gd.pos, d.Lq, gd.T, d.Lkv);
-  VLPK_CHECK_ARG(gd.prefix != nullptr && gd.text != nullptr && gd.slots != nullptr, "attention group: null pointer");
-  const int width = d.heads * HD, images = d.B / gd.G;
   AttnTmaps tm;
-  memset(&tm, 0, sizeof(tm));
-  VLPK_TRY(make_seq_tmap(&tm.q, d.q, width, d.Lq, d.B, d.ld_q));
-  VLPK_TRY(make_seq_tmap(&tm.k, gd.prefix, width, gd.P, images, d.ld_kv, static_cast<int64_t>(gd.prefix_rows) * d.ld_kv));
-  VLPK_TRY(make_seq_tmap(&tm.v, static_cast<const __nv_bfloat16*>(gd.prefix) + width, width, gd.P, images, d.ld_kv,
-                         static_cast<int64_t>(gd.prefix_rows) * d.ld_kv));
-  VLPK_TRY(make_seq_tmap(&tm.o, d.o, width, d.Lq, d.B, d.ld_o));
-  tm.dq = tm.dk = tm.dv = tm.o;
   GroupKv g;
-  g.text = static_cast<const __nv_bfloat16*>(gd.text);
-  g.slots = gd.slots;
-  g.ld = d.ld_kv;
-  g.H = width; g.G = gd.G; g.P = gd.P; g.pos = gd.pos; g.T = gd.T;
-  g.text_rows = static_cast<long long>(d.B) * gd.T;
-  const dim3 grid(gd.G * d.heads, images, (d.Lq + TL - 1) / TL);
+  VLPK_TRY(group_setup(d, gd, &tm, &g));
+  const dim3 grid(gd.G * d.heads, d.B / gd.G, (d.Lq + TL - 1) / TL);
   LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * d.Lkv * HD, stream);
   if (use_tiled(d)) {
     AttnTiledArgs a = tiled_args(d);
@@ -1344,13 +1365,8 @@ int launch_attn_fwd_group(const AttnDesc& d, const AttnGroupKv& gd, cudaStream_t
     VLPK_CUDA(launch_ex(attn_fwd_group_tiled_kernel, grid, dim3(ATT_THREADS), FwdTiledSmem::DYN, stream, 1, tm, a, g));
     return 0;
   }
-  AttnArgs a;
-  a.B = d.B; a.heads = d.heads; a.Lq = d.Lq; a.Lkv = d.Lkv;
-  a.mask_bits = d.mask_bits; a.mask_rows = d.mask_rows;
-  a.lse = d.lse; a.o_ptr = nullptr; a.do_ptr = nullptr; a.ld_o = d.ld_o;
-  a.drop = d.drop;
+  AttnArgs a = fwd_args(d);
   a.keep_out = nullptr;
-  a.dbias_part = nullptr;
   static bool attr_set = false;
   if (!attr_set) {
     VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem::DYN));
@@ -1360,7 +1376,8 @@ int launch_attn_fwd_group(const AttnDesc& d, const AttnGroupKv& gd, cudaStream_t
   return 0;
 }
 
-int launch_attn_fwd_self(const AttnDesc& d, const AttnSelfKv& sd, cudaStream_t stream) {
+// Shape, mask and self-row rules of the self-key forwards (contiguous or shared-prefix K/V).
+static int check_self(const AttnDesc& d, const AttnSelfKv& sd) {
   VLPK_CHECK_ARG(d.head_dim == HD, "attention self: head_dim %d unsupported (only 64)", d.head_dim);
   VLPK_CHECK_ARG(d.B >= 1 && d.heads >= 1 && d.Lq >= 1 && d.Lq <= MAX_SLOTS && d.Lkv >= 1 && d.Lkv <= MAX_SLOTS,
                  "attention self: B=%d heads=%d Lq=%d Lkv=%d (lengths in [1,512])", d.B, d.heads, d.Lq, d.Lkv);
@@ -1368,19 +1385,30 @@ int launch_attn_fwd_self(const AttnDesc& d, const AttnSelfKv& sd, cudaStream_t s
                  "attention self: kv_slots=%d for Lkv=%d (0 needs Lkv <= 128, else 128 * ceil(Lkv / 128))", d.kv_slots, d.Lkv);
   VLPK_CHECK_ARG(d.mask_bits != nullptr && d.mask_rows == d.Lq, "attention self: one mask row per query row needed (%d for Lq=%d)",
                  d.mask_rows, d.Lq);
-  VLPK_CHECK_ARG(d.q && d.k && d.v && d.o && sd.k && sd.v, "attention self: null pointer");
+  VLPK_CHECK_ARG(d.q && d.o && sd.k && sd.v, "attention self: null pointer");
   VLPK_CHECK_ARG(d.drop.p == 0.f && d.keep_out == nullptr, "attention self: forward only, without dropout");
   const auto a16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15u) == 0; };
   VLPK_CHECK_ARG(a16(sd.k) && a16(sd.v) && sd.ld % 8 == 0 && sd.batch_stride % 8 == 0 && sd.ld >= d.heads * HD,
                  "attention self: self keys / values need 16-byte rows (ld=%lld, batch stride=%lld)", static_cast<long long>(sd.ld),
                  static_cast<long long>(sd.batch_stride));
-  AttnTmaps tm;
-  VLPK_TRY(fwd_tmaps(d, &tm));
+  return 0;
+}
+
+static SelfKv self_kv(const AttnDesc& d, const AttnSelfKv& sd) {
   SelfKv sk;
   sk.k = static_cast<const __nv_bfloat16*>(sd.k);
   sk.v = static_cast<const __nv_bfloat16*>(sd.v);
   sk.ld = sd.ld;
   sk.bstride = sd.batch_stride != 0 ? sd.batch_stride : static_cast<int64_t>(d.Lq) * sd.ld;
+  return sk;
+}
+
+int launch_attn_fwd_self(const AttnDesc& d, const AttnSelfKv& sd, cudaStream_t stream) {
+  VLPK_TRY(check_self(d, sd));
+  VLPK_CHECK_ARG(d.k && d.v, "attention self: null pointer");
+  AttnTmaps tm;
+  VLPK_TRY(fwd_tmaps(d, &tm));
+  const SelfKv sk = self_kv(d, sd);
   LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * (d.Lkv + 1) * HD, stream);
   if (use_tiled(d)) {
     const AttnTiledArgs a = tiled_args(d);
@@ -1400,6 +1428,37 @@ int launch_attn_fwd_self(const AttnDesc& d, const AttnSelfKv& sd, cudaStream_t s
     attr_set = true;
   }
   VLPK_CUDA(launch_ex(attn_fwd_self_kernel, dim3(d.heads, d.B), dim3(ATT_THREADS), FwdSmem::DYN, stream, 1, tm, a, sk));
+  return 0;
+}
+
+int launch_attn_fwd_group_self(const AttnDesc& d, const AttnGroupKv& gd, const AttnSelfKv& sd, cudaStream_t stream) {
+  VLPK_TRY(check_self(d, sd));
+  VLPK_CHECK_ARG(gd.P >= 1 && gd.P <= gd.prefix_rows && gd.pos >= 0 && gd.P + gd.pos <= d.Lkv && d.Lkv - gd.P <= gd.T,
+                 "attention group self: P=%d (prefix rows %d) pos=%d Lkv=%d T=%d (needs P + pos <= Lkv <= P + T)", gd.P, gd.prefix_rows,
+                 gd.pos, d.Lkv, gd.T);
+  AttnTmaps tm;
+  GroupKv g;
+  VLPK_TRY(group_setup(d, gd, &tm, &g));
+  const SelfKv sk = self_kv(d, sd);
+  const dim3 grid(gd.G * d.heads, d.B / gd.G, (d.Lq + TL - 1) / TL);
+  LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * (d.Lkv + 1) * HD, stream);
+  if (use_tiled(d)) {
+    const AttnTiledArgs a = tiled_args(d);
+    static bool attr_set = false;
+    if (!attr_set) {
+      VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_group_self_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdTiledSmem::DYN));
+      attr_set = true;
+    }
+    VLPK_CUDA(launch_ex(attn_fwd_group_self_tiled_kernel, grid, dim3(ATT_THREADS), FwdTiledSmem::DYN, stream, 1, tm, a, g, sk));
+    return 0;
+  }
+  const AttnArgs a = fwd_args(d);  // keep_out is null: checked above
+  static bool attr_set = false;
+  if (!attr_set) {
+    VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_group_self_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem::DYN));
+    attr_set = true;
+  }
+  VLPK_CUDA(launch_ex(attn_fwd_group_self_kernel, dim3(grid.x, grid.y), dim3(ATT_THREADS), FwdSmem::DYN, stream, 1, tm, a, g, sk));
   return 0;
 }
 

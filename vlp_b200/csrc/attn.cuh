@@ -31,15 +31,17 @@ struct AttnDesc {
   float* dbias = nullptr;  // optional [3 * heads * 64] fp32: += column sums of dQ | dK | dV, summed over sequences in a fixed order
 };
 
-// Keys of d.B hypotheses in groups of G per image (vlpk_layer_cached_group_fwd): hypothesis b reads key r < P from row r of image
-// b / G's prefix [images, prefix_rows, ld_kv], key P + j from text row slots[b * T + j] (j < pos) or b * T + j (its own new rows) of
-// text [B * T, ld_kv]; K at column 0, V at column heads * 64 of both.  mask_bits has one sequence per image.
+// Keys of d.B hypotheses in groups of G per image (vlpk_layer_cached_group_fwd, vlpk_encoder_score_group_fwd): hypothesis b reads
+// key r < P from row r of image b / G's prefix [images, prefix_rows, ld_kv], key P + j from text row slots[b * T + j] (j < pos) or
+// b * T + j (its own rows) of text [B * T rows, ld_text]; K at column 0, V at column heads * 64 of both.  slots may be NULL when
+// pos = 0.  mask_bits has one sequence per image.  Q / ctx take d.q_batch_stride / d.o_batch_stride.
 struct AttnGroupKv {
   const void* prefix = nullptr;
   int prefix_rows = 0, P = 0;
   const void* text = nullptr;
   const int32_t* slots = nullptr;
   int T = 0, G = 1, pos = 0;
+  int64_t ld_text = 0;  // row stride of text (0: d.ld_kv)
 };
 
 // Lq, Lkv <= 128: the single-tile kernels; longer sequences (or the "attn_tiled" test option): the KV-tiled kernels.
@@ -56,6 +58,9 @@ struct AttnSelfKv {
   int64_t ld = 0, batch_stride = 0;
 };
 int launch_attn_fwd_self(const AttnDesc& d, const AttnSelfKv& s, cudaStream_t stream);
+// launch_attn_fwd_self with the keys of launch_attn_fwd_group (d.k / d.v unused): key P + j, j < Lkv - P, from the hypothesis' text
+// rows, then each query row's own key.  Needs P + pos <= Lkv <= P + T.
+int launch_attn_fwd_group_self(const AttnDesc& d, const AttnGroupKv& g, const AttnSelfKv& s, cudaStream_t stream);
 void set_attn_tiled(bool on);
 // Attention probabilities exp(s - lse) of query rows [row0, Lq) into p [B, heads, Lq - row0, ld_p] (sequences p_batch_stride floats
 // apart, 0 = heads * (Lq - row0) * ld_p) from d.q / d.k / d.mask_bits / d.lse; q_batch_stride as d.kv_batch_stride for Q.

@@ -302,6 +302,39 @@ def encoder_score_fwd(x, shared_bits, query_bits, T, heads, I, params):
     return acts.y[(n_layers - 1) % 2], acts
 
 
+def encoder_score_group_fwd(x, prefix, word_bits, query_bits, T, G, heads, I, params):
+    """vlpk_encoder_score_group_fwd: the caption matrix's pass of the layer stack, forward only.  x: [B * G, 2T - 1, H] embeddings of
+    the (image, caption) pairs, G per image, each its T - 1 words then its T query rows; prefix: one [B, P, 2H] bf16 K | V cache of the
+    images' prefix rows per layer; word_bits [B, T - 1, S' / 32] (None when T = 1) / query_bits [B, T, S' / 32]: the packed masks of
+    the word and query rows over the keys [prefix | words] (S = P + T - 1), one sequence per image.  params: PARAMS_PER_LAYER per
+    layer.  Returns the last layer's output [B * G, 2T - 1, H] and its _Acts (two buffers used in turn, whatever the depth)."""
+    xc = _bf16c(x)
+    BG, R, H = xc.shape
+    n_layers = len(params) // PARAMS_PER_LAYER
+    B, P = prefix[0].shape[:2]
+    S = P + T - 1
+    if R != 2 * T - 1 or G < 1 or B * G != BG or len(prefix) != n_layers:
+        raise ValueError(f"vlp_b200: caption-matrix rows {tuple(xc.shape)} do not fit T={T}, G={G}, {B} images and {n_layers} layers")
+    for t in prefix:
+        if not (t.dtype == BF16 and t.is_contiguous() and tuple(t.shape) == (B, P, 2 * H)):
+            raise ValueError(f"vlp_b200: every prefix cache must be a contiguous bf16 [{B}, {P}, {2 * H}] tensor")
+    slots = kv_slots(S, S)
+    for bits, rows in ((word_bits, T - 1), (query_bits, T)):
+        if bits is None and rows == 0:
+            continue
+        _check_mask_words(bits, S)
+        if tuple(bits.shape[:2]) != (B, rows) or bits.dtype != torch.int32 or not bits.is_contiguous():
+            raise ValueError(f"vlp_b200: packed caption-matrix mask {tuple(bits.shape)} does not fit {B} images, {rows} rows")
+    pk = [_bf16c(p) for p in params]
+    acts = _Acts(min(n_layers, 2), BG, R, H, heads, I, xc.device)
+    structs = (L.VlpkLayerActs * n_layers)(*[acts.structs[i % 2] for i in range(n_layers)])
+    caches = (C.c_void_p * n_layers)(*[t.data_ptr() for t in prefix])
+    shape = L.VlpkShape(BG, S, S, H, heads, I, slots)
+    L.call("vlpk_encoder_score_group_fwd", C.byref(shape), int(T), int(G), int(P), n_layers, _weight_structs(pk, n_layers), xc.data_ptr(),
+           caches, P, L.ptr(word_bits), query_bits.data_ptr(), structs, L.stream())
+    return acts.y[(n_layers - 1) % 2], acts
+
+
 def attn_probs(q, k, lse, mask_bits, row0=0, out=None):
     """Attention probabilities of one layer (vlpk_attn_probs): P[b, h, i - row0, j] = exp(q_i . k_j / 8 + mask_add - lse[b, h, i]) for
     query rows [row0, Lq), fp32, not differentiable — the reference's attention_probs before dropout.

@@ -24,7 +24,7 @@ from torch import nn
 from . import ops
 from .beam import beam_search
 from .decode import check_decode, greedy_decode, sample_decode
-from .score import score_captions
+from .score import score_caption_matrix, score_captions
 
 logger = logging.getLogger(__name__)
 
@@ -892,3 +892,16 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         if torch.is_tensor(token_type_ids):
             _check_seq_len(self.config, token_type_ids.size(-1))
         return score_captions(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, caption_ids, task_idx)
+
+    def score_caption_matrix(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, caption_ids, task_idx=None,
+                             max_rows=None):
+        """Image x caption log-likelihoods (score.score_caption_matrix): the decoder's own input tuple for B images, as forward takes
+        it, and int64 caption_ids [C, T], C captions shared by all images (0-padded after the end, T <= out_len - in_len).  Returns
+        fp32 [B, C, T]: out[b, c] is score_captions of image b with caption c.  Each image's prefix runs through the layers once;
+        every (image, caption) pair adds only its 2T - 1 caption rows.  task_idx (relaxed head) is per image.  max_rows bounds the
+        head rows B * chunk * T of one chunk of captions (default score.MATRIX_MAX_ROWS, about 10 GB at BERT-base).  Inference only,
+        with score_captions' refusals (ValueError before any launch), and for C < 1 or max_rows < B * T."""
+        if torch.is_tensor(token_type_ids):
+            _check_seq_len(self.config, token_type_ids.size(-1))
+        return score_caption_matrix(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, caption_ids,
+                                    task_idx, max_rows)
