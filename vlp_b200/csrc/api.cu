@@ -154,11 +154,10 @@ int wgrad_join(cudaStream_t main) {
   return 0;
 }
 
-struct KvCache {       // incremental decode with a persistent K/V cache (vlpk_layer_cached_fwd)
+struct KvCache {       // incremental decode with a persistent K/V cache (vlpk_layer_cached_fwd, vlpk_layer_cached_group_fwd's text cache)
   void* base = nullptr;  // [B, rows, 2H] bf16: key | value projections of the rows this layer has seen
   int rows = 0;          // allocated rows per sequence
   int pos = 0;           // rows already valid; the call appends the Lq new rows at [pos, pos + Lq)
-  const AttnGroupKv* group = nullptr;  // vlpk_layer_cached_group_fwd: base / rows / pos are the text cache, keys from the group loader
 };
 
 // Packed QKV projection of M rows x [M, H] -> qkv [M, 3H]: the three [H,H] weights read in place as N-segments.
@@ -171,6 +170,20 @@ int qkv_fwd(int M, int H, const VlpkLayerWeights* w, const void* x, void* qkv, c
   g.B[0] = w->wq; g.B[1] = w->wk; g.B[2] = w->wv;
   g.bias[0] = static_cast<const bf16*>(w->bq); g.bias[1] = static_cast<const bf16*>(w->bk); g.bias[2] = static_cast<const bf16*>(w->bv);
   g.D0 = qkv; g.ldd0 = 3 * H;
+  g.epi = EPI_STORE;
+  g.bn = (H % 256 == 0) ? 0 : 128;
+  return launch_gemm(g, st);
+}
+
+// K | V projection of M rows x [M, H] -> kv [M, 2H]: the two [H,H] weights read in place as N-segments.
+int kv_fwd(int M, int H, const VlpkLayerWeights* w, const void* x, void* kv, cudaStream_t st) {
+  GemmDesc g;
+  g.M = M; g.N = 2 * H; g.K = H;
+  g.A = x; g.lda = H;
+  g.nseg = 2; g.b_seg_rows = H; g.ldb = H;
+  g.B[0] = w->wk; g.B[1] = w->wv;
+  g.bias[0] = static_cast<const bf16*>(w->bk); g.bias[1] = static_cast<const bf16*>(w->bv);
+  g.D0 = kv; g.ldd0 = 2 * H;
   g.epi = EPI_STORE;
   g.bn = (H % 256 == 0) ? 0 : 128;
   return launch_gemm(g, st);
@@ -193,7 +206,7 @@ int attn_out_ln(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, Vl
 
 int mha_fwd_impl(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, const void* x_kv, const uint32_t* bits, int mask_rows,
                  VlpkLayerActs* a, float p_attn, float p_hidden, const VlpkDropout* drop, uint64_t layer_id, cudaStream_t st,
-                 const KvCache* cache = nullptr) {
+                 const KvCache* cache = nullptr, const AttnGroupKv* group = nullptr) {
   const int H = s->H, Mq = s->B * s->Lq, Mkv = s->B * s->Lkv;
   const bool incr = (cache == nullptr && x_kv != nullptr && x_kv != x);
   const DropoutCfg none = make_dropout(0.f, 0, 0);
@@ -205,20 +218,12 @@ int mha_fwd_impl(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, c
   ad.keep_out = (ad.drop.p > 0.f) ? a->drop_attn : nullptr;   // forward stores its keep-decisions for backward
   if (cache != nullptr) {
     // Q and K|V of the NEW rows only; K|V are appended to the cache (rows [pos, pos + Lq) of every sequence), attention reads the cache
-    if (cache->group == nullptr)
+    // (with a group: the image's prefix cache, then the text cache)
+    if (group == nullptr)
       VLPK_CHECK_ARG(a->kv != nullptr && cache->base != nullptr && cache->pos >= 0 && cache->pos + s->Lq == s->Lkv && s->Lkv <= cache->rows,
                      "mha_cached_fwd: pos=%d + Lq=%d must equal Lkv=%d <= cache rows %d", cache->pos, s->Lq, s->Lkv, cache->rows);
     VLPK_TRY(fwd_linear(Mq, H, H, x, H, w->wq, H, w->bq, a->qkv, H, EPI_STORE, nullptr, 0, none, st));
-    GemmDesc g;
-    g.M = Mq; g.N = 2 * H; g.K = H;
-    g.A = x; g.lda = H;
-    g.nseg = 2; g.b_seg_rows = H; g.ldb = H;
-    g.B[0] = w->wk; g.B[1] = w->wv;
-    g.bias[0] = static_cast<const bf16*>(w->bk); g.bias[1] = static_cast<const bf16*>(w->bv);
-    g.D0 = a->kv; g.ldd0 = 2 * H;
-    g.epi = EPI_STORE;
-    g.bn = (H % 256 == 0) ? 0 : 128;
-    VLPK_TRY(launch_gemm(g, st));
+    VLPK_TRY(kv_fwd(Mq, H, w, x, a->kv, st));
     bf16* dst = static_cast<bf16*>(cache->base) + static_cast<size_t>(cache->pos) * 2 * H;
     VLPK_CUDA(cudaMemcpy2DAsync(dst, static_cast<size_t>(cache->rows) * 2 * H * sizeof(bf16), a->kv, static_cast<size_t>(s->Lq) * 2 * H * sizeof(bf16),
                                 static_cast<size_t>(s->Lq) * 2 * H * sizeof(bf16), s->B, cudaMemcpyDeviceToDevice, st));
@@ -227,10 +232,6 @@ int mha_fwd_impl(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, c
     ad.v = static_cast<const bf16*>(cache->base) + H;
     ad.ld_kv = 2 * H;
     ad.kv_batch_stride = static_cast<int64_t>(cache->rows) * 2 * H;
-    if (cache->group != nullptr) {
-      VLPK_TRY(launch_attn_fwd_group(ad, *cache->group, st));
-      return attn_out_ln(s, w, x, a, p_hidden, drop, layer_id, st);
-    }
   } else if (!incr) {
     VLPK_CHECK_ARG(s->Lq == s->Lkv, "mha_fwd: Lq != Lkv requires x_kv");
     VLPK_TRY(qkv_fwd(Mq, H, w, x, a->qkv, st));
@@ -241,22 +242,13 @@ int mha_fwd_impl(const VlpkShape* s, const VlpkLayerWeights* w, const void* x, c
   } else {
     VLPK_CHECK_ARG(a->kv != nullptr, "mha_fwd: incremental decode needs acts.kv");
     VLPK_TRY(fwd_linear(Mq, H, H, x, H, w->wq, H, w->bq, a->qkv, H, EPI_STORE, nullptr, 0, none, st));
-    GemmDesc g;
-    g.M = Mkv; g.N = 2 * H; g.K = H;
-    g.A = x_kv; g.lda = H;
-    g.nseg = 2; g.b_seg_rows = H; g.ldb = H;
-    g.B[0] = w->wk; g.B[1] = w->wv;
-    g.bias[0] = static_cast<const bf16*>(w->bk); g.bias[1] = static_cast<const bf16*>(w->bv);
-    g.D0 = a->kv; g.ldd0 = 2 * H;
-    g.epi = EPI_STORE;
-    g.bn = (H % 256 == 0) ? 0 : 128;
-    VLPK_TRY(launch_gemm(g, st));
+    VLPK_TRY(kv_fwd(Mkv, H, w, x_kv, a->kv, st));
     ad.q = a->qkv; ad.ld_q = H;
     ad.k = a->kv;
     ad.v = static_cast<const bf16*>(a->kv) + H;
     ad.ld_kv = 2 * H;
   }
-  VLPK_TRY(launch_attn_fwd(ad, st));
+  VLPK_TRY(launch_attn_fwd(ad, group, nullptr, st));
   return attn_out_ln(s, w, x, a, p_hidden, drop, layer_id, st);
 }
 
@@ -404,80 +396,70 @@ __global__ void relu_bwd_kernel(bf16* __restrict__ dpre, const bf16* __restrict_
   *reinterpret_cast<uint4*>(dpre + i) = make_uint4(o[0], o[1], o[2], o[3]);
 }
 
-// One layer of vlpk_encoder_score_fwd over B sequences of S + T rows (S shared rows, then T query rows).  s: Lq = Lkv = S.
-int score_layer_fwd(const VlpkShape* s, int T, const VlpkLayerWeights* w, const void* x, const uint32_t* shared_bits,
+// One layer of the scoring stacks over s->B sequences of R rows: the first K = R - T rows attend to the keys through key_bits, then
+// the T query rows through query_bits, each also to its own key.
+//   group null (vlpk_encoder_score_fwd): R = S + T; the keys are the K = S = s->Lq shared rows themselves.
+//   group (vlpk_encoder_score_group_fwd): pairs, G per image, of R = 2T - 1 rows, K = T - 1 of them words (no launch when T = 1).
+//   A pair's s->Lkv = P + T - 1 keys are the P rows of its image's prefix cache (group: prefix, prefix_rows, P, G), then its words.
+int score_layer_fwd(const VlpkShape* s, int T, const AttnGroupKv* group, const VlpkLayerWeights* w, const void* x, const uint32_t* key_bits,
                     const uint32_t* query_bits, VlpkLayerActs* a, uint64_t layer_id, cudaStream_t st) {
-  const int H = s->H, S = s->Lq, R = S + T;
-  const DropoutCfg none = make_dropout(0.f, 0, 0);
+  const int H = s->H, K = group != nullptr ? T - 1 : s->Lq, R = K + T;
   VLPK_TRY(qkv_fwd(s->B * R, H, w, x, a->qkv, st));
   const bf16* qkv = static_cast<const bf16*>(a->qkv);
-  // shared rows against the shared rows
+  AttnGroupKv g;  // keys P + j: word j of the pair, read in place from its rows of the packed qkv
+  if (group != nullptr) {
+    g = *group;
+    g.text = qkv + H; g.ld_text = 3 * H; g.T = R; g.pos = 0;
+  }
   AttnDesc ad;
-  ad.B = s->B; ad.heads = s->heads; ad.Lq = S; ad.Lkv = S; ad.kv_slots = s->kv_slots;
-  ad.q = qkv; ad.k = qkv + H; ad.v = qkv + 2 * H;
-  ad.ld_q = ad.ld_kv = 3 * H;
-  ad.q_batch_stride = ad.kv_batch_stride = static_cast<int64_t>(R) * 3 * H;
+  ad.B = s->B; ad.heads = s->heads; ad.Lkv = s->Lkv; ad.kv_slots = s->kv_slots;
+  ad.q = qkv; ad.ld_q = 3 * H; ad.q_batch_stride = static_cast<int64_t>(R) * 3 * H;
+  ad.k = qkv + H; ad.v = qkv + 2 * H; ad.kv_batch_stride = static_cast<int64_t>(R) * 3 * H;  // unused with a group
+  ad.ld_kv = group != nullptr ? 2 * H : 3 * H;  // the prefix cache's rows, or the packed qkv's
   ad.o = a->ctx; ad.ld_o = H; ad.o_batch_stride = static_cast<int64_t>(R) * H;
-  ad.mask_bits = shared_bits; ad.mask_rows = S;
   ad.lse = a->lse;
-  ad.drop = none;
-  VLPK_TRY(launch_attn_fwd(ad, st));
-  // query rows against the shared rows, each plus its own key
+  ad.drop = make_dropout(0.f, 0, 0);
+  if (K > 0) {
+    AttnDesc kd = ad;
+    kd.Lq = K;
+    kd.mask_bits = key_bits; kd.mask_rows = K;
+    VLPK_TRY(launch_attn_fwd(kd, group != nullptr ? &g : nullptr, nullptr, st));
+  }
   AttnDesc qd = ad;
   qd.Lq = T;
-  qd.q = qkv + static_cast<size_t>(S) * 3 * H;
-  qd.o = static_cast<bf16*>(a->ctx) + static_cast<size_t>(S) * H;
+  qd.q = qkv + static_cast<size_t>(K) * 3 * H;
+  qd.o = static_cast<bf16*>(a->ctx) + static_cast<size_t>(K) * H;
   qd.mask_bits = query_bits; qd.mask_rows = T;
-  qd.lse = a->lse + static_cast<size_t>(s->B) * s->heads * S;
+  qd.lse = a->lse + static_cast<size_t>(s->B) * s->heads * K;
   AttnSelfKv sk;
-  sk.k = qkv + static_cast<size_t>(S) * 3 * H + H;
-  sk.v = qkv + static_cast<size_t>(S) * 3 * H + 2 * H;
+  sk.k = qkv + static_cast<size_t>(K) * 3 * H + H;
+  sk.v = qkv + static_cast<size_t>(K) * 3 * H + 2 * H;
   sk.ld = 3 * H; sk.batch_stride = static_cast<int64_t>(R) * 3 * H;
-  VLPK_TRY(launch_attn_fwd_self(qd, sk, st));
-  VlpkShape rows = *s;  // the row-wise tail (output projection, LayerNorms, FFN) over all B * (S + T) rows
+  VLPK_TRY(launch_attn_fwd(qd, group != nullptr ? &g : nullptr, &sk, st));
+  VlpkShape rows = *s;  // the row-wise tail (output projection, LayerNorms, FFN) over all B * R rows
   rows.Lq = rows.Lkv = R;
   VLPK_TRY(attn_out_ln(&rows, w, x, a, 0.f, nullptr, layer_id, st));
   return ffn_fwd_impl(&rows, w, a, 0.f, nullptr, layer_id, st);
 }
 
-// One layer of vlpk_encoder_score_group_fwd over s->B pairs (G per image) of 2T - 1 rows: T - 1 word rows, then T query rows.
-// s: Lq = Lkv = S = P + T - 1, the keys of a pair: P prefix rows of its image, then its words.
-int score_group_layer_fwd(const VlpkShape* s, int T, int G, int P, int prefix_rows, const VlpkLayerWeights* w, const void* x,
-                          const void* prefix, const uint32_t* word_bits, const uint32_t* query_bits, VlpkLayerActs* a, uint64_t layer_id,
-                          cudaStream_t st) {
-  const int H = s->H, W = T - 1, R = 2 * T - 1;
-  VLPK_TRY(qkv_fwd(s->B * R, H, w, x, a->qkv, st));
-  const bf16* qkv = static_cast<const bf16*>(a->qkv);
-  AttnGroupKv g;  // keys P + j: word j of the pair, read in place from its rows of the packed qkv
-  g.prefix = prefix; g.prefix_rows = prefix_rows; g.P = P;
-  g.text = qkv + H; g.ld_text = 3 * H; g.T = R; g.G = G; g.pos = 0;
-  AttnDesc ad;
-  ad.B = s->B; ad.heads = s->heads; ad.Lkv = s->Lkv; ad.kv_slots = s->kv_slots;
-  ad.ld_q = 3 * H; ad.q_batch_stride = static_cast<int64_t>(R) * 3 * H;
-  ad.ld_kv = 2 * H;
-  ad.ld_o = H; ad.o_batch_stride = static_cast<int64_t>(R) * H;
-  ad.drop = make_dropout(0.f, 0, 0);
-  if (W > 0) {  // word rows against the prefix and the words up to their own
-    AttnDesc wd = ad;
-    wd.Lq = W; wd.q = qkv; wd.o = a->ctx;
-    wd.mask_bits = word_bits; wd.mask_rows = W;
-    wd.lse = a->lse;
-    VLPK_TRY(launch_attn_fwd_group(wd, g, st));
+// The layer loop of both scoring stacks; with a group, group->prefix is set to prefix[i] for layer i.
+int score_stack_fwd(const VlpkShape* s, int T, int n_layers, const VlpkLayerWeights* w, const void* x, AttnGroupKv* group,
+                    const void* const* prefix, const uint32_t* key_bits, const uint32_t* query_bits, VlpkLayerActs* acts, cudaStream_t st) {
+  const void* cur = x;
+  for (int i = 0; i < n_layers; ++i) {
+    if (group != nullptr) group->prefix = prefix[i];
+    VLPK_TRY(score_layer_fwd(s, T, group, &w[i], cur, key_bits, query_bits, &acts[i], i, st));
+    cur = acts[i].y;
   }
-  // query rows against the prefix and the words, each plus its own key
-  AttnDesc qd = ad;
-  qd.Lq = T; qd.q = qkv + static_cast<size_t>(W) * 3 * H; qd.o = static_cast<bf16*>(a->ctx) + static_cast<size_t>(W) * H;
-  qd.mask_bits = query_bits; qd.mask_rows = T;
-  qd.lse = a->lse + static_cast<size_t>(s->B) * s->heads * W;
-  AttnSelfKv sk;
-  sk.k = qkv + static_cast<size_t>(W) * 3 * H + H;
-  sk.v = qkv + static_cast<size_t>(W) * 3 * H + 2 * H;
-  sk.ld = 3 * H; sk.batch_stride = static_cast<int64_t>(R) * 3 * H;
-  VLPK_TRY(launch_attn_fwd_group_self(qd, g, sk, st));
-  VlpkShape rows = *s;  // the row-wise tail over all B * (2T - 1) rows
-  rows.Lq = rows.Lkv = R;
-  VLPK_TRY(attn_out_ln(&rows, w, x, a, 0.f, nullptr, layer_id, st));
-  return ffn_fwd_impl(&rows, w, a, 0.f, nullptr, layer_id, st);
+  return 0;
+}
+
+// Bytes of one layer's activations over `rows` rows per sequence: eight bf16 buffers (qkv, ctx, t1, y1, u, hmid, t2, y: 8H + 2I per
+// row) plus kv_elems bf16 of K | V, then the fp32 logsumexp and the two float2 LayerNorm statistics per row.
+size_t act_bytes(const VlpkShape* s, size_t rows, size_t kv_elems) {
+  const size_t H = s->H, I = s->I, M = static_cast<size_t>(s->B) * rows;
+  const size_t lse = (static_cast<size_t>(s->B) * s->heads * rows + 3) / 4 * 4;  // keeps the float2 statistics behind it aligned
+  return 2 * (M * (3 * H + 5 * H + 2 * I) + kv_elems) + 4 * (lse + 4 * M);
 }
 
 }  // namespace
@@ -640,7 +622,7 @@ int vlpk_attn_core_fwd_wide(int B, int heads, int Lq, int Lkv, const void* q, in
   d.o = ctx; d.ld_o = ld_ctx;
   d.mask_bits = mask_bits; d.mask_rows = mask_rows; d.lse = lse;
   d.drop = mk_drop(drop, drop ? drop->p : 0.f, site);
-  return launch_attn_fwd(d, S(stream));
+  return launch_attn_fwd(d, nullptr, nullptr, S(stream));
 }
 
 int vlpk_attn_core_fwd(int B, int heads, int Lq, int Lkv, const void* q, int64_t ld_q, const void* k, const void* v, int64_t ld_kv,
@@ -660,7 +642,7 @@ int vlpk_attn_core_self_fwd(int B, int heads, int Lq, int Lkv, const void* q, in
   d.mask_bits = mask_bits; d.mask_rows = Lq; d.lse = lse;
   AttnSelfKv s;
   s.k = k_self; s.v = v_self; s.ld = ld_q; s.batch_stride = q_bstride;
-  return launch_attn_fwd_self(d, s, S(stream));
+  return launch_attn_fwd(d, nullptr, &s, S(stream));
 }
 
 int vlpk_attn_core_group_self_fwd(int B, int G, int heads, int Lq, int Lkv, int P, const void* q, int64_t ld_q, int64_t q_bstride,
@@ -678,7 +660,7 @@ int vlpk_attn_core_group_self_fwd(int B, int G, int heads, int Lq, int Lkv, int 
   g.text = text; g.T = T; g.G = G; g.pos = 0; g.ld_text = ld_text;
   AttnSelfKv s;
   s.k = k_self; s.v = v_self; s.ld = ld_q; s.batch_stride = q_bstride;
-  return launch_attn_fwd_group_self(d, g, s, S(stream));
+  return launch_attn_fwd(d, &g, &s, S(stream));
 }
 
 int vlpk_attn_probs(int B, int heads, int Lq, int Lkv, int row0, const void* q, int64_t ld_q, int64_t q_bstride, const void* k, int64_t ld_k,
@@ -796,8 +778,8 @@ int vlpk_layer_cached_group_fwd(const VlpkShape* s, const VlpkLayerWeights* w, c
   g.prefix = prefix; g.prefix_rows = prefix_rows; g.P = P;
   g.text = text; g.slots = slots; g.T = T; g.G = G; g.pos = pos;
   KvCache c;
-  c.base = text; c.rows = T; c.pos = pos; c.group = &g;
-  VLPK_TRY(mha_fwd_impl(s, w, x, nullptr, mask_bits, mask_rows, a, 0.f, 0.f, nullptr, layer_id, S(stream), &c));
+  c.base = text; c.rows = T; c.pos = pos;
+  VLPK_TRY(mha_fwd_impl(s, w, x, nullptr, mask_bits, mask_rows, a, 0.f, 0.f, nullptr, layer_id, S(stream), &c, &g));
   return ffn_fwd_impl(s, w, a, 0.f, nullptr, layer_id, S(stream));
 }
 
@@ -805,9 +787,7 @@ int vlpk_workspace_bytes(const VlpkShape* s, size_t* out3) {
   VLPK_TRY(check_shape(s));
   VLPK_CHECK_ARG(out3 != nullptr, "workspace_bytes: null output");
   const size_t H = s->H, I = s->I, Mq = static_cast<size_t>(s->B) * s->Lq, Mkv = static_cast<size_t>(s->B) * s->Lkv;
-  const size_t kv = (s->Lkv != s->Lq) ? Mkv * 2 * H : 0;
-  const size_t lse = (static_cast<size_t>(s->B) * s->heads * s->Lq + 3) / 4 * 4;  // keeps the float2 statistics behind it aligned
-  out3[0] = 2 * (Mq * (3 * H + 5 * H + 2 * I) + kv) + 4 * (lse + 4 * Mq);
+  out3[0] = act_bytes(s, s->Lq, (s->Lkv != s->Lq) ? Mkv * 2 * H : 0);
   out3[1] = 2 * (Mq * (7 * H + I + 3 * H));
   out3[2] = 4 * (3 * H * H + 3 * H + H * H + H + 2 * H + I * H + I + H * I + H + 2 * H);
   return 0;
@@ -831,9 +811,7 @@ int vlpk_encoder_score_workspace_bytes(const VlpkShape* s, int T, size_t* out1) 
   VLPK_CHECK_ARG(out1 != nullptr, "encoder_score_workspace_bytes: null output");
   VLPK_CHECK_ARG(s->Lq == s->Lkv && T >= 1 && T <= 512, "encoder_score: Lq=%d must equal Lkv=%d (the shared rows S), T=%d in [1,512]", s->Lq,
                  s->Lkv, T);
-  const size_t H = s->H, I = s->I, M = static_cast<size_t>(s->B) * (s->Lq + T);
-  const size_t lse = (static_cast<size_t>(s->B) * s->heads * (s->Lq + T) + 3) / 4 * 4;
-  out1[0] = 2 * M * (3 * H + 5 * H + 2 * I) + 4 * (lse + 4 * M);
+  out1[0] = act_bytes(s, s->Lq + T, 0);
   return 0;
 }
 
@@ -853,12 +831,7 @@ int vlpk_encoder_score_fwd(const VlpkShape* s, int T, int n_layers, const VlpkLa
                    "encoder_score: layer %d acts missing or misaligned (16-byte bf16 buffers, 4-byte lse, 8-byte statistics), or its output "
                    "aliases its input", i);
   }
-  const void* cur = x;
-  for (int i = 0; i < n_layers; ++i) {
-    VLPK_TRY(score_layer_fwd(s, T, &w[i], cur, shared_bits, query_bits, &acts[i], i, S(stream)));
-    cur = acts[i].y;
-  }
-  return 0;
+  return score_stack_fwd(s, T, n_layers, w, x, nullptr, nullptr, shared_bits, query_bits, acts, S(stream));
 }
 
 int vlpk_encoder_score_group_workspace_bytes(const VlpkShape* s, int T, size_t* out1) {
@@ -866,9 +839,7 @@ int vlpk_encoder_score_group_workspace_bytes(const VlpkShape* s, int T, size_t* 
   VLPK_CHECK_ARG(out1 != nullptr, "encoder_score_group_workspace_bytes: null output");
   VLPK_CHECK_ARG(s->Lq == s->Lkv && T >= 1 && T <= s->Lkv, "encoder_score_group: Lq=%d must equal Lkv=%d (the keys S), T=%d in [1, S]", s->Lq,
                  s->Lkv, T);
-  const size_t H = s->H, I = s->I, M = static_cast<size_t>(s->B) * (2 * T - 1);
-  const size_t lse = (static_cast<size_t>(s->B) * s->heads * (2 * T - 1) + 3) / 4 * 4;
-  out1[0] = 2 * M * (3 * H + 5 * H + 2 * I) + 4 * (lse + 4 * M);
+  out1[0] = act_bytes(s, 2 * T - 1, 0);
   return 0;
 }
 
@@ -893,12 +864,9 @@ int vlpk_encoder_score_group_fwd(const VlpkShape* s, int T, int G, int P, int n_
                    "encoder_score_group: layer %d prefix cache or acts missing or misaligned (16-byte bf16 buffers, 4-byte lse, 8-byte "
                    "statistics), or its output aliases its input", i);
   }
-  const void* cur = x;
-  for (int i = 0; i < n_layers; ++i) {
-    VLPK_TRY(score_group_layer_fwd(s, T, G, P, prefix_rows, &w[i], cur, prefix[i], word_bits, query_bits, &acts[i], i, S(stream)));
-    cur = acts[i].y;
-  }
-  return 0;
+  AttnGroupKv g;
+  g.prefix_rows = prefix_rows; g.P = P; g.G = G;
+  return score_stack_fwd(s, T, n_layers, w, x, &g, prefix, word_bits, query_bits, acts, S(stream));
 }
 
 int vlpk_encoder_bwd(const VlpkShape* s, int n_layers, const VlpkLayerWeights* w, const void* x, const uint32_t* mask_bits, int mask_rows,

@@ -1240,16 +1240,16 @@ static AttnTiledArgs tiled_args(const AttnDesc& d) {
   return a;
 }
 
-static int launch_attn_fwd_tiled(const AttnDesc& d, const AttnTmaps& tm, cudaStream_t stream) {
-  AttnTiledArgs a = tiled_args(d);
-  a.keep_out = d.keep_out;
+// Launches Kernel with ATT_THREADS threads and `smem` bytes of dynamic shared memory, raising its limit to `smem` on the first launch.
+// The flag is per kernel (a template argument), not per kernel type: kernels of one signature need different limits.
+template <auto Kernel, typename... Args>
+static int launch_attn_kernel(dim3 grid, int smem, cudaStream_t stream, const Args&... args) {
   static bool attr_set = false;
   if (!attr_set) {
-    VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdTiledSmem::DYN));
+    VLPK_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_set = true;
   }
-  LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * d.Lkv * HD, stream);
-  VLPK_CUDA(launch_ex(attn_fwd_tiled_kernel, dim3(d.heads, d.B, (d.Lq + TL - 1) / TL), dim3(ATT_THREADS), FwdTiledSmem::DYN, stream, 1, tm, a));
+  VLPK_CUDA(launch_ex(Kernel, grid, dim3(ATT_THREADS), smem, stream, 1, args...));
   return 0;
 }
 
@@ -1262,21 +1262,14 @@ static int launch_attn_bwd_tiled(const AttnDesc& d, const AttnTmaps& tm, cudaStr
     a.dbias_part = scratch_f32(SCRATCH_ATTN_DBIAS, static_cast<size_t>(d.B) * a.tiles * nbias, stream);
     if (a.dbias_part == nullptr) return -1;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    VLPK_CUDA(cudaFuncSetAttribute(attn_bwd_dq_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdDqSmem::DYN));
-    VLPK_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdDkvSmem::DYN));
-    attr_set = true;
-  }
   const double flops = 10.0 * d.B * d.heads * d.Lq * d.Lkv * HD;  // algorithmic: the recomputed products are not counted
   {
     LaunchScope scope(CAT_ATTN_BWD, 0.4 * flops, stream);
-    VLPK_CUDA(launch_ex(attn_bwd_dq_tiled_kernel, dim3(d.heads, d.B, a.tiles), dim3(ATT_THREADS), BwdDqSmem::DYN, stream, 1, tm, a));
+    VLPK_TRY(launch_attn_kernel<attn_bwd_dq_tiled_kernel>(dim3(d.heads, d.B, a.tiles), BwdDqSmem::DYN, stream, tm, a));
   }
   {
     LaunchScope scope(CAT_ATTN_BWD, 0.6 * flops, stream);
-    VLPK_CUDA(launch_ex(attn_bwd_dkv_tiled_kernel, dim3(d.heads, d.B, (d.Lkv + TL - 1) / TL), dim3(ATT_THREADS), BwdDkvSmem::DYN, stream, 1,
-                        tm, a));
+    VLPK_TRY(launch_attn_kernel<attn_bwd_dkv_tiled_kernel>(dim3(d.heads, d.B, (d.Lkv + TL - 1) / TL), BwdDkvSmem::DYN, stream, tm, a));
   }
   if (d.dbias != nullptr) VLPK_TRY(launch_sum_parts(a.dbias_part, d.B * a.tiles, nbias, d.dbias, stream));
   return 0;
@@ -1306,22 +1299,6 @@ static AttnArgs fwd_args(const AttnDesc& d) {
   return a;
 }
 
-int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream) {
-  VLPK_TRY(check_common(d));
-  AttnTmaps tm;
-  VLPK_TRY(fwd_tmaps(d, &tm));
-  if (use_tiled(d)) return launch_attn_fwd_tiled(d, tm, stream);
-  const AttnArgs a = fwd_args(d);
-  static bool attr_set = false;
-  if (!attr_set) {
-    VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem::DYN));
-    attr_set = true;
-  }
-  LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * d.Lkv * HD, stream);
-  VLPK_CUDA(launch_ex(attn_fwd_kernel, dim3(d.heads, d.B), dim3(ATT_THREADS), FwdSmem::DYN, stream, 1, tm, a));
-  return 0;
-}
-
 // Tensor maps and loader arguments of a shared-prefix forward: Q / ctx of the d.B hypotheses with their strides, K / V boxes over
 // the P prefix rows of each image, text rows gd.ld_text (0: d.ld_kv) elements apart.
 static int group_setup(const AttnDesc& d, const AttnGroupKv& gd, AttnTmaps* tm, GroupKv* g) {
@@ -1343,36 +1320,6 @@ static int group_setup(const AttnDesc& d, const AttnGroupKv& gd, AttnTmaps* tm, 
   g->ld = ld_text;
   g->H = width; g->G = gd.G; g->P = gd.P; g->pos = gd.pos; g->T = gd.T;
   g->text_rows = static_cast<long long>(d.B) * gd.T;
-  return 0;
-}
-
-int launch_attn_fwd_group(const AttnDesc& d, const AttnGroupKv& gd, cudaStream_t stream) {
-  VLPK_TRY(check_common(d));
-  VLPK_CHECK_ARG(gd.P >= 1 && gd.P <= gd.prefix_rows && gd.pos >= 0 && gd.pos + d.Lq <= gd.T && gd.P + gd.pos + d.Lq == d.Lkv,
-                 "attention group: P=%d (prefix rows %d) pos=%d Lq=%d T=%d Lkv=%d", gd.P, gd.prefix_rows, gd.pos, d.Lq, gd.T, d.Lkv);
-  AttnTmaps tm;
-  GroupKv g;
-  VLPK_TRY(group_setup(d, gd, &tm, &g));
-  const dim3 grid(gd.G * d.heads, d.B / gd.G, (d.Lq + TL - 1) / TL);
-  LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * d.Lkv * HD, stream);
-  if (use_tiled(d)) {
-    AttnTiledArgs a = tiled_args(d);
-    static bool attr_set = false;
-    if (!attr_set) {
-      VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_group_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdTiledSmem::DYN));
-      attr_set = true;
-    }
-    VLPK_CUDA(launch_ex(attn_fwd_group_tiled_kernel, grid, dim3(ATT_THREADS), FwdTiledSmem::DYN, stream, 1, tm, a, g));
-    return 0;
-  }
-  AttnArgs a = fwd_args(d);
-  a.keep_out = nullptr;
-  static bool attr_set = false;
-  if (!attr_set) {
-    VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem::DYN));
-    attr_set = true;
-  }
-  VLPK_CUDA(launch_ex(attn_fwd_group_kernel, dim3(grid.x, grid.y), dim3(ATT_THREADS), FwdSmem::DYN, stream, 1, tm, a, g));
   return 0;
 }
 
@@ -1403,63 +1350,47 @@ static SelfKv self_kv(const AttnDesc& d, const AttnSelfKv& sd) {
   return sk;
 }
 
-int launch_attn_fwd_self(const AttnDesc& d, const AttnSelfKv& sd, cudaStream_t stream) {
-  VLPK_TRY(check_self(d, sd));
-  VLPK_CHECK_ARG(d.k && d.v, "attention self: null pointer");
+int launch_attn_fwd(const AttnDesc& d, const AttnGroupKv* gd, const AttnSelfKv* sd, cudaStream_t stream) {
+  // Each key source keeps its own rules: check_self takes lengths check_common refuses, and the two group rules differ.
+  if (sd == nullptr) VLPK_TRY(check_common(d));
+  else VLPK_TRY(check_self(d, *sd));
   AttnTmaps tm;
-  VLPK_TRY(fwd_tmaps(d, &tm));
-  const SelfKv sk = self_kv(d, sd);
-  LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * (d.Lkv + 1) * HD, stream);
-  if (use_tiled(d)) {
-    const AttnTiledArgs a = tiled_args(d);
-    static bool attr_set = false;
-    if (!attr_set) {
-      VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_self_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdTiledSmem::DYN));
-      attr_set = true;
-    }
-    VLPK_CUDA(launch_ex(attn_fwd_self_tiled_kernel, dim3(d.heads, d.B, (d.Lq + TL - 1) / TL), dim3(ATT_THREADS), FwdTiledSmem::DYN, stream,
-                        1, tm, a, sk));
-    return 0;
+  GroupKv g{};
+  if (gd == nullptr) {
+    if (sd != nullptr) VLPK_CHECK_ARG(d.k && d.v, "attention self: null pointer");
+    VLPK_TRY(fwd_tmaps(d, &tm));
+  } else {
+    if (sd == nullptr)
+      VLPK_CHECK_ARG(gd->P >= 1 && gd->P <= gd->prefix_rows && gd->pos >= 0 && gd->pos + d.Lq <= gd->T && gd->P + gd->pos + d.Lq == d.Lkv,
+                     "attention group: P=%d (prefix rows %d) pos=%d Lq=%d T=%d Lkv=%d", gd->P, gd->prefix_rows, gd->pos, d.Lq, gd->T, d.Lkv);
+    else
+      VLPK_CHECK_ARG(gd->P >= 1 && gd->P <= gd->prefix_rows && gd->pos >= 0 && gd->P + gd->pos <= d.Lkv && d.Lkv - gd->P <= gd->T,
+                     "attention group self: P=%d (prefix rows %d) pos=%d Lkv=%d T=%d (needs P + pos <= Lkv <= P + T)", gd->P, gd->prefix_rows,
+                     gd->pos, d.Lkv, gd->T);
+    VLPK_TRY(group_setup(d, *gd, &tm, &g));
   }
-  const AttnArgs a = fwd_args(d);  // keep_out is null: checked above
-  static bool attr_set = false;
-  if (!attr_set) {
-    VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_self_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem::DYN));
-    attr_set = true;
+  const SelfKv sk = sd != nullptr ? self_kv(d, *sd) : SelfKv{};
+  unsigned char* keep_out = gd != nullptr ? nullptr : d.keep_out;  // with a self key d.keep_out is null: check_self refuses it
+  const int G = gd != nullptr ? gd->G : 1;
+  const bool tiled = use_tiled(d);
+  const dim3 grid(G * d.heads, d.B / G, tiled ? (d.Lq + TL - 1) / TL : 1);
+  LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * (d.Lkv + (sd != nullptr ? 1 : 0)) * HD, stream);
+  if (tiled) {
+    AttnTiledArgs a = tiled_args(d);
+    a.keep_out = keep_out;
+    constexpr int smem = FwdTiledSmem::DYN;
+    if (gd != nullptr && sd != nullptr) return launch_attn_kernel<attn_fwd_group_self_tiled_kernel>(grid, smem, stream, tm, a, g, sk);
+    if (gd != nullptr) return launch_attn_kernel<attn_fwd_group_tiled_kernel>(grid, smem, stream, tm, a, g);
+    if (sd != nullptr) return launch_attn_kernel<attn_fwd_self_tiled_kernel>(grid, smem, stream, tm, a, sk);
+    return launch_attn_kernel<attn_fwd_tiled_kernel>(grid, smem, stream, tm, a);
   }
-  VLPK_CUDA(launch_ex(attn_fwd_self_kernel, dim3(d.heads, d.B), dim3(ATT_THREADS), FwdSmem::DYN, stream, 1, tm, a, sk));
-  return 0;
-}
-
-int launch_attn_fwd_group_self(const AttnDesc& d, const AttnGroupKv& gd, const AttnSelfKv& sd, cudaStream_t stream) {
-  VLPK_TRY(check_self(d, sd));
-  VLPK_CHECK_ARG(gd.P >= 1 && gd.P <= gd.prefix_rows && gd.pos >= 0 && gd.P + gd.pos <= d.Lkv && d.Lkv - gd.P <= gd.T,
-                 "attention group self: P=%d (prefix rows %d) pos=%d Lkv=%d T=%d (needs P + pos <= Lkv <= P + T)", gd.P, gd.prefix_rows,
-                 gd.pos, d.Lkv, gd.T);
-  AttnTmaps tm;
-  GroupKv g;
-  VLPK_TRY(group_setup(d, gd, &tm, &g));
-  const SelfKv sk = self_kv(d, sd);
-  const dim3 grid(gd.G * d.heads, d.B / gd.G, (d.Lq + TL - 1) / TL);
-  LaunchScope scope(CAT_ATTN_FWD, 4.0 * d.B * d.heads * d.Lq * (d.Lkv + 1) * HD, stream);
-  if (use_tiled(d)) {
-    const AttnTiledArgs a = tiled_args(d);
-    static bool attr_set = false;
-    if (!attr_set) {
-      VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_group_self_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdTiledSmem::DYN));
-      attr_set = true;
-    }
-    VLPK_CUDA(launch_ex(attn_fwd_group_self_tiled_kernel, grid, dim3(ATT_THREADS), FwdTiledSmem::DYN, stream, 1, tm, a, g, sk));
-    return 0;
-  }
-  const AttnArgs a = fwd_args(d);  // keep_out is null: checked above
-  static bool attr_set = false;
-  if (!attr_set) {
-    VLPK_CUDA(cudaFuncSetAttribute(attn_fwd_group_self_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwdSmem::DYN));
-    attr_set = true;
-  }
-  VLPK_CUDA(launch_ex(attn_fwd_group_self_kernel, dim3(grid.x, grid.y), dim3(ATT_THREADS), FwdSmem::DYN, stream, 1, tm, a, g, sk));
-  return 0;
+  AttnArgs a = fwd_args(d);
+  a.keep_out = keep_out;
+  constexpr int smem = FwdSmem::DYN;
+  if (gd != nullptr && sd != nullptr) return launch_attn_kernel<attn_fwd_group_self_kernel>(grid, smem, stream, tm, a, g, sk);
+  if (gd != nullptr) return launch_attn_kernel<attn_fwd_group_kernel>(grid, smem, stream, tm, a, g);
+  if (sd != nullptr) return launch_attn_kernel<attn_fwd_self_kernel>(grid, smem, stream, tm, a, sk);
+  return launch_attn_kernel<attn_fwd_kernel>(grid, smem, stream, tm, a);
 }
 
 int launch_attn_bwd(const AttnDesc& d, cudaStream_t stream) {
@@ -1477,29 +1408,18 @@ int launch_attn_bwd(const AttnDesc& d, cudaStream_t stream) {
   VLPK_TRY(make_seq_tmap(&tm.dk, d.dk, width, d.Lkv, d.B, d.ld_dqkv));
   VLPK_TRY(make_seq_tmap(&tm.dv, d.dv, width, d.Lkv, d.B, d.ld_dqkv));
   if (use_tiled(d)) return launch_attn_bwd_tiled(d, tm, stream);
-  AttnArgs a;
-  a.B = d.B; a.heads = d.heads; a.Lq = d.Lq; a.Lkv = d.Lkv;
-  a.mask_bits = d.mask_bits; a.mask_rows = d.mask_rows;
-  a.lse = d.lse;
+  AttnArgs a = fwd_args(d);
   a.o_ptr = reinterpret_cast<const __nv_bfloat16*>(d.o);
   a.do_ptr = reinterpret_cast<const __nv_bfloat16*>(d.d_o);
-  a.ld_o = d.ld_o;
-  a.drop = d.drop;
   a.keep_out = nullptr;
-  a.dbias_part = nullptr;
   const long long nbias = 3LL * d.heads * HD;
   if (d.dbias != nullptr) {
     a.dbias_part = scratch_f32(SCRATCH_ATTN_DBIAS, static_cast<size_t>(d.B) * nbias, stream);
     if (a.dbias_part == nullptr) return -1;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    VLPK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, BwdSmem::DYN));
-    attr_set = true;
-  }
   {
     LaunchScope scope(CAT_ATTN_BWD, 10.0 * d.B * d.heads * d.Lq * d.Lkv * HD, stream);
-    VLPK_CUDA(launch_ex(attn_bwd_kernel, dim3(d.heads, d.B), dim3(ATT_THREADS), BwdSmem::DYN, stream, 1, tm, a));
+    VLPK_TRY(launch_attn_kernel<attn_bwd_kernel>(dim3(d.heads, d.B), BwdSmem::DYN, stream, tm, a));
   }
   if (d.dbias != nullptr) VLPK_TRY(launch_sum_parts(a.dbias_part, d.B, nbias, d.dbias, stream));
   return 0;
@@ -1536,16 +1456,10 @@ int launch_attn_probs(const AttnDesc& d, int64_t q_batch_stride, int row0, float
   a.ld_p = ld_p;
   a.p_bstride = pbs;
   a.vec2 = (reinterpret_cast<uintptr_t>(p) & 7u) == 0 && ld_p % 2 == 0 && pbs % 2 == 0;
-  static bool attr_set = false;
-  if (!attr_set) {
-    VLPK_CUDA(cudaFuncSetAttribute(attn_probs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ProbsSmem::DYN));
-    attr_set = true;
-  }
   // bandwidth kernel: fp32 P written, Q / K / lse read
   const double bytes = 4.0 * d.B * d.heads * rows * d.Lkv + 2.0 * d.B * width * (rows + d.Lkv) + 4.0 * d.B * d.heads * rows;
   LaunchScope scope(CAT_MISC, bytes, stream);
-  VLPK_CUDA(launch_ex(attn_probs_kernel, dim3(d.heads, d.B, (rows + TL - 1) / TL), dim3(ATT_THREADS), ProbsSmem::DYN, stream, 1, tm, a));
-  return 0;
+  return launch_attn_kernel<attn_probs_kernel>(dim3(d.heads, d.B, (rows + TL - 1) / TL), ProbsSmem::DYN, stream, tm, a);
 }
 
 }  // namespace vlpk

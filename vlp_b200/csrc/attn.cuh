@@ -35,6 +35,9 @@ struct AttnDesc {
 // key r < P from row r of image b / G's prefix [images, prefix_rows, ld_kv], key P + j from text row slots[b * T + j] (j < pos) or
 // b * T + j (its own rows) of text [B * T rows, ld_text]; K at column 0, V at column heads * 64 of both.  slots may be NULL when
 // pos = 0.  mask_bits has one sequence per image.  Q / ctx take d.q_batch_stride / d.o_batch_stride.
+// Forward only, no dropout: d.k / d.v / d.kv_batch_stride unused, d.ld_kv is the row stride of prefix and text.  Needs
+// P + pos + Lq == Lkv and pos + Lq <= T; with a self key (AttnSelfKv), P + pos <= Lkv <= P + T instead: key P + j, j < Lkv - P, from
+// the hypothesis' text rows, then each query row's own key.
 struct AttnGroupKv {
   const void* prefix = nullptr;
   int prefix_rows = 0, P = 0;
@@ -44,11 +47,6 @@ struct AttnGroupKv {
   int64_t ld_text = 0;  // row stride of text (0: d.ld_kv)
 };
 
-// Lq, Lkv <= 128: the single-tile kernels; longer sequences (or the "attn_tiled" test option): the KV-tiled kernels.
-int launch_attn_fwd(const AttnDesc& d, cudaStream_t stream);
-// Forward only, no dropout: d.k / d.v / d.kv_batch_stride unused, d.ld_kv is the row stride of prefix and text.
-int launch_attn_fwd_group(const AttnDesc& d, const AttnGroupKv& g, cudaStream_t stream);
-int launch_attn_bwd(const AttnDesc& d, cudaStream_t stream);
 // Query row i of sequence b also attends to one extra key, its own (k_self, v_self) row: k_self + b * self_batch_stride + i * ld_self
 // (v_self alike), never masked.  Forward only, no dropout; d.mask_rows must be d.Lq.  Lq, Lkv in [1, 512]: the single-tile kernel when
 // both are <= 128 (kv_slots 0), else the tiled one (kv_slots = 128 * ceil(Lkv / 128), or 0 for Lkv <= 128: the 128-slot layout).
@@ -57,10 +55,11 @@ struct AttnSelfKv {
   const void* v = nullptr;
   int64_t ld = 0, batch_stride = 0;
 };
-int launch_attn_fwd_self(const AttnDesc& d, const AttnSelfKv& s, cudaStream_t stream);
-// launch_attn_fwd_self with the keys of launch_attn_fwd_group (d.k / d.v unused): key P + j, j < Lkv - P, from the hypothesis' text
-// rows, then each query row's own key.  Needs P + pos <= Lkv <= P + T.
-int launch_attn_fwd_group_self(const AttnDesc& d, const AttnGroupKv& g, const AttnSelfKv& s, cudaStream_t stream);
+
+// Keys from d.k / d.v, or from a shared prefix (group non-null); self non-null adds each query row's own key.  Lq, Lkv <= 128: the
+// single-tile kernels; longer sequences (or the "attn_tiled" test option): the KV-tiled kernels.
+int launch_attn_fwd(const AttnDesc& d, const AttnGroupKv* group, const AttnSelfKv* self, cudaStream_t stream);
+int launch_attn_bwd(const AttnDesc& d, cudaStream_t stream);
 void set_attn_tiled(bool on);
 // Attention probabilities exp(s - lse) of query rows [row0, Lq) into p [B, heads, Lq - row0, ld_p] (sequences p_batch_stride floats
 // apart, 0 = heads * (Lq - row0) * ld_p) from d.q / d.k / d.mask_bits / d.lse; q_batch_stride as d.kv_batch_stride for Q.
