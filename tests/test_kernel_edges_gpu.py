@@ -201,25 +201,6 @@ def _layer(H, B=3, Lq=123, seed=0):
     return dict(H=H, I=I, M=B * Lq, gen=gen, params=params, x=x.view(B * Lq, H), bits=bits, shape=shape, ws=ws, acts=acts)
 
 
-def _scratch_view(buf, M, H, I, name):
-    sizes = {"dz2": M * H, "dt2": M * H, "du": M * I, "dy1": M * H, "dz1": M * H, "dt1": M * H, "dctx": M * H, "dqkv": 3 * M * H, "dx": M * H}
-    off = 0
-    for n in L.SCRATCH_FIELDS:
-        if n == name:
-            return buf[off:off + sizes[n]].view(M, sizes[n] // M)
-        off += sizes[n]
-    raise KeyError(name)
-
-
-def _grad_seg(arena, H, I, name):
-    off = 0
-    for n, sz in zip(L.GRAD_FIELDS, ops._layer_sizes(H, I)):
-        if n == name:
-            return arena[off:off + sz]
-        off += sz
-    raise KeyError(name)
-
-
 def _check(name, family, got, ref, E):
     e, t = kc.check_gemm(name, got, ref, E)
     _note(f"{family} elementwise", e)
@@ -269,7 +250,7 @@ def _mha_bwd(lay, dy1, wgrad_stream):
     L.call("vlpk_mha_bwd", C.byref(lay["shape"]), lay["ws"], lay["x"].data_ptr(), lay["bits"].data_ptr(), lay["bits"].shape[1],
            lay["acts"].structs, dy1.data_ptr(), dx.data_ptr(), C.byref(g), C.byref(st), 0.0, 0.0, None, 0, L.stream())
     torch.cuda.synchronize()
-    return arena, buf, dx
+    return ops.carve(arena, ops.grad_layout(H, I)), ops.carve(buf, ops.scratch_layout(M, H, I)), dx
 
 
 @pytest.mark.parametrize("wgrad_stream", [0, 1])
@@ -278,18 +259,17 @@ def test_mha_bwd_qkv_dgrad_and_bias_gradient(H, wgrad_stream):
     lay = _layer(H, seed=1)
     I, M, p = lay["I"], lay["M"], lay["params"]
     dy1 = abi_cases._rn(lay["gen"], DEV, M, H, scale=0.1)
-    arena, buf, dx = _mha_bwd(lay, dy1, wgrad_stream)
-    dqkv = _scratch_view(buf, M, H, I, "dqkv")
-    dz1 = _scratch_view(buf, M, H, I, "dz1")
+    grads, scr, dx = _mha_bwd(lay, dy1, wgrad_stream)
+    dqkv, dz1 = scr["dqkv"], scr["dz1"]
     # dx = dqkv [M, 3H] Wqkv [3H, H] + dz1: 3-segment MN-major B operand, ADD epilogue
     acc, E = kc.gemm_ref(dqkv, torch.cat(p[0:3]).t())
     ref, Er = kc.epilogue_ref(ADD, acc, E, aux=dz1)["d0"]
     _check(f"mha_bwd dx H{H}", "entry bf16", dx, ref, Er)
     kc.assert_guard_intact(dx, "mha_bwd dx")
-    _note("bias-gradient sums", kc.check_colsum(f"mha_bwd bqkv H{H}", _grad_seg(arena, H, I, "bqkv"), dqkv))
+    _note("bias-gradient sums", kc.check_colsum(f"mha_bwd bqkv H{H}", grads["bqkv"], dqkv))
     # run to run: the q/k/v bias gradient is summed in a fixed order over the sequences
-    arena2, _, _ = _mha_bwd(lay, dy1, wgrad_stream)
-    assert torch.equal(_grad_seg(arena, H, I, "bqkv"), _grad_seg(arena2, H, I, "bqkv"))
+    grads2, _, _ = _mha_bwd(lay, dy1, wgrad_stream)
+    assert torch.equal(grads["bqkv"], grads2["bqkv"])
 
 
 @pytest.mark.parametrize("wgrad_stream", [0, 1])
@@ -306,14 +286,14 @@ def test_ffn_bwd_gelu_dgrad_and_fused_colsum(H, wgrad_stream):
     L.call("vlpk_ffn_bwd", C.byref(lay["shape"]), lay["ws"], lay["acts"].structs, dy.data_ptr(), dy1.data_ptr(), C.byref(g), C.byref(st),
            0.0, None, 0, L.stream())
     torch.cuda.synchronize()
-    dz2 = _scratch_view(buf, M, H, I, "dz2")          # p = 0: dt2 = dz2
-    du = _scratch_view(buf, M, H, I, "du")
+    scr = ops.carve(buf, ops.scratch_layout(M, H, I))
+    dz2, du = scr["dz2"], scr["du"]          # p = 0: dt2 = dz2
     u = abi_cases.act_view(lay["acts"], 0, "u", M, I)
     # du = (dt2 W2) * gelu'(u): MUL epilogue; db1 = column sums of du fused into the same epilogue
     acc, E = kc.gemm_ref(dz2, p[12].t())
     ref, Er = kc.epilogue_ref(MUL, acc, E, aux=u)["d0"]
     _check(f"ffn_bwd du H{H}", "entry bf16", du, ref, Er)
-    _note("bias-gradient sums", kc.check_colsum(f"ffn_bwd b1 H{H}", _grad_seg(arena, H, I, "b1"), du))
+    _note("bias-gradient sums", kc.check_colsum(f"ffn_bwd b1 H{H}", ops.carve(arena, ops.grad_layout(H, I))["b1"], du))
     # dy1 = du W1 + dz2
     acc, E = kc.gemm_ref(du, p[10].t())
     ref, Er = kc.epilogue_ref(ADD, acc, E, aux=dz2)["d0"]

@@ -60,32 +60,25 @@ def s2s_mask(B, L, n_src, dev):
 
 def grad_struct(arena_row, H, I):
     gs = L.VlpkLayerGrads()
-    off = 0
-    for name, sz in zip(L.GRAD_FIELDS, ops._layer_sizes(H, I)):
-        setattr(gs, name, arena_row[off:off + sz].data_ptr())
-        off += sz
-    assert off == arena_row.numel()
+    ops.carve(arena_row, ops.grad_layout(H, I), gs)
     return gs
 
 
 def bwd_scratch(M, H, I, dev):
-    sizes = {"dz2": M * H, "dt2": M * H, "du": M * I, "dy1": M * H, "dz1": M * H, "dt1": M * H, "dctx": M * H, "dqkv": 3 * M * H, "dx": M * H}
-    buf = torch.empty(sum(sizes.values()), device=dev, dtype=BF16)
+    layout = ops.scratch_layout(M, H, I)
+    buf = torch.empty(ops.layout_numel(layout), device=dev, dtype=BF16)
     st = L.VlpkBwdScratch()
-    off = 0
-    for name in L.SCRATCH_FIELDS:
-        setattr(st, name, buf[off:off + sizes[name]].data_ptr())
-        off += sizes[name]
+    ops.carve(buf, layout, st)
     return st, buf
 
 
 def act_view(acts, layer, name, rows, width):
-    off = 0
-    for n, sz in acts.bf_sizes:
-        if n == name:
-            return acts.bf[layer][off:off + sz].view(rows, width)
-        off += sz
-    raise KeyError(name)
+    return acts.view(layer, name).view(rows, width)
+
+
+def _point(struct, views):
+    for n, t in views.items():
+        setattr(struct, n, t.data_ptr())
 
 
 def split_backward_case(dev, B=3, Lq=123, H=128, heads=2, I=512, p=0.1, seed=1234):
@@ -149,52 +142,44 @@ def incremental_case(dev, B=2, Lq=2, Lkv=50, H=128, heads=2, I=512):
 
 # ---- encoder stack and cached decode layer (tests/test_encoder_stack_gpu.py) ------------------------------------------------------
 def guarded_acts(n_layers, B, Lq, H, heads, I, dev, drop_bits=False, decode=False):
-    """Per-layer VlpkLayerActs whose every buffer is a NaN-guarded view (tools/kernel_check.guarded).  decode: the layout of
-    vlpk_layer_cached_fwd (qkv holds Q [B*Lq, H], kv the new rows' K | V [B*Lq, 2H]).  drop_bits: attention keep-bits followed by 64
-    guard bytes of 0xA5.  Returns (structs, [dict of views per layer], keep-bit buffer or None)."""
-    M = B * Lq
+    """Per-layer VlpkLayerActs whose every buffer is a NaN-guarded view (tools/kernel_check.guarded) of its ops.act_layout shape.
+    decode: the layout of vlpk_layer_cached_fwd (qkv holds Q [B*Lq, H], kv the new rows' K | V [B*Lq, 2H]).  drop_bits: attention
+    keep-bits followed by 64 guard bytes of 0xA5.  Returns (structs, [dict of views per layer], keep-bit buffer or None)."""
     structs = (L.VlpkLayerActs * n_layers)()
     nb = B * heads * Lq * ops.key_slots(Lq) // 8
     bits = torch.full((n_layers, nb + 64), 0xA5, dtype=torch.uint8, device=dev) if drop_bits else None
-    views = []
-    widths = [("qkv", H if decode else 3 * H), ("ctx", H), ("t1", H), ("y1", H), ("u", I), ("hmid", I), ("t2", H), ("y", H)]
+    bf, f32 = ops.act_layout(B, Lq, H, heads, I, Lkv=Lq if decode else None)
+    fields = {n: (s, BF16) for n, s in bf} | {n: (s, torch.float32) for n, s in f32 if n is not None}
     if decode:
-        widths.append(("kv", 2 * H))
+        # the cached layer stores only Q in qkv: guarding exactly [B*Lq, H] catches a store past Q, which ops' 3H-wide buffer would hide
+        fields["qkv"] = ((B * Lq, H), BF16)
+    views = []
     for i in range(n_layers):
-        v = {n: kc.guarded(M, c, device=dev) for n, c in widths}
-        v["lse"] = kc.guarded(1, B * heads * Lq, dtype=torch.float32, device=dev)
-        v["stats1"] = kc.guarded(M, 2, dtype=torch.float32, device=dev)
-        v["stats2"] = kc.guarded(M, 2, dtype=torch.float32, device=dev)
-        for n, t in v.items():
-            setattr(structs[i], n, t.data_ptr())
-        if not decode:
-            structs[i].kv = None
+        v = {n: kc.guarded(*s, dtype=dt, device=dev) for n, (s, dt) in fields.items()}
+        _point(structs[i], v)
         structs[i].drop_attn = None if bits is None else bits[i].data_ptr()
         views.append(v)
     return structs, views, bits
 
 
 def guarded_scratch(M, H, I, dev):
-    """VlpkBwdScratch of NaN-guarded views: (struct, dict of views)."""
-    widths = {"dz2": H, "dt2": H, "du": I, "dy1": H, "dz1": H, "dt1": H, "dctx": H, "dqkv": 3 * H, "dx": H}
-    st, v = L.VlpkBwdScratch(), {}
-    for n in L.SCRATCH_FIELDS:
-        v[n] = kc.guarded(M, widths[n], device=dev)
-        setattr(st, n, v[n].data_ptr())
+    """VlpkBwdScratch of NaN-guarded views of the ops.scratch_layout shapes: (struct, dict of views)."""
+    st, v = L.VlpkBwdScratch(), {n: kc.guarded(*s, device=dev) for n, s in ops.scratch_layout(M, H, I)}
+    _point(st, v)
     return st, v
 
 
 def guarded_grads(priors, H, I, dev):
-    """Per-layer VlpkLayerGrads of NaN-guarded fp32 views holding the given prior contents ([{name: tensor}] per layer, shapes of
-    layer_check.grad_shapes).  Returns (structs, [dict of 2-D guarded views per layer])."""
+    """Per-layer VlpkLayerGrads of NaN-guarded fp32 views of the ops.grad_layout shapes (a 1-D gradient as one row) holding the
+    given prior contents ([{name: tensor}] per layer).  Returns (structs, [dict of 2-D guarded views per layer])."""
     structs = (L.VlpkLayerGrads * len(priors))()
     views = []
     for i, pr in enumerate(priors):
         v = {}
-        for n in L.GRAD_FIELDS:
-            t = pr[n] if pr[n].dim() == 2 else pr[n][None]
-            v[n] = kc.guard_fill(kc.guarded(t.shape[0], t.shape[1], dtype=torch.float32, device=dev), t)
-            setattr(structs[i], n, v[n].data_ptr())
+        for n, s in ops.grad_layout(H, I):
+            rows, cols = s if len(s) == 2 else (1, s[0])
+            v[n] = kc.guard_fill(kc.guarded(rows, cols, dtype=torch.float32, device=dev), pr[n].reshape(rows, cols))
+        _point(structs[i], v)
         views.append(v)
     return structs, views
 

@@ -25,7 +25,8 @@ worst tile / block / row / column.  Everything runs on whatever device its tenso
 import torch
 
 from tools import kernel_check as kc
-from vlp_b200._lib import GRAD_FIELDS, WEIGHT_FIELDS
+from vlp_b200 import ops
+from vlp_b200._lib import WEIGHT_FIELDS
 
 F64 = torch.float64
 STORE, GELU, ADD, MUL, REDUCE = 0, 1, 3, 4, 6
@@ -43,8 +44,8 @@ def weights(params):
 
 
 def grad_shapes(H, I):
-    return {"wqkv": (3 * H, H), "bqkv": (3 * H,), "wo": (H, H), "bo": (H,), "ln1_g": (H,), "ln1_b": (H,), "w1": (I, H), "b1": (I,),
-            "w2": (H, I), "b2": (H,), "ln2_g": (H,), "ln2_b": (H,)}
+    """{field: shape} of one layer's gradient arena (vlp_b200.ops.grad_layout)."""
+    return dict(ops.grad_layout(H, I))
 
 
 def _wqkv(w):

@@ -6,6 +6,7 @@ these ops anywhere in the package, so a missing library is a hard error.
 """
 import ctypes as C
 import itertools
+import math
 import os
 
 import torch
@@ -116,62 +117,81 @@ def pack_mask(mask, mode="additive"):
 PARAMS_PER_LAYER = 16  # order == _lib.WEIGHT_FIELDS
 
 
+# Per-layer buffer layouts: [(field, shape)] in allocation order, each field's buffer packed right behind the previous one.  A field
+# named None is padding.  vlpk_workspace_bytes states the same sizes on the library side.
+def act_layout(B, Lq, H, heads, I, Lkv=None):
+    """One layer's activations of B x Lq rows: (bf16 layout, fp32 layout).  Lkv: rows per sequence of "kv", the K | V projections
+    that the incremental and cached layers keep apart from qkv; qkv keeps its 3H width there although their kernels store only Q."""
+    M = B * Lq
+    bf = [("qkv", (M, 3 * H)), ("ctx", (M, H)), ("t1", (M, H)), ("y1", (M, H)), ("u", (M, I)), ("hmid", (M, I)), ("t2", (M, H)),
+          ("y", (M, H))]
+    if Lkv is not None:
+        bf.append(("kv", (B * Lkv, 2 * H)))
+    n_lse = B * heads * Lq
+    # lse padded up to 4 floats so that the float2 statistics behind it stay 8-byte aligned for odd B * heads * Lq
+    return bf, [("lse", (1, n_lse)), (None, (-n_lse % 4,)), ("stats1", (M, 2)), ("stats2", (M, 2))]
+
+
+def scratch_layout(M, H, I):
+    """The bf16 backward scratch of one layer of M rows."""
+    return [("dz2", (M, H)), ("dt2", (M, H)), ("du", (M, I)), ("dy1", (M, H)), ("dz1", (M, H)), ("dt1", (M, H)), ("dctx", (M, H)),
+            ("dqkv", (M, 3 * H)), ("dx", (M, H))]
+
+
+def grad_layout(H, I):
+    """One layer's fp32 gradient arena: the parameter gradients, q / k / v stacked in wqkv and bqkv."""
+    return [("wqkv", (3 * H, H)), ("bqkv", (3 * H,)), ("wo", (H, H)), ("bo", (H,)), ("ln1_g", (H,)), ("ln1_b", (H,)), ("w1", (I, H)),
+            ("b1", (I,)), ("w2", (H, I)), ("b2", (H,)), ("ln2_g", (H,)), ("ln2_b", (H,))]
+
+
 def _layer_sizes(H, I):
-    # fp32 gradient arena layout of one layer, order == _lib.GRAD_FIELDS
-    return [3 * H * H, 3 * H, H * H, H, H, H, I * H, I, H * I, H, H, H]
+    """Element counts of grad_layout's fields, in its order."""
+    return [math.prod(shape) for _, shape in grad_layout(H, I)]
+
+
+def layout_numel(layout):
+    return sum(math.prod(shape) for _, shape in layout)
+
+
+def carve(flat, layout, struct=None):
+    """{field: view} of the 1-D tensor flat cut by layout; when struct is given, each field of it is set to its view's pointer."""
+    views, off = {}, 0
+    for name, shape in layout:
+        n = math.prod(shape)
+        if name is not None:
+            views[name] = flat[off:off + n].view(shape)
+            if struct is not None:
+                setattr(struct, name, views[name].data_ptr())
+        off += n
+    return views
 
 
 def _grad_views(arena, H, I):
-    """Views of one layer's fp32 (or converted) arena in the order of WEIGHT_FIELDS."""
-    sizes = _layer_sizes(H, I)
-    offs = [0]
-    for s in sizes:
-        offs.append(offs[-1] + s)
-    seg = {n: arena[offs[i]:offs[i + 1]] for i, n in enumerate(L.GRAD_FIELDS)}
-    wqkv, bqkv = seg["wqkv"].view(3, H, H), seg["bqkv"].view(3, H)
-    return [wqkv[0], wqkv[1], wqkv[2], bqkv[0], bqkv[1], bqkv[2], seg["wo"].view(H, H), seg["bo"], seg["ln1_g"], seg["ln1_b"],
-            seg["w1"].view(I, H), seg["b1"], seg["w2"].view(H, I), seg["b2"], seg["ln2_g"], seg["ln2_b"]]
+    """Views of one layer's fp32 (or converted) arena in the order of WEIGHT_FIELDS (wqkv and bqkv split into q, k, v)."""
+    g = carve(arena, grad_layout(H, I))
+    return [*g["wqkv"].view(3, H, H), *g["bqkv"].view(3, H)] + [g[n] for n in L.WEIGHT_FIELDS[6:]]
 
 
 class _Acts:
-    """Per-layer activation buffers (one bf16 + one fp32 allocation for the whole stack)."""
+    """Per-layer activation buffers (one bf16 + one fp32 allocation for the whole stack, each layer's row cut by act_layout)."""
 
     def __init__(self, n_layers, B, Lq, H, heads, I, device, Lkv=None, drop_bits=False):
-        M = B * Lq
-        self.bf_sizes = [("qkv", M * 3 * H), ("ctx", M * H), ("t1", M * H), ("y1", M * H), ("u", M * I), ("hmid", M * I), ("t2", M * H),
-                         ("y", M * H)]
-        if Lkv is not None:
-            self.bf_sizes.append(("kv", B * Lkv * 2 * H))
-        # lse rounded up to 4 floats so that the float2 statistics behind it stay 8-byte aligned for odd B * heads * Lq
-        self.f_sizes = [("lse", (B * heads * Lq + 3) // 4 * 4), ("stats1", 2 * M), ("stats2", 2 * M)]
-        per_bf = sum(s for _, s in self.bf_sizes)
-        per_f = sum(s for _, s in self.f_sizes)
-        self.bf = torch.empty(n_layers, per_bf, device=device, dtype=BF16)
-        self.f32 = torch.empty(n_layers, per_f, device=device, dtype=torch.float32)
+        bf, f32 = act_layout(B, Lq, H, heads, I, Lkv)
+        self.bf = torch.empty(n_layers, layout_numel(bf), device=device, dtype=BF16)
+        self.f32 = torch.empty(n_layers, layout_numel(f32), device=device, dtype=torch.float32)
         self.structs = (L.VlpkLayerActs * n_layers)()
         # training with dropout: 1 bit per attention probability (key_slots(Lq) per query row: the training path has Lkv = Lq),
         # written by the forward attention kernel and re-read by the backward one instead of re-evaluating Philox
         self.bits = torch.empty(n_layers, B * heads * Lq * key_slots(Lq) // 8, device=device, dtype=torch.uint8) if drop_bits else None
-        self.y = []
-        for i in range(n_layers):
-            st = self.structs[i]
-            off = 0
-            base = self.bf[i]
-            for name, sz in self.bf_sizes:
-                setattr(st, name, base[off:off + sz].data_ptr())
-                if name == "y":
-                    self.y.append(base[off:off + sz].view(B, Lq, H))
-                off += sz
-            if Lkv is None:
-                st.kv = None
-            st.drop_attn = None
-            if self.bits is not None:
-                st.drop_attn = self.bits[i].data_ptr()
-            off = 0
-            basef = self.f32[i]
-            for name, sz in self.f_sizes:
-                setattr(st, name, basef[off:off + sz].data_ptr())
-                off += sz
+        self._views = [{**carve(self.bf[i], bf, self.structs[i]), **carve(self.f32[i], f32, self.structs[i])} for i in range(n_layers)]
+        if self.bits is not None:
+            for i in range(n_layers):
+                self.structs[i].drop_attn = self.bits[i].data_ptr()
+        self.y = [v["y"].view(B, Lq, H) for v in self._views]
+
+    def view(self, i, name):
+        """Layer i's buffer `name`, shaped as act_layout states it."""
+        return self._views[i][name]
 
 
 def _weight_structs(params, n_layers):
@@ -230,30 +250,22 @@ class EncoderStackFn(torch.autograd.Function):
                                "(retain_graph=True) is not supported")
         x, acts = ctx.x, ctx.acts
         B, Lq, H = x.shape
-        M = B * Lq
         dev = x.device
         if dys[-1] is None:
             dys = list(dys)
             dys[-1] = torch.zeros_like(x)
         dyc = [None if d is None else _bf16c(d) for d in dys]
         dy_ptrs = (C.c_void_p * n_layers)(*[None if d is None else d.data_ptr() for d in dyc])
-        per_layer = sum(_layer_sizes(H, I))
+        grads_l = grad_layout(H, I)
+        per_layer = layout_numel(grads_l)
         arena = torch.zeros(n_layers, per_layer, device=dev, dtype=torch.float32)
         gs = (L.VlpkLayerGrads * n_layers)()
-        sizes = _layer_sizes(H, I)
         for i in range(n_layers):
-            off = 0
-            for name, sz in zip(L.GRAD_FIELDS, sizes):
-                setattr(gs[i], name, arena[i, off:off + sz].data_ptr())
-                off += sz
-        scr_sizes = {"dz2": M * H, "dt2": M * H, "du": M * I, "dy1": M * H, "dz1": M * H, "dt1": M * H, "dctx": M * H, "dqkv": 3 * M * H,
-                     "dx": M * H}
-        scratch = torch.empty(sum(scr_sizes.values()), device=dev, dtype=BF16)
+            carve(arena[i], grads_l, gs[i])
+        scratch_l = scratch_layout(B * Lq, H, I)
+        scratch = torch.empty(layout_numel(scratch_l), device=dev, dtype=BF16)
         ws_s = L.VlpkBwdScratch()
-        off = 0
-        for name in L.SCRATCH_FIELDS:
-            setattr(ws_s, name, scratch[off:off + scr_sizes[name]].data_ptr())
-            off += scr_sizes[name]
+        carve(scratch, scratch_l, ws_s)
         dx0 = torch.empty_like(x)
         shape = L.VlpkShape(B, Lq, Lq, H, heads, I, kv_slots(Lq, Lq))
         ws = _weight_structs(ctx.pk, n_layers)
@@ -374,13 +386,13 @@ def attn_probs(q, k, lse, mask_bits, row0=0, out=None):
 
 def _acts_maps(acts, i, B, Lq, H, heads, mask_bits, row0=0, out=None, k=None):
     """attn_probs of layer i of an _Acts: q in place in its qkv buffer (ld 3H, or ld H in the decode layouts that pass k)."""
-    qkv = acts.bf[i][:B * Lq * 3 * H]
-    lse = acts.f32[i][:B * heads * Lq].view(B, heads, Lq)
+    qkv = acts.view(i, "qkv")
+    lse = acts.view(i, "lse").view(B, heads, Lq)
     if k is None:
         v = qkv.view(B, Lq, 3 * H)
         q, k = v[..., :H], v[..., H:2 * H]
     else:
-        q = qkv[:B * Lq * H].view(B, Lq, H)
+        q = qkv.view(3, B, Lq, H)[0]
     return attn_probs(q, k, lse, mask_bits, row0, out)
 
 
@@ -402,18 +414,8 @@ def layer_incremental_fwd(hidden, history, mask_bits, heads, I, params, maps=Non
            None, 0, L.stream())
     if maps is None:
         return acts.y[0]
-    k = _acts_region(acts, 0, "kv").view(B, Lkv, 2 * H)[..., :H]
+    k = acts.view(0, "kv").view(B, Lkv, 2 * H)[..., :H]
     return acts.y[0], _acts_maps(acts, 0, B, Lq, H, heads, mask_bits, maps[0], maps[1], k=k)
-
-
-def _acts_region(acts, i, name):
-    """Layer i's flat bf16 buffer `name` of an _Acts."""
-    off = 0
-    for n, sz in acts.bf_sizes:
-        if n == name:
-            return acts.bf[i][off:off + sz]
-        off += sz
-    raise KeyError(name)
 
 
 # ------------------------------------------------------------------------------------------------
