@@ -433,6 +433,26 @@ int vlpk_sample_tokens(int rows, int V, const void* logits, int64_t ld, const vo
                        uint64_t seed, int f, int64_t* seq, int T_cap, float* score, int32_t* finished, int32_t* live, int eos_id, int pad_id,
                        int block_eos, int n, const int32_t* ignore, int n_ignore, void* stream);
 
+/* Diverse beam search (Vijayakumar et al., AAAI 2018): the selection of frame f (0 <= f < T_cap) for B images of K beams in G groups
+ * of Kg = K / G, with a Hamming penalty, one call per frame (two launches), no host synchronisation.  Rows are b (f = 0) or b*K + k.
+ *   logp[i, w]  x = logits[i*ld + w] + bias[w], rounded to the logits' dtype (fp32 = 0: bf16, 1: fp32; bias may be NULL);
+ *     logp = x - logsumexp(x) in fp32; then, as beam search does, -10000 is added at the words the duplicate-n-gram rule of
+ *     vlpk_beam_ngram_block blocks (n > 0, f >= n; the history carry hist_out[i] = hist_in[b*K + prev_ptr[i]] ‖ prev_wid[i] runs at
+ *     every f >= 1 with n > 0), and logp[eos_id] = -10000 if block_eos.
+ *   cand(i, w)  logp at f = 0; logp + prev_eos[i] * -10000 + prev_score[i] after (frame f-1's traces, [B, K]).
+ *   groups      g = 0 .. G-1 in turn: group g's parents are beams [g*Kg, (g+1)*Kg) (row b at f = 0); it keeps the Kg (parent, word)
+ *     pairs with the largest cand - diversity_penalty * cnt(w), cnt(w) = beams of groups < g that chose w in this frame; ties go
+ *     to the lower parent, then the lower word.  Its r-th pair becomes beam g*Kg + r.
+ *   traces      wid / ptr int64 [B, K] (ptr a beam index in [0, K), 0 at f = 0), score fp32 [B, K] the unpenalised cand, eos fp32
+ *     [B, K] (wid == eos_id).  top_w int32 / top_lp fp32 [rows, K] are scratch (each row's top K words).
+ * Bitwise reproducible.  Returns < 0 without launching for K outside [1, 64], G not dividing K, V < K, ld < V, a penalty that is
+ * negative or not finite, f outside [0, T_cap), fp32 not 0 / 1, a NULL pointer that is needed, hist_in == hist_out, or
+ * (V + V/32 + T_cap) * 4 bytes above 200 KB of shared memory. */
+int vlpk_diverse_beam_step(int B, int K, int G, int f, int V, const void* logits, int64_t ld, const void* bias, int fp32, float diversity_penalty,
+                           int eos_id, int block_eos, int T_cap, int n, const int32_t* hist_in, int32_t* hist_out, const int32_t* ignore,
+                           int n_ignore, const int64_t* prev_wid, const int64_t* prev_ptr, const float* prev_score, const float* prev_eos,
+                           int32_t* top_w, float* top_lp, int64_t* wid, int64_t* ptr, float* score, float* eos, void* stream);
+
 /* utilities */
 int vlpk_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 int vlpk_colsum(const void* x, int64_t ld, int64_t M, int N, float* out, void* stream);

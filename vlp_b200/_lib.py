@@ -132,6 +132,8 @@ _SIGS = {
     "vlpk_beam_ngram_block": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_int, _P, c_i64, c_int, _P]),
     "vlpk_sample_tokens": (c_int, [c_int, c_int, _P, c_i64, _P, c_int, c_int, c_int, c_float, c_u64, c_int, _P, c_int, _P, _P, _P, c_int,
                                    c_int, c_int, c_int, _P, c_int, _P]),
+    "vlpk_diverse_beam_step": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, c_i64, _P, c_int, c_float, c_int, c_int, c_int, c_int, _P,
+                                       _P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "vlpk_f32_to_bf16": (c_int, [_P, _P, c_i64, _P]),
     "vlpk_colsum": (c_int, [_P, c_i64, c_i64, c_int, _P, _P]),
     "vlpk_debug_dropout_mask": (c_int, [C.POINTER(VlpkDropout), c_u64, c_i64, _P, _P]),

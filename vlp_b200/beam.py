@@ -8,6 +8,7 @@ best-hypothesis selection + back-tracking (:1431-1472) as vectorised tensor ops,
 device: no host synchronisation inside or after the loop, so a blocked decode can be captured as a CUDA graph too.
 Per-sample `task_idx` (the relaxed MLM head, relax_projection > 1) is expanded to the B*K beam rows with the other inputs; the
 reference does not expand it (:1297 vs :1325-1373), so its relaxed beam search only runs at B = 1.
+Diverse beam search (num_beam_groups > 1, diverse_beam_search) runs the same data flow and trace format with its own per-frame selection.
 Every step runs the fused layers on the two new rows (token, [MASK]) through decode.DecodeState, which also expands the history to the
 beams after the first step and reorders it by the back pointers after every later one.
 """
@@ -97,6 +98,79 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
     if N > 1:
         out["nbest_seq"], out["nbest_scores"] = nbest(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len, N)
     return out
+
+
+def diverse_beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None,
+                        output_attentions=False):
+    """Diverse beam search (Vijayakumar et al., AAAI 2018): the K = dec.search_beam_size beams of an image in G = dec.num_beam_groups
+    groups of Kg = K / G.  Every frame, the groups choose in turn; group g extends its own beams and ranks each (parent, word) by its
+    beam score minus dec.diversity_penalty times the number of beams of groups < g that chose the word in this frame.  The traces keep
+    the unpenalised scores, so the final selection compares the groups on model log-probabilities.  One vlpk_diverse_beam_step per
+    frame reads the head's logits (decoder output without the bias) once and writes the frame's traces in place, the n-gram blocking
+    and the min_len [EOS] block included; nothing synchronises with the host.
+
+    Output: beam_search's dict (pred_seq, scores, wids, ptrs; attentions, nbest_seq / nbest_scores as there), plus group_seq int64
+    [B, G, out_len] and group_scores fp32 [B, G]: the final-selection rule applied to each group's Kg beams alone."""
+    K, G = dec.search_beam_size, dec.num_beam_groups
+    B, in_len = input_ids.shape
+    out_len = token_type_ids.shape[1]
+    T = out_len - in_len
+    dev = input_ids.device
+    N = dec.num_return_sequences
+    state = DecodeState(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, K if N > 1 else None)
+    ngram = int(dec.ngram_size) if dec.forbid_duplicate_ngrams else 0
+    ignore = _ignore_tensor(dec, dev) if ngram else None
+    hist = [torch.empty(B * K, T, dtype=torch.int32, device=dev) for _ in range(2)] if ngram else [None, None]
+    sc, eos = (torch.zeros(T, B, K, dtype=torch.float32, device=dev) for _ in range(2))
+    wi, pt = (torch.zeros(T, B, K, dtype=torch.int64, device=dev) for _ in range(2))
+    top_w = torch.empty(B * K, K, dtype=torch.int32, device=dev)
+    top_lp = torch.empty(B * K, K, dtype=torch.float32, device=dev)
+    pred = dec.cls.predictions
+    maps = new_attention_maps(dec, T, B * K, out_len, dev) if output_attentions else None
+    rows = torch.arange(B, device=dev).unsqueeze(1) * K
+    curr_ids = input_ids
+    for frame in range(T):
+        buf = None
+        if maps is not None:
+            buf = maps[frame] if frame else maps[0].view(B, K, *maps.shape[2:])[:, 0]
+        h = pred.select_task(pred.transform(state.step(curr_ids, buf).to(pred.decoder.weight.dtype)), task_idx)
+        logits = pred.decoder(h)                                          # [B or B*K, 1, V]; the kernel adds the bias
+        ops.diverse_beam_step(logits, pred.bias.to(logits.dtype), frame, G, dec.diversity_penalty, wi, pt, sc, eos, top_w, top_lp,
+                              dec.eos_id, block_eos=bool(dec.min_len) and frame + 1 <= dec.min_len, ngram=ngram, ignore=ignore,
+                              hist_in=hist[(frame - 1) % 2], hist_out=hist[frame % 2])
+        if frame == 0:
+            state.expand(K)
+            task_idx = expand_task_idx(task_idx, B, K)
+        else:
+            state.reorder((pt[frame] + rows).reshape(-1))
+        curr_ids = wi[frame].reshape(B * K, 1)
+
+    out = {"pred_seq": backtrack(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len)}
+    if maps is not None:
+        out["attentions"] = beam_maps(maps, *best_path(sc, wi, pt, dec.eos_id, dec.length_penalty), pt)
+    for k, t in (("scores", sc), ("wids", wi), ("ptrs", pt)):
+        padded = t.new_zeros((B, out_len, K))
+        padded[:, :T] = t.permute(1, 0, 2)
+        out[k] = padded
+    if N > 1:
+        out["nbest_seq"], out["nbest_scores"] = nbest(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len, N)
+    out["group_seq"], out["group_scores"] = group_best(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len, G)
+    return out
+
+
+def group_best(sc, wi, pt, eos_id, length_penalty, out_len, G):
+    """Each group's best hypothesis under the final-selection rule over its own Kg = K / G beams (a diverse beam search's parents
+    stay in their group): (group_seq int64 [B, G, out_len] zero padded, group_scores [B, G] — the rule's values)."""
+    T, B, K = sc.shape
+    Kg = K // G
+    seqs, vals = [], []
+    for g in range(G):
+        beams = slice(g * Kg, (g + 1) * Kg)
+        sg, wg = sc[:, :, beams], wi[:, :, beams]
+        pg = pt[:, :, beams] % Kg                                         # the parent's place in the group: ptr - g*Kg (0 at frame 0)
+        seqs.append(backtrack(sg, wg, pg, eos_id, length_penalty, out_len))
+        vals.append(candidate_values(sg, wg, eos_id, length_penalty).max(1).values)
+    return torch.stack(seqs, 1), torch.stack(vals, 1)
 
 
 def backtrack(sc, wi, pt, eos_id, length_penalty, out_len):

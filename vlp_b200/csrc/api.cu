@@ -1000,6 +1000,22 @@ int vlpk_sample_tokens(int rows, int V, const void* logits, int64_t ld, const vo
   return launch_sample(a, S(stream));
 }
 
+int vlpk_diverse_beam_step(int B, int K, int G, int f, int V, const void* logits, int64_t ld, const void* bias, int fp32, float diversity_penalty,
+                           int eos_id, int block_eos, int T_cap, int n, const int32_t* hist_in, int32_t* hist_out, const int32_t* ignore,
+                           int n_ignore, const int64_t* prev_wid, const int64_t* prev_ptr, const float* prev_score, const float* prev_eos,
+                           int32_t* top_w, float* top_lp, int64_t* wid, int64_t* ptr, float* score, float* eos, void* stream) {
+  DiverseBeamArgs a;
+  a.B = B; a.K = K; a.G = G; a.f = f; a.V = V;
+  a.logits = logits; a.ld = ld; a.bias = bias; a.fp32 = fp32;
+  a.lambda = diversity_penalty; a.eos_id = eos_id; a.block_eos = block_eos;
+  a.T_cap = T_cap; a.n = n; a.hist_in = hist_in; a.hist_out = hist_out; a.ignore = ignore; a.n_ignore = n_ignore;
+  a.prev_wid = reinterpret_cast<const long long*>(prev_wid); a.prev_ptr = reinterpret_cast<const long long*>(prev_ptr);
+  a.prev_score = prev_score; a.prev_eos = prev_eos;
+  a.top_w = top_w; a.top_lp = top_lp;
+  a.wid = reinterpret_cast<long long*>(wid); a.ptr = reinterpret_cast<long long*>(ptr); a.score = score; a.eos = eos;
+  return launch_diverse_beam_step(a, S(stream));
+}
+
 int vlpk_colsum(const void* x, int64_t ld, int64_t M, int N, float* out, void* stream) {
   VLPK_CHECK_ARG(x && out, "colsum: null pointer");
   return launch_colsum(x, ld, M, N, out, S(stream));

@@ -304,6 +304,188 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Diverse beam search (Vijayakumar et al., AAAI 2018) of one frame f: K beams per image in G groups of Kg = K / G, with a Hamming
+// diversity penalty lambda.  Two launches.
+//
+// diverse_beam_rows_kernel, one CTA of SAMPLE_THREADS per row (B rows at f = 0, B*K after):
+//   history  at f >= 1 with n > 0, hist_out[i] = hist_in[b*K + prev_ptr[i]] ‖ prev_wid[i], exactly as beam_ngram_block_kernel.
+//   logp     x[v] = head_logit(row, bias, v); logp[v] = (x[v] - max x) - log(sum exp(x - max x)) in fp32; then -10000 is added at
+//            the words the duplicate-n-gram rule blocks (f >= n), and logp[eos] = -10000 while block_eos: beam search's order and
+//            values.
+//   top K    the K words ranked first by (logp descending, word ascending), found as a threshold on order_key(logp) by binary
+//            search over the key's bits plus a scan of the ties in index order (no sort), written in rank order to
+//            top_w / top_lp [row, 0:K].
+// diverse_beam_merge_kernel, one CTA per image: groups choose in order g = 0 .. G-1.  Group g's candidates are its parents'
+//   (beams [g*Kg, (g+1)*Kg); row b at f = 0) row top K with cand = logp + eos_prev * -10000 + score_prev (cand = logp at f = 0);
+//   it keeps the Kg with the largest cand - lambda * cnt(w), cnt(w) = beams of groups < g that chose w in this frame, ties to the
+//   lower parent then the lower word, in rank order as beams g*Kg ..  The traces get the unpenalised cand.
+// Group g penalises at most g*Kg <= K - Kg words, so any (row, word) outside the row's top K has at least Kg unpenalised words of
+// the same row ranked strictly ahead of it: the row top K hold every pair a group can keep.  Every sum runs in a fixed order
+// (chunk, then a fixed shuffle tree) and the merge only compares, so a frame is bitwise reproducible.
+constexpr int MERGE_THREADS = 256;
+constexpr int DIVERSE_MAX_CAND = DIVERSE_MAX_BEAMS * DIVERSE_MAX_BEAMS;       // Kg * K <= K * K candidates per group
+
+template <typename T>
+__global__ void __launch_bounds__(SAMPLE_THREADS) diverse_beam_rows_kernel(DiverseBeamArgs a) {
+  extern __shared__ float rows_smem[];
+  __shared__ float redf[33];
+  __shared__ int redi[33], prei[SAMPLE_THREADS + 1];
+  __shared__ int sel_w[DIVERSE_MAX_BEAMS];
+  __shared__ float sel_lp[DIVERSE_MAX_BEAMS];
+  const int V = a.V, K = a.K, tid = threadIdx.x, row = blockIdx.x;
+  float* val = rows_smem;                                            // [V] logp
+  unsigned* bits = reinterpret_cast<unsigned*>(val + V);             // [ceil(V/32)] blocked words
+  int* hist = reinterpret_cast<int*>(bits + ((V + 31) >> 5));        // [T_cap] history
+
+  bool blocked = false;
+  if (a.n > 0 && a.f >= 1) {                                         // uniform
+    const int f = a.f;
+    const long long p = f > 1 ? a.prev_ptr[row] : 0;
+    const bool parent_ok = p >= 0 && p < K;
+    const int* src = a.hist_in + (static_cast<size_t>(row / K) * K + (parent_ok ? p : 0)) * a.T_cap;
+    int* dst = a.hist_out + static_cast<size_t>(row) * a.T_cap;
+    for (int t = tid; t < f - 1; t += SAMPLE_THREADS) {
+      const int w = parent_ok ? src[t] : -1;
+      hist[t] = w;
+      dst[t] = w;
+    }
+    if (tid == 0) {
+      const long long w64 = a.prev_wid[row];
+      const int w = (w64 >= INT_MIN && w64 <= INT_MAX) ? static_cast<int>(w64) : -1;
+      hist[f - 1] = w;
+      dst[f - 1] = w;
+    }
+    if (f >= a.n) blocked = ngram_candidates(hist, f, a.n, V, a.ignore, a.n_ignore, bits);
+  }
+
+  const T* lrow = static_cast<const T*>(a.logits) + static_cast<size_t>(row) * a.ld;
+  const T* bias = static_cast<const T*>(a.bias);
+  float mx = -INFINITY;
+  for (int v = tid; v < V; v += SAMPLE_THREADS) {
+    const float x = head_logit(lrow, bias, v);
+    val[v] = x;
+    mx = fmaxf(mx, x);
+  }
+  mx = block_reduce(mx, redf, [](float p, float q) { return fmaxf(p, q); });
+
+  // from here on thread t owns words [lo, hi)
+  const int C = ((V + SAMPLE_THREADS - 1) / SAMPLE_THREADS) | 1;
+  const int lo = min(tid * C, V), hi = min(lo + C, V);
+  float z = 0.f;
+  for (int v = lo; v < hi; ++v) z += expf(val[v] - mx);
+  const float lse = logf(block_reduce(z, redf, [](float p, float q) { return p + q; }));
+  float top = -INFINITY;
+  for (int v = lo; v < hi; ++v) {
+    float lp = (val[v] - mx) - lse;
+    if (blocked && ((bits[v >> 5] >> (v & 31)) & 1u)) lp += -10000.0f;
+    if (a.block_eos && v == a.eos_id) lp = -10000.0f;
+    val[v] = lp;
+    top = fmaxf(top, lp);
+  }
+  top = block_reduce(top, redf, [](float p, float q) { return fmaxf(p, q); });
+
+  // tau = the largest key with at least K words at or above it
+  auto count = [&](unsigned t) {
+    int c = 0;
+    for (int v = lo; v < hi; ++v) c += order_key(val[v]) >= t;
+    return block_reduce(c, redi, [](int p, int q) { return p + q; });
+  };
+  unsigned klo = 0, khi = order_key(top);
+  if (count(khi) >= K) {
+    klo = khi;
+  } else {
+    khi -= 1;
+    while (klo < khi) {                                              // uniform: every thread sees the same counts
+      const unsigned mid = klo + (khi - klo + 1) / 2;
+      if (count(mid) >= K) klo = mid; else khi = mid - 1;
+    }
+  }
+  const unsigned tau = klo;
+  const int take = K - (tau == 0xffffffffu ? 0 : count(tau + 1));   // words tied at tau to keep, lowest index first
+
+  int ties = 0;
+  for (int v = lo; v < hi; ++v) ties += order_key(val[v]) == tau;
+  block_exclusive_scan(ties, redi, prei);
+  const int ties_before = prei[tid];
+  int rank = ties_before, kept = 0;
+  for (int v = lo; v < hi; ++v) {
+    const unsigned k = order_key(val[v]);
+    kept += k > tau || (k == tau && rank++ < take);
+  }
+  block_exclusive_scan(kept, redi, prei);                            // the chunk's first slot among the K kept words
+  int slot = prei[tid];
+  rank = ties_before;
+  for (int v = lo; v < hi; ++v) {
+    const unsigned k = order_key(val[v]);
+    if (k > tau || (k == tau && rank++ < take)) {
+      sel_w[slot] = v;
+      sel_lp[slot] = val[v];
+      ++slot;
+    }
+  }
+  __syncthreads();
+  if (tid < K) {                                                     // rank order: (logp descending, word ascending)
+    const float lp = sel_lp[tid];
+    const unsigned kt = order_key(lp);
+    const int w = sel_w[tid];
+    int r = 0;
+    for (int j = 0; j < K; ++j) {
+      const unsigned kj = order_key(sel_lp[j]);
+      r += kj > kt || (kj == kt && sel_w[j] < w);
+    }
+    a.top_w[static_cast<size_t>(row) * K + r] = w;
+    a.top_lp[static_cast<size_t>(row) * K + r] = lp;
+  }
+}
+
+__global__ void __launch_bounds__(MERGE_THREADS) diverse_beam_merge_kernel(DiverseBeamArgs a) {
+  __shared__ float pen[DIVERSE_MAX_CAND];
+  __shared__ int word[DIVERSE_MAX_CAND];
+  __shared__ int chosen[DIVERSE_MAX_BEAMS];                          // words of the beams chosen so far in this frame
+  const int b = blockIdx.x, K = a.K, Kg = a.K / a.G, tid = threadIdx.x;
+  const bool first = a.f == 0;
+  const int nc = first ? K : Kg * K;                                 // one group's candidates: its parents' row top K
+  const size_t base = static_cast<size_t>(b) * K;
+  // candidate c of group g: parent beam g*Kg + c / K (the image's row at f = 0), the (c % K)-th word of the parent's row top K
+  auto parent = [&](int g, int c) { return first ? 0 : g * Kg + c / K; };
+  auto slot = [&](int g, int c) { return (first ? static_cast<size_t>(b) : base + parent(g, c)) * K + c % K; };
+  auto cand = [&](int g, int c) {
+    const float lp = a.top_lp[slot(g, c)];
+    const size_t p = base + parent(g, c);
+    return first ? lp : lp + a.prev_eos[p] * -10000.0f + a.prev_score[p];
+  };
+  for (int g = 0; g < a.G; ++g) {
+    for (int c = tid; c < nc; c += MERGE_THREADS) {
+      const int w = a.top_w[slot(g, c)];
+      int cnt = 0;
+      for (int q = 0; q < g * Kg; ++q) cnt += chosen[q] == w;
+      pen[c] = __fsub_rn(cand(g, c), __fmul_rn(a.lambda, static_cast<float>(cnt)));
+      word[c] = w;
+    }
+    __syncthreads();
+    for (int c = tid; c < nc; c += MERGE_THREADS) {
+      const float v = pen[c];
+      const int w = word[c], pc = c / K;
+      int r = 0;                                                     // candidates ranked ahead of c; only r < Kg matters
+      for (int d = 0; d < nc && r < Kg; ++d) {
+        const float u = pen[d];
+        const int pd = d / K;
+        r += u > v || (u == v && (pd < pc || (pd == pc && word[d] < w)));
+      }
+      if (r < Kg) {
+        const int k = g * Kg + r;
+        chosen[k] = w;
+        a.wid[base + k] = w;
+        a.ptr[base + k] = parent(g, c);
+        a.score[base + k] = cand(g, c);                              // unpenalised
+        a.eos[base + k] = w == a.eos_id ? 1.0f : 0.0f;
+      }
+    }
+    __syncthreads();
+  }
+}
+
 }  // namespace
 
 size_t sample_smem_bytes(int T_cap, int V) {
@@ -340,6 +522,58 @@ int launch_sample(const SampleArgs& a, cudaStream_t s) {
     }
     sample_kernel<bf16><<<a.rows, SAMPLE_THREADS, smem, s>>>(a);
   }
+  VLPK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int launch_diverse_beam_step(const DiverseBeamArgs& a, cudaStream_t s) {
+  VLPK_CHECK_ARG(a.B >= 0 && a.K >= 1 && a.K <= DIVERSE_MAX_BEAMS, "diverse_beam_step: B=%d K=%d (K must lie in [1, %d])", a.B, a.K,
+                 DIVERSE_MAX_BEAMS);
+  VLPK_CHECK_ARG(a.G >= 1 && a.K % a.G == 0, "diverse_beam_step: G=%d groups do not divide K=%d beams", a.G, a.K);
+  VLPK_CHECK_ARG(a.V >= a.K && a.ld >= a.V, "diverse_beam_step: V=%d ld=%lld K=%d (ld >= V >= K needed)", a.V, a.ld, a.K);
+  VLPK_CHECK_ARG(a.fp32 == 0 || a.fp32 == 1, "diverse_beam_step: fp32=%d (0 bf16, 1 fp32)", a.fp32);
+  VLPK_CHECK_ARG(isfinite(a.lambda) && a.lambda >= 0.f, "diverse_beam_step: diversity penalty %g (finite and >= 0 needed)",
+                 static_cast<double>(a.lambda));
+  VLPK_CHECK_ARG(a.T_cap >= 1 && a.f >= 0 && a.f < a.T_cap, "diverse_beam_step: frame f=%d outside [0, T_cap=%d)", a.f, a.T_cap);
+  VLPK_CHECK_ARG(a.n >= 0 && a.n_ignore >= 0 && (a.n_ignore == 0 || a.ignore), "diverse_beam_step: n=%d, ignore set of %d words", a.n,
+                 a.n_ignore);
+  VLPK_CHECK_ARG(a.logits && a.top_w && a.top_lp && a.wid && a.ptr && a.score && a.eos,
+                 "diverse_beam_step: null pointer (logits, top_w, top_lp, wid, ptr, score, eos)");
+  VLPK_CHECK_ARG(a.f == 0 || (a.prev_score && a.prev_eos), "diverse_beam_step: null pointer (prev_score, prev_eos are needed at f=%d)",
+                 a.f);
+  const bool hist = a.n > 0 && a.f >= 1;
+  VLPK_CHECK_ARG(!hist || (a.hist_out && a.prev_wid), "diverse_beam_step: null pointer (hist_out, prev_wid are needed at f=%d)", a.f);
+  VLPK_CHECK_ARG(!hist || a.f == 1 || (a.hist_in && a.prev_ptr), "diverse_beam_step: null pointer (hist_in, prev_ptr are needed at f=%d)",
+                 a.f);
+  VLPK_CHECK_ARG(!hist || a.hist_in != a.hist_out, "diverse_beam_step: hist_in and hist_out must be different buffers");
+  const size_t smem = sample_smem_bytes(a.T_cap, a.V);
+  VLPK_CHECK_ARG(smem <= SAMPLE_SMEM_MAX, "diverse_beam_step: T_cap=%d V=%d need %zu bytes of shared memory (at most %zu)", a.T_cap, a.V,
+                 smem, SAMPLE_SMEM_MAX);
+  if (a.B == 0) return 0;
+  const int rows = a.f == 0 ? a.B : a.B * a.K;
+  {
+    LaunchScope scope(CAT_MISC, (a.fp32 ? 8.0 : 4.0) * rows * a.V, s);
+    if (a.fp32) {
+      static bool attr_set = false;
+      if (!attr_set) {
+        VLPK_CUDA(cudaFuncSetAttribute(diverse_beam_rows_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       static_cast<int>(SAMPLE_SMEM_MAX)));
+        attr_set = true;
+      }
+      diverse_beam_rows_kernel<float><<<rows, SAMPLE_THREADS, smem, s>>>(a);
+    } else {
+      static bool attr_set = false;
+      if (!attr_set) {
+        VLPK_CUDA(cudaFuncSetAttribute(diverse_beam_rows_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       static_cast<int>(SAMPLE_SMEM_MAX)));
+        attr_set = true;
+      }
+      diverse_beam_rows_kernel<bf16><<<rows, SAMPLE_THREADS, smem, s>>>(a);
+    }
+    VLPK_CUDA(cudaGetLastError());
+  }
+  LaunchScope scope(CAT_MISC, 8.0 * rows * a.K, s);
+  diverse_beam_merge_kernel<<<a.B, MERGE_THREADS, 0, s>>>(a);
   VLPK_CUDA(cudaGetLastError());
   return 0;
 }

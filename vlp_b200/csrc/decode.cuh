@@ -53,4 +53,38 @@ struct SampleArgs {
 size_t sample_smem_bytes(int T_cap, int V);
 int launch_sample(const SampleArgs& a, cudaStream_t s);
 
+// Diverse beam search: one frame's selection, K beams per image in G groups with a Hamming penalty (see decode.cu).
+constexpr int DIVERSE_MAX_BEAMS = SAMPLE_MAX_TOPK;
+
+struct DiverseBeamArgs {
+  int B = 0, K = 1, G = 1;            // images, beams per image, groups (G divides K; Kg = K / G)
+  int f = 0;                          // frame: rows = B at f = 0 (one per image), B*K after (row b*K + k)
+  int V = 0;
+  const void* logits = nullptr;       // [rows, ld] bf16 or fp32 decoder outputs, without the bias
+  long long ld = 0;
+  const void* bias = nullptr;         // [V] same dtype, or null
+  int fp32 = 0;                       // dtype of logits and bias: 0 bf16, 1 fp32
+  float lambda = 0.f;                 // diversity penalty per earlier-group use of a word, >= 0
+  int eos_id = -1;
+  int block_eos = 0;                  // 1: frame below min_len, logp[eos] = -10000
+  int T_cap = 0;                      // words per history row; frames f < T_cap
+  int n = 0;                          // duplicate-n-gram blocking: n-gram size, 0 = off
+  const int* hist_in = nullptr;       // [B*K, T_cap] int32 history of frame f-1 (read at f >= 2)
+  int* hist_out = nullptr;            // [B*K, T_cap] int32 history of frame f (f words; written at f >= 1)
+  const int* ignore = nullptr;
+  int n_ignore = 0;
+  const long long* prev_wid = nullptr;    // [B, K] frame f-1's traces (f >= 1)
+  const long long* prev_ptr = nullptr;
+  const float* prev_score = nullptr;
+  const float* prev_eos = nullptr;
+  int* top_w = nullptr;               // [rows, K] scratch: each row's top K words and log-probabilities
+  float* top_lp = nullptr;
+  long long* wid = nullptr;           // [B, K] frame f's traces
+  long long* ptr = nullptr;
+  float* score = nullptr;
+  float* eos = nullptr;
+};
+
+int launch_diverse_beam_step(const DiverseBeamArgs& a, cudaStream_t s);
+
 }  // namespace vlpk

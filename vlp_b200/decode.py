@@ -2,6 +2,8 @@
 shares (DecodeState), and the greedy and top-k / top-p sampling loops.  Beam search's loop is beam.beam_search; each loop owns only
 its choice of word.
 """
+import math
+
 import torch
 import torch.nn.functional as F
 
@@ -13,12 +15,13 @@ PAD_ID = 0
 
 
 def check_decode(sampling_method, topk, topp, beam_size, num_return_sequences=1, forbid_duplicate_ngrams=False, ngram_size=3,
-                 use_kv_cache=True, output_attentions=False, ngram_in_greedy=False):
+                 use_kv_cache=True, output_attentions=False, ngram_in_greedy=False, num_beam_groups=1, diversity_penalty=0.0):
     """Raises ValueError, before anything is launched, for decode settings the decoder does not take.  Greedy decode ignores the
     n-gram settings, so a bad ngram_size is refused for beam search and sampling only, or in every mode with ngram_in_greedy."""
     if sampling_method not in SAMPLING_METHODS:
         raise ValueError(f"vlp_b200: sampling_method must be one of {', '.join(SAMPLING_METHODS)}, got {sampling_method!r}")
     sampling = sampling_method != "beam_search"
+    check_beam_groups(num_beam_groups, diversity_penalty, sampling_method, beam_size)
     if sampling:
         if int(beam_size) != 1:
             raise ValueError(f"vlp_b200: sampling_method={sampling_method!r} needs beam size 1, got {beam_size}")
@@ -44,6 +47,28 @@ def check_decode(sampling_method, topk, topp, beam_size, num_return_sequences=1,
         raise ValueError("vlp_b200: num_return_sequences > 1 needs use_kv_cache (the shared image-prefix cache)")
     if output_attentions:
         raise ValueError("vlp_b200: output_attentions is not available with num_return_sequences > 1")
+
+
+def check_beam_groups(num_beam_groups, diversity_penalty, sampling_method, beam_size):
+    """The diverse beam search settings (beam.diverse_beam_search): G groups of K / G beams, a Hamming penalty lambda >= 0."""
+    G, lam = num_beam_groups, diversity_penalty
+    if isinstance(G, bool) or not isinstance(G, int) or G < 1:
+        raise ValueError(f"vlp_b200: num_beam_groups must be an integer >= 1, got {G!r}")
+    if isinstance(lam, bool) or not isinstance(lam, (int, float)) or not math.isfinite(lam) or lam < 0:
+        raise ValueError(f"vlp_b200: diversity_penalty must be a finite number >= 0, got {lam!r}")
+    if G == 1:
+        if lam > 0:
+            raise ValueError("vlp_b200: diversity_penalty > 0 needs num_beam_groups > 1 (it penalises words earlier groups chose)")
+        return
+    K = int(beam_size)
+    if sampling_method != "beam_search":
+        raise ValueError(f"vlp_b200: num_beam_groups > 1 needs beam search, got sampling_method={sampling_method!r}")
+    if K <= 1:
+        raise ValueError(f"vlp_b200: num_beam_groups={G} needs beam search (beam size > 1), got beam size {K}")
+    if K % G:
+        raise ValueError(f"vlp_b200: num_beam_groups={G} does not divide the beam size {K}")
+    if K > ops.MAX_TOPK:
+        raise ValueError(f"vlp_b200: diverse beam search takes beam sizes up to {ops.MAX_TOPK}, got {K}")
 
 
 class DecodeState:

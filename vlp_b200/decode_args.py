@@ -27,6 +27,9 @@ _OPTIONS = (
     ("--seed", dict(type=int, default=123, help="random seed (keys the sampling draws)")),
     ("--num_return_sequences", dict(type=int, default=1, help="captions per image: the N best of beam search (N <= --beam_size) or N "
                                                               "top-k / top-p samples, over one K/V cache of the image prefix")),
+    ("--num_beam_groups", dict(type=int, default=1, help="diverse beam search: split the --beam_size beams into this many groups, "
+                                                         "each penalised for words earlier groups chose in the same step")),
+    ("--diversity_penalty", dict(type=float, default=0.0, help="diverse beam search: penalty per earlier group's use of a word, >= 0")),
 )
 
 
@@ -44,7 +47,7 @@ def check_decode_args(args):
     """ValueError for a combination BertForSeq2SeqDecoder refuses (raised before any model is built); --ngram_size is checked with
     --forbid_duplicate_ngrams in every mode, greedy included."""
     check_decode(args.sampling_method, args.topk, args.topp, args.beam_size, args.num_return_sequences, args.forbid_duplicate_ngrams,
-                 args.ngram_size, ngram_in_greedy=True)
+                 args.ngram_size, ngram_in_greedy=True, num_beam_groups=args.num_beam_groups, diversity_penalty=args.diversity_penalty)
 
 
 def parse_decode_args(parser, argv=None):
@@ -71,4 +74,8 @@ def decoder_kwargs(args, tokenizer=None):
               topk=args.topk, topp=args.topp, seed=args.seed)
     if args.num_return_sequences != 1:
         kw["num_return_sequences"] = args.num_return_sequences       # the decoder's default otherwise
+    if args.num_beam_groups != 1:
+        kw["num_beam_groups"] = args.num_beam_groups
+    if args.diversity_penalty != 0:
+        kw["diversity_penalty"] = args.diversity_penalty
     return kw

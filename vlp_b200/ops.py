@@ -696,3 +696,52 @@ def sample_tokens(logits, bias, mode, topk, topp, seed, f, seq, score, finished,
            int(topk), float(topp), int(seed) & 0xFFFFFFFFFFFFFFFF, int(f), seq.data_ptr(), seq.shape[1], L.ptr(score), finished.data_ptr(),
            live.data_ptr(), int(eos_id), int(pad_id), int(bool(block_eos)), int(ngram), ignore.data_ptr() if n_ign else None, n_ign,
            L.stream())
+
+
+# ------------------------------------------------------------------------------------------------
+# diverse beam search
+# ------------------------------------------------------------------------------------------------
+def diverse_beam_step(logits, bias, f, G, penalty, wid, ptr, score, eos, top_w, top_lp, eos_id, block_eos=False, ngram=0, ignore=None,
+                      hist_in=None, hist_out=None):
+    """The selection of diverse-beam frame f (vlpk_diverse_beam_step): K beams per image in G groups with a Hamming penalty.  logits:
+    the head's decoder outputs without its bias, [rows, ..., V] with unit stride in V, bf16 or fp32, rows = B at f = 0 and B*K after;
+    bias: [V] of the same dtype, or None.  wid / ptr (int64) and score / eos (fp32): the traces, contiguous [T, B, K]; frame f is
+    written and frame f-1 read.  top_w (int32) / top_lp (fp32): contiguous [B*K, K] scratch.  ngram > 0: duplicate-n-gram blocking
+    over the int32 [B*K, T_cap] histories hist_in (frame f-1) and hist_out (frame f), two different tensors used in turn; ignore:
+    int32 device tensor of exempt word ids, or None.  block_eos: the frame is below min_len."""
+    tensors = ((logits, "logits"), (wid, "beam word ids"), (ptr, "beam back pointers"), (score, "beam scores"), (eos, "beam eos flags"),
+               (top_w, "top-K scratch"), (top_lp, "top-K scratch"))
+    extra = ((bias, "logit bias"), (ignore, "n-gram ignore set"), (hist_in, "n-gram history"), (hist_out, "n-gram history"))
+    for t, what in tensors + tuple((t, w) for t, w in extra if t is not None):
+        _require_cuda(t, what)
+    if wid.dim() != 3 or any(t.shape != wid.shape or not t.is_contiguous() for t in (wid, ptr, score, eos)) \
+            or wid.dtype != torch.int64 or ptr.dtype != torch.int64 or score.dtype != torch.float32 or eos.dtype != torch.float32:
+        raise RuntimeError("vlp_b200: beam traces must be contiguous [T, B, K] tensors: int64 word ids and pointers, fp32 scores and "
+                           "eos flags")
+    T, B, K = wid.shape
+    if not 0 <= f < T:
+        raise ValueError(f"vlp_b200: frame {f} outside the traces' {T} frames")
+    V = logits.shape[-1]
+    lg = logits.reshape(-1, V) if logits.dim() != 2 else logits
+    if logits.dtype not in (BF16, torch.float32) or lg.stride(1) != 1 or lg.shape[0] != (B if f == 0 else B * K):
+        raise RuntimeError("vlp_b200: diverse-beam logits must be bf16 or fp32 [rows, V] with unit column stride, rows = B at frame 0 "
+                           "and B*K after")
+    if bias is not None and (bias.dtype != logits.dtype or bias.shape != (V,) or not bias.is_contiguous()):
+        raise RuntimeError("vlp_b200: the logit bias must be a contiguous [V] tensor of the logits' dtype")
+    if top_w.dtype != torch.int32 or top_lp.dtype != torch.float32 or top_w.shape != (B * K, K) or top_lp.shape != (B * K, K) \
+            or not (top_w.is_contiguous() and top_lp.is_contiguous()):
+        raise RuntimeError("vlp_b200: the top-K scratch must be contiguous int32 and fp32 [B*K, K] tensors")
+    T_cap = T
+    if ngram:
+        if hist_in is None or hist_out is None or hist_in.shape != hist_out.shape or hist_out.dim() != 2 or hist_out.shape[0] != B * K \
+                or hist_in.dtype != torch.int32 or hist_out.dtype != torch.int32 or not (hist_in.is_contiguous() and hist_out.is_contiguous()):
+            raise RuntimeError("vlp_b200: n-gram histories must be two contiguous int32 [B*K, T_cap] tensors")
+        T_cap = hist_out.shape[1]
+    if ignore is not None and (ignore.dtype != torch.int32 or ignore.dim() != 1 or not ignore.is_contiguous()):
+        raise RuntimeError("vlp_b200: the n-gram ignore set must be a contiguous 1-D int32 tensor of word ids")
+    n_ign = 0 if ignore is None or not ngram else ignore.numel()
+    prev = (wid[f - 1], ptr[f - 1], score[f - 1], eos[f - 1]) if f else (None,) * 4
+    L.call("vlpk_diverse_beam_step", B, K, int(G), int(f), V, lg.data_ptr(), lg.stride(0), L.ptr(bias), int(logits.dtype == torch.float32),
+           float(penalty), int(eos_id), int(bool(block_eos)), T_cap, int(ngram), L.ptr(hist_in if ngram else None),
+           L.ptr(hist_out if ngram else None), ignore.data_ptr() if n_ign else None, n_ign, *(L.ptr(t) for t in prev), top_w.data_ptr(),
+           top_lp.data_ptr(), wid[f].data_ptr(), ptr[f].data_ptr(), score[f].data_ptr(), eos[f].data_ptr(), L.stream())

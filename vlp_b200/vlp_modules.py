@@ -22,7 +22,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import ops
-from .beam import beam_search
+from .beam import beam_search, diverse_beam_search
 from .decode import check_decode, greedy_decode, sample_decode
 from .score import score_caption_matrix, score_captions
 
@@ -832,7 +832,7 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
 
     def __init__(self, config, mask_word_id=0, num_labels=2, search_beam_size=1, length_penalty=1.0, eos_id=0, forbid_duplicate_ngrams=False,
                  forbid_ignore_set=None, ngram_size=3, min_len=0, enable_butd=False, len_vis_input=49, sampling_method="beam_search", topk=1,
-                 topp=1.0, seed=0, num_return_sequences=1):
+                 topp=1.0, seed=0, num_return_sequences=1, num_beam_groups=1, diversity_penalty=0.0):
         super().__init__(config)
         self.bert = BertModelIncr(config)
         self.cls = BertPreTrainingHeads(config, self.bert.embeddings.word_embeddings.weight, num_labels=num_labels)
@@ -851,9 +851,12 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         # "topk" / "topp": stochastic decode on the device (decode.sample_decode) instead of greedy / beam search; beam size 1.
         # N > 1: N captions per image (beam search's N best hypotheses, or N samples) over one K/V cache of the image prefix.
         # forward checks every decode setting again, the n-gram settings included, since callers may change these attributes.
-        check_decode(sampling_method, topk, topp, search_beam_size, num_return_sequences)
+        # G > 1: diverse beam search, the K beams in G groups of K / G with a Hamming penalty (beam.diverse_beam_search).
+        check_decode(sampling_method, topk, topp, search_beam_size, num_return_sequences, num_beam_groups=num_beam_groups,
+                     diversity_penalty=diversity_penalty)
         self.sampling_method, self.topk, self.topp, self.seed = sampling_method, topk, topp, seed
         self.num_return_sequences = num_return_sequences
+        self.num_beam_groups, self.diversity_penalty = num_beam_groups, diversity_penalty
         self.use_kv_cache = True     # False: the reference's data flow (K, V of the whole prefix re-projected at every step, modeling.py:273-277)
         self._build_region_projections(config, enable_butd)
 
@@ -869,16 +872,21 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         out["attentions"]: fp32 [B, out_len - in_len, layers, heads, out_len], for every output word the attention probabilities of the
         [MASK] query row that predicted it, over keys [0, out_len) (keys not yet visible, and frames not decoded, are 0).
         num_return_sequences N > 1: beam search adds out["nbest_seq"] int64 [B, N, out_len] and out["nbest_scores"] fp32 [B, N];
-        top-k / top-p sampling returns ids and scores [B, N, out_len - in_len]."""
+        top-k / top-p sampling returns ids and scores [B, N, out_len - in_len].
+        num_beam_groups G > 1: diverse beam search, whose out also holds each group's best caption, out["group_seq"] int64
+        [B, G, out_len] and out["group_scores"] fp32 [B, G]."""
         self.cls.predictions.check_task_idx(task_idx)          # before anything is launched
         _check_seq_len(self.config, token_type_ids.size(1))
         check_decode(self.sampling_method, self.topk, self.topp, self.search_beam_size, self.num_return_sequences,
-                     self.forbid_duplicate_ngrams, self.ngram_size, self.use_kv_cache, output_attentions)
+                     self.forbid_duplicate_ngrams, self.ngram_size, self.use_kv_cache, output_attentions,
+                     num_beam_groups=self.num_beam_groups, diversity_penalty=self.diversity_penalty)
         with torch.no_grad():
             vis_feats, vis_pe = self.project_regions(vis_feats, vis_pe)
             inputs = (self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx)
             if self.sampling_method != "beam_search":
                 return sample_decode(*inputs, seed, output_attentions=output_attentions)
+            if self.num_beam_groups > 1:
+                return diverse_beam_search(*inputs, output_attentions=output_attentions)
             if self.search_beam_size > 1:
                 return beam_search(*inputs, output_attentions=output_attentions)
             return greedy_decode(*inputs, sample_mode, output_attentions=output_attentions)
