@@ -141,14 +141,16 @@ def incremental_case(dev, B=2, Lq=2, Lkv=50, H=128, heads=2, I=512):
 
 
 # ---- encoder stack and cached decode layer (tests/test_encoder_stack_gpu.py) ------------------------------------------------------
-def guarded_acts(n_layers, B, Lq, H, heads, I, dev, drop_bits=False, decode=False):
+def guarded_acts(n_layers, B, Lq, H, heads, I, dev, drop_bits=False, decode=False, Lkv=None):
     """Per-layer VlpkLayerActs whose every buffer is a NaN-guarded view (tools/kernel_check.guarded) of its ops.act_layout shape.
-    decode: the layout of vlpk_layer_cached_fwd (qkv holds Q [B*Lq, H], kv the new rows' K | V [B*Lq, 2H]).  drop_bits: attention
-    keep-bits followed by 64 guard bytes of 0xA5.  Returns (structs, [dict of views per layer], keep-bit buffer or None)."""
+    Lq: rows per sequence (R = S + T or 2T - 1 for the scoring stacks).  decode: the layout of vlpk_layer_cached_fwd and of the
+    re-projecting decode layer (qkv holds Q [B*Lq, H], kv the K | V of Lkv rows per sequence [B*Lkv, 2H]; Lkv defaults to Lq, the
+    cached layer's new rows).  drop_bits: attention keep-bits followed by 64 guard bytes of 0xA5.  Returns (structs, [dict of views
+    per layer], keep-bit buffer or None)."""
     structs = (L.VlpkLayerActs * n_layers)()
     nb = B * heads * Lq * ops.key_slots(Lq) // 8
     bits = torch.full((n_layers, nb + 64), 0xA5, dtype=torch.uint8, device=dev) if drop_bits else None
-    bf, f32 = ops.act_layout(B, Lq, H, heads, I, Lkv=Lq if decode else None)
+    bf, f32 = ops.act_layout(B, Lq, H, heads, I, Lkv=(Lkv or Lq) if decode else None)
     fields = {n: (s, BF16) for n, s in bf} | {n: (s, torch.float32) for n, s in f32 if n is not None}
     if decode:
         # the cached layer stores only Q in qkv: guarding exactly [B*Lq, H] catches a store past Q, which ops' 3H-wide buffer would hide
@@ -278,6 +280,137 @@ def cached_decode_calls(dev, H, B, src, n_steps, cache_rows, seed=0):
                structs, 0, L.stream())
         yield dict(pos=pos, Lq=Lq, Lkv=Lkv, B=B, H=H, I=I, heads=heads, x=x, mask=m, bits=bits, acts=views[0], before=before, cache=cache,
                    params=params)
+
+
+# ---- scoring stacks and the re-projecting decode layer (tests/test_score_stack_gpu.py) ----------------------------------------------
+def score_masks(kind, B, S, T, gen):
+    """0/1 masks (shared [B, S, S], query [B, T, S]) of B sequences of S shared keys and T query rows.
+    s2s: vlp_b200.score.layout at in_len = S - T + 1; ragged: the same with the last 3 (b % 5) prefix positions of sequence b padding,
+    seen by no row; bernoulli: every bit a coin flip; dead_row: s2s with one query row per sequence seeing no shared key (only
+    itself); beyond: Bernoulli(0.8), and score_bits sets every bit past S as well."""
+    from vlp_b200 import score
+    if kind in ("bernoulli", "beyond"):
+        p = 0.5 if kind == "bernoulli" else 0.8
+        return (torch.rand(B, S, S, generator=gen) < p).long(), (torch.rand(B, T, S, generator=gen) < p).long()
+    in_len = S - T + 1
+    _, _, shared_keep, query_keep = score.layout(in_len, T)
+    shared, query = shared_keep.long().expand(B, S, S).clone(), query_keep.long().expand(B, T, S).clone()
+    for b in range(B):
+        if kind == "ragged":
+            pad = 3 * (b % 5)
+            shared[b, :, in_len - pad:in_len] = 0
+            query[b, :, in_len - pad:in_len] = 0
+        elif kind == "dead_row":
+            query[b, (7 * b + 3) % T] = 0
+    return shared, query
+
+
+def score_bits(m, dev, beyond=False):
+    """Packed bits of a 0/1 mask [B, rows, S]; beyond: every bit at key slots [S, key_slots(S)) set too (vlpk_mask_pack never sets
+    them), which the kernels must ignore."""
+    bits = ops.pack_mask(m.to(dev), "zero_one")
+    S = m.shape[2]
+    if beyond and S < ops.key_slots(S):
+        hi = torch.zeros(bits.shape[2], dtype=torch.int64)
+        for j in range(S, ops.key_slots(S)):
+            hi[j // 32] |= 1 << (j % 32)
+        bits = bits | torch.where(hi >= 2 ** 31, hi - 2 ** 32, hi).to(torch.int32).to(dev)
+    return bits
+
+
+def score_stack_inputs(dev, B, S, T, H, I, n_layers, mask="s2s", seed=0):
+    """One vlpk_encoder_score_fwd case: B sequences of R = S + T rows (S shared, then T query rows)."""
+    gen = torch.Generator().manual_seed(seed)
+    heads, R = H // 64, S + T
+    params = [t for _ in range(n_layers) for t in layer_params(gen, dev, H, I)]
+    x = _rn(gen, dev, B * R, H)
+    shared, query = score_masks(mask, B, S, T, gen)
+    return dict(B=B, S=S, T=T, R=R, K=S, H=H, I=I, heads=heads, n_layers=n_layers, params=params, x=x,
+                key_bits=score_bits(shared, dev, mask == "beyond"), query_bits=score_bits(query, dev, mask == "beyond"),
+                shape=L.VlpkShape(B, S, S, H, heads, I, ops.kv_slots(S, S)), ws=ops._weight_structs(params, n_layers), dev=dev)
+
+
+def score_stack_run(c, x=None):
+    """vlpk_encoder_score_fwd on x (default c["x"]) into per-layer NaN-guarded acts: [dict of views per layer]."""
+    x = c["x"] if x is None else x
+    structs, views, _ = guarded_acts(c["n_layers"], c["B"], c["R"], c["H"], c["heads"], c["I"], c["dev"])
+    L.call("vlpk_encoder_score_fwd", C.byref(c["shape"]), c["T"], c["n_layers"], c["ws"], x.data_ptr(), c["key_bits"].data_ptr(),
+           c["query_bits"].data_ptr(), structs, L.stream())
+    return views
+
+
+def score_shared_run(c):
+    """vlpk_encoder_fwd over the S shared rows alone under the shared mask into per-layer NaN-guarded acts: [dict of views per layer]."""
+    B, S, R, H = c["B"], c["S"], c["R"], c["H"]
+    x = c["x"].view(B, R, H)[:, :S].reshape(B * S, H).contiguous()
+    structs, views, _ = guarded_acts(c["n_layers"], B, S, H, c["heads"], c["I"], c["dev"])
+    bits = c["key_bits"]
+    L.call("vlpk_encoder_fwd", C.byref(c["shape"]), c["n_layers"], c["ws"], x.data_ptr(), bits.data_ptr(), bits.shape[1], structs, 0.0, 0.0,
+           None, L.stream())
+    return views
+
+
+def group_stack_inputs(dev, images, G, P, T, H, I, n_layers, mask="s2s", seed=0):
+    """One vlpk_encoder_score_group_fwd case: images x G pairs of R = 2T - 1 rows (T - 1 words, then T query rows), keys [the image's
+    P prefix rows | the pair's words], S = P + T - 1.  Every layer's prefix cache has prefix_rows = P + 3 rows per image, those past
+    P NaN."""
+    gen = torch.Generator().manual_seed(seed)
+    heads, B, R, S = H // 64, images * G, 2 * T - 1, P + T - 1
+    params = [t for _ in range(n_layers) for t in layer_params(gen, dev, H, I)]
+    x = _rn(gen, dev, B * R, H)
+    prefix = []
+    for _ in range(n_layers):
+        t = torch.full((images, P + 3, 2 * H), float("nan"), dtype=BF16, device=dev)
+        t[:, :P] = _rn(gen, dev, images, P, 2 * H)
+        prefix.append(t)
+    shared, query = score_masks(mask, images, S, T, gen)
+    beyond = mask == "beyond"
+    return dict(images=images, G=G, P=P, B=B, S=S, T=T, R=R, K=T - 1, H=H, I=I, heads=heads, n_layers=n_layers, params=params, x=x,
+                prefix=prefix, key_bits=score_bits(shared[:, P:], dev, beyond) if T > 1 else None, query_bits=score_bits(query, dev, beyond),
+                shape=L.VlpkShape(B, S, S, H, heads, I, ops.kv_slots(S, S)), ws=ops._weight_structs(params, n_layers), dev=dev)
+
+
+def group_stack_run(c, x=None, prefix=None):
+    """vlpk_encoder_score_group_fwd on x / prefix (default c's) into per-layer NaN-guarded acts: [dict of views per layer]."""
+    x = c["x"] if x is None else x
+    prefix = c["prefix"] if prefix is None else prefix
+    n = c["n_layers"]
+    structs, views, _ = guarded_acts(n, c["B"], c["R"], c["H"], c["heads"], c["I"], c["dev"])
+    caches = (C.c_void_p * n)(*[t.data_ptr() for t in prefix])
+    L.call("vlpk_encoder_score_group_fwd", C.byref(c["shape"]), c["T"], c["G"], c["P"], n, c["ws"], x.data_ptr(), caches, prefix[0].shape[1],
+           L.ptr(c["key_bits"]), c["query_bits"].data_ptr(), structs, L.stream())
+    return views
+
+
+def incr_layer_inputs(dev, B, Lq, Lkv, H, I, mask_rows, seed=0):
+    """One re-projecting decode layer case: x_kv [B*Lkv, H] = cat(history, x), x its last Lq rows per sequence.  The mask [B, mask_rows,
+    Lkv]: row r sees the positions up to its own, the first 2 (b % 4) of sequence b padding; one row: the last row's."""
+    gen = torch.Generator().manual_seed(seed)
+    heads = H // 64
+    params = layer_params(gen, dev, H, I)
+    x_kv = _rn(gen, dev, B * Lkv, H)
+    x = x_kv.view(B, Lkv, H)[:, Lkv - Lq:].reshape(B * Lq, H).contiguous()
+    m = torch.tril(torch.ones(Lq, Lkv, dtype=torch.long), diagonal=Lkv - Lq).expand(B, Lq, Lkv).clone()
+    for b in range(B):
+        m[b, :, :2 * (b % 4)] = 0
+    m = m[:, Lq - mask_rows:].contiguous()
+    return dict(B=B, Lq=Lq, Lkv=Lkv, H=H, I=I, heads=heads, params=params, x=x, x_kv=x_kv, bits=ops.pack_mask(m.to(dev), "zero_one"),
+                shape=L.VlpkShape(B, Lq, Lkv, H, heads, I, ops.kv_slots(Lq, Lkv)), ws=ops._weight_structs(params, 1), dev=dev)
+
+
+def incr_layer_run(c):
+    """vlpk_layer_fwd and vlpk_mha_incr_fwd with x_kv, each into its own NaN-guarded acts: (layer views, attention-half views)."""
+    out = []
+    for entry in ("vlpk_layer_fwd", "vlpk_mha_incr_fwd"):
+        structs, views, _ = guarded_acts(1, c["B"], c["Lq"], c["H"], c["heads"], c["I"], c["dev"], decode=True, Lkv=c["Lkv"])
+        bits = c["bits"]
+        head = (C.byref(c["shape"]), C.byref(c["ws"][0]), c["x"].data_ptr(), c["x_kv"].data_ptr(), bits.data_ptr(), bits.shape[1], structs)
+        if entry == "vlpk_layer_fwd":
+            L.call(entry, *head, 0.0, 0.0, None, 0, L.stream())
+        else:
+            L.call(entry, *head, 0, L.stream())
+        out.append(views[0])
+    return tuple(out)
 
 
 # ---- fused BertAdam step (tests/test_adam_kernel_gpu.py) ----------------------------------------------------------------------------

@@ -21,6 +21,15 @@ Backward stages (dy: gradient of y)
   7 dx        dqkv [Wq|Wk|Wv] + dz1; wqkv += dqkv^T x            GEMM, GEMM f32
 Every fp32 parameter gradient is checked as prior + sum onto the arena's prior contents.  Failures name the layer, the stage and the
 worst tile / block / row / column.  Everything runs on whatever device its tensors live on.
+
+The forward-only layouts (score_layer_fwd and mha_fwd_impl with x_kv, csrc/api.cu) differ from the training layer in stages 1-2 only:
+  score  (vlpk_encoder_score_fwd)        B sequences of R = S + T rows.  The S shared rows attend to the S shared keys (key launch);
+                                         the T query rows attend to the shared keys and each to its own key (query launch).
+  group  (vlpk_encoder_score_group_fwd)  B = images x G pairs of R = 2T - 1 rows.  The keys of a pair are the P first rows of its
+                                         image's prefix cache, then its own T - 1 word rows; the word rows attend to them (key launch,
+                                         none when T = 1), the T query rows attend to them and each to its own key.
+  incr   (vlpk_layer_fwd / vlpk_mha_incr_fwd with x_kv)  q = x Wq^T + bq [B*Lq, H] in acts.qkv, K | V of x_kv [B*Lkv, 2H] in acts.kv.
+The lse of a scoring layer is the key launch's [B, heads, K] block followed by the query launch's [B, heads, T] block.
 """
 import torch
 
@@ -29,6 +38,7 @@ from vlp_b200 import ops
 from vlp_b200._lib import WEIGHT_FIELDS
 
 F64 = torch.float64
+BF = torch.bfloat16
 STORE, GELU, ADD, MUL, REDUCE = 0, 1, 3, 4, 6
 
 FWD_STAGES = ["fwd1 qkv", "fwd2 ctx/lse", "fwd3 t1", "fwd4 y1/stats1", "fwd5 u/hmid", "fwd6 t2", "fwd7 y/stats2"]
@@ -174,6 +184,102 @@ def reference_layer(w, x, allow, keep, p, B, L, heads, dy, prior):
     return A, S, {n: G[n][1] for n in G}
 
 
+# ---- forward-only layouts: scoring (score, group) and the re-projecting decode layer (incr) -------------------------------------
+def _bqkv(w):
+    return torch.cat((w["bq"], w["bk"], w["bv"]))
+
+
+def self_key_attn_ref(q, k, v, ks, vs, allow):
+    """fp64 attention of q [B,h,Lq,64] over k / v [B,h,Lkv,64] (additive -10000 where allow [B,Lq,Lkv] is False, scale 1/8), each
+    query row also attending to its own key ks / vs [B,h,Lq,64], never masked.  Returns dict(ctx, lse, E)."""
+    q, k, v, ks, vs = (t.to(F64) for t in (q, k, v, ks, vs))
+    s = torch.cat((q @ k.transpose(-1, -2) / 8.0 + (~allow[:, None]).to(F64) * -10000.0, (q * ks).sum(-1, keepdim=True) / 8.0), -1)
+    P = torch.softmax(s, -1)
+    n = k.shape[2]
+    return {"ctx": P[..., :n] @ v + P[..., n:] * vs, "lse": torch.logsumexp(s, -1), "E": P[..., :n] @ v.abs() + P[..., n:] * vs.abs()}
+
+
+def score_keys(qkv, B, R, K, heads, prefix=None, P=0, G=1):
+    """The keys of a scoring layer, (k, v) [B, heads, Lkv, 64]: the first K rows of each sequence of qkv [B*R, 3H], behind the
+    first P rows of its image's prefix cache (prefix [images, prefix_rows, 2H], G sequences per image) when prefix is given."""
+    _, k, v = _split(qkv, B, R, heads)
+    k, v = k[:, :, :K], v[:, :, :K]
+    if prefix is not None:
+        H = heads * 64
+        pre = prefix[:, :P].repeat_interleave(G, 0)
+        k = torch.cat((kc.heads_view(pre[..., :H], B, P, heads), k), 2)
+        v = torch.cat((kc.heads_view(pre[..., H:], B, P, heads), v), 2)
+    return k, v
+
+
+def score_attn_refs(qkv, B, R, K, heads, key_allow, query_allow, prefix=None, P=0, G=1):
+    """fp64 stage 2 of one scoring layer from its own qkv [B*R, 3H]: {"keys": attn_ref of the first K rows of every sequence (None
+    when K = 0), "query": self_key_attn_ref of its last R - K rows}, both over score_keys.  key_allow [., K, Lkv] / query_allow
+    [., R - K, Lkv]: one mask per sequence, or with a prefix one per image."""
+    q, ks, vs = _split(qkv, B, R, heads)
+    k, v = score_keys(qkv, B, R, K, heads, prefix, P, G)
+    rep = lambda a: a.repeat_interleave(G, 0)
+    return {"keys": kc.attn_ref(q[:, :, :K], k, v, rep(key_allow)) if K > 0 else None,
+            "query": self_key_attn_ref(q[:, :, K:], k, v, ks[:, :, K:], vs[:, :, K:], rep(query_allow))}
+
+
+def score_lse(lse, B, R, K, heads):
+    """A scoring layer's lse buffer -> (the key launch's [B, heads, K] block, the query launch's [B, heads, R - K] block)."""
+    flat = lse.reshape(-1)
+    n = B * heads * K
+    return flat[:n].view(B, heads, K), flat[n:n + B * heads * (R - K)].view(B, heads, R - K)
+
+
+def incr_attn_ref(A, B, Lq, Lkv, heads, allow):
+    """fp64 stage 2 of the re-projecting decode layer from its own q (A["qkv"] [B*Lq, H]) and K | V (A["kv"] [B*Lkv, 2H])."""
+    H = heads * 64
+    kv = A["kv"].reshape(B, Lkv, 2 * H)
+    return kc.attn_ref(kc.heads_view(A["qkv"], B, Lq, heads), kc.heads_view(kv, B, Lkv, heads), kc.heads_view(kv[..., H:], B, Lkv, heads),
+                       allow)
+
+
+def _store(rounded):
+    return (lambda t, dt: t.to(dt)) if rounded else (lambda t, dt: t)
+
+
+def compose_tail(w, x, A, store):
+    """Forward stages 3-7 chained on A["ctx"]: fills t1, y1, stats1, u, hmid, t2, y and stats2 of A.  store(t, dtype) is what a
+    stored output becomes before the next stage reads it."""
+    f32 = torch.float32
+    A["t1"] = store(ref_linear(A["ctx"], w["wo"], w["bo"])["d0"][0], BF)
+    l1 = kc.ln_ref(A["t1"], x, w["ln1_g"], w["ln1_b"])
+    A["y1"], A["stats1"] = store(l1["y"][0], BF), store(torch.stack((l1["mean"], l1["rstd"]), -1), f32)
+    g = ref_linear(A["y1"], w["w1"], w["b1"], GELU)
+    A["u"], A["hmid"] = store(g["d0"][0], BF), store(g["d1"][0], BF)
+    A["t2"] = store(ref_linear(A["hmid"], w["w2"], w["b2"])["d0"][0], BF)
+    l2 = kc.ln_ref(A["t2"], A["y1"], w["ln2_g"], w["ln2_b"])
+    A["y"], A["stats2"] = store(l2["y"][0], BF), store(torch.stack((l2["mean"], l2["rstd"]), -1), f32)
+    return A
+
+
+def compose_score_layer(w, x, B, R, K, heads, key_allow, query_allow, prefix=None, P=0, G=1, rounded=False):
+    """One scoring layer chained stage by stage, no kernel anywhere: every activation, lse as its two blocks.  rounded: every stored
+    output is rounded as the kernels store it (bf16 activations, fp32 lse and statistics) before the next stage reads it; else all
+    fp64.  Test support: in fp64 this must agree with the oracle's bert_layer over the equivalent plain sequence."""
+    st = _store(rounded)
+    A = {"qkv": st(ref_linear(x, _wqkv(w), _bqkv(w))["d0"][0], BF)}
+    f = score_attn_refs(A["qkv"], B, R, K, heads, key_allow, query_allow, prefix, P, G)
+    parts = [f["query"]] if f["keys"] is None else [f["keys"], f["query"]]
+    A["ctx"] = st(_merge(torch.cat([a["ctx"] for a in parts], 2)), BF)
+    A["lse"] = st(torch.cat([a["lse"].reshape(-1) for a in parts]), torch.float32)
+    return compose_tail(w, x, A, st)
+
+
+def compose_incr_layer(w, x, x_kv, B, Lq, Lkv, heads, allow, rounded=False):
+    """The re-projecting decode layer chained stage by stage (as compose_score_layer): x [B*Lq, H] query rows, x_kv [B*Lkv, H]."""
+    st = _store(rounded)
+    A = {"qkv": st(ref_linear(x, w["wq"], w["bq"])["d0"][0], BF),
+         "kv": st(ref_linear(x_kv, torch.cat((w["wk"], w["wv"])), torch.cat((w["bk"], w["bv"])))["d0"][0], BF)}
+    f = incr_attn_ref(A, B, Lq, Lkv, heads, allow)
+    A["ctx"], A["lse"] = st(_merge(f["ctx"]), BF), st(f["lse"].reshape(-1), torch.float32)
+    return compose_tail(w, x, A, st)
+
+
 # ---- checks --------------------------------------------------------------------------------------------------------------------
 class Worst(dict):
     """Largest share of each bound family used so far."""
@@ -217,6 +323,40 @@ def check_tail(tag, A, R, worst):
     check_gemm_stage(worst, f"{tag} {s[4]}: u (gelu')", A["u"], R["u"])
     check_gemm_stage(worst, f"{tag} {s[4]}: hmid", A["hmid"], R["hmid"])
     check_gemm_stage(worst, f"{tag} {s[5]}: t2", A["t2"], R["t2"])
+
+
+def _check_attn(what, worst, got_ctx, got_lse, ref):
+    e, t = kc.check_attn_block(f"{what} ctx", got_ctx, ref["ctx"], ref["E"], kc.ATTN_FWD_BLOCK)
+    worst.note("attn fwd elementwise", e)
+    worst.note("attn fwd block", t)
+    worst.note("attn lse", kc.check_lse(f"{what} lse", got_lse, ref["lse"]))
+
+
+def check_score_layer_fwd(tag, w, x, A, B, R, K, heads, key_allow, query_allow, worst, prefix=None, P=0, G=1):
+    """Every activation of one scoring layer over B*R rows (A: qkv, ctx, lse, t1, y1, stats1, u, hmid, t2, y, stats2) against
+    score_attn_refs and tail_refs of its own inputs x [B*R, H] and A.  The two attention launches are checked apart: a failure
+    names the launch, and its rows count from the launch's first row."""
+    s = FWD_STAGES
+    check_gemm_stage(worst, f"{tag} {s[0]}: qkv", A["qkv"], ref_linear(x, _wqkv(w), _bqkv(w))["d0"])
+    f = score_attn_refs(A["qkv"], B, R, K, heads, key_allow, query_allow, prefix, P, G)
+    ctx = kc.heads_view(A["ctx"], B, R, heads)
+    lse_k, lse_q = score_lse(A["lse"], B, R, K, heads)
+    if K > 0:
+        rows = "word" if prefix is not None else "shared"
+        _check_attn(f"{tag} {s[1]}: {rows} rows 0..{K - 1} (key launch)", worst, ctx[:, :, :K], lse_k, f["keys"])
+    _check_attn(f"{tag} {s[1]}: query rows {K}..{R - 1} (query launch)", worst, ctx[:, :, K:], lse_q, f["query"])
+    check_tail(tag, A, tail_refs(w, x, A, {}, 0.0), worst)
+
+
+def check_incr_layer_fwd(tag, w, x, x_kv, A, B, Lq, Lkv, heads, allow, worst):
+    """Every activation of the re-projecting decode layer (A: qkv holding q [B*Lq, H], kv [B*Lkv, 2H], ctx, lse, t1 ... stats2)
+    against the references of its own inputs x [B*Lq, H], x_kv [B*Lkv, H] and A."""
+    s = FWD_STAGES
+    check_gemm_stage(worst, f"{tag} {s[0]}: q", A["qkv"], ref_linear(x, w["wq"], w["bq"])["d0"])
+    check_gemm_stage(worst, f"{tag} {s[0]}: kv", A["kv"], ref_linear(x_kv, torch.cat((w["wk"], w["wv"])), torch.cat((w["bk"], w["bv"])))["d0"])
+    _check_attn(f"{tag} {s[1]}:", worst, kc.heads_view(A["ctx"], B, Lq, heads), A["lse"].reshape(B, heads, Lq),
+                incr_attn_ref(A, B, Lq, Lkv, heads, allow))
+    check_tail(tag, A, tail_refs(w, x, A, {}, 0.0), worst)
 
 
 def check_layer_bwd(tag, w, x, allow, A, dy, S, prior, keep, p, B, L, heads, worst):
