@@ -453,6 +453,55 @@ int vlpk_diverse_beam_step(int B, int K, int G, int f, int V, const void* logits
                            int n_ignore, const int64_t* prev_wid, const int64_t* prev_ptr, const float* prev_score, const float* prev_eos,
                            int32_t* top_w, float* top_lp, int64_t* wid, int64_t* ptr, float* score, float* eos, void* stream);
 
+/* Constrained beam search (Anderson et al., EMNLP 2017): the selection of frame f (0 <= f < T_cap) for B images whose captions must
+ * contain C constraints, one call per frame (two launches), no host synchronisation.
+ *   constraints  cons int64 [B, C, A, P], 0-padded: constraint j of image b is the disjunction of its alternatives, each a run of
+ *     1 .. P word ids (the leading non-zero entries; an alternative whose first entry is 0 is absent).  A constraint with no
+ *     alternative is satisfied from the start.
+ *   states       a hypothesis' state s is the set of constraints met so far (bit j: an alternative of j occurred as a contiguous run
+ *     of its generated words).  S = 2^C states of K beams each: image b's slots are [0, S*K), slot s*K + k is beam k of state s.
+ *     Rows are b (f = 0, in the root state: the set of empty constraints) or b*S*K + slot.
+ *   logp[i, w]   as vlpk_diverse_beam_step: x = logits + bias rounded to the logits' dtype (fp32 = 0: bf16, 1: fp32), logp = x -
+ *     logsumexp(x) in fp32, -10000 added at the words the duplicate-n-gram rule of vlpk_beam_ngram_block blocks (n > 0, f >= n),
+ *     logp[eos_id] = -10000 if block_eos.  The history carry hist_out[i] = hist_in[b*S*K + prev_ptr[i]] ‖ prev_wid[i] runs at every
+ *     f >= 1, whatever n.
+ *   cand(i, w)   logp at f = 0; logp + prev_eos[i] * -10000 + prev_score[i] after (frame f-1's traces, [B, S*K]).
+ *   dest(i, w)   s_i ∪ {j : w completes an alternative a of j}: a[-1] == w and the row's last len(a) - 1 words equal a[:-1].
+ *   selection    state s' keeps the K (row, word) pairs with dest == s' and the largest finite cand, ties to the lower parent slot, then
+ *     the lower word; its r-th pair becomes slot s'*K + r.  Slots it cannot fill are empty: word 0, pointer 0, score -inf, eos 0.
+ *   traces       wid / ptr int64 [B, S*K] (ptr a slot in [0, S*K), 0 at f = 0), score fp32 [B, S*K] the cand, eos fp32 [B, S*K]
+ *     (wid == eos_id).  top_w int32 / top_lp fp32 [rows, K + C*A] and top_dest int32 [rows, C*A] are scratch: each row's top K
+ *     words that keep it in its state, then its completing words and their destinations.
+ * Limits: 1 <= C <= 4, 1 <= A <= 4, 1 <= P <= 8, 1 <= K <= 64, S*K <= 256 (so K <= 16 at C = 4 and K <= 64 at C <= 2), V >= K + C*A.
+ * Bitwise reproducible.  Returns < 0 without launching for a value outside these limits, ld < V, f outside [0, T_cap), fp32 not 0 / 1,
+ * a NULL pointer that is needed, hist_in == hist_out, or (V + V/32 + T_cap) * 4 bytes above 200 KB of shared memory. */
+typedef struct VlpkConstrainedBeamArgs {
+  int32_t B, K, C, A, P;             /* images, beams per state, constraints, alternatives per constraint, words per alternative */
+  int32_t f, V;                      /* frame; vocabulary */
+  const void* logits;                /* [rows, ld] bf16 or fp32 decoder outputs, without the bias */
+  int64_t ld;
+  const void* bias;                  /* [V] same dtype, or NULL */
+  int32_t fp32, eos_id, block_eos;
+  int32_t T_cap, n;                  /* history width (frames); duplicate-n-gram size, 0 = off */
+  const int32_t* hist_in;            /* [B*S*K, T_cap] frame f-1's histories (read at f >= 2) */
+  int32_t* hist_out;                 /* [B*S*K, T_cap] frame f's histories (f words, written at f >= 1) */
+  const int32_t* ignore;             /* [n_ignore] word ids exempt from n-gram blocking */
+  int32_t n_ignore;
+  const int64_t* cons;               /* [B, C, A, P] */
+  const int64_t* prev_wid;           /* [B, S*K] frame f-1's traces (f >= 1; prev_ptr at f >= 2) */
+  const int64_t* prev_ptr;
+  const float* prev_score;
+  const float* prev_eos;
+  int32_t* top_w;                    /* [rows, K + C*A] scratch */
+  float* top_lp;                     /* [rows, K + C*A] scratch */
+  int32_t* top_dest;                 /* [rows, C*A] scratch */
+  int64_t* wid;                      /* [B, S*K] frame f's traces */
+  int64_t* ptr;
+  float* score;
+  float* eos;
+} VlpkConstrainedBeamArgs;
+int vlpk_constrained_beam_step(const VlpkConstrainedBeamArgs* args, void* stream);
+
 /* utilities */
 int vlpk_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 int vlpk_colsum(const void* x, int64_t ld, int64_t M, int N, float* out, void* stream);

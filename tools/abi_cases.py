@@ -544,3 +544,8 @@ def adam_run(tensors, table, hyper, det=False, reserved_sms=0):
         if reserved_sms:
             L.invoke("vlpk_set_reserved_sms", 0)
         torch.use_deterministic_algorithms(before)
+
+
+def constrained_beam_args(**fields):
+    """A VlpkConstrainedBeamArgs for vlpk_constrained_beam_step (vlpk.h) from keyword fields; unset fields are 0 / NULL."""
+    return L.VlpkConstrainedBeamArgs(**fields)

@@ -52,6 +52,14 @@ class VlpkAdamTensor(C.Structure):
                 ("weight_decay", c_float), ("param_dtype", C.c_int32), ("grad_dtype", C.c_int32), ("reserved", C.c_int32)]
 
 
+class VlpkConstrainedBeamArgs(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("B", "K", "C", "A", "P", "f", "V")] + [("logits", c_void_p), ("ld", c_i64), ("bias", c_void_p)] \
+        + [(n, C.c_int32) for n in ("fp32", "eos_id", "block_eos", "T_cap", "n")] \
+        + [("hist_in", c_void_p), ("hist_out", c_void_p), ("ignore", c_void_p), ("n_ignore", C.c_int32)] \
+        + [(n, c_void_p) for n in ("cons", "prev_wid", "prev_ptr", "prev_score", "prev_eos", "top_w", "top_lp", "top_dest", "wid", "ptr",
+                                   "score", "eos")]
+
+
 # name -> (restype, argtypes); mirrors include/vlpk.h one to one
 _P = c_void_p
 _SIGS = {
@@ -134,6 +142,7 @@ _SIGS = {
                                    c_int, c_int, c_int, _P, c_int, _P]),
     "vlpk_diverse_beam_step": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, c_i64, _P, c_int, c_float, c_int, c_int, c_int, c_int, _P,
                                        _P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "vlpk_constrained_beam_step": (c_int, [C.POINTER(VlpkConstrainedBeamArgs), _P]),
     "vlpk_f32_to_bf16": (c_int, [_P, _P, c_i64, _P]),
     "vlpk_colsum": (c_int, [_P, c_i64, c_i64, c_int, _P, _P]),
     "vlpk_debug_dropout_mask": (c_int, [C.POINTER(VlpkDropout), c_u64, c_i64, _P, _P]),

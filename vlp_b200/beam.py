@@ -9,6 +9,7 @@ device: no host synchronisation inside or after the loop, so a blocked decode ca
 Per-sample `task_idx` (the relaxed MLM head, relax_projection > 1) is expanded to the B*K beam rows with the other inputs; the
 reference does not expand it (:1297 vs :1325-1373), so its relaxed beam search only runs at B = 1.
 Diverse beam search (num_beam_groups > 1, diverse_beam_search) runs the same data flow and trace format with its own per-frame selection.
+Constrained beam search (constraints, constrained_beam_search) runs it too, over K beams in each of 2^C constraint states.
 Every step runs the fused layers on the two new rows (token, [MASK]) through decode.DecodeState, which also expands the history to the
 beams after the first step and reorders it by the back pointers after every later one.
 """
@@ -158,6 +159,107 @@ def diverse_beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, posit
     return out
 
 
+def constrained_beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, cons, task_idx=None,
+                            output_attentions=False):
+    """Constrained beam search (Anderson et al., EMNLP 2017): captions that must contain given words or phrases.  cons: int64 [B, C, A,
+    P] on the device, 0-padded: constraint j of image b is met when one of its A alternatives (each a run of up to P word ids) occurs as
+    a contiguous run of the generated words; a constraint with no alternative is met from the start.  A hypothesis' state is the set s
+    of constraints met so far; each of the S = 2^C states keeps K = dec.search_beam_size beams, slot s*K + k of an image being beam k of
+    state s.  Every frame, each (parent, word) pair goes to the state s_parent ∪ {constraints the word completes}, and each state keeps
+    its K best pairs (beam search's scores, ties to the lower parent slot, then the lower word); a state with fewer candidates leaves
+    empty slots (word 0, pointer 0, score -inf).  One vlpk_constrained_beam_step per frame reads the head's logits once, carries the
+    word histories by back pointer and writes the frame's traces in place, the n-gram blocking and the min_len [EOS] block included;
+    the S*K hypotheses of an image share one copy of its prefix K/V (per-hypothesis caches with output_attentions, which the shared
+    cache does not produce), and nothing synchronises with the host.
+
+    Output: beam_search's dict over the S*K slots (scores, wids, ptrs [B, out_len, S*K]; attentions along pred_seq's path), with
+      pred_seq         the accept state's best caption under the final-selection rule (counting live slots only), or, where the accept
+                       state has none, the best of the states with the most constraints met (higher value, then lower state);
+      constraints_met  bool [B]: the accept state had a candidate;
+      state_seq        int64 [B, S, out_len] and state_scores fp32 [B, S]: each state's own best (-inf where it has none);
+      nbest_seq / nbest_scores (num_return_sequences N > 1): the accept state's N best."""
+    K, C = dec.search_beam_size, cons.shape[1]
+    S = 1 << C
+    SK = S * K
+    B, in_len = input_ids.shape
+    out_len = token_type_ids.shape[1]
+    T = out_len - in_len
+    dev = input_ids.device
+    N = dec.num_return_sequences
+    W = K + C * cons.shape[2]
+    # one copy of each image's prefix K/V for its S*K hypotheses; the attention maps come from per-hypothesis caches
+    state = DecodeState(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, None if output_attentions else SK)
+    ngram = int(dec.ngram_size) if dec.forbid_duplicate_ngrams else 0
+    ignore = _ignore_tensor(dec, dev) if ngram else None
+    hist = [torch.empty(B * SK, T, dtype=torch.int32, device=dev) for _ in range(2)]       # the constraint match reads them always
+    sc, eos = (torch.zeros(T, B, SK, dtype=torch.float32, device=dev) for _ in range(2))
+    wi, pt = (torch.zeros(T, B, SK, dtype=torch.int64, device=dev) for _ in range(2))
+    top_w = torch.empty(B * SK, W, dtype=torch.int32, device=dev)
+    top_lp = torch.empty(B * SK, W, dtype=torch.float32, device=dev)
+    top_dest = torch.empty(B * SK, W - K, dtype=torch.int32, device=dev)
+    pred = dec.cls.predictions
+    maps = new_attention_maps(dec, T, B * SK, out_len, dev) if output_attentions else None
+    rows = torch.arange(B, device=dev).unsqueeze(1) * SK
+    curr_ids = input_ids
+    for frame in range(T):
+        buf = None
+        if maps is not None:
+            buf = maps[frame] if frame else maps[0].view(B, SK, *maps.shape[2:])[:, 0]
+        h = pred.select_task(pred.transform(state.step(curr_ids, buf).to(pred.decoder.weight.dtype)), task_idx)
+        logits = pred.decoder(h)                                          # [B or B*S*K, 1, V]; the kernel adds the bias
+        ops.constrained_beam_step(logits, pred.bias.to(logits.dtype), frame, cons, wi, pt, sc, eos, top_w, top_lp, top_dest, dec.eos_id,
+                                  block_eos=bool(dec.min_len) and frame + 1 <= dec.min_len, ngram=ngram, ignore=ignore,
+                                  hist_in=hist[(frame - 1) % 2], hist_out=hist[frame % 2])
+        if frame == 0:
+            state.expand(SK)
+            task_idx = expand_task_idx(task_idx, B, SK)
+        else:
+            state.reorder((pt[frame] + rows).reshape(-1))
+        curr_ids = wi[frame].reshape(B * SK, 1)
+
+    lp = dec.length_penalty
+    paths = [best_path(sc, wi, pt, dec.eos_id, lp, beams=slice(s * K, (s + 1) * K)) for s in range(S)]
+    state_seq = torch.stack([_path_tokens(wi, *path, out_len) for path in paths], 1)                    # [B, S, out_len]
+    state_scores = torch.stack([candidate_values(sc[:, :, s * K:(s + 1) * K], wi[:, :, s * K:(s + 1) * K], dec.eos_id, lp, live=True)
+                                .max(1).values for s in range(S)], 1)                                  # [B, S]
+    chosen = state_choice(state_scores)
+    bidx = torch.arange(B, device=dev)
+    out = {"pred_seq": state_seq[bidx, chosen], "constraints_met": torch.isfinite(state_scores[:, S - 1])}
+    if maps is not None:
+        active = torch.stack([a for a, _ in paths])[chosen, :, bidx].t()                             # [T, B]: the chosen state's path
+        pos = torch.stack([p for _, p in paths])[chosen, :, bidx].t()
+        out["attentions"] = beam_maps(maps, active, pos, pt)
+    for k, t in (("scores", sc), ("wids", wi), ("ptrs", pt)):
+        padded = t.new_zeros((B, out_len, SK))
+        padded[:, :T] = t.permute(1, 0, 2)
+        out[k] = padded
+    if N > 1:
+        out["nbest_seq"], out["nbest_scores"] = nbest(sc, wi, pt, dec.eos_id, lp, out_len, N, beams=slice((S - 1) * K, SK))
+    out["state_seq"], out["state_scores"] = state_seq, state_scores
+    return out
+
+
+def state_choice(state_scores):
+    """The state pred_seq comes from, [B]: among the states with a candidate (finite value), the most constraints met, then the higher
+    value, then the lower state; the accept state S - 1 whenever it has one.  0 where no state has a candidate."""
+    B, S = state_scores.shape
+    states = torch.arange(S, device=state_scores.device)
+    met = sum((states >> j) & 1 for j in range(max(S.bit_length() - 1, 1)))                   # constraints met by each state
+    finite = torch.isfinite(state_scores)
+    most = torch.where(finite, met, torch.full_like(met, -1)).max(1, keepdim=True).values                    # [B, 1]
+    val = torch.where(finite & (met == most), state_scores, torch.full_like(state_scores, -math.inf))
+    return val.argmax(1)                                                  # first maximum: the lower state
+
+
+def _path_tokens(wi, active, pos, out_len):
+    """The words of a best_path (active / pos [T, B]) as a zero-padded [B, out_len] sequence."""
+    T, B, _ = wi.shape
+    seq = torch.zeros(B, out_len, dtype=torch.long, device=wi.device)
+    tok = wi.gather(2, pos.unsqueeze(-1)).squeeze(-1)
+    seq[:, :T] = torch.where(active, tok, torch.zeros_like(tok)).t()
+    return seq
+
+
 def group_best(sc, wi, pt, eos_id, length_penalty, out_len, G):
     """Each group's best hypothesis under the final-selection rule over its own Kg = K / G beams (a diverse beam search's parents
     stay in their group): (group_seq int64 [B, G, out_len] zero padded, group_scores [B, G] — the rule's values)."""
@@ -197,29 +299,39 @@ def beam_maps(maps, active, pos, pt):
     return torch.where(keep, got, torch.zeros_like(got)).transpose(0, 1)
 
 
-def candidate_values(sc, wi, eos_id, length_penalty):
+def candidate_values(sc, wi, eos_id, length_penalty, live=False):
     """The final-selection rule's value of every (frame, beam), [B, T*K] in (frame, beam) order — the reference's loop order: score +
-    length_penalty * (frame + 1) for a candidate ([EOS] word, or the last frame, within frames <= last[b]), -inf otherwise."""
+    length_penalty * (frame + 1) for a candidate ([EOS] word, or the last frame, within frames <= last[b]), -inf otherwise.
+    live: the beams may hold empty slots (score -inf, constrained beam search); the all-[EOS] test that sets last[b] then counts the
+    live slots only, and a frame with no live slot never ends the search."""
     T, B, K = sc.shape
     dev = sc.device
     frames = torch.arange(T, device=dev).view(T, 1)
-    all_eos = (wi == eos_id).all(-1)                                      # [T,B]
+    if live:
+        alive = torch.isfinite(sc)
+        all_eos = ((wi == eos_id) | ~alive).all(-1) & alive.any(-1)
+    else:
+        all_eos = (wi == eos_id).all(-1)                                  # [T,B]
     last = torch.where(all_eos.any(0), all_eos.float().argmax(0), torch.full((B,), T - 1, device=dev))      # [B]
     cand = (frames <= last.unsqueeze(0)).unsqueeze(-1) & ((wi == eos_id) | (frames == last.unsqueeze(0)).unsqueeze(-1))
     val = torch.where(cand, sc + length_penalty * (frames + 1).unsqueeze(-1).to(sc.dtype), torch.full_like(sc, -math.inf))
     return val.permute(1, 0, 2).reshape(B, T * K)
 
 
-def nbest(sc, wi, pt, eos_id, length_penalty, out_len, n):
+def nbest(sc, wi, pt, eos_id, length_penalty, out_len, n, beams=None):
     """The n highest-ranked candidates of the final-selection rule, each back-tracked as backtrack() does its best one: (nbest_seq
     int64 [B, n, out_len] zero padded, nbest_scores [B, n] — the rule's values).  Equal values keep (frame, beam) order, so entry 0
-    is backtrack()'s hypothesis; the list is not deduplicated.  Every beam of the last frame is a candidate, so n <= K always fills."""
+    is backtrack()'s hypothesis; the list is not deduplicated.  Every beam of the last frame is a candidate, so n <= K always fills.
+    beams: a slice of the slots (one state of constrained beam search) whose candidates are ranked, under the live-slot rule of
+    candidate_values; the back pointers still run over every slot.  Entries past its live candidates are -inf and zero words."""
     T, B, K = sc.shape
     dev = sc.device
-    flat = candidate_values(sc, wi, eos_id, length_penalty)
+    sel = slice(0, K) if beams is None else beams
+    flat = candidate_values(sc[:, :, sel], wi[:, :, sel], eos_id, length_penalty, live=beams is not None)
+    Ks = flat.shape[1] // T
     val, idx = torch.sort(flat, dim=1, descending=True, stable=True)
     val, idx = val[:, :n], idx[:, :n]                                     # [B, n]
-    frame, pos = torch.div(idx, K, rounding_mode="floor"), idx % K
+    frame, pos = torch.div(idx, Ks, rounding_mode="floor"), idx % Ks + sel.start
     found = torch.isfinite(val)
     toks = [None] * T
     for fid in range(T - 1, -1, -1):                                      # walk the back pointers from `frame` down to 0
@@ -231,14 +343,16 @@ def nbest(sc, wi, pt, eos_id, length_penalty, out_len, n):
     return seq, val
 
 
-def best_path(sc, wi, pt, eos_id, length_penalty):
+def best_path(sc, wi, pt, eos_id, length_penalty, beams=None):
     """The hypothesis backtrack() selects, frame by frame: (active [T,B] — frame t belongs to it —, pos [T,B] — its beam index at
-    frame t)."""
+    frame t).  beams: as nbest's, the best of those slots under the live-slot rule (pos still indexes every slot)."""
     T, B, K = sc.shape
     dev = sc.device
-    flat = candidate_values(sc, wi, eos_id, length_penalty)
+    sel = slice(0, K) if beams is None else beams
+    flat = candidate_values(sc[:, :, sel], wi[:, :, sel], eos_id, length_penalty, live=beams is not None)
+    Ks = flat.shape[1] // T
     best = flat.argmax(-1)                                                # first maximal value
-    frame, pos = torch.div(best, K, rounding_mode="floor"), best % K
+    frame, pos = torch.div(best, Ks, rounding_mode="floor"), best % Ks + sel.start
     found = torch.isfinite(flat.gather(1, best.unsqueeze(1)).squeeze(1))
     bidx = torch.arange(B, device=dev)
     actives, poss = [None] * T, [None] * T

@@ -1016,6 +1016,11 @@ int vlpk_diverse_beam_step(int B, int K, int G, int f, int V, const void* logits
   return launch_diverse_beam_step(a, S(stream));
 }
 
+int vlpk_constrained_beam_step(const VlpkConstrainedBeamArgs* args, void* stream) {
+  VLPK_CHECK_ARG(args, "constrained_beam_step: null argument struct");
+  return launch_constrained_beam_step(*args, S(stream));
+}
+
 int vlpk_colsum(const void* x, int64_t ld, int64_t M, int N, float* out, void* stream) {
   VLPK_CHECK_ARG(x && out, "colsum: null pointer");
   return launch_colsum(x, ld, M, N, out, S(stream));

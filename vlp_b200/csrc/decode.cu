@@ -486,6 +486,260 @@ __global__ void __launch_bounds__(MERGE_THREADS) diverse_beam_merge_kernel(Diver
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Constrained beam search (Anderson et al., EMNLP 2017) of one frame f: K beams in each of S = 2^C constraint states per image, slot
+// s*K + k of image b being beam k of state s.  Two launches; vlpk.h states the semantics.
+//
+// constrained_beam_rows_kernel, one CTA of SAMPLE_THREADS per row (B rows at f = 0, B*S*K after):
+//   history  at f >= 1, hist_out[i] = hist_in[b*S*K + prev_ptr[i]] ‖ prev_wid[i], exactly as beam_ngram_block_kernel, always: the
+//            constraint match reads it whether or not n-grams are blocked.
+//   logp     as diverse_beam_rows_kernel (n-gram and min_len blocks included).
+//   complete each of the image's C*A alternatives a of a constraint j not in the row's state s_i is tested by one thread: w = a[-1]
+//            completes it when the row's last len(a) - 1 words are a[:-1].  The distinct such words, with dest = s_i ∪ the bits they
+//            complete, go to top_w / top_lp / top_dest [row, K + e] (word -1 and dest -1 past the last), and leave the row's word set.
+//   top K    of the remaining words (those whose dest is s_i), by the threshold search of diverse_beam_rows_kernel, in rank order to
+//            top_w / top_lp [row, 0:K].  A completing word's logp is replaced by a value whose order_key is 0, below every real
+//            key; V >= K + C*A keeps at least K words above it.
+// constrained_beam_merge_kernel, one CTA per (state s', image b): the candidates of s' are the top K of its own K rows (at f = 0 the
+//   image's row, if s' is the root state) and every completing entry of the image's rows with dest == s', with cand = logp +
+//   eos_prev * -10000 + score_prev (logp at f = 0); non-finite ones (rows of empty slots) are dropped.  They are staged in dynamic
+//   shared memory in any order; every (parent, word) pair is distinct, so the rank by (cand descending, parent ascending, word
+//   ascending) does not depend on it.  The K first fill slots s'*K .. in rank order, the rest are left empty.
+// Every other word w of a row keeps it in its state, and any such pair outside the row's top K has K pairs of the same row and state
+// ranked strictly ahead of it: the rows' top K plus their completing words hold every pair a state can keep.
+__device__ __forceinline__ int cbs_root_state(const VlpkConstrainedBeamArgs& a, int b) {
+  int s = 0;
+  for (int j = 0; j < a.C; ++j) {
+    bool empty = true;
+    for (int q = 0; q < a.A; ++q) empty &= a.cons[((static_cast<size_t>(b) * a.C + j) * a.A + q) * a.P] == 0;
+    s |= empty ? 1 << j : 0;
+  }
+  return s;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(SAMPLE_THREADS) constrained_beam_rows_kernel(VlpkConstrainedBeamArgs a) {
+  extern __shared__ float cbs_smem[];
+  __shared__ float redf[33];
+  __shared__ int redi[33], prei[SAMPLE_THREADS + 1];
+  __shared__ int sel_w[CBS_MAX_BEAMS];
+  __shared__ float sel_lp[CBS_MAX_BEAMS];
+  constexpr int MAX_CA = CBS_MAX_CONSTRAINTS * CBS_MAX_ALTS;
+  __shared__ int hit[MAX_CA], comp_w[MAX_CA], comp_d[MAX_CA];
+  __shared__ int n_comp;
+  const int V = a.V, K = a.K, tid = threadIdx.x, row = blockIdx.x, f = a.f;
+  const int CA = a.C * a.A, SK = K << a.C, W = K + CA;
+  const int b = f == 0 ? row : row / SK;
+  const int state = f == 0 ? cbs_root_state(a, b) : (row % SK) / K;
+  float* val = cbs_smem;                                             // [V] logp
+  unsigned* bits = reinterpret_cast<unsigned*>(val + V);             // [ceil(V/32)] blocked words
+  int* hist = reinterpret_cast<int*>(bits + ((V + 31) >> 5));        // [T_cap] history
+
+  if (f >= 1) {                                                      // uniform
+    const long long p = f > 1 ? a.prev_ptr[row] : 0;
+    const bool parent_ok = p >= 0 && p < SK;
+    const int* src = a.hist_in + (static_cast<size_t>(b) * SK + (parent_ok ? p : 0)) * a.T_cap;
+    int* dst = a.hist_out + static_cast<size_t>(row) * a.T_cap;
+    for (int t = tid; t < f - 1; t += SAMPLE_THREADS) {
+      const int w = parent_ok ? src[t] : -1;
+      hist[t] = w;
+      dst[t] = w;
+    }
+    if (tid == 0) {
+      const long long w64 = a.prev_wid[row];
+      const int w = (w64 >= INT_MIN && w64 <= INT_MAX) ? static_cast<int>(w64) : -1;
+      hist[f - 1] = w;
+      dst[f - 1] = w;
+    }
+  }
+  __syncthreads();
+  const bool blocked = a.n > 0 && f >= a.n && ngram_candidates(hist, f, a.n, V, a.ignore, a.n_ignore, bits);
+
+  if (tid < CA) {                                                    // alternative tid: constraint tid / A
+    const int64_t* alt = a.cons + (static_cast<size_t>(b) * CA + tid) * a.P;
+    int len = 0;
+    while (len < a.P && alt[len] != 0) ++len;
+    int w = -1;
+    if (len > 0 && len - 1 <= f && !((state >> (tid / a.A)) & 1) && alt[len - 1] >= 0 && alt[len - 1] < V) {
+      bool match = true;
+      for (int t = 0; t < len - 1 && match; ++t) match = hist[f - (len - 1) + t] == alt[t];
+      if (match) w = static_cast<int>(alt[len - 1]);
+    }
+    hit[tid] = w;
+  }
+  __syncthreads();
+  if (tid == 0) {                                                    // distinct completing words in alternative order
+    int m = 0;
+    for (int q = 0; q < CA; ++q) {
+      const int w = hit[q];
+      if (w < 0) continue;
+      int e = 0;
+      while (e < m && comp_w[e] != w) ++e;
+      if (e == m) {
+        comp_w[m] = w;
+        comp_d[m++] = state;
+      }
+      comp_d[e] |= 1 << (q / a.A);
+    }
+    n_comp = m;
+  }
+
+  const T* lrow = static_cast<const T*>(a.logits) + static_cast<size_t>(row) * a.ld;
+  const T* bias = static_cast<const T*>(a.bias);
+  float mx = -INFINITY;
+  for (int v = tid; v < V; v += SAMPLE_THREADS) {
+    const float x = head_logit(lrow, bias, v);
+    val[v] = x;
+    mx = fmaxf(mx, x);
+  }
+  mx = block_reduce(mx, redf, [](float p, float q) { return fmaxf(p, q); });
+
+  // from here on thread t owns words [lo, hi)
+  const int Cw = ((V + SAMPLE_THREADS - 1) / SAMPLE_THREADS) | 1;
+  const int lo = min(tid * Cw, V), hi = min(lo + Cw, V);
+  float z = 0.f;
+  for (int v = lo; v < hi; ++v) z += expf(val[v] - mx);
+  const float lse = logf(block_reduce(z, redf, [](float p, float q) { return p + q; }));
+  for (int v = lo; v < hi; ++v) {
+    float lp = (val[v] - mx) - lse;
+    if (blocked && ((bits[v >> 5] >> (v & 31)) & 1u)) lp += -10000.0f;
+    if (a.block_eos && v == a.eos_id) lp = -10000.0f;
+    val[v] = lp;
+  }
+  __syncthreads();
+  const size_t out = static_cast<size_t>(row) * W;
+  if (tid < CA) {                                                    // completing entries, then out of the top-K search
+    const bool used = tid < n_comp;
+    const int w = used ? comp_w[tid] : -1;
+    a.top_w[out + K + tid] = w;
+    a.top_lp[out + K + tid] = used ? val[w] : -INFINITY;
+    a.top_dest[static_cast<size_t>(row) * CA + tid] = used ? comp_d[tid] : -1;
+    if (used) val[w] = __int_as_float(-1);                         // a NaN whose order_key is 0
+  }
+  __syncthreads();
+  float top = -INFINITY;
+  for (int v = lo; v < hi; ++v) top = fmaxf(top, val[v]);            // fmaxf skips the excluded NaNs
+  top = block_reduce(top, redf, [](float p, float q) { return fmaxf(p, q); });
+
+  // tau = the largest key with at least K words at or above it
+  auto count = [&](unsigned t) {
+    int c = 0;
+    for (int v = lo; v < hi; ++v) c += order_key(val[v]) >= t;
+    return block_reduce(c, redi, [](int p, int q) { return p + q; });
+  };
+  unsigned klo = 0, khi = order_key(top);
+  if (count(khi) >= K) {
+    klo = khi;
+  } else {
+    khi -= 1;
+    while (klo < khi) {                                              // uniform: every thread sees the same counts
+      const unsigned mid = klo + (khi - klo + 1) / 2;
+      if (count(mid) >= K) klo = mid; else khi = mid - 1;
+    }
+  }
+  const unsigned tau = klo;
+  const int take = K - (tau == 0xffffffffu ? 0 : count(tau + 1));   // words tied at tau to keep, lowest index first
+
+  int ties = 0;
+  for (int v = lo; v < hi; ++v) ties += order_key(val[v]) == tau;
+  block_exclusive_scan(ties, redi, prei);
+  const int ties_before = prei[tid];
+  int rank = ties_before, kept = 0;
+  for (int v = lo; v < hi; ++v) {
+    const unsigned k = order_key(val[v]);
+    kept += k > tau || (k == tau && rank++ < take);
+  }
+  block_exclusive_scan(kept, redi, prei);                            // the chunk's first slot among the K kept words
+  int slot = prei[tid];
+  rank = ties_before;
+  for (int v = lo; v < hi; ++v) {
+    const unsigned k = order_key(val[v]);
+    if (k > tau || (k == tau && rank++ < take)) {
+      sel_w[slot] = v;
+      sel_lp[slot] = val[v];
+      ++slot;
+    }
+  }
+  __syncthreads();
+  if (tid < K) {                                                     // rank order: (logp descending, word ascending)
+    const float lp = sel_lp[tid];
+    const unsigned kt = order_key(lp);
+    const int w = sel_w[tid];
+    int r = 0;
+    for (int j = 0; j < K; ++j) {
+      const unsigned kj = order_key(sel_lp[j]);
+      r += kj > kt || (kj == kt && sel_w[j] < w);
+    }
+    a.top_w[out + r] = w;
+    a.top_lp[out + r] = lp;
+  }
+}
+
+size_t cbs_merge_smem_bytes(int K, int C, int A) {                   // one state's candidates at most: value, parent, word
+  return (static_cast<size_t>(K) * K + (static_cast<size_t>(K) << C) * C * A) * 12;
+}
+
+__global__ void __launch_bounds__(MERGE_THREADS) constrained_beam_merge_kernel(VlpkConstrainedBeamArgs a) {
+  extern __shared__ float cbs_smem[];
+  __shared__ int n_cand;
+  const int s = blockIdx.x, b = blockIdx.y, K = a.K, tid = threadIdx.x;
+  const int CA = a.C * a.A, SK = K << a.C, W = K + CA;
+  const bool first = a.f == 0;
+  const int n_stay = first ? (s == cbs_root_state(a, b) ? K : 0) : K * K;     // top-K entries of the state's own rows
+  const int n_all = n_stay + (first ? 1 : SK) * CA;                            // ... then every row's completing entries
+  float* val = cbs_smem;
+  int* par = reinterpret_cast<int*>(val + n_all);
+  int* word = par + n_all;
+  if (tid == 0) n_cand = 0;
+  __syncthreads();
+  for (int c = tid; c < n_all; c += MERGE_THREADS) {
+    int p, e;                                                        // parent slot, entry of its row
+    if (c < n_stay) {
+      p = first ? 0 : s * K + c / K;
+      e = c % K;
+    } else {
+      p = first ? 0 : (c - n_stay) / CA;
+      e = K + (c - n_stay) % CA;
+    }
+    const size_t r = first ? static_cast<size_t>(b) : static_cast<size_t>(b) * SK + p;
+    if (e >= K && a.top_dest[r * CA + (e - K)] != s) continue;
+    const int w = a.top_w[r * W + e];
+    if (w < 0) continue;
+    const float lp = a.top_lp[r * W + e];
+    const float v = first ? lp : lp + a.prev_eos[r] * -10000.0f + a.prev_score[r];
+    if (!isfinite(v)) continue;
+    const int i = atomicAdd(&n_cand, 1);
+    val[i] = v;
+    par[i] = p;
+    word[i] = w;
+  }
+  __syncthreads();
+  const int n = n_cand;
+  const size_t base = static_cast<size_t>(b) * SK + s * K;
+  for (int c = tid; c < n; c += MERGE_THREADS) {
+    const float v = val[c];
+    const int w = word[c], pc = par[c];
+    int r = 0;                                                       // candidates ranked ahead of c; only r < K matters
+    for (int d = 0; d < n && r < K; ++d) {
+      const float u = val[d];
+      const int pd = par[d];
+      r += u > v || (u == v && (pd < pc || (pd == pc && word[d] < w)));
+    }
+    if (r < K) {
+      a.wid[base + r] = w;
+      a.ptr[base + r] = pc;
+      a.score[base + r] = v;
+      a.eos[base + r] = w == a.eos_id ? 1.0f : 0.0f;
+    }
+  }
+  for (int k = n + tid; k < K; k += MERGE_THREADS) {                 // empty slots
+    a.wid[base + k] = 0;
+    a.ptr[base + k] = 0;
+    a.score[base + k] = -INFINITY;
+    a.eos[base + k] = 0.0f;
+  }
+}
+
 }  // namespace
 
 size_t sample_smem_bytes(int T_cap, int V) {
@@ -574,6 +828,63 @@ int launch_diverse_beam_step(const DiverseBeamArgs& a, cudaStream_t s) {
   }
   LaunchScope scope(CAT_MISC, 8.0 * rows * a.K, s);
   diverse_beam_merge_kernel<<<a.B, MERGE_THREADS, 0, s>>>(a);
+  VLPK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int launch_constrained_beam_step(const VlpkConstrainedBeamArgs& a, cudaStream_t s) {
+  VLPK_CHECK_ARG(a.C >= 1 && a.C <= CBS_MAX_CONSTRAINTS && a.A >= 1 && a.A <= CBS_MAX_ALTS && a.P >= 1 && a.P <= CBS_MAX_WORDS,
+                 "constrained_beam_step: C=%d A=%d P=%d (C in [1, %d], A in [1, %d], P in [1, %d])", a.C, a.A, a.P, CBS_MAX_CONSTRAINTS,
+                 CBS_MAX_ALTS, CBS_MAX_WORDS);
+  VLPK_CHECK_ARG(a.B >= 0 && a.K >= 1 && a.K <= CBS_MAX_BEAMS && (a.K << a.C) <= CBS_MAX_SLOTS,
+                 "constrained_beam_step: B=%d K=%d C=%d (K in [1, %d] and 2^C * K <= %d needed)", a.B, a.K, a.C, CBS_MAX_BEAMS, CBS_MAX_SLOTS);
+  VLPK_CHECK_ARG(a.V >= a.K + a.C * a.A && a.ld >= a.V, "constrained_beam_step: V=%d ld=%lld (ld >= V >= K + C*A = %d needed)", a.V,
+                 static_cast<long long>(a.ld), a.K + a.C * a.A);
+  VLPK_CHECK_ARG(a.fp32 == 0 || a.fp32 == 1, "constrained_beam_step: fp32=%d (0 bf16, 1 fp32)", a.fp32);
+  VLPK_CHECK_ARG(a.T_cap >= 1 && a.f >= 0 && a.f < a.T_cap, "constrained_beam_step: frame f=%d outside [0, T_cap=%d)", a.f, a.T_cap);
+  VLPK_CHECK_ARG(a.n >= 0 && a.n_ignore >= 0 && (a.n_ignore == 0 || a.ignore), "constrained_beam_step: n=%d, ignore set of %d words", a.n,
+                 a.n_ignore);
+  VLPK_CHECK_ARG(a.logits && a.cons && a.top_w && a.top_lp && a.top_dest && a.wid && a.ptr && a.score && a.eos,
+                 "constrained_beam_step: null pointer (logits, cons, top_w, top_lp, top_dest, wid, ptr, score, eos)");
+  VLPK_CHECK_ARG(a.f == 0 || (a.prev_score && a.prev_eos && a.prev_wid && a.hist_out),
+                 "constrained_beam_step: null pointer (prev_score, prev_eos, prev_wid, hist_out are needed at f=%d)", a.f);
+  VLPK_CHECK_ARG(a.f <= 1 || (a.hist_in && a.prev_ptr), "constrained_beam_step: null pointer (hist_in, prev_ptr are needed at f=%d)", a.f);
+  VLPK_CHECK_ARG(a.f == 0 || a.hist_in != a.hist_out, "constrained_beam_step: hist_in and hist_out must be different buffers");
+  const size_t smem = sample_smem_bytes(a.T_cap, a.V);
+  VLPK_CHECK_ARG(smem <= SAMPLE_SMEM_MAX, "constrained_beam_step: T_cap=%d V=%d need %zu bytes of shared memory (at most %zu)", a.T_cap,
+                 a.V, smem, SAMPLE_SMEM_MAX);
+  if (a.B == 0) return 0;
+  const int SK = a.K << a.C, rows = a.f == 0 ? a.B : a.B * SK;
+  {
+    LaunchScope scope(CAT_MISC, (a.fp32 ? 8.0 : 4.0) * rows * a.V, s);
+    if (a.fp32) {
+      static bool attr_set = false;
+      if (!attr_set) {
+        VLPK_CUDA(cudaFuncSetAttribute(constrained_beam_rows_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       static_cast<int>(SAMPLE_SMEM_MAX)));
+        attr_set = true;
+      }
+      constrained_beam_rows_kernel<float><<<rows, SAMPLE_THREADS, smem, s>>>(a);
+    } else {
+      static bool attr_set = false;
+      if (!attr_set) {
+        VLPK_CUDA(cudaFuncSetAttribute(constrained_beam_rows_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       static_cast<int>(SAMPLE_SMEM_MAX)));
+        attr_set = true;
+      }
+      constrained_beam_rows_kernel<bf16><<<rows, SAMPLE_THREADS, smem, s>>>(a);
+    }
+    VLPK_CUDA(cudaGetLastError());
+  }
+  const size_t merge_smem = cbs_merge_smem_bytes(a.K, a.C, a.A);
+  static bool attr_set = false;
+  if (!attr_set) {
+    VLPK_CUDA(cudaFuncSetAttribute(constrained_beam_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   static_cast<int>(cbs_merge_smem_bytes(CBS_MAX_BEAMS, 2, CBS_MAX_ALTS))));
+    attr_set = true;
+  }
+  LaunchScope scope(CAT_MISC, 8.0 * rows * (a.K + a.C * a.A), s);
+  constrained_beam_merge_kernel<<<dim3(1 << a.C, a.B), MERGE_THREADS, merge_smem, s>>>(a);
   VLPK_CUDA(cudaGetLastError());
   return 0;
 }

@@ -1,5 +1,6 @@
 // vlp_b200 — beam-search duplicate-n-gram blocking on the device (see decode.cu).
 #pragma once
+#include "../../include/vlpk.h"
 #include "common.cuh"
 
 namespace vlpk {
@@ -86,5 +87,10 @@ struct DiverseBeamArgs {
 };
 
 int launch_diverse_beam_step(const DiverseBeamArgs& a, cudaStream_t s);
+
+// Constrained beam search: one frame's selection, K beams in each of the 2^C constraint states (see decode.cu and vlpk.h).
+constexpr int CBS_MAX_CONSTRAINTS = 4, CBS_MAX_ALTS = 4, CBS_MAX_WORDS = 8, CBS_MAX_BEAMS = 64, CBS_MAX_SLOTS = 256;
+
+int launch_constrained_beam_step(const VlpkConstrainedBeamArgs& a, cudaStream_t s);
 
 }  // namespace vlpk

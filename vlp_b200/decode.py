@@ -15,13 +15,25 @@ PAD_ID = 0
 
 
 def check_decode(sampling_method, topk, topp, beam_size, num_return_sequences=1, forbid_duplicate_ngrams=False, ngram_size=3,
-                 use_kv_cache=True, output_attentions=False, ngram_in_greedy=False, num_beam_groups=1, diversity_penalty=0.0):
+                 use_kv_cache=True, output_attentions=False, ngram_in_greedy=False, num_beam_groups=1, diversity_penalty=0.0,
+                 constraints=False):
     """Raises ValueError, before anything is launched, for decode settings the decoder does not take.  Greedy decode ignores the
-    n-gram settings, so a bad ngram_size is refused for beam search and sampling only, or in every mode with ngram_in_greedy."""
+    n-gram settings, so a bad ngram_size is refused for beam search and sampling only, or in every mode with ngram_in_greedy.
+    constraints: the decode is a constrained beam search (the table itself is checked by check_constraints)."""
     if sampling_method not in SAMPLING_METHODS:
         raise ValueError(f"vlp_b200: sampling_method must be one of {', '.join(SAMPLING_METHODS)}, got {sampling_method!r}")
     sampling = sampling_method != "beam_search"
     check_beam_groups(num_beam_groups, diversity_penalty, sampling_method, beam_size)
+    if constraints:
+        if sampling:
+            raise ValueError(f"vlp_b200: constraints need beam search, got sampling_method={sampling_method!r}")
+        if num_beam_groups != 1:
+            raise ValueError("vlp_b200: constraints do not combine with num_beam_groups > 1 (diverse beam search)")
+        if not use_kv_cache:
+            raise ValueError("vlp_b200: constraints need use_kv_cache (the shared image-prefix cache of every state's beams)")
+        if isinstance(num_return_sequences, int) and num_return_sequences > int(beam_size):
+            raise ValueError(f"vlp_b200: num_return_sequences={num_return_sequences} exceeds the beam size {beam_size} of the accept "
+                             "state")
     if sampling:
         if int(beam_size) != 1:
             raise ValueError(f"vlp_b200: sampling_method={sampling_method!r} needs beam size 1, got {beam_size}")
@@ -69,6 +81,66 @@ def check_beam_groups(num_beam_groups, diversity_penalty, sampling_method, beam_
         raise ValueError(f"vlp_b200: num_beam_groups={G} does not divide the beam size {K}")
     if K > ops.MAX_TOPK:
         raise ValueError(f"vlp_b200: diverse beam search takes beam sizes up to {ops.MAX_TOPK}, got {K}")
+
+
+CONSTRAINT_LIMITS = dict(C=4, A=4, P=8, K=64, slots=256)      # vlpk_constrained_beam_step's limits; slots = 2^C * K
+
+
+def constraint_table(constraints):
+    """The host int64 [1, C, A, P] table of a constraint list shared by every image: constraints[j] is a list of alternatives, each a
+    word id or a list of word ids (a phrase), 0-padded to the longest.  A constraint given as an empty list is met from the start.
+    ValueError for anything else."""
+    msg = "vlp_b200: constraints must be a non-empty list of constraints, each a list of alternatives, each a word id or a list of ids"
+    if isinstance(constraints, (str, bytes)) or not isinstance(constraints, (list, tuple)) or not constraints:
+        raise ValueError(msg)
+    table = []
+    for alts in constraints:
+        if isinstance(alts, (str, bytes)) or not isinstance(alts, (list, tuple)):
+            raise ValueError(msg)
+        rows = []
+        for a in alts:
+            a = [a] if isinstance(a, int) and not isinstance(a, bool) else a
+            if isinstance(a, (str, bytes)) or not isinstance(a, (list, tuple)) or not a \
+                    or any(isinstance(w, bool) or not isinstance(w, int) for w in a):
+                raise ValueError(msg)
+            rows.append(list(a))
+        table.append(rows)
+    A = max(1, max(len(alts) for alts in table))
+    P = max(1, max((len(a) for alts in table for a in alts), default=1))
+    out = torch.zeros(1, len(table), A, P, dtype=torch.int64)
+    for j, alts in enumerate(table):
+        for q, a in enumerate(alts):
+            out[0, j, q, :len(a)] = torch.tensor(a, dtype=torch.int64)
+    return out
+
+
+def check_constraints(cons, vocab_size, beam_size, max_words=None, values=True):
+    """ValueError, before anything is launched, for a constraint table [B, C, A, P] the constrained beam search does not take: sizes
+    past its limits (C <= 4, A <= 4, P <= 8, beam size <= 64 and 2^C * beam size <= 256, vocab >= beam size + C*A); with values, ids
+    outside [0, vocab_size), a 0 inside an alternative (0 is padding), or an alternative longer than max_words (out_len - in_len), read
+    from a host copy of the table."""
+    lim = CONSTRAINT_LIMITS
+    if not torch.is_tensor(cons) or cons.dim() != 4 or cons.dtype != torch.int64:
+        raise ValueError("vlp_b200: constraints must be an int64 tensor [B, C, A, P] (C constraints of A alternatives of P word ids)")
+    _, C, A, P = cons.shape
+    if not (1 <= C <= lim["C"] and 1 <= A <= lim["A"] and 1 <= P <= lim["P"]):
+        raise ValueError(f"vlp_b200: constraints [B, C={C}, A={A}, P={P}] exceed the limits C <= {lim['C']}, A <= {lim['A']}, "
+                         f"P <= {lim['P']}")
+    K = int(beam_size)
+    if not (1 <= K <= lim["K"] and (K << C) <= lim["slots"]):
+        raise ValueError(f"vlp_b200: constrained beam search keeps 2^C * K <= {lim['slots']} hypotheses per image with K <= {lim['K']}; "
+                         f"got C={C}, beam size {K}")
+    if vocab_size < K + C * A:
+        raise ValueError(f"vlp_b200: constrained beam search needs a vocabulary of at least beam size + C*A = {K + C * A} words")
+    if not values:
+        return
+    c = cons.cpu()
+    if bool(((c < 0) | (c >= vocab_size)).any()):
+        raise ValueError(f"vlp_b200: constraint word ids must lie in [0, {vocab_size})")
+    if bool(((c[..., 1:] != 0) & (c[..., :-1] == 0)).any()):
+        raise ValueError("vlp_b200: a constraint alternative has a 0 (padding) before a word id")
+    if max_words is not None and bool(((c != 0).sum(-1) > max_words).any()):
+        raise ValueError(f"vlp_b200: a constraint alternative is longer than the {max_words} words the decode generates")
 
 
 class DecodeState:

@@ -10,7 +10,19 @@ A script that already defines one of these options (decode_img2txt.py has its ow
 import argparse
 
 from . import ops
-from .decode import SAMPLING_METHODS, check_decode
+from .decode import CONSTRAINT_LIMITS, SAMPLING_METHODS, check_decode
+
+
+def constraint_spec(text):
+    """--constraints "dog,dogs|frisbee" -> [["dog", "dogs"], ["frisbee"]]: '|' separates constraints, ',' the alternatives of one;
+    argparse.ArgumentTypeError (a usage error) for an empty constraint or alternative, or more than the search takes."""
+    cons = [[a.strip() for a in c.split(",")] for c in text.split("|")]
+    if any(not a for c in cons for a in c):
+        raise argparse.ArgumentTypeError(f"empty constraint or alternative in {text!r} ('|' separates constraints, ',' alternatives)")
+    if len(cons) > CONSTRAINT_LIMITS["C"] or any(len(c) > CONSTRAINT_LIMITS["A"] for c in cons):
+        raise argparse.ArgumentTypeError(f"at most {CONSTRAINT_LIMITS['C']} constraints of {CONSTRAINT_LIMITS['A']} alternatives, "
+                                         f"got {text!r}")
+    return cons
 
 _OPTIONS = (
     ("--beam_size", dict(type=int, default=1, help="beam size for beam search; 1 = greedy, and required when sampling")),
@@ -30,6 +42,9 @@ _OPTIONS = (
     ("--num_beam_groups", dict(type=int, default=1, help="diverse beam search: split the --beam_size beams into this many groups, "
                                                          "each penalised for words earlier groups chose in the same step")),
     ("--diversity_penalty", dict(type=float, default=0.0, help="diverse beam search: penalty per earlier group's use of a word, >= 0")),
+    ("--constraints", dict(type=constraint_spec, default=None, help="constrained beam search: words or phrases every caption must "
+                                                                   "contain, e.g. 'dog,dogs|frisbee' ('|' separates constraints, "
+                                                                   "',' the alternatives of one)")),
 )
 
 
@@ -47,7 +62,8 @@ def check_decode_args(args):
     """ValueError for a combination BertForSeq2SeqDecoder refuses (raised before any model is built); --ngram_size is checked with
     --forbid_duplicate_ngrams in every mode, greedy included."""
     check_decode(args.sampling_method, args.topk, args.topp, args.beam_size, args.num_return_sequences, args.forbid_duplicate_ngrams,
-                 args.ngram_size, ngram_in_greedy=True, num_beam_groups=args.num_beam_groups, diversity_penalty=args.diversity_penalty)
+                 args.ngram_size, ngram_in_greedy=True, num_beam_groups=args.num_beam_groups, diversity_penalty=args.diversity_penalty,
+                 constraints=getattr(args, "constraints", None) is not None)
 
 
 def parse_decode_args(parser, argv=None):
@@ -62,7 +78,8 @@ def parse_decode_args(parser, argv=None):
 
 def decoder_kwargs(args, tokenizer=None):
     """BertForSeq2SeqDecoder keyword arguments of the parsed options.  tokenizer (convert_tokens_to_ids) maps --forbid_ignore_word
-    to word ids, as decode_img2txt.py does; without one the option must be empty."""
+    to word ids, as decode_img2txt.py does, and tokenizes every --constraints alternative into wordpieces (tokenize, then
+    convert_tokens_to_ids); without one both options must be empty."""
     check_decode_args(args)
     ignore = None
     if args.forbid_ignore_word:
@@ -78,4 +95,8 @@ def decoder_kwargs(args, tokenizer=None):
         kw["num_beam_groups"] = args.num_beam_groups
     if args.diversity_penalty != 0:
         kw["diversity_penalty"] = args.diversity_penalty
+    if getattr(args, "constraints", None) is not None:
+        if tokenizer is None:
+            raise ValueError("vlp_b200: --constraints needs a tokenizer to map its words to wordpiece ids")
+        kw["constraints"] = [[list(tokenizer.convert_tokens_to_ids(tokenizer.tokenize(a))) for a in c] for c in args.constraints]
     return kw

@@ -745,3 +745,66 @@ def diverse_beam_step(logits, bias, f, G, penalty, wid, ptr, score, eos, top_w, 
            float(penalty), int(eos_id), int(bool(block_eos)), T_cap, int(ngram), L.ptr(hist_in if ngram else None),
            L.ptr(hist_out if ngram else None), ignore.data_ptr() if n_ign else None, n_ign, *(L.ptr(t) for t in prev), top_w.data_ptr(),
            top_lp.data_ptr(), wid[f].data_ptr(), ptr[f].data_ptr(), score[f].data_ptr(), eos[f].data_ptr(), L.stream())
+
+
+# ------------------------------------------------------------------------------------------------
+# constrained beam search
+# ------------------------------------------------------------------------------------------------
+def constrained_beam_step(logits, bias, f, cons, wid, ptr, score, eos, top_w, top_lp, top_dest, eos_id, block_eos=False, ngram=0, ignore=None,
+                          hist_in=None, hist_out=None):
+    """The selection of constrained-beam frame f (vlpk_constrained_beam_step): K beams in each of the S = 2^C constraint states of an
+    image.  logits: the head's decoder outputs without its bias, [rows, ..., V] with unit stride in V, bf16 or fp32, rows = B at f = 0
+    and B*S*K after; bias: [V] of the same dtype, or None.  cons: contiguous int64 [B, C, A, P] constraint table.  wid / ptr (int64)
+    and score / eos (fp32): the traces, contiguous [T, B, S*K]; frame f is written and frame f-1 read.  top_w (int32) / top_lp (fp32):
+    contiguous [B*S*K, K + C*A] scratch, top_dest (int32) [B*S*K, C*A].  hist_in / hist_out: the int32 [B*S*K, T_cap] histories of
+    frames f-1 and f, two different tensors used in turn (needed at f >= 1, whatever ngram).  ngram > 0: duplicate-n-gram blocking;
+    ignore: int32 device tensor of exempt word ids, or None.  block_eos: the frame is below min_len."""
+    tensors = ((logits, "logits"), (cons, "constraint table"), (wid, "beam word ids"), (ptr, "beam back pointers"), (score, "beam scores"),
+               (eos, "beam eos flags"), (top_w, "top-K scratch"), (top_lp, "top-K scratch"), (top_dest, "top-K scratch"))
+    extra = ((bias, "logit bias"), (ignore, "n-gram ignore set"), (hist_in, "word history"), (hist_out, "word history"))
+    for t, what in tensors + tuple((t, w) for t, w in extra if t is not None):
+        _require_cuda(t, what)
+    if cons.dim() != 4 or cons.dtype != torch.int64 or not cons.is_contiguous():
+        raise RuntimeError("vlp_b200: the constraint table must be a contiguous int64 [B, C, A, P] tensor")
+    Bc, C, A, P = cons.shape
+    if wid.dim() != 3 or any(t.shape != wid.shape or not t.is_contiguous() for t in (wid, ptr, score, eos)) \
+            or wid.dtype != torch.int64 or ptr.dtype != torch.int64 or score.dtype != torch.float32 or eos.dtype != torch.float32:
+        raise RuntimeError("vlp_b200: beam traces must be contiguous [T, B, S*K] tensors: int64 word ids and pointers, fp32 scores and "
+                           "eos flags")
+    T, B, SK = wid.shape
+    if Bc != B or C < 1 or SK % (1 << C):
+        raise RuntimeError(f"vlp_b200: a constraint table [{Bc}, {C}, ...] does not match traces of {B} images and {SK} slots "
+                           "(2^C states of K beams)")
+    K = SK >> C
+    if not 0 <= f < T:
+        raise ValueError(f"vlp_b200: frame {f} outside the traces' {T} frames")
+    V = logits.shape[-1]
+    lg = logits.reshape(-1, V) if logits.dim() != 2 else logits
+    if logits.dtype not in (BF16, torch.float32) or lg.stride(1) != 1 or lg.shape[0] != (B if f == 0 else B * SK):
+        raise RuntimeError("vlp_b200: constrained-beam logits must be bf16 or fp32 [rows, V] with unit column stride, rows = B at frame 0 "
+                           "and B*S*K after")
+    if bias is not None and (bias.dtype != logits.dtype or bias.shape != (V,) or not bias.is_contiguous()):
+        raise RuntimeError("vlp_b200: the logit bias must be a contiguous [V] tensor of the logits' dtype")
+    W = K + C * A
+    if top_w.dtype != torch.int32 or top_lp.dtype != torch.float32 or top_dest.dtype != torch.int32 or top_w.shape != (B * SK, W) \
+            or top_lp.shape != (B * SK, W) or top_dest.shape != (B * SK, C * A) \
+            or not (top_w.is_contiguous() and top_lp.is_contiguous() and top_dest.is_contiguous()):
+        raise RuntimeError("vlp_b200: the top-K scratch must be contiguous int32 / fp32 [B*S*K, K + C*A] and int32 [B*S*K, C*A] tensors")
+    T_cap = T
+    if hist_out is not None or f:
+        if hist_in is None or hist_out is None or hist_in.shape != hist_out.shape or hist_out.dim() != 2 or hist_out.shape[0] != B * SK \
+                or hist_in.dtype != torch.int32 or hist_out.dtype != torch.int32 or not (hist_in.is_contiguous() and hist_out.is_contiguous()):
+            raise RuntimeError("vlp_b200: word histories must be two contiguous int32 [B*S*K, T_cap] tensors")
+        T_cap = hist_out.shape[1]
+    if ignore is not None and (ignore.dtype != torch.int32 or ignore.dim() != 1 or not ignore.is_contiguous()):
+        raise RuntimeError("vlp_b200: the n-gram ignore set must be a contiguous 1-D int32 tensor of word ids")
+    n_ign = 0 if ignore is None or not ngram else ignore.numel()
+    prev = (wid[f - 1], ptr[f - 1], score[f - 1], eos[f - 1]) if f else (None,) * 4
+    a = L.VlpkConstrainedBeamArgs(B=B, K=K, C=C, A=A, P=P, f=int(f), V=V, logits=lg.data_ptr(), ld=lg.stride(0), bias=L.ptr(bias),
+                                  fp32=int(logits.dtype == torch.float32), eos_id=int(eos_id), block_eos=int(bool(block_eos)), T_cap=T_cap,
+                                  n=int(ngram), hist_in=L.ptr(hist_in), hist_out=L.ptr(hist_out),
+                                  ignore=ignore.data_ptr() if n_ign else None, n_ignore=n_ign, cons=cons.data_ptr(),
+                                  prev_wid=L.ptr(prev[0]), prev_ptr=L.ptr(prev[1]), prev_score=L.ptr(prev[2]), prev_eos=L.ptr(prev[3]),
+                                  top_w=top_w.data_ptr(), top_lp=top_lp.data_ptr(), top_dest=top_dest.data_ptr(), wid=wid[f].data_ptr(),
+                                  ptr=ptr[f].data_ptr(), score=score[f].data_ptr(), eos=eos[f].data_ptr())
+    L.call("vlpk_constrained_beam_step", L.C.byref(a), L.stream())

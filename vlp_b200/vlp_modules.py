@@ -22,8 +22,8 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import ops
-from .beam import beam_search, diverse_beam_search
-from .decode import check_decode, greedy_decode, sample_decode
+from .beam import beam_search, constrained_beam_search, diverse_beam_search
+from .decode import check_constraints, check_decode, constraint_table, greedy_decode, sample_decode
 from .score import score_caption_matrix, score_captions
 
 logger = logging.getLogger(__name__)
@@ -832,7 +832,7 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
 
     def __init__(self, config, mask_word_id=0, num_labels=2, search_beam_size=1, length_penalty=1.0, eos_id=0, forbid_duplicate_ngrams=False,
                  forbid_ignore_set=None, ngram_size=3, min_len=0, enable_butd=False, len_vis_input=49, sampling_method="beam_search", topk=1,
-                 topp=1.0, seed=0, num_return_sequences=1, num_beam_groups=1, diversity_penalty=0.0):
+                 topp=1.0, seed=0, num_return_sequences=1, num_beam_groups=1, diversity_penalty=0.0, constraints=None):
         super().__init__(config)
         self.bert = BertModelIncr(config)
         self.cls = BertPreTrainingHeads(config, self.bert.embeddings.word_embeddings.weight, num_labels=num_labels)
@@ -852,8 +852,13 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         # N > 1: N captions per image (beam search's N best hypotheses, or N samples) over one K/V cache of the image prefix.
         # forward checks every decode setting again, the n-gram settings included, since callers may change these attributes.
         # G > 1: diverse beam search, the K beams in G groups of K / G with a Hamming penalty (beam.diverse_beam_search).
+        # constraints: constrained beam search (beam.constrained_beam_search) with these word-id lists for every image: constraints[j]
+        # is a list of alternatives, each a word id or a list of ids; forward's `constraints` tensor overrides them per call.
         check_decode(sampling_method, topk, topp, search_beam_size, num_return_sequences, num_beam_groups=num_beam_groups,
-                     diversity_penalty=diversity_penalty)
+                     diversity_penalty=diversity_penalty, constraints=constraints is not None)
+        self.constraints = None if constraints is None else constraint_table(constraints)
+        if self.constraints is not None:
+            check_constraints(self.constraints, config.vocab_size, search_beam_size)
         self.sampling_method, self.topk, self.topp, self.seed = sampling_method, topk, topp, seed
         self.num_return_sequences = num_return_sequences
         self.num_beam_groups, self.diversity_penalty = num_beam_groups, diversity_penalty
@@ -866,7 +871,7 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         return [torch.empty(batch, rows, 2 * H, device=device, dtype=torch.bfloat16) for _ in self.bert.encoder.layer]
 
     def forward(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, sample_mode="greedy",
-                seed=None, output_attentions=False):
+                seed=None, output_attentions=False, constraints=None):
         """seed: the sampling seed of this call (sampling_method "topk" / "topp"); None uses self.seed.
         output_attentions: greedy / sample / top-k / top-p decode return (ids, scores, attentions) and beam search adds
         out["attentions"]: fp32 [B, out_len - in_len, layers, heads, out_len], for every output word the attention probabilities of the
@@ -874,22 +879,48 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         num_return_sequences N > 1: beam search adds out["nbest_seq"] int64 [B, N, out_len] and out["nbest_scores"] fp32 [B, N];
         top-k / top-p sampling returns ids and scores [B, N, out_len - in_len].
         num_beam_groups G > 1: diverse beam search, whose out also holds each group's best caption, out["group_seq"] int64
-        [B, G, out_len] and out["group_scores"] fp32 [B, G]."""
+        [B, G, out_len] and out["group_scores"] fp32 [B, G].
+        constraints: int64 [B, C, A, P] (or [1, C, A, P] for every image), 0-padded word ids, this call's constraints in place of
+        the constructor's: constrained beam search, whose out also holds out["constraints_met"] bool [B], out["state_seq"] int64
+        [B, 2^C, out_len] and out["state_scores"] fp32 [B, 2^C] (beam.constrained_beam_search).  A device tensor's ids are checked
+        from a host copy, except while a CUDA graph is being captured."""
         self.cls.predictions.check_task_idx(task_idx)          # before anything is launched
         _check_seq_len(self.config, token_type_ids.size(1))
+        cons = self.constraints if constraints is None else constraints
         check_decode(self.sampling_method, self.topk, self.topp, self.search_beam_size, self.num_return_sequences,
                      self.forbid_duplicate_ngrams, self.ngram_size, self.use_kv_cache, output_attentions,
-                     num_beam_groups=self.num_beam_groups, diversity_penalty=self.diversity_penalty)
+                     num_beam_groups=self.num_beam_groups, diversity_penalty=self.diversity_penalty, constraints=cons is not None)
+        if cons is not None:
+            cons = self._constraint_tensor(cons, constraints is None, input_ids, token_type_ids.size(1) - input_ids.size(1))
         with torch.no_grad():
             vis_feats, vis_pe = self.project_regions(vis_feats, vis_pe)
             inputs = (self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx)
             if self.sampling_method != "beam_search":
                 return sample_decode(*inputs, seed, output_attentions=output_attentions)
+            if cons is not None:
+                return constrained_beam_search(*inputs[:-1], cons, task_idx, output_attentions=output_attentions)
             if self.num_beam_groups > 1:
                 return diverse_beam_search(*inputs, output_attentions=output_attentions)
             if self.search_beam_size > 1:
                 return beam_search(*inputs, output_attentions=output_attentions)
             return greedy_decode(*inputs, sample_mode, output_attentions=output_attentions)
+
+    def _constraint_tensor(self, cons, shared, input_ids, max_words):
+        """Checks a constraint table and returns it as a contiguous int64 [B, C, A, P] tensor on the decode's device.  The
+        constructor's table (shared) is copied to each device once and kept, as the n-gram ignore set is, so a CUDA graph captured
+        after a first call makes no host-to-device copy."""
+        B, dev = input_ids.size(0), input_ids.device
+        capturing = dev.type == "cuda" and torch.cuda.is_current_stream_capturing()
+        check_constraints(cons, self.config.vocab_size, self.search_beam_size, max_words, values=not capturing)
+        if cons.size(0) not in (1, B):
+            raise ValueError(f"vlp_b200: constraints for {cons.size(0)} images, the batch has {B}")
+        if shared:
+            cache = self.__dict__.setdefault("_constraint_cache", {})
+            key = (str(dev), tuple(cons.flatten().tolist()), tuple(cons.shape))
+            if key not in cache:
+                cache[key] = cons.to(dev)
+            cons = cache[key]
+        return cons.to(dev).expand(B, *cons.shape[1:]).contiguous()
 
     def score_captions(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, caption_ids, task_idx=None):
         """log p(c_t | image, c_<t) of given captions in one teacher-forced pass (score.score_captions): the decoder's own input tuple,
