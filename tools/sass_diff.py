@@ -20,7 +20,9 @@ def kernels(path):
                 ks[cur] = hashlib.md5("\n".join(buf).encode()).hexdigest()
             cur, buf = m.group(1), []
         elif cur and "/*" in line:
-            buf.append(re.sub(r"/\*[0-9a-fx]+\*/", "", line).strip())     # instruction text without addresses / encodings
+            # instruction text without addresses / encodings; cuobjdump pads every line to the widest instruction of the whole
+            # dump, so the padding changes with any kernel and is collapsed
+            buf.append(" ".join(re.sub(r"/\*[^*]*\*/", " ", line).split()))
     if cur:
         ks[cur] = hashlib.md5("\n".join(buf).encode()).hexdigest()
     # anonymous-namespace prefixes carry a per-file hash

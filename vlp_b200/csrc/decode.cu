@@ -283,13 +283,26 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
     for (int v = lo; v < hi; ++v) {
       const unsigned k = key(v);
       if (!(k > tau || (k == tau && rank++ < take))) continue;
-      found = v;                                                     // the last kept word, should rounding leave goal above acc
-      acc += weight(v);
-      if (goal < acc) break;
+      const float w = weight(v);                                     // found: the last kept word of positive weight, should rounding
+      if (w > 0.f) found = v;                                        // leave goal above acc (top-k keeps words whose e underflows)
+      if (goal < (acc += w)) break;
     }
   }
   int pick = block_reduce(found, redi, [](int p, int q) { return min(p, q); });
-  if (pick == INT_MAX) {                                              // goal fell outside every chunk (rounding): first argmax
+  if (pick == INT_MAX) {
+    // No walked chunk drew: the scan's prefixes pref[t] and pref[t + 1] are summed in different orders, so goal can fall in a chunk
+    // whose kept weight is 0, or in none.  Take the last kept word of positive weight in the chunks that start at or before goal.
+    int last = -1;
+    if (pref[tid] <= goal) {
+      rank = prei[tid];
+      for (int v = lo; v < hi; ++v) {
+        const unsigned k = key(v);
+        if ((k > tau || (k == tau && rank++ < take)) && weight(v) > 0.f) last = v;
+      }
+    }
+    pick = block_reduce(last, redi, [](int p, int q) { return max(p, q); });
+  }
+  if (pick < 0) {                                                     // non-finite sums: the first argmax
     int first = INT_MAX;
     for (int v = lo; v < hi && first == INT_MAX; ++v) if (val[v] == (topp ? 1.0f : mx)) first = v;
     pick = block_reduce(first, redi, [](int p, int q) { return min(p, q); });
