@@ -141,6 +141,12 @@ int vlpk_mask_pack(const void* mask, int dtype, int mode, int B, int rows, int k
  * mode[b] (0 = bidirectional, 1 = seq2seq), L <= 512.  Output: [B, L, S / 32] u32, the packed bitmask vlpk_mask_pack would produce
  * from the loader's matrix. */
 int vlpk_mask_synth(const int32_t* len_b, const int32_t* mode, int len_a, int B, int L, uint32_t* out, void* stream);
+/* Several seq2seq captions per image in one packed sequence: B images, G captions each, pair p = b * G + g with len_b[p] text tokens
+ * and an L-row sample of P = len_a + 2 prefix rows and T = L - P text rows.  Image b's packed sequence has L' = P + G * T rows: the
+ * shared prefix, then each pair's T text rows.  Output: [B, L', S' / 32] u32, S' = 128 * ceil(L' / 128); each caption's rows see the
+ * prefix and, as in vlpk_mask_synth's seq2seq mask, their own caption's text up to themselves; no row sees another caption's text.
+ * Returns < 0 with nothing launched for G < 1, L' > 512, a NULL pointer or an out not 16-byte aligned. */
+int vlpk_mask_synth_grouped(const int32_t* len_b, int G, int len_a, int B, int T, uint32_t* out, void* stream);
 
 /* y[M,N] = dropout(act(x[M,K] w[N,K]^T + b)) — vis_embed / vis_pe_embed Linears (modeling.py:1003-1018, 1035-1036).
  * K need not be tile aligned but ldx/ldw (elements) must be multiples of 8. */

@@ -71,6 +71,7 @@ _SIGS = {
     "vlpk_debug_plan_gemm": (c_int, [c_int] * 10 + [C.POINTER(c_int)]),
     "vlpk_mask_pack": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_i64, c_i64, _P, _P]),
     "vlpk_mask_synth": (c_int, [_P, _P, c_int, c_int, c_int, _P, _P]),
+    "vlpk_mask_synth_grouped": (c_int, [_P, c_int, c_int, c_int, c_int, _P, _P]),
     "vlpk_linear_fwd": (c_int, [c_int, c_int, c_int, _P, c_i64, _P, c_i64, _P, _P, c_i64, c_int, C.POINTER(VlpkDropout), c_u64, _P]),
     "vlpk_linear_bwd": (c_int, [c_int, c_int, c_int, _P, c_i64, _P, c_i64, _P, c_i64, _P, c_i64, _P, _P, c_i64, _P, c_i64, _P,
                                 c_int, c_float, _P]),

@@ -497,6 +497,10 @@ int vlpk_mask_synth(const int32_t* len_b, const int32_t* mode, int len_a, int B,
   return launch_mask_synth(len_b, mode, len_a, B, L, out, S(stream));
 }
 
+int vlpk_mask_synth_grouped(const int32_t* len_b, int G, int len_a, int B, int T, uint32_t* out, void* stream) {
+  return launch_mask_synth_grouped(len_b, G, len_a, B, T, out, S(stream));
+}
+
 int vlpk_linear_fwd(int M, int N, int K, const void* x, int64_t ldx, const void* w, int64_t ldw, const void* bias, void* y, int64_t ldy,
                     int act, const VlpkDropout* drop, uint64_t site, void* stream) {
   VLPK_CHECK_ARG(x && w && y, "linear_fwd: null pointer");

@@ -632,6 +632,50 @@ int launch_mask_synth(const int* len_b, const int* mode, int len_a, int B, int L
   return 0;
 }
 
+// The packed seq2seq mask of G captions per image: one sequence of Lp = P + G * T rows per image, P = len_a + 2 prefix rows shared by
+// the image's G pairs, then the T text rows of each pair in turn (pair b * G + g has len_b[b * G + g] text tokens).  Per caption it
+// is mask_synth's seq2seq rule, with no text key of another caption:
+//   prefix row                  : columns [0, P)
+//   text row j < nt of caption g : columns [0, P) and [P + g * T, P + g * T + j]   (nt = min(len_b + 1, T): the text and its [SEP])
+//   padding row of caption g     : columns [0, P)
+// At G = 1 this is mask_synth's s2s mask bit for bit.  Rows have ceil(Lp / 128) chunks of 4 words.
+__global__ void __launch_bounds__(256) mask_synth_grouped_kernel(const int* __restrict__ len_b, int G, int len_a, int B, int T, int Lp,
+                                                                  int chunks, uint32_t* __restrict__ out) {
+  const long long idx = static_cast<long long>(blockIdx.x) * 8 + (threadIdx.x >> 5);
+  if (idx >= static_cast<long long>(B) * Lp) return;  // warp-uniform
+  const int lane = threadIdx.x & 31;
+  const int b = static_cast<int>(idx / Lp), r = static_cast<int>(idx % Lp);
+  const int P = len_a + 2;
+  int lo = 0, hi = -1;  // text keys [lo, hi] of this row
+  if (r >= P) {
+    const int g = (r - P) / T, t = (r - P) % T;
+    if (t < min(len_b[b * G + g] + 1, T)) lo = P + g * T, hi = r;
+  }
+  for (int c = 0; c < chunks; ++c) {
+    uint32_t w[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int j = 128 * c + lane + 32 * i;
+      w[i] = __ballot_sync(0xffffffffu, j < P || (j >= lo && j <= hi));
+    }
+    if (lane == 0) reinterpret_cast<uint4*>(out)[idx * chunks + c] = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
+int launch_mask_synth_grouped(const int* len_b, int G, int len_a, int B, int T, uint32_t* out, cudaStream_t s) {
+  VLPK_CHECK_ARG(len_b != nullptr && out != nullptr, "mask_synth_grouped: null pointer");
+  VLPK_CHECK_ARG(G >= 1 && B > 0 && T >= 1 && len_a >= 0, "mask_synth_grouped: G=%d B=%d T=%d len_a=%d", G, B, T, len_a);
+  const long long Lp = len_a + 2 + static_cast<long long>(G) * T;
+  VLPK_CHECK_ARG(Lp <= MASK_MAX_KV, "mask_synth_grouped: packed length %lld = len_a + 2 + G * T exceeds 512", Lp);
+  VLPK_CHECK_ARG(!misaligned(out, 15), "mask_synth_grouped: the bitmask buffer must be 16-byte aligned");
+  const long long n = static_cast<long long>(B) * Lp;
+  LaunchScope scope(CAT_MISC, 0.0, s);
+  mask_synth_grouped_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(len_b, G, len_a, B, T, static_cast<int>(Lp),
+                                                                               static_cast<int>((Lp + 127) / 128), out);
+  VLPK_CUDA(cudaGetLastError());
+  return 0;
+}
+
 // ------------------------------------------------------------------------------------------------
 // column sums (bias gradients) and fp32 -> bf16 conversion
 // ------------------------------------------------------------------------------------------------

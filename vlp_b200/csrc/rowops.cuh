@@ -64,6 +64,7 @@ int launch_embed_bwd(const EmbedArgs& a, cudaStream_t s);
 int launch_mask_pack(const void* mask, int dtype, int mode, int B, int rows, int kv, long long stride_b, long long stride_r,
                      uint32_t* out, cudaStream_t s);
 int launch_mask_synth(const int* len_b, const int* mode, int len_a, int B, int L, uint32_t* out, cudaStream_t s);
+int launch_mask_synth_grouped(const int* len_b, int G, int len_a, int B, int T, uint32_t* out, cudaStream_t s);
 int launch_colsum(const void* x, long long ld, long long M, int N, float* out, cudaStream_t s);
 // out[i] += sum_{p < parts} part[p * n + i], in the order p = 0, 1, ... (the same bits on every run)
 int launch_sum_parts(const float* part, int parts, long long n, float* out, cudaStream_t s);

@@ -27,7 +27,7 @@ import torch
 
 from . import _lib as L
 from . import ops
-from .staging import PackedAttentionMask
+from .staging import GroupedCaptionMask, PackedAttentionMask
 
 
 class GraphedStep:
@@ -41,6 +41,8 @@ class GraphedStep:
         for k, v in example_batch.items():
             if isinstance(v, PackedAttentionMask):
                 self.static[k] = PackedAttentionMask(v.bits.clone(), v.L)
+            elif isinstance(v, GroupedCaptionMask):
+                self.static[k] = GroupedCaptionMask(v.bits.clone(), v.G, v.T, v.len_a, v.L)
             elif torch.is_tensor(v) and v.is_cuda:
                 self.static[k] = v.clone()
         if ops._seed_dev is None:
@@ -75,6 +77,11 @@ class GraphedStep:
             if isinstance(dst, PackedAttentionMask):
                 if not isinstance(src, PackedAttentionMask):
                     raise RuntimeError(f"vlp_b200.graph: '{k}' was captured as a PackedAttentionMask")
+                dst.bits.copy_(src.bits, non_blocking=True)
+            elif isinstance(dst, GroupedCaptionMask):
+                if not isinstance(src, GroupedCaptionMask) or (src.G, src.T, src.len_a) != (dst.G, dst.T, dst.len_a):
+                    raise RuntimeError(f"vlp_b200.graph: '{k}' was captured as a GroupedCaptionMask of G={dst.G}, T={dst.T}, "
+                                       f"len_a={dst.len_a}")
                 dst.bits.copy_(src.bits, non_blocking=True)
             elif src.data_ptr() != dst.data_ptr():
                 dst.copy_(src, non_blocking=True)

@@ -85,6 +85,74 @@ class PackedAttentionMask:
         return cls(bits, L_)
 
 
+class GroupedCaptionMask:
+    """The packed self-attention mask of G seq2seq captions per image (vlpk_mask_synth_grouped): int32 [B, L', S' / 32] for B images,
+    L' = P + G * T with P = len_a + 2 prefix rows shared by the image's captions and T = L - P text rows per caption.  Passed as
+    `attention_mask` with `captions_per_image=G` to BertForPreTrainingLossMask.forward."""
+
+    def __init__(self, bits, G, T, len_a, L_):
+        self._vlpk_bits = bits
+        self.G, self.T, self.len_a, self.L = int(G), int(T), int(len_a), int(L_)
+
+    @property
+    def bits(self):
+        return self._vlpk_bits
+
+    @property
+    def packed_len(self):
+        return self.len_a + 2 + self.G * self.T
+
+    @property
+    def is_cuda(self):
+        return self._vlpk_bits.is_cuda
+
+    @property
+    def device(self):
+        return self._vlpk_bits.device
+
+    def dim(self):
+        return 3
+
+    @staticmethod
+    def check(G, len_a, L_):
+        """(T, L') of G captions of L-row samples with len_a regions; ValueError when G < 1 or L' exceeds ops.MAX_SEQ."""
+        G, len_a, L_ = int(G), int(len_a), int(L_)
+        T = L_ - len_a - 2
+        if G < 1 or T < 1 or len_a < 0:
+            raise ValueError(f"vlp_b200: captions_per_image={G} with len_a={len_a}, L={L_} describes no packed sequence")
+        Lp = len_a + 2 + G * T
+        if Lp > ops.MAX_SEQ:
+            raise ValueError(f"vlp_b200: {G} captions per image pack to {Lp} rows; the attention kernels take up to {ops.MAX_SEQ}")
+        return T, Lp
+
+    @classmethod
+    def synthesize(cls, len_b, G, len_a, L_, out=None):
+        """len_b: int32 CUDA tensor [B * G], the text tokens of pair b * G + g.  One kernel launch."""
+        ops._require_cuda(len_b, "len_b")
+        if not (len_b.dtype == torch.int32 and len_b.dim() == 1):
+            raise RuntimeError("vlp_b200.staging: len_b must be a 1-d int32 CUDA tensor")
+        T, Lp = cls.check(G, len_a, L_)
+        if len_b.numel() == 0 or len_b.numel() % int(G):
+            raise ValueError(f"vlp_b200.staging: {len_b.numel()} pairs do not form whole images of {G} captions")
+        B = len_b.numel() // int(G)
+        shape = (B, Lp, ops.key_slots(Lp) // 32)
+        if out is not None and not (tuple(out.shape) == shape and out.dtype == torch.int32 and out.is_cuda and out.is_contiguous()):
+            raise ValueError(f"vlp_b200.staging: out must be a contiguous int32 CUDA tensor of shape {shape}")
+        bits = out if out is not None else torch.empty(shape, device=len_b.device, dtype=torch.int32)
+        L.call("vlpk_mask_synth_grouped", len_b.contiguous().data_ptr(), int(G), int(len_a), B, T, bits.data_ptr(), L.stream())
+        return cls(bits, G, T, len_a, L_)
+
+    @classmethod
+    def from_pair_masks(cls, input_mask, G, len_a):
+        """The loader's [B * G, L, L] 0/1 masks (host or device) of B images x G seq2seq pairs -> the packed mask, via describe_mask.
+        ValueError if any pair is bidirectional: its prefix rows see its text, so it cannot share a prefix."""
+        len_b, s2s = describe_mask(input_mask.cpu(), len_a)
+        if not bool(s2s.all()):
+            raise ValueError("vlp_b200: only seq2seq pairs can share an image prefix; the batch holds a bidirectional pair")
+        dev = input_mask.device if input_mask.is_cuda else torch.device("cuda", torch.cuda.current_device())
+        return cls.synthesize(len_b.to(dev), G, len_a, input_mask.shape[-1])
+
+
 class BatchStager:
     """Pinned, `depth`-deep host->device staging of training batches.
 
@@ -96,10 +164,18 @@ class BatchStager:
             loss = model(b["img"], b["vis_pe"], b["input_ids"], b["segment_ids"], b["input_mask"], ...)   # carried len_b / mode
 
     Host batches may carry either "input_mask" (the loader's int64 matrix: copied as is, 121 KB per sample) or "len_b" + "mode"
-    (int32 [B]: the mask is synthesised on the device).  Features are staged in `feature_dtype`."""
+    (int32 [B]: the mask is synthesised on the device).  Features are staged in `feature_dtype`.
 
-    def __init__(self, device, len_vis_input=100, max_len=123, feature_dtype=BF16, depth=2):
+    captions_per_image=G > 1: batches of B images x G seq2seq captions for BertForPreTrainingLossMask(..., captions_per_image=G).
+    "img" / "vis_pe" have B rows, the text fields B * G rows (pair b * G + g is image b's caption g), and either "len_b" (int32
+    [B * G], with "mode" if the loader gives it) or the loader's "input_mask" matrices (read on the host through describe_mask, not
+    copied); a bidirectional pair is refused with ValueError.  b["input_mask"] is a GroupedCaptionMask."""
+
+    def __init__(self, device, len_vis_input=100, max_len=123, feature_dtype=BF16, depth=2, captions_per_image=1):
         self.device = torch.device(device)
+        self.G = int(captions_per_image)
+        if self.G > 1:
+            GroupedCaptionMask.check(self.G, len_vis_input, max_len)
         self.len_a, self.max_len, self.fdt, self.depth = int(len_vis_input), int(max_len), feature_dtype, int(depth)
         self.copy_stream = torch.cuda.Stream(device=self.device)
         self._slots = [None] * self.depth            # pinned host mirrors, allocated on first use per slot
@@ -120,6 +196,19 @@ class BatchStager:
         if self._put - self._got >= self.depth:
             raise RuntimeError("BatchStager: all slots in flight; call get() first")
         hb = self._as_dict(batch)
+        if self.G > 1:
+            hb = dict(hb)
+            if "input_mask" in hb:                   # the loader's matrices: their (len_b, mode), checked like from_pair_masks
+                len_b, s2s = describe_mask(torch.as_tensor(hb.pop("input_mask")), self.len_a)
+                if not bool(s2s.all()):
+                    raise ValueError("BatchStager: only seq2seq pairs can share an image prefix; the batch holds a bidirectional pair")
+                if "len_b" in hb and not torch.equal(torch.as_tensor(hb["len_b"]).to(torch.int32), len_b):
+                    raise ValueError("BatchStager: len_b disagrees with the text lengths of input_mask")
+                hb["len_b"] = len_b
+            if "len_b" not in hb:
+                raise ValueError("BatchStager: captions_per_image > 1 needs len_b (int32 [B * G]) or input_mask in every batch")
+            if "mode" in hb and not bool((torch.as_tensor(hb.pop("mode")) == 1).all()):
+                raise ValueError("BatchStager: only seq2seq pairs can share an image prefix; the batch holds a bidirectional pair")
         s = self._put % self.depth
         self._put += 1
         pinned = self._slots[s]
@@ -143,7 +232,9 @@ class BatchStager:
         with torch.cuda.stream(self.copy_stream):
             self.copy_stream.wait_event(self._consumed[s])       # the previous occupant of this slot has been consumed
             dev = {k: v.to(self.device, non_blocking=True) for k, v in staged.items()}
-            if "input_mask" not in dev:
+            if self.G > 1:
+                dev["input_mask"] = GroupedCaptionMask.synthesize(dev["len_b"], self.G, self.len_a, self.max_len)
+            elif "input_mask" not in dev:
                 dev["input_mask"] = PackedAttentionMask.synthesize(dev["len_b"], dev["mode"], self.len_a, self.max_len)
             self._ready[s].record(self.copy_stream)
         self._dev[s] = dev
@@ -169,7 +260,7 @@ class BatchStager:
         cur.wait_event(self._ready[s])
         dev = self._dev[s]
         for v in dev.values():                        # the caching allocator must not recycle these before the compute stream is done
-            t = v.bits if isinstance(v, PackedAttentionMask) else v
+            t = v.bits if isinstance(v, (PackedAttentionMask, GroupedCaptionMask)) else v
             t.record_stream(cur)
         return _Staged(dev, self._consumed[s], cur)
 

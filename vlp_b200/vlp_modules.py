@@ -22,6 +22,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import ops
+from .staging import GroupedCaptionMask
 from .beam import beam_search, constrained_beam_search, diverse_beam_search
 from .decode import check_constraints, check_decode, constraint_table, greedy_decode, sample_decode
 from .score import score_caption_matrix, score_captions
@@ -127,12 +128,13 @@ class BertLayerNorm(nn.Module):
         return F.layer_norm(x, (x.shape[-1],), self.weight, self.bias, self.variance_epsilon)
 
 
-def _check_seq_len(config, L):
+def _check_seq_len(config, L, positions=True):
     """Sequence lengths the model takes, checked before anything is launched: the attention kernels stop at ops.MAX_SEQ (512) and
-    the position table at max_position_embeddings (the reference fails there with an index error)."""
+    the position table at max_position_embeddings (the reference fails there with an index error).  positions=False: the rows carry
+    explicit positions that their caller has checked, so only the attention limit applies."""
     if L > ops.MAX_SEQ:
         raise ValueError(f"vlp_b200: sequence length {L} exceeds {ops.MAX_SEQ}, the longest the attention kernels take")
-    if L > config.max_position_embeddings:
+    if positions and L > config.max_position_embeddings:
         raise ValueError(f"vlp_b200: sequence length {L} exceeds max_position_embeddings {config.max_position_embeddings}")
 
 
@@ -596,12 +598,14 @@ class BertModel(PreTrainedBertModel):
         return ext
 
     def forward(self, vis_feats, vis_pe, input_ids, token_type_ids=None, attention_mask=None, output_all_encoded_layers=True, len_vis_input=49,
-                output_attentions=False):
+                output_attentions=False, position_ids=None):
         """output_attentions=True returns (encoded_layers, pooled_output, attentions): one fp32 [B, heads, L, L] map per layer, the
-        reference's attention_probs before dropout (what a forward hook on its attention.self.dropout receives)."""
-        _check_seq_len(self.config, input_ids.size(1))
+        reference's attention_probs before dropout (what a forward hook on its attention.self.dropout receives).
+        position_ids: int64 [B, L] position of every row (None: 0 .. L - 1), as packed captions per image use it; the caller keeps
+        them below max_position_embeddings."""
+        _check_seq_len(self.config, input_ids.size(1), positions=position_ids is None)
         ext = self.get_extended_attention_mask(input_ids, token_type_ids, attention_mask)
-        embedding_output = self.embeddings(vis_feats, vis_pe, input_ids, token_type_ids, len_vis_input=len_vis_input)
+        embedding_output = self.embeddings(vis_feats, vis_pe, input_ids, token_type_ids, position_ids, len_vis_input=len_vis_input)
         encoded_layers = self.encoder(embedding_output, ext, output_all_encoded_layers=output_all_encoded_layers,
                                       output_attentions=bool(output_attentions))
         if output_attentions:
@@ -751,11 +755,22 @@ class BertForPreTrainingLossMask(PreTrainedBertModel, _RegionProjections):
 
     def forward(self, vis_feats, vis_pe, input_ids, token_type_ids=None, attention_mask=None, masked_lm_labels=None, ans_labels=None,
                 next_sentence_label=None, masked_pos=None, masked_weights=None, task_idx=None, vis_masked_pos=[], mask_image_regions=False,
-                drop_worst_ratio=0.2, vqa_inference=False):
+                drop_worst_ratio=0.2, vqa_inference=False, captions_per_image=1):
+        """captions_per_image=G > 1 (or a GroupedCaptionMask as attention_mask): B images with G seq2seq captions each in one packed
+        pass per image (_pack_captions).  vis_feats / vis_pe have B rows; input_ids, token_type_ids, masked_lm_labels, masked_pos,
+        masked_weights and task_idx have B * G rows, pair b * G + g being image b's caption g as the loader builds it; attention_mask is
+        the GroupedCaptionMask of those pairs.  Losses, their gradients and last_prediction_scores are those of the B * G pairs."""
         if not vqa_inference and masked_pos is not None and masked_pos.numel() > 0:
             self.cls.predictions.check_task_idx(task_idx)      # before anything is launched
-        _check_seq_len(self.config, input_ids.size(1))
+        _check_seq_len(self.config, input_ids.size(1))         # grouped: positions stay below L; _pack_captions checks L' alone
+        grouped = captions_per_image != 1 or isinstance(attention_mask, GroupedCaptionMask)
+        if grouped:
+            packed = self._pack_captions(vis_feats, input_ids, token_type_ids, attention_mask, masked_pos, captions_per_image,
+                                         ans_labels, mask_image_regions, vqa_inference)
         vis_feats, vis_pe = self.project_regions(vis_feats, vis_pe)
+        if grouped:
+            return self._grouped_loss(vis_feats, vis_pe, packed, attention_mask, masked_lm_labels, next_sentence_label, masked_pos,
+                                      masked_weights, task_idx, drop_worst_ratio)
 
         if vqa_inference:                                    # modeling.py:1039-1047
             assert ans_labels is None
@@ -774,6 +789,16 @@ class BertForPreTrainingLossMask(PreTrainedBertModel, _RegionProjections):
                                                    len_vis_input=self.len_vis_input)
         if masked_lm_labels is None or next_sentence_label is None:
             raise NotImplementedError
+        if masked_pos.numel() == 0:
+            masked_lm_loss = pooled_output.new(1).fill_(0).float()
+        else:
+            gathered = torch.gather(sequence_output, 1, masked_pos.unsqueeze(2).expand(-1, -1, sequence_output.size(-1)))
+            masked_lm_loss = self._mlm_loss(gathered, pooled_output, masked_lm_labels, masked_weights, task_idx, drop_worst_ratio)
+        return self._loss_tail(masked_lm_loss, sequence_output, pooled_output, vis_feats, vis_pe, vis_masked_pos, mask_image_regions,
+                               ans_labels)
+
+    def _mlm_loss(self, gathered, pooled_output, masked_lm_labels, masked_weights, task_idx, drop_worst_ratio):
+        """modeling.py:1068-1109: the masked-LM loss of the gathered hidden states [B, P, H], normalised over the batch."""
 
         def loss_mask_and_normalize(loss, mask, ratio):      # modeling.py:1083-1093
             mask = mask.type_as(loss)
@@ -782,31 +807,89 @@ class BertForPreTrainingLossMask(PreTrainedBertModel, _RegionProjections):
             denominator = torch.sum(mask.sum(-1)[keep_ind]) + 1e-5
             return (keep_loss / denominator).sum()
 
-        if masked_pos.numel() == 0:
+        if self.fused_mlm_head:                              # decoder + bias + CE in libvlpk, SURVEY.md §8f-3
+            pred = self.cls.predictions
+            hid = pred.select_task(pred.transform(gathered.to(pred.decoder.weight.dtype)), task_idx)
+            eps = self.crit_mask_lm_smoothed.label_smoothing if self.crit_mask_lm_smoothed is not None else 0.0
+            loss_flat, scores = ops.DecoderCEFn.apply(hid.reshape(-1, hid.size(-1)), pred.decoder.weight, pred.bias,
+                                                      masked_lm_labels.reshape(-1), eps)
+            self.last_prediction_scores = scores.view(*masked_lm_labels.shape, -1)
+            masked_lm_loss = loss_flat.view_as(masked_lm_labels)
+        else:
+            prediction_scores_masked, _ = self.cls(gathered, pooled_output, task_idx=task_idx)
+            self.last_prediction_scores = prediction_scores_masked
+            if self.crit_mask_lm_smoothed is not None:       # modeling.py:1104-1106
+                masked_lm_loss = self.crit_mask_lm_smoothed(F.log_softmax(prediction_scores_masked.float(), dim=-1), masked_lm_labels)
+            else:
+                # same per-position CE as crit_mask_lm(scores.transpose(1, 2).float(), labels) (modeling.py:1108-1109), evaluated
+                # on the contiguous [B*P, V] view so that the softmax reduces over the unit-stride dimension
+                V = prediction_scores_masked.size(-1)
+                masked_lm_loss = F.cross_entropy(prediction_scores_masked.reshape(-1, V).float(), masked_lm_labels.reshape(-1),
+                                                 reduction="none").view_as(masked_lm_labels)
+        return loss_mask_and_normalize(masked_lm_loss.float(), masked_weights, drop_worst_ratio)
+
+    def _pack_captions(self, vis_feats, input_ids, token_type_ids, attention_mask, masked_pos, G, ans_labels, mask_image_regions,
+                       vqa_inference):
+        """Checks a grouped call (ValueError before any launch) and returns the packed (ids, token types, positions) [B, L'] and the
+        flat packed row [B * G, P_m] of every masked position.  Image b's packed sequence is the prefix of pair b * G (rows [0, P),
+        P = len_vis_input + 2), then row P + j of pair b * G + g at row P + g * T + j with its own position P + j (T = L - P)."""
+        if self.tasks == "vqa2" or vqa_inference:
+            raise ValueError("vlp_b200: captions_per_image groups seq2seq caption pairs; VQA samples cannot share an image prefix")
+        if mask_image_regions:
+            raise ValueError("vlp_b200: captions_per_image does not support mask_image_regions")
+        if not isinstance(attention_mask, GroupedCaptionMask):
+            raise ValueError("vlp_b200: captions_per_image > 1 takes a staging.GroupedCaptionMask as attention_mask")
+        if attention_mask.G != int(G):
+            raise ValueError(f"vlp_b200: the GroupedCaptionMask groups {attention_mask.G} captions per image, captions_per_image={G}")
+        G = attention_mask.G
+        N, L_ = input_ids.shape
+        R = self.len_vis_input
+        T, Lp = GroupedCaptionMask.check(G, R, L_)
+        if attention_mask.len_a != R or attention_mask.L != L_:
+            raise ValueError(f"vlp_b200: the GroupedCaptionMask is for len_a={attention_mask.len_a}, L={attention_mask.L}; the batch has "
+                             f"len_a={R}, L={L_}")
+        if N % G:
+            raise ValueError(f"vlp_b200: {N} caption pairs do not form whole images of captions_per_image={G}")
+        B = N // G
+        if vis_feats.size(0) != B:
+            raise ValueError(f"vlp_b200: {N} pairs at captions_per_image={G} are {B} images; vis_feats has {vis_feats.size(0)} rows")
+        if tuple(attention_mask.bits.shape[:2]) != (B, Lp):
+            raise ValueError(f"vlp_b200: the GroupedCaptionMask has {tuple(attention_mask.bits.shape[:2])} rows, [{B}, {Lp}] needed")
+        P = R + 2
+        dev = input_ids.device
+        k = torch.arange(Lp, device=dev)
+        text = (k - P).clamp_min(0)
+        src = torch.where(k < P, k, text // T * L_ + P + text % T)             # column of input_ids.view(B, G * L) behind packed row k
+        pos = torch.where(k < P, k, P + text % T).unsqueeze(0).expand(B, Lp).contiguous()
+
+        def pack(t):
+            return None if t is None else t.reshape(B, G * L_).index_select(1, src)
+
+        flat = None
+        if masked_pos is not None and masked_pos.numel() > 0:
+            pair = torch.arange(N, device=dev).unsqueeze(1)
+            flat = pair // G * Lp + torch.where(masked_pos >= P, masked_pos + pair % G * T, masked_pos)
+        return pack(input_ids), pack(token_type_ids), pos, flat
+
+    def _grouped_loss(self, vis_feats, vis_pe, packed, attention_mask, masked_lm_labels, next_sentence_label, masked_pos, masked_weights,
+                      task_idx, drop_worst_ratio):
+        """The masked-LM loss of B images x G captions from one packed pass per image (forward with captions_per_image > 1)."""
+        ids, types, pos, flat = packed
+        sequence_output, pooled_output = self.bert(vis_feats, vis_pe, ids, types, attention_mask, output_all_encoded_layers=False,
+                                                   len_vis_input=self.len_vis_input, position_ids=pos)
+        if masked_lm_labels is None or next_sentence_label is None:
+            raise NotImplementedError
+        if flat is None:
             masked_lm_loss = pooled_output.new(1).fill_(0).float()
         else:
-            gathered = torch.gather(sequence_output, 1, masked_pos.unsqueeze(2).expand(-1, -1, sequence_output.size(-1)))
-            if self.fused_mlm_head:                          # decoder + bias + CE in libvlpk, SURVEY.md §8f-3
-                pred = self.cls.predictions
-                hid = pred.select_task(pred.transform(gathered.to(pred.decoder.weight.dtype)), task_idx)
-                eps = self.crit_mask_lm_smoothed.label_smoothing if self.crit_mask_lm_smoothed is not None else 0.0
-                loss_flat, scores = ops.DecoderCEFn.apply(hid.reshape(-1, hid.size(-1)), pred.decoder.weight, pred.bias,
-                                                          masked_lm_labels.reshape(-1), eps)
-                self.last_prediction_scores = scores.view(*masked_lm_labels.shape, -1)
-                masked_lm_loss = loss_flat.view_as(masked_lm_labels)
-            else:
-                prediction_scores_masked, _ = self.cls(gathered, pooled_output, task_idx=task_idx)
-                self.last_prediction_scores = prediction_scores_masked
-                if self.crit_mask_lm_smoothed is not None:   # modeling.py:1104-1106
-                    masked_lm_loss = self.crit_mask_lm_smoothed(F.log_softmax(prediction_scores_masked.float(), dim=-1), masked_lm_labels)
-                else:
-                    # same per-position CE as crit_mask_lm(scores.transpose(1, 2).float(), labels) (modeling.py:1108-1109), evaluated
-                    # on the contiguous [B*P, V] view so that the softmax reduces over the unit-stride dimension
-                    V = prediction_scores_masked.size(-1)
-                    masked_lm_loss = F.cross_entropy(prediction_scores_masked.reshape(-1, V).float(), masked_lm_labels.reshape(-1),
-                                                     reduction="none").view_as(masked_lm_labels)
-            masked_lm_loss = loss_mask_and_normalize(masked_lm_loss.float(), masked_weights, drop_worst_ratio)
+            H = sequence_output.size(-1)
+            rows = sequence_output.reshape(1, -1, H)
+            gathered = torch.gather(rows, 1, flat.reshape(1, -1, 1).expand(-1, -1, H)).view(*flat.shape, H)
+            masked_lm_loss = self._mlm_loss(gathered, pooled_output, masked_lm_labels, masked_weights, task_idx, drop_worst_ratio)
+        return masked_lm_loss, masked_lm_loss.new(1).fill_(0), masked_lm_loss.new(1).fill_(0)
 
+    def _loss_tail(self, masked_lm_loss, sequence_output, pooled_output, vis_feats, vis_pe, vis_masked_pos, mask_image_regions, ans_labels):
+        """modeling.py:1113-1143: the region pretext and VQA losses next to the masked-LM loss, and the returned triple."""
         if mask_image_regions:                               # Selfie-like pretext, modeling.py:1113-1131
             vf = vis_feats.float()
             idx = (vis_masked_pos - 1).unsqueeze(-1)
