@@ -38,6 +38,34 @@ def _dup_ngram_candidates(seq, n, ignore):
     return sorted(out)
 
 
+def _step_maps(maps, frame, B, W):
+    """The buffer of step `frame`'s [MASK]-row maps in maps [T, B*W, ...]: step 0 has B input rows, written at rows b*W; None
+    without maps."""
+    if maps is None:
+        return None
+    return maps[frame] if frame else maps[0].view(B, W, *maps.shape[2:])[:, 0]
+
+
+def _follow_beams(state, frame, ptrs, task_idx):
+    """Moves the decode state to frame `frame`'s W beams per image (ptrs [B, W] their back pointers): expands each image's row to
+    them after frame 0, per-sample task_idx included, and reorders by the back pointers after every later frame.  Returns task_idx."""
+    B, W = ptrs.shape
+    if frame == 0:
+        state.expand(W)
+        return expand_task_idx(task_idx, B, W)                          # per-sample ids follow their beams (relaxed head)
+    state.reorder((ptrs + torch.arange(B, device=ptrs.device).unsqueeze(1) * W).reshape(-1))      # beam i continues hypothesis parent[i]
+    return task_idx
+
+
+def _padded_traces(out, sc, wi, pt, out_len):
+    """out["scores"], out["wids"], out["ptrs"]: the traces [T, B, W] as [B, out_len, W], zero past frame T."""
+    T, B, W = sc.shape
+    for k, t in (("scores", sc), ("wids", wi), ("ptrs", pt)):
+        padded = t.new_zeros((B, out_len, W))
+        padded[:, :T] = t.permute(1, 0, 2)
+        out[k] = padded
+
+
 def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, output_attentions=False):
     """output_attentions: out["attentions"] [B, out_len - in_len, layers, heads, out_len] holds, for frame t of pred_seq, the [MASK]-row
     maps of step t taken from the row its hypothesis continued (beam_maps)."""
@@ -56,10 +84,7 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
     maps = new_attention_maps(dec, out_len - in_len, B * K, out_len, dev) if output_attentions else None
     curr_ids = input_ids
     for frame in range(out_len - in_len):
-        buf = None
-        if maps is not None:
-            buf = maps[frame] if frame else maps[0].view(B, K, *maps.shape[2:])[:, 0]
-        scores, _ = dec.cls(state.step(curr_ids, buf), None, task_idx=task_idx)
+        scores, _ = dec.cls(state.step(curr_ids, _step_maps(maps, frame, B, K)), None, task_idx=task_idx)
         logp = F.log_softmax(scores.float(), dim=-1)                      # [B or B*K, 1, V]
         if dec.forbid_duplicate_ngrams and frame >= 1:
             # history of frame `frame` from the previous frame's words and back pointers; blocks in place once it holds n words
@@ -80,22 +105,14 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
         step_ids.append(k_ids)
         beam_eos.append((k_ids == dec.eos_id).float())
         total_scores.append(k_scores)
-        if frame == 0:
-            state.expand(K)
-            task_idx = expand_task_idx(task_idx, B, K)                     # per-sample ids follow their beams (relaxed head)
-        else:
-            state.reorder((back + torch.arange(B, device=dev).unsqueeze(1) * K).reshape(-1))      # beam i continues hypothesis parent[i]
+        task_idx = _follow_beams(state, frame, back, task_idx)
         curr_ids = k_ids.reshape(B * K, 1)
 
     sc, wi, pt = torch.stack(total_scores), torch.stack(step_ids), torch.stack(step_ptrs)
     out = {"pred_seq": backtrack(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len)}
     if maps is not None:
         out["attentions"] = beam_maps(maps, *best_path(sc, wi, pt, dec.eos_id, dec.length_penalty), pt)
-    T = len(total_scores)
-    for k, t in (("scores", torch.stack(total_scores)), ("wids", torch.stack(step_ids)), ("ptrs", torch.stack(step_ptrs))):
-        padded = t.new_zeros((B, out_len, K))
-        padded[:, :T] = t.permute(1, 0, 2)
-        out[k] = padded
+    _padded_traces(out, sc, wi, pt, out_len)
     if N > 1:
         out["nbest_seq"], out["nbest_scores"] = nbest(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len, N)
     return out
@@ -128,31 +145,20 @@ def diverse_beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, posit
     top_lp = torch.empty(B * K, K, dtype=torch.float32, device=dev)
     pred = dec.cls.predictions
     maps = new_attention_maps(dec, T, B * K, out_len, dev) if output_attentions else None
-    rows = torch.arange(B, device=dev).unsqueeze(1) * K
     curr_ids = input_ids
     for frame in range(T):
-        buf = None
-        if maps is not None:
-            buf = maps[frame] if frame else maps[0].view(B, K, *maps.shape[2:])[:, 0]
-        h = pred.select_task(pred.transform(state.step(curr_ids, buf).to(pred.decoder.weight.dtype)), task_idx)
+        h = pred.select_task(pred.transform(state.step(curr_ids, _step_maps(maps, frame, B, K)).to(pred.decoder.weight.dtype)), task_idx)
         logits = pred.decoder(h)                                          # [B or B*K, 1, V]; the kernel adds the bias
         ops.diverse_beam_step(logits, pred.bias.to(logits.dtype), frame, G, dec.diversity_penalty, wi, pt, sc, eos, top_w, top_lp,
                               dec.eos_id, block_eos=bool(dec.min_len) and frame + 1 <= dec.min_len, ngram=ngram, ignore=ignore,
                               hist_in=hist[(frame - 1) % 2], hist_out=hist[frame % 2])
-        if frame == 0:
-            state.expand(K)
-            task_idx = expand_task_idx(task_idx, B, K)
-        else:
-            state.reorder((pt[frame] + rows).reshape(-1))
+        task_idx = _follow_beams(state, frame, pt[frame], task_idx)
         curr_ids = wi[frame].reshape(B * K, 1)
 
     out = {"pred_seq": backtrack(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len)}
     if maps is not None:
         out["attentions"] = beam_maps(maps, *best_path(sc, wi, pt, dec.eos_id, dec.length_penalty), pt)
-    for k, t in (("scores", sc), ("wids", wi), ("ptrs", pt)):
-        padded = t.new_zeros((B, out_len, K))
-        padded[:, :T] = t.permute(1, 0, 2)
-        out[k] = padded
+    _padded_traces(out, sc, wi, pt, out_len)
     if N > 1:
         out["nbest_seq"], out["nbest_scores"] = nbest(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len, N)
     out["group_seq"], out["group_scores"] = group_best(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len, G)
@@ -199,22 +205,14 @@ def constrained_beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, p
     top_dest = torch.empty(B * SK, W - K, dtype=torch.int32, device=dev)
     pred = dec.cls.predictions
     maps = new_attention_maps(dec, T, B * SK, out_len, dev) if output_attentions else None
-    rows = torch.arange(B, device=dev).unsqueeze(1) * SK
     curr_ids = input_ids
     for frame in range(T):
-        buf = None
-        if maps is not None:
-            buf = maps[frame] if frame else maps[0].view(B, SK, *maps.shape[2:])[:, 0]
-        h = pred.select_task(pred.transform(state.step(curr_ids, buf).to(pred.decoder.weight.dtype)), task_idx)
+        h = pred.select_task(pred.transform(state.step(curr_ids, _step_maps(maps, frame, B, SK)).to(pred.decoder.weight.dtype)), task_idx)
         logits = pred.decoder(h)                                          # [B or B*S*K, 1, V]; the kernel adds the bias
         ops.constrained_beam_step(logits, pred.bias.to(logits.dtype), frame, cons, wi, pt, sc, eos, top_w, top_lp, top_dest, dec.eos_id,
                                   block_eos=bool(dec.min_len) and frame + 1 <= dec.min_len, ngram=ngram, ignore=ignore,
                                   hist_in=hist[(frame - 1) % 2], hist_out=hist[frame % 2])
-        if frame == 0:
-            state.expand(SK)
-            task_idx = expand_task_idx(task_idx, B, SK)
-        else:
-            state.reorder((pt[frame] + rows).reshape(-1))
+        task_idx = _follow_beams(state, frame, pt[frame], task_idx)
         curr_ids = wi[frame].reshape(B * SK, 1)
 
     lp = dec.length_penalty
@@ -229,10 +227,7 @@ def constrained_beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, p
         active = torch.stack([a for a, _ in paths])[chosen, :, bidx].t()                             # [T, B]: the chosen state's path
         pos = torch.stack([p for _, p in paths])[chosen, :, bidx].t()
         out["attentions"] = beam_maps(maps, active, pos, pt)
-    for k, t in (("scores", sc), ("wids", wi), ("ptrs", pt)):
-        padded = t.new_zeros((B, out_len, SK))
-        padded[:, :T] = t.permute(1, 0, 2)
-        out[k] = padded
+    _padded_traces(out, sc, wi, pt, out_len)
     if N > 1:
         out["nbest_seq"], out["nbest_scores"] = nbest(sc, wi, pt, dec.eos_id, lp, out_len, N, beams=slice((S - 1) * K, SK))
     out["state_seq"], out["state_scores"] = state_seq, state_scores

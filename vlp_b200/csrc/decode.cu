@@ -1,17 +1,8 @@
-// vlp_b200 — duplicate-n-gram blocking for beam search (the reference's forbid_duplicate_ngrams, modeling.py:1375-1428, and its
-// get_dup_ngram_candidates, :1391-1406), on the device so that a blocked decode needs no host synchronisation and can be captured
-// in a CUDA graph.
-//
-// One launch per beam frame f >= 1, one CTA per hypothesis row i = b*K + k:
-//   history  hist_out[i, :f-1] = hist_in[b*K + ptr[i], :f-1],  hist_out[i, f-1] = wid[i]        (the reference's partial_seqs)
-//   blocking (f >= n) seq = hist_out[i, :f], tail = seq[-(n-1):] (the whole of seq when n = 1, as in the reference);
-//            no candidates if a tail word is ignored, else w = seq[s+n-1] for every s <= f-n with seq[s:s+n-1] == tail, unless w
-//            is ignored; logp[i, w] += -10000 once per distinct candidate.
-// The history row lives in shared memory, so its length is bounded by shared memory and not by the CTA's threads.  Candidates are
-// collected in a V-bit shared bitmap (integer atomicOr: the set does not depend on scheduling) and each set bit is applied by one
-// thread with one fp32 add, so every (row, word) is written at most once and the result is bitwise reproducible.  Word ids outside
-// [0, V) never become candidates; a back pointer outside [0, K) gives a history of -1 words (never a candidate, never matching a
-// real tail).
+// vlp_b200 — the decoders' per-frame selection on the device, so that a decode needs no host synchronisation and can be captured in
+// a CUDA graph.  Four selectors: duplicate-n-gram blocking for beam search (beam_ngram_block_kernel), top-k / top-p sampling
+// (sample_kernel), diverse beam search (diverse_beam_rows / _merge) and constrained beam search (constrained_beam_rows / _merge).
+// Shared blocks: the history carry (to_word, carry_history), the n-gram candidates, and for the row kernels their shared memory
+// and chunks (row_smem, row_chunk), the log-softmax (row_logp), the threshold search (threshold_key) and the top K (row_top_k).
 #include "decode.cuh"
 
 #include <climits>
@@ -21,6 +12,18 @@
 namespace vlpk {
 namespace {
 
+// ---------------------------------------------------------------------------------------------------------------------------
+// Duplicate-n-gram blocking for beam search (the reference's forbid_duplicate_ngrams, modeling.py:1375-1428, and its
+// get_dup_ngram_candidates, :1391-1406).  One launch per beam frame f >= 1, one CTA per hypothesis row i = b*K + k:
+//   history  hist_out[i, :f-1] = hist_in[b*K + ptr[i], :f-1],  hist_out[i, f-1] = wid[i]        (the reference's partial_seqs)
+//   blocking (f >= n) seq = hist_out[i, :f], tail = seq[-(n-1):] (the whole of seq when n = 1, as in the reference);
+//            no candidates if a tail word is ignored, else w = seq[s+n-1] for every s <= f-n with seq[s:s+n-1] == tail, unless w
+//            is ignored; logp[i, w] += -10000 once per distinct candidate.
+// The history row lives in shared memory, so its length is bounded by shared memory and not by the CTA's threads.  Candidates are
+// collected in a V-bit shared bitmap (integer atomicOr: the set does not depend on scheduling) and each set bit is applied by one
+// thread with one fp32 add, so every (row, word) is written at most once and the result is bitwise reproducible.  Word ids outside
+// [0, V) never become candidates; a back pointer outside [0, K) gives a history of -1 words (never a candidate, never matching a
+// real tail).
 constexpr int NGRAM_THREADS = 256;
 constexpr size_t NGRAM_SMEM_MAX = 48 * 1024;
 
@@ -28,6 +31,32 @@ __device__ __forceinline__ bool is_ignored(int w, const int* ignore, int n_ignor
   for (int j = 0; j < n_ignore; ++j)
     if (__ldg(ignore + j) == w) return true;
   return false;
+}
+
+// An int64 word id as int32; ids outside int32 become -1, which is never a candidate and never matches a real word.
+__device__ __forceinline__ int to_word(long long w) { return (w >= INT_MIN && w <= INT_MAX) ? static_cast<int>(w) : -1; }
+
+// The history of frame f >= 1 of `row`, written to hist_out's row and to seq (shared memory): the f-1 words of its parent, row
+// (row / width) * width + prev_ptr[row] of hist_in (read at f > 1; a pointer outside [0, width) gives -1 words), then
+// prev_wid[row].  The CTA's threads stride over the words; the caller orders seq with a barrier before reading it.  I64: the
+// traces' 64-bit integer type.
+template <typename I64>
+__device__ __forceinline__ void carry_history(const int* hist_in, int* hist_out, int* seq, const I64* prev_ptr, const I64* prev_wid,
+                                              int row, int width, int f, int T_cap) {
+  const long long p = f > 1 ? prev_ptr[row] : 0;
+  const bool parent_ok = p >= 0 && p < width;
+  const int* src = hist_in + (static_cast<size_t>(row / width) * width + (parent_ok ? p : 0)) * T_cap;
+  int* dst = hist_out + static_cast<size_t>(row) * T_cap;
+  for (int t = threadIdx.x; t < f - 1; t += blockDim.x) {
+    const int w = parent_ok ? src[t] : -1;
+    seq[t] = w;
+    dst[t] = w;
+  }
+  if (threadIdx.x == 0) {
+    const int w = to_word(prev_wid[row]);
+    seq[f - 1] = w;
+    dst[f - 1] = w;
+  }
 }
 
 // The candidates of history seq[0:f], f >= n, as set bits of `bits` ([ceil(V/32)] words, cleared here).  seq must be complete in
@@ -67,22 +96,7 @@ __global__ void __launch_bounds__(NGRAM_THREADS) beam_ngram_block_kernel(NgramBl
   const int f = a.f;
   const int tid = threadIdx.x;
 
-  // history of frame f: the parent's f-1 words, then this frame's word
-  const long long p = f > 1 ? a.ptr[i] : 0;
-  const bool parent_ok = p >= 0 && p < a.K;
-  const int* src = a.hist_in + (static_cast<size_t>(i / a.K) * a.K + (parent_ok ? p : 0)) * a.T_cap;
-  int* dst = a.hist_out + static_cast<size_t>(i) * a.T_cap;
-  for (int t = tid; t < f - 1; t += blockDim.x) {
-    const int w = parent_ok ? src[t] : -1;
-    seq[t] = w;
-    dst[t] = w;
-  }
-  if (tid == 0) {
-    const long long w64 = a.wid[i];
-    const int w = (w64 >= INT_MIN && w64 <= INT_MAX) ? static_cast<int>(w64) : -1;
-    seq[f - 1] = w;
-    dst[f - 1] = w;
-  }
+  carry_history(a.hist_in, a.hist_out, seq, a.ptr, a.wid, i, a.K, f, a.T_cap);      // history of frame f
   if (f < a.n) return;                                             // uniform: too short for an n-gram
 
   if (!ngram_candidates(seq, f, a.n, a.V, a.ignore, a.n_ignore, bits)) return;      // no candidate: the row is not touched
@@ -99,23 +113,36 @@ __global__ void __launch_bounds__(NGRAM_THREADS) beam_ngram_block_kernel(NgramBl
   }
 }
 
+size_t ngram_block_smem_bytes(int T_cap, int V) {
+  return (static_cast<size_t>(T_cap) + (static_cast<size_t>(V) + 31) / 32) * 4;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------------
-// Top-k / top-p sampling of one decode frame f, one CTA of SAMPLE_THREADS per row:
-//   x[v]   = logits[row, v] + bias[v], rounded to the logits' dtype (bit for bit the head's `decoder(h) + bias`), plus -10000 at
-//            the words the duplicate-n-gram rule above blocks for history seq[row, :f] (n > 0, f >= n), and x[eos] = -10000 while
-//            block_eos is set (beam search's order and values); e[v] = exp(x[v] - max x), Z = sum e.
-//   order  words ranked by (x descending, index ascending).  top-k keeps the first k; top-p keeps the shortest prefix whose e
-//            sum reaches topp * Z (always at least the first argmax, so topp -> 0 is greedy).  The cut is found as a threshold on
-//            an order-preserving 32-bit key (x for top-k, e for top-p) by binary search over the key's bits — no sort — and words
-//            tied at the threshold are taken lowest index first, as many as needed.
-//   draw   u = Philox(seed; frame f, row) in [0, 1); the chosen word is the first kept word, in index order, whose running e sum
-//          exceeds u * (kept e sum).  seq[row, f] = word, score[row, f] = log(e[word] / Z).
-// Each thread owns one contiguous chunk of the row in shared memory and every sum is taken in a fixed order (chunk, then a
-// fixed shuffle tree), so the result depends on (seed, f, row, logits) only: not on the batch, the grid or the run.
-// Finished rows write pad_id and score 0; a row that draws eos_id is marked finished and decrements *live.
+// Shared blocks of the row kernels (sample_kernel, diverse_beam_rows_kernel, constrained_beam_rows_kernel): one CTA of
+// SAMPLE_THREADS per row of V words.
 using bf16 = __nv_bfloat16;
 constexpr int SAMPLE_THREADS = 1024;                               // 32 warps: the block reductions below rely on it
 constexpr size_t SAMPLE_SMEM_MAX = 200 * 1024;
+
+// Their dynamic shared memory: val [V] floats, bits [ceil(V/32)] blocked words, hist [T_cap] history.
+size_t row_smem_bytes(int T_cap, int V) {
+  return (static_cast<size_t>(V) + (static_cast<size_t>(V) + 31) / 32 + static_cast<size_t>(T_cap)) * 4;
+}
+
+__device__ __forceinline__ void row_smem(int V, float*& val, unsigned*& bits, int*& hist) {
+  extern __shared__ float row_smem_base[];
+  val = row_smem_base;
+  bits = reinterpret_cast<unsigned*>(val + V);
+  hist = reinterpret_cast<int*>(bits + ((V + 31) >> 5));
+}
+
+// The words [lo, hi) thread t owns in the row passes; an odd chunk length keeps the threads' strided reads in distinct banks.
+struct Chunk { int lo, hi; };
+__device__ __forceinline__ Chunk row_chunk(int V) {
+  const int C = ((V + SAMPLE_THREADS - 1) / SAMPLE_THREADS) | 1;
+  const int lo = min(static_cast<int>(threadIdx.x) * C, V);
+  return {lo, min(lo + C, V)};
+}
 
 __device__ __forceinline__ float head_logit(const bf16* l, const bf16* b, int v) {
   const float x = __bfloat162float(l[v]);
@@ -177,16 +204,127 @@ __device__ __forceinline__ void block_exclusive_scan(T v, T* red, T* pre) {
   __syncthreads();
 }
 
+// The largest key t <= khi for which at_least(t) holds, by binary search over the key's bits.  at_least must hold at 0, hold
+// below every key where it holds, and give every thread the same answer.
+template <typename F>
+__device__ __forceinline__ unsigned threshold_key(unsigned khi, F at_least) {
+  if (at_least(khi)) return khi;
+  unsigned klo = 0;
+  khi -= 1;
+  while (klo < khi) {                                                // uniform: every thread sees the same answers
+    const unsigned mid = klo + (khi - klo + 1) / 2;
+    if (at_least(mid)) klo = mid; else khi = mid - 1;
+  }
+  return klo;
+}
+
+// The beam kernels' log-softmax of row `row` into val [V]: x[v] = head_logit(row, bias, v); logp[v] = (x[v] - max x) -
+// log(sum exp(x - max x)) in fp32; then -10000 is added at the words set in bits while blocked, and logp[eos] = -10000 while
+// block_eos: beam search's order and values.  Each thread leaves its own chunk of val written (no barrier after it).
+template <typename T, typename Args>
+__device__ __forceinline__ void row_logp(const Args& a, int row, bool blocked, const unsigned* bits, float* val, float* redf) {
+  const int V = a.V;
+  const T* lrow = static_cast<const T*>(a.logits) + static_cast<size_t>(row) * a.ld;
+  const T* bias = static_cast<const T*>(a.bias);
+  float mx = -INFINITY;
+  for (int v = threadIdx.x; v < V; v += SAMPLE_THREADS) {
+    const float x = head_logit(lrow, bias, v);
+    val[v] = x;
+    mx = fmaxf(mx, x);
+  }
+  mx = block_reduce(mx, redf, [](float p, float q) { return fmaxf(p, q); });
+
+  const Chunk ch = row_chunk(V);
+  float z = 0.f;
+  for (int v = ch.lo; v < ch.hi; ++v) z += expf(val[v] - mx);
+  const float lse = logf(block_reduce(z, redf, [](float p, float q) { return p + q; }));
+  for (int v = ch.lo; v < ch.hi; ++v) {
+    float lp = (val[v] - mx) - lse;
+    if (blocked && ((bits[v >> 5] >> (v & 31)) & 1u)) lp += -10000.0f;
+    if (a.block_eos && v == a.eos_id) lp = -10000.0f;
+    val[v] = lp;
+  }
+}
+
+// The K words of val [V] ranked first by (value descending, word ascending), written in rank order to out_w / out_lp [0:K]: a
+// threshold on order_key(val) by binary search over the key's bits plus a scan of the ties in index order (no sort).  Each
+// thread's chunk of val must be complete; the search starts from the maximum, which skips NaNs (the constrained kernel's
+// excluded words).  redf / redi: [33], prei: [SAMPLE_THREADS + 1], sel_w / sel_lp: [K] shared.
+__device__ __forceinline__ void row_top_k(const float* val, int V, int K, int* out_w, float* out_lp, float* redf, int* redi,
+                                          int* prei, int* sel_w, float* sel_lp) {
+  const int tid = threadIdx.x;
+  const Chunk ch = row_chunk(V);
+  const int lo = ch.lo, hi = ch.hi;
+  float top = -INFINITY;
+  for (int v = lo; v < hi; ++v) top = fmaxf(top, val[v]);
+  top = block_reduce(top, redf, [](float p, float q) { return fmaxf(p, q); });
+
+  // tau = the largest key with at least K words at or above it
+  auto count = [&](unsigned t) {
+    int c = 0;
+    for (int v = lo; v < hi; ++v) c += order_key(val[v]) >= t;
+    return block_reduce(c, redi, [](int p, int q) { return p + q; });
+  };
+  const unsigned tau = threshold_key(order_key(top), [&](unsigned t) { return count(t) >= K; });
+  const int take = K - (tau == 0xffffffffu ? 0 : count(tau + 1));   // words tied at tau to keep, lowest index first
+
+  int ties = 0;
+  for (int v = lo; v < hi; ++v) ties += order_key(val[v]) == tau;
+  block_exclusive_scan(ties, redi, prei);
+  const int ties_before = prei[tid];
+  int rank = ties_before, kept = 0;
+  for (int v = lo; v < hi; ++v) {
+    const unsigned k = order_key(val[v]);
+    kept += k > tau || (k == tau && rank++ < take);
+  }
+  block_exclusive_scan(kept, redi, prei);                            // the chunk's first slot among the K kept words
+  int slot = prei[tid];
+  rank = ties_before;
+  for (int v = lo; v < hi; ++v) {
+    const unsigned k = order_key(val[v]);
+    if (k > tau || (k == tau && rank++ < take)) {
+      sel_w[slot] = v;
+      sel_lp[slot] = val[v];
+      ++slot;
+    }
+  }
+  __syncthreads();
+  if (tid < K) {                                                     // rank order: (logp descending, word ascending)
+    const float lp = sel_lp[tid];
+    const unsigned kt = order_key(lp);
+    const int w = sel_w[tid];
+    int r = 0;
+    for (int j = 0; j < K; ++j) {
+      const unsigned kj = order_key(sel_lp[j]);
+      r += kj > kt || (kj == kt && sel_w[j] < w);
+    }
+    out_w[r] = w;
+    out_lp[r] = lp;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------
+// Top-k / top-p sampling of one decode frame f, one CTA of SAMPLE_THREADS per row:
+//   x[v]   = logits[row, v] + bias[v], rounded to the logits' dtype (bit for bit the head's `decoder(h) + bias`), plus -10000 at
+//            the words the duplicate-n-gram rule above blocks for history seq[row, :f] (n > 0, f >= n), and x[eos] = -10000 while
+//            block_eos is set (beam search's order and values); e[v] = exp(x[v] - max x), Z = sum e.
+//   order  words ranked by (x descending, index ascending).  top-k keeps the first k; top-p keeps the shortest prefix whose e
+//            sum reaches topp * Z (always at least the first argmax, so topp -> 0 is greedy).  The cut is found as a threshold on
+//            an order-preserving 32-bit key (x for top-k, e for top-p) by binary search over the key's bits — no sort — and words
+//            tied at the threshold are taken lowest index first, as many as needed.
+//   draw   u = Philox(seed; frame f, row) in [0, 1); the chosen word is the first kept word, in index order, whose running e sum
+//          exceeds u * (kept e sum).  seq[row, f] = word, score[row, f] = log(e[word] / Z).
+// Each thread owns one contiguous chunk of the row in shared memory and every sum is taken in a fixed order (chunk, then a
+// fixed shuffle tree), so the result depends on (seed, f, row, logits) only: not on the batch, the grid or the run.
+// Finished rows write pad_id and score 0; a row that draws eos_id is marked finished and decrements *live.
 template <typename T>
 __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
-  extern __shared__ float sample_smem[];
   __shared__ float redf[33], pref[SAMPLE_THREADS + 1];
   __shared__ int redi[33], prei[SAMPLE_THREADS + 1];
   const int V = a.V, tid = threadIdx.x, row = blockIdx.x;
-  const int nwords = (V + 31) >> 5;
-  float* val = sample_smem;                                          // [V] x (top-k) or e (top-p)
-  unsigned* bits = reinterpret_cast<unsigned*>(val + V);             // [nwords] blocked words
-  int* hist = reinterpret_cast<int*>(bits + nwords);                 // [T_cap] history
+  float* val;                                                        // [V] x (top-k) or e (top-p)
+  unsigned* bits; int* hist;
+  row_smem(V, val, bits, hist);
   long long* out = a.seq + static_cast<size_t>(row) * a.T_cap;
   if (a.finished[row]) {                                             // uniform
     if (tid == 0) {
@@ -198,10 +336,7 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
 
   bool blocked = false;
   if (a.n > 0 && a.f >= a.n) {
-    for (int t = tid; t < a.f; t += SAMPLE_THREADS) {
-      const long long w = out[t];
-      hist[t] = (w >= INT_MIN && w <= INT_MAX) ? static_cast<int>(w) : -1;
-    }
+    for (int t = tid; t < a.f; t += SAMPLE_THREADS) hist[t] = to_word(out[t]);
     blocked = ngram_candidates(hist, a.f, a.n, V, a.ignore, a.n_ignore, bits);
   }
 
@@ -218,9 +353,9 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
   }
   mx = block_reduce(mx, redf, [](float p, float q) { return fmaxf(p, q); });
 
-  // from here on thread t owns words [lo, hi); an odd chunk length keeps the threads' strided reads in distinct banks
-  const int C = ((V + SAMPLE_THREADS - 1) / SAMPLE_THREADS) | 1;
-  const int lo = min(tid * C, V), hi = min(lo + C, V);
+  // from here on thread t owns words [lo, hi)
+  const Chunk ch = row_chunk(V);
+  const int lo = ch.lo, hi = ch.hi;
   const bool topp = a.mode == SAMPLE_TOPP;
   float z = 0.f;
   for (int v = lo; v < hi; ++v) {
@@ -240,17 +375,7 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
   };
   const float target = topp ? a.topp * Z : static_cast<float>(min(a.topk, V));
   // tau = the largest key with mass(tau) >= target; mass(0) >= target always holds
-  unsigned klo = 0, khi = topp ? __float_as_uint(1.0f) : order_key(mx);
-  if (mass(khi) >= target) {
-    klo = khi;
-  } else {
-    khi -= 1;
-    while (klo < khi) {                                              // uniform: every thread sees the same masses
-      const unsigned mid = klo + (khi - klo + 1) / 2;
-      if (mass(mid) >= target) klo = mid; else khi = mid - 1;
-    }
-  }
-  const unsigned tau = klo;
+  const unsigned tau = threshold_key(topp ? __float_as_uint(1.0f) : order_key(mx), [&](unsigned t) { return mass(t) >= target; });
   const float above = tau == 0xffffffffu ? 0.f : mass(tau + 1);
   int take;                                                           // words tied at tau to keep, lowest index first
   if (!topp) {
@@ -341,115 +466,23 @@ constexpr int DIVERSE_MAX_CAND = DIVERSE_MAX_BEAMS * DIVERSE_MAX_BEAMS;       //
 
 template <typename T>
 __global__ void __launch_bounds__(SAMPLE_THREADS) diverse_beam_rows_kernel(DiverseBeamArgs a) {
-  extern __shared__ float rows_smem[];
   __shared__ float redf[33];
   __shared__ int redi[33], prei[SAMPLE_THREADS + 1];
   __shared__ int sel_w[DIVERSE_MAX_BEAMS];
   __shared__ float sel_lp[DIVERSE_MAX_BEAMS];
-  const int V = a.V, K = a.K, tid = threadIdx.x, row = blockIdx.x;
-  float* val = rows_smem;                                            // [V] logp
-  unsigned* bits = reinterpret_cast<unsigned*>(val + V);             // [ceil(V/32)] blocked words
-  int* hist = reinterpret_cast<int*>(bits + ((V + 31) >> 5));        // [T_cap] history
+  const int V = a.V, K = a.K, row = blockIdx.x;
+  float* val;                                                        // [V] logp
+  unsigned* bits; int* hist;
+  row_smem(V, val, bits, hist);
 
   bool blocked = false;
   if (a.n > 0 && a.f >= 1) {                                         // uniform
-    const int f = a.f;
-    const long long p = f > 1 ? a.prev_ptr[row] : 0;
-    const bool parent_ok = p >= 0 && p < K;
-    const int* src = a.hist_in + (static_cast<size_t>(row / K) * K + (parent_ok ? p : 0)) * a.T_cap;
-    int* dst = a.hist_out + static_cast<size_t>(row) * a.T_cap;
-    for (int t = tid; t < f - 1; t += SAMPLE_THREADS) {
-      const int w = parent_ok ? src[t] : -1;
-      hist[t] = w;
-      dst[t] = w;
-    }
-    if (tid == 0) {
-      const long long w64 = a.prev_wid[row];
-      const int w = (w64 >= INT_MIN && w64 <= INT_MAX) ? static_cast<int>(w64) : -1;
-      hist[f - 1] = w;
-      dst[f - 1] = w;
-    }
-    if (f >= a.n) blocked = ngram_candidates(hist, f, a.n, V, a.ignore, a.n_ignore, bits);
+    carry_history(a.hist_in, a.hist_out, hist, a.prev_ptr, a.prev_wid, row, K, a.f, a.T_cap);
+    if (a.f >= a.n) blocked = ngram_candidates(hist, a.f, a.n, V, a.ignore, a.n_ignore, bits);
   }
-
-  const T* lrow = static_cast<const T*>(a.logits) + static_cast<size_t>(row) * a.ld;
-  const T* bias = static_cast<const T*>(a.bias);
-  float mx = -INFINITY;
-  for (int v = tid; v < V; v += SAMPLE_THREADS) {
-    const float x = head_logit(lrow, bias, v);
-    val[v] = x;
-    mx = fmaxf(mx, x);
-  }
-  mx = block_reduce(mx, redf, [](float p, float q) { return fmaxf(p, q); });
-
-  // from here on thread t owns words [lo, hi)
-  const int C = ((V + SAMPLE_THREADS - 1) / SAMPLE_THREADS) | 1;
-  const int lo = min(tid * C, V), hi = min(lo + C, V);
-  float z = 0.f;
-  for (int v = lo; v < hi; ++v) z += expf(val[v] - mx);
-  const float lse = logf(block_reduce(z, redf, [](float p, float q) { return p + q; }));
-  float top = -INFINITY;
-  for (int v = lo; v < hi; ++v) {
-    float lp = (val[v] - mx) - lse;
-    if (blocked && ((bits[v >> 5] >> (v & 31)) & 1u)) lp += -10000.0f;
-    if (a.block_eos && v == a.eos_id) lp = -10000.0f;
-    val[v] = lp;
-    top = fmaxf(top, lp);
-  }
-  top = block_reduce(top, redf, [](float p, float q) { return fmaxf(p, q); });
-
-  // tau = the largest key with at least K words at or above it
-  auto count = [&](unsigned t) {
-    int c = 0;
-    for (int v = lo; v < hi; ++v) c += order_key(val[v]) >= t;
-    return block_reduce(c, redi, [](int p, int q) { return p + q; });
-  };
-  unsigned klo = 0, khi = order_key(top);
-  if (count(khi) >= K) {
-    klo = khi;
-  } else {
-    khi -= 1;
-    while (klo < khi) {                                              // uniform: every thread sees the same counts
-      const unsigned mid = klo + (khi - klo + 1) / 2;
-      if (count(mid) >= K) klo = mid; else khi = mid - 1;
-    }
-  }
-  const unsigned tau = klo;
-  const int take = K - (tau == 0xffffffffu ? 0 : count(tau + 1));   // words tied at tau to keep, lowest index first
-
-  int ties = 0;
-  for (int v = lo; v < hi; ++v) ties += order_key(val[v]) == tau;
-  block_exclusive_scan(ties, redi, prei);
-  const int ties_before = prei[tid];
-  int rank = ties_before, kept = 0;
-  for (int v = lo; v < hi; ++v) {
-    const unsigned k = order_key(val[v]);
-    kept += k > tau || (k == tau && rank++ < take);
-  }
-  block_exclusive_scan(kept, redi, prei);                            // the chunk's first slot among the K kept words
-  int slot = prei[tid];
-  rank = ties_before;
-  for (int v = lo; v < hi; ++v) {
-    const unsigned k = order_key(val[v]);
-    if (k > tau || (k == tau && rank++ < take)) {
-      sel_w[slot] = v;
-      sel_lp[slot] = val[v];
-      ++slot;
-    }
-  }
-  __syncthreads();
-  if (tid < K) {                                                     // rank order: (logp descending, word ascending)
-    const float lp = sel_lp[tid];
-    const unsigned kt = order_key(lp);
-    const int w = sel_w[tid];
-    int r = 0;
-    for (int j = 0; j < K; ++j) {
-      const unsigned kj = order_key(sel_lp[j]);
-      r += kj > kt || (kj == kt && sel_w[j] < w);
-    }
-    a.top_w[static_cast<size_t>(row) * K + r] = w;
-    a.top_lp[static_cast<size_t>(row) * K + r] = lp;
-  }
+  row_logp<T>(a, row, blocked, bits, val, redf);
+  row_top_k(val, V, K, a.top_w + static_cast<size_t>(row) * K, a.top_lp + static_cast<size_t>(row) * K, redf, redi, prei, sel_w,
+            sel_lp);
 }
 
 __global__ void __launch_bounds__(MERGE_THREADS) diverse_beam_merge_kernel(DiverseBeamArgs a) {
@@ -532,7 +565,6 @@ __device__ __forceinline__ int cbs_root_state(const VlpkConstrainedBeamArgs& a, 
 
 template <typename T>
 __global__ void __launch_bounds__(SAMPLE_THREADS) constrained_beam_rows_kernel(VlpkConstrainedBeamArgs a) {
-  extern __shared__ float cbs_smem[];
   __shared__ float redf[33];
   __shared__ int redi[33], prei[SAMPLE_THREADS + 1];
   __shared__ int sel_w[CBS_MAX_BEAMS];
@@ -544,27 +576,11 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) constrained_beam_rows_kernel(V
   const int CA = a.C * a.A, SK = K << a.C, W = K + CA;
   const int b = f == 0 ? row : row / SK;
   const int state = f == 0 ? cbs_root_state(a, b) : (row % SK) / K;
-  float* val = cbs_smem;                                             // [V] logp
-  unsigned* bits = reinterpret_cast<unsigned*>(val + V);             // [ceil(V/32)] blocked words
-  int* hist = reinterpret_cast<int*>(bits + ((V + 31) >> 5));        // [T_cap] history
+  float* val;                                                        // [V] logp
+  unsigned* bits; int* hist;
+  row_smem(V, val, bits, hist);
 
-  if (f >= 1) {                                                      // uniform
-    const long long p = f > 1 ? a.prev_ptr[row] : 0;
-    const bool parent_ok = p >= 0 && p < SK;
-    const int* src = a.hist_in + (static_cast<size_t>(b) * SK + (parent_ok ? p : 0)) * a.T_cap;
-    int* dst = a.hist_out + static_cast<size_t>(row) * a.T_cap;
-    for (int t = tid; t < f - 1; t += SAMPLE_THREADS) {
-      const int w = parent_ok ? src[t] : -1;
-      hist[t] = w;
-      dst[t] = w;
-    }
-    if (tid == 0) {
-      const long long w64 = a.prev_wid[row];
-      const int w = (w64 >= INT_MIN && w64 <= INT_MAX) ? static_cast<int>(w64) : -1;
-      hist[f - 1] = w;
-      dst[f - 1] = w;
-    }
-  }
+  if (f >= 1) carry_history(a.hist_in, a.hist_out, hist, a.prev_ptr, a.prev_wid, row, SK, f, a.T_cap);      // uniform
   __syncthreads();
   const bool blocked = a.n > 0 && f >= a.n && ngram_candidates(hist, f, a.n, V, a.ignore, a.n_ignore, bits);
 
@@ -597,28 +613,7 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) constrained_beam_rows_kernel(V
     n_comp = m;
   }
 
-  const T* lrow = static_cast<const T*>(a.logits) + static_cast<size_t>(row) * a.ld;
-  const T* bias = static_cast<const T*>(a.bias);
-  float mx = -INFINITY;
-  for (int v = tid; v < V; v += SAMPLE_THREADS) {
-    const float x = head_logit(lrow, bias, v);
-    val[v] = x;
-    mx = fmaxf(mx, x);
-  }
-  mx = block_reduce(mx, redf, [](float p, float q) { return fmaxf(p, q); });
-
-  // from here on thread t owns words [lo, hi)
-  const int Cw = ((V + SAMPLE_THREADS - 1) / SAMPLE_THREADS) | 1;
-  const int lo = min(tid * Cw, V), hi = min(lo + Cw, V);
-  float z = 0.f;
-  for (int v = lo; v < hi; ++v) z += expf(val[v] - mx);
-  const float lse = logf(block_reduce(z, redf, [](float p, float q) { return p + q; }));
-  for (int v = lo; v < hi; ++v) {
-    float lp = (val[v] - mx) - lse;
-    if (blocked && ((bits[v >> 5] >> (v & 31)) & 1u)) lp += -10000.0f;
-    if (a.block_eos && v == a.eos_id) lp = -10000.0f;
-    val[v] = lp;
-  }
+  row_logp<T>(a, row, blocked, bits, val, redf);
   __syncthreads();
   const size_t out = static_cast<size_t>(row) * W;
   if (tid < CA) {                                                    // completing entries, then out of the top-K search
@@ -630,62 +625,7 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) constrained_beam_rows_kernel(V
     if (used) val[w] = __int_as_float(-1);                         // a NaN whose order_key is 0
   }
   __syncthreads();
-  float top = -INFINITY;
-  for (int v = lo; v < hi; ++v) top = fmaxf(top, val[v]);            // fmaxf skips the excluded NaNs
-  top = block_reduce(top, redf, [](float p, float q) { return fmaxf(p, q); });
-
-  // tau = the largest key with at least K words at or above it
-  auto count = [&](unsigned t) {
-    int c = 0;
-    for (int v = lo; v < hi; ++v) c += order_key(val[v]) >= t;
-    return block_reduce(c, redi, [](int p, int q) { return p + q; });
-  };
-  unsigned klo = 0, khi = order_key(top);
-  if (count(khi) >= K) {
-    klo = khi;
-  } else {
-    khi -= 1;
-    while (klo < khi) {                                              // uniform: every thread sees the same counts
-      const unsigned mid = klo + (khi - klo + 1) / 2;
-      if (count(mid) >= K) klo = mid; else khi = mid - 1;
-    }
-  }
-  const unsigned tau = klo;
-  const int take = K - (tau == 0xffffffffu ? 0 : count(tau + 1));   // words tied at tau to keep, lowest index first
-
-  int ties = 0;
-  for (int v = lo; v < hi; ++v) ties += order_key(val[v]) == tau;
-  block_exclusive_scan(ties, redi, prei);
-  const int ties_before = prei[tid];
-  int rank = ties_before, kept = 0;
-  for (int v = lo; v < hi; ++v) {
-    const unsigned k = order_key(val[v]);
-    kept += k > tau || (k == tau && rank++ < take);
-  }
-  block_exclusive_scan(kept, redi, prei);                            // the chunk's first slot among the K kept words
-  int slot = prei[tid];
-  rank = ties_before;
-  for (int v = lo; v < hi; ++v) {
-    const unsigned k = order_key(val[v]);
-    if (k > tau || (k == tau && rank++ < take)) {
-      sel_w[slot] = v;
-      sel_lp[slot] = val[v];
-      ++slot;
-    }
-  }
-  __syncthreads();
-  if (tid < K) {                                                     // rank order: (logp descending, word ascending)
-    const float lp = sel_lp[tid];
-    const unsigned kt = order_key(lp);
-    const int w = sel_w[tid];
-    int r = 0;
-    for (int j = 0; j < K; ++j) {
-      const unsigned kj = order_key(sel_lp[j]);
-      r += kj > kt || (kj == kt && sel_w[j] < w);
-    }
-    a.top_w[out + r] = w;
-    a.top_lp[out + r] = lp;
-  }
+  row_top_k(val, V, K, a.top_w + out, a.top_lp + out, redf, redi, prei, sel_w, sel_lp);
 }
 
 size_t cbs_merge_smem_bytes(int K, int C, int A) {                   // one state's candidates at most: value, parent, word
@@ -753,11 +693,43 @@ __global__ void __launch_bounds__(MERGE_THREADS) constrained_beam_merge_kernel(V
   }
 }
 
-}  // namespace
-
-size_t sample_smem_bytes(int T_cap, int V) {
-  return (static_cast<size_t>(V) + (static_cast<size_t>(V) + 31) / 32 + static_cast<size_t>(T_cap)) * 4;
+// Raises Kernel's dynamic shared memory limit to `bytes` on the first call; the flag is per kernel (a template argument).
+template <auto Kernel>
+int allow_dynamic_smem(int bytes) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    VLPK_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    attr_set = true;
+  }
+  return 0;
 }
+
+// One CTA of SAMPLE_THREADS per row, with `smem` bytes of row_smem, of the fp32 or the bf16 instantiation of a row kernel.
+template <auto KernelF, auto KernelB, typename Args>
+int launch_rows(int rows, size_t smem, cudaStream_t s, const Args& a) {
+  LaunchScope scope(CAT_MISC, (a.fp32 ? 8.0 : 4.0) * rows * a.V, s);
+  if (a.fp32) {
+    VLPK_TRY(allow_dynamic_smem<KernelF>(static_cast<int>(SAMPLE_SMEM_MAX)));
+    KernelF<<<rows, SAMPLE_THREADS, smem, s>>>(a);
+  } else {
+    VLPK_TRY(allow_dynamic_smem<KernelB>(static_cast<int>(SAMPLE_SMEM_MAX)));
+    KernelB<<<rows, SAMPLE_THREADS, smem, s>>>(a);
+  }
+  VLPK_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// The checks every row-kernel launcher shares: the logits' dtype, the frame, the n-gram settings and row_smem's size.
+int check_frame(const char* name, int V, int fp32, int T_cap, int f, int n, int n_ignore, const int* ignore, size_t smem) {
+  VLPK_CHECK_ARG(fp32 == 0 || fp32 == 1, "%s: fp32=%d (0 bf16, 1 fp32)", name, fp32);
+  VLPK_CHECK_ARG(T_cap >= 1 && f >= 0 && f < T_cap, "%s: frame f=%d outside [0, T_cap=%d)", name, f, T_cap);
+  VLPK_CHECK_ARG(n >= 0 && n_ignore >= 0 && (n_ignore == 0 || ignore), "%s: n=%d, ignore set of %d words", name, n, n_ignore);
+  VLPK_CHECK_ARG(smem <= SAMPLE_SMEM_MAX, "%s: T_cap=%d V=%d need %zu bytes of shared memory (at most %zu)", name, T_cap, V, smem,
+                 SAMPLE_SMEM_MAX);
+  return 0;
+}
+
+}  // namespace
 
 int launch_sample(const SampleArgs& a, cudaStream_t s) {
   VLPK_CHECK_ARG(a.rows >= 0 && a.V >= 1 && a.ld >= a.V, "sample: rows=%d V=%d ld=%lld (ld must be >= V >= 1)", a.rows, a.V, a.ld);
@@ -765,32 +737,11 @@ int launch_sample(const SampleArgs& a, cudaStream_t s) {
   VLPK_CHECK_ARG(a.mode != SAMPLE_TOPK || (a.topk >= 1 && a.topk <= SAMPLE_MAX_TOPK), "sample: topk=%d outside [1, %d]", a.topk,
                  SAMPLE_MAX_TOPK);
   VLPK_CHECK_ARG(a.mode != SAMPLE_TOPP || (a.topp > 0.f && a.topp <= 1.f), "sample: topp=%g outside (0, 1]", static_cast<double>(a.topp));
-  VLPK_CHECK_ARG(a.fp32 == 0 || a.fp32 == 1, "sample: fp32=%d (0 bf16, 1 fp32)", a.fp32);
-  VLPK_CHECK_ARG(a.T_cap >= 1 && a.f >= 0 && a.f < a.T_cap, "sample: frame f=%d outside [0, T_cap=%d)", a.f, a.T_cap);
-  VLPK_CHECK_ARG(a.n >= 0 && a.n_ignore >= 0 && (a.n_ignore == 0 || a.ignore), "sample: n=%d, ignore set of %d words", a.n, a.n_ignore);
+  const size_t smem = row_smem_bytes(a.T_cap, a.V);
+  VLPK_TRY(check_frame("sample", a.V, a.fp32, a.T_cap, a.f, a.n, a.n_ignore, a.ignore, smem));
   VLPK_CHECK_ARG(a.logits && a.seq && a.finished && a.live, "sample: null pointer (logits, seq, finished, live)");
-  const size_t smem = sample_smem_bytes(a.T_cap, a.V);
-  VLPK_CHECK_ARG(smem <= SAMPLE_SMEM_MAX, "sample: T_cap=%d V=%d need %zu bytes of shared memory (at most %zu)", a.T_cap, a.V, smem,
-                 SAMPLE_SMEM_MAX);
   if (a.rows == 0) return 0;
-  LaunchScope scope(CAT_MISC, (a.fp32 ? 8.0 : 4.0) * a.rows * a.V, s);
-  if (a.fp32) {
-    static bool attr_set = false;
-    if (!attr_set) {
-      VLPK_CUDA(cudaFuncSetAttribute(sample_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(SAMPLE_SMEM_MAX)));
-      attr_set = true;
-    }
-    sample_kernel<float><<<a.rows, SAMPLE_THREADS, smem, s>>>(a);
-  } else {
-    static bool attr_set = false;
-    if (!attr_set) {
-      VLPK_CUDA(cudaFuncSetAttribute(sample_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(SAMPLE_SMEM_MAX)));
-      attr_set = true;
-    }
-    sample_kernel<bf16><<<a.rows, SAMPLE_THREADS, smem, s>>>(a);
-  }
-  VLPK_CUDA(cudaGetLastError());
-  return 0;
+  return launch_rows<sample_kernel<float>, sample_kernel<bf16>>(a.rows, smem, s, a);
 }
 
 int launch_diverse_beam_step(const DiverseBeamArgs& a, cudaStream_t s) {
@@ -798,12 +749,10 @@ int launch_diverse_beam_step(const DiverseBeamArgs& a, cudaStream_t s) {
                  DIVERSE_MAX_BEAMS);
   VLPK_CHECK_ARG(a.G >= 1 && a.K % a.G == 0, "diverse_beam_step: G=%d groups do not divide K=%d beams", a.G, a.K);
   VLPK_CHECK_ARG(a.V >= a.K && a.ld >= a.V, "diverse_beam_step: V=%d ld=%lld K=%d (ld >= V >= K needed)", a.V, a.ld, a.K);
-  VLPK_CHECK_ARG(a.fp32 == 0 || a.fp32 == 1, "diverse_beam_step: fp32=%d (0 bf16, 1 fp32)", a.fp32);
   VLPK_CHECK_ARG(isfinite(a.lambda) && a.lambda >= 0.f, "diverse_beam_step: diversity penalty %g (finite and >= 0 needed)",
                  static_cast<double>(a.lambda));
-  VLPK_CHECK_ARG(a.T_cap >= 1 && a.f >= 0 && a.f < a.T_cap, "diverse_beam_step: frame f=%d outside [0, T_cap=%d)", a.f, a.T_cap);
-  VLPK_CHECK_ARG(a.n >= 0 && a.n_ignore >= 0 && (a.n_ignore == 0 || a.ignore), "diverse_beam_step: n=%d, ignore set of %d words", a.n,
-                 a.n_ignore);
+  const size_t smem = row_smem_bytes(a.T_cap, a.V);
+  VLPK_TRY(check_frame("diverse_beam_step", a.V, a.fp32, a.T_cap, a.f, a.n, a.n_ignore, a.ignore, smem));
   VLPK_CHECK_ARG(a.logits && a.top_w && a.top_lp && a.wid && a.ptr && a.score && a.eos,
                  "diverse_beam_step: null pointer (logits, top_w, top_lp, wid, ptr, score, eos)");
   VLPK_CHECK_ARG(a.f == 0 || (a.prev_score && a.prev_eos), "diverse_beam_step: null pointer (prev_score, prev_eos are needed at f=%d)",
@@ -813,32 +762,9 @@ int launch_diverse_beam_step(const DiverseBeamArgs& a, cudaStream_t s) {
   VLPK_CHECK_ARG(!hist || a.f == 1 || (a.hist_in && a.prev_ptr), "diverse_beam_step: null pointer (hist_in, prev_ptr are needed at f=%d)",
                  a.f);
   VLPK_CHECK_ARG(!hist || a.hist_in != a.hist_out, "diverse_beam_step: hist_in and hist_out must be different buffers");
-  const size_t smem = sample_smem_bytes(a.T_cap, a.V);
-  VLPK_CHECK_ARG(smem <= SAMPLE_SMEM_MAX, "diverse_beam_step: T_cap=%d V=%d need %zu bytes of shared memory (at most %zu)", a.T_cap, a.V,
-                 smem, SAMPLE_SMEM_MAX);
   if (a.B == 0) return 0;
   const int rows = a.f == 0 ? a.B : a.B * a.K;
-  {
-    LaunchScope scope(CAT_MISC, (a.fp32 ? 8.0 : 4.0) * rows * a.V, s);
-    if (a.fp32) {
-      static bool attr_set = false;
-      if (!attr_set) {
-        VLPK_CUDA(cudaFuncSetAttribute(diverse_beam_rows_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       static_cast<int>(SAMPLE_SMEM_MAX)));
-        attr_set = true;
-      }
-      diverse_beam_rows_kernel<float><<<rows, SAMPLE_THREADS, smem, s>>>(a);
-    } else {
-      static bool attr_set = false;
-      if (!attr_set) {
-        VLPK_CUDA(cudaFuncSetAttribute(diverse_beam_rows_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       static_cast<int>(SAMPLE_SMEM_MAX)));
-        attr_set = true;
-      }
-      diverse_beam_rows_kernel<bf16><<<rows, SAMPLE_THREADS, smem, s>>>(a);
-    }
-    VLPK_CUDA(cudaGetLastError());
-  }
+  VLPK_TRY((launch_rows<diverse_beam_rows_kernel<float>, diverse_beam_rows_kernel<bf16>>(rows, smem, s, a)));
   LaunchScope scope(CAT_MISC, 8.0 * rows * a.K, s);
   diverse_beam_merge_kernel<<<a.B, MERGE_THREADS, 0, s>>>(a);
   VLPK_CUDA(cudaGetLastError());
@@ -853,57 +779,22 @@ int launch_constrained_beam_step(const VlpkConstrainedBeamArgs& a, cudaStream_t 
                  "constrained_beam_step: B=%d K=%d C=%d (K in [1, %d] and 2^C * K <= %d needed)", a.B, a.K, a.C, CBS_MAX_BEAMS, CBS_MAX_SLOTS);
   VLPK_CHECK_ARG(a.V >= a.K + a.C * a.A && a.ld >= a.V, "constrained_beam_step: V=%d ld=%lld (ld >= V >= K + C*A = %d needed)", a.V,
                  static_cast<long long>(a.ld), a.K + a.C * a.A);
-  VLPK_CHECK_ARG(a.fp32 == 0 || a.fp32 == 1, "constrained_beam_step: fp32=%d (0 bf16, 1 fp32)", a.fp32);
-  VLPK_CHECK_ARG(a.T_cap >= 1 && a.f >= 0 && a.f < a.T_cap, "constrained_beam_step: frame f=%d outside [0, T_cap=%d)", a.f, a.T_cap);
-  VLPK_CHECK_ARG(a.n >= 0 && a.n_ignore >= 0 && (a.n_ignore == 0 || a.ignore), "constrained_beam_step: n=%d, ignore set of %d words", a.n,
-                 a.n_ignore);
+  const size_t smem = row_smem_bytes(a.T_cap, a.V);
+  VLPK_TRY(check_frame("constrained_beam_step", a.V, a.fp32, a.T_cap, a.f, a.n, a.n_ignore, a.ignore, smem));
   VLPK_CHECK_ARG(a.logits && a.cons && a.top_w && a.top_lp && a.top_dest && a.wid && a.ptr && a.score && a.eos,
                  "constrained_beam_step: null pointer (logits, cons, top_w, top_lp, top_dest, wid, ptr, score, eos)");
   VLPK_CHECK_ARG(a.f == 0 || (a.prev_score && a.prev_eos && a.prev_wid && a.hist_out),
                  "constrained_beam_step: null pointer (prev_score, prev_eos, prev_wid, hist_out are needed at f=%d)", a.f);
   VLPK_CHECK_ARG(a.f <= 1 || (a.hist_in && a.prev_ptr), "constrained_beam_step: null pointer (hist_in, prev_ptr are needed at f=%d)", a.f);
   VLPK_CHECK_ARG(a.f == 0 || a.hist_in != a.hist_out, "constrained_beam_step: hist_in and hist_out must be different buffers");
-  const size_t smem = sample_smem_bytes(a.T_cap, a.V);
-  VLPK_CHECK_ARG(smem <= SAMPLE_SMEM_MAX, "constrained_beam_step: T_cap=%d V=%d need %zu bytes of shared memory (at most %zu)", a.T_cap,
-                 a.V, smem, SAMPLE_SMEM_MAX);
   if (a.B == 0) return 0;
   const int SK = a.K << a.C, rows = a.f == 0 ? a.B : a.B * SK;
-  {
-    LaunchScope scope(CAT_MISC, (a.fp32 ? 8.0 : 4.0) * rows * a.V, s);
-    if (a.fp32) {
-      static bool attr_set = false;
-      if (!attr_set) {
-        VLPK_CUDA(cudaFuncSetAttribute(constrained_beam_rows_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       static_cast<int>(SAMPLE_SMEM_MAX)));
-        attr_set = true;
-      }
-      constrained_beam_rows_kernel<float><<<rows, SAMPLE_THREADS, smem, s>>>(a);
-    } else {
-      static bool attr_set = false;
-      if (!attr_set) {
-        VLPK_CUDA(cudaFuncSetAttribute(constrained_beam_rows_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       static_cast<int>(SAMPLE_SMEM_MAX)));
-        attr_set = true;
-      }
-      constrained_beam_rows_kernel<bf16><<<rows, SAMPLE_THREADS, smem, s>>>(a);
-    }
-    VLPK_CUDA(cudaGetLastError());
-  }
-  const size_t merge_smem = cbs_merge_smem_bytes(a.K, a.C, a.A);
-  static bool attr_set = false;
-  if (!attr_set) {
-    VLPK_CUDA(cudaFuncSetAttribute(constrained_beam_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   static_cast<int>(cbs_merge_smem_bytes(CBS_MAX_BEAMS, 2, CBS_MAX_ALTS))));
-    attr_set = true;
-  }
+  VLPK_TRY((launch_rows<constrained_beam_rows_kernel<float>, constrained_beam_rows_kernel<bf16>>(rows, smem, s, a)));
+  VLPK_TRY(allow_dynamic_smem<constrained_beam_merge_kernel>(static_cast<int>(cbs_merge_smem_bytes(CBS_MAX_BEAMS, 2, CBS_MAX_ALTS))));
   LaunchScope scope(CAT_MISC, 8.0 * rows * (a.K + a.C * a.A), s);
-  constrained_beam_merge_kernel<<<dim3(1 << a.C, a.B), MERGE_THREADS, merge_smem, s>>>(a);
+  constrained_beam_merge_kernel<<<dim3(1 << a.C, a.B), MERGE_THREADS, cbs_merge_smem_bytes(a.K, a.C, a.A), s>>>(a);
   VLPK_CUDA(cudaGetLastError());
   return 0;
-}
-
-size_t ngram_block_smem_bytes(int T_cap, int V) {
-  return (static_cast<size_t>(T_cap) + (static_cast<size_t>(V) + 31) / 32) * 4;
 }
 
 int launch_beam_ngram_block(const NgramBlockArgs& a, cudaStream_t s) {

@@ -1,4 +1,5 @@
-// vlp_b200 — beam-search duplicate-n-gram blocking on the device (see decode.cu).
+// vlp_b200 — the per-frame selection of the device decoders: n-gram blocking, sampling, diverse and constrained beam search
+// (see decode.cu).
 #pragma once
 #include "../../include/vlpk.h"
 #include "common.cuh"
@@ -21,7 +22,6 @@ struct NgramBlockArgs {
   int V = 0;
 };
 
-size_t ngram_block_smem_bytes(int T_cap, int V);
 int launch_beam_ngram_block(const NgramBlockArgs& a, cudaStream_t s);
 
 // Top-k / top-p sampling of one decode frame, one CTA per row (see decode.cu).
@@ -51,7 +51,6 @@ struct SampleArgs {
   int n_ignore = 0;
 };
 
-size_t sample_smem_bytes(int T_cap, int V);
 int launch_sample(const SampleArgs& a, cudaStream_t s);
 
 // Diverse beam search: one frame's selection, K beams per image in G groups with a Hamming penalty (see decode.cu).

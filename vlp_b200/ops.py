@@ -628,6 +628,59 @@ def layer_cached_group_fwd(hidden, prefix, P, text, slots, G, pos, mask_bits, he
 
 
 # ------------------------------------------------------------------------------------------------
+# the per-frame selectors' tensor contracts
+# ------------------------------------------------------------------------------------------------
+def _require_cuda_all(*pairs):
+    """_require_cuda over (tensor, what) pairs; None tensors are skipped."""
+    for t, what in pairs:
+        if t is not None:
+            _require_cuda(t, what)
+
+
+def _logit_rows(logits, what, rows=None, rows_rule=""):
+    """The head's logits [rows, ..., V] as (lg [rows, V], V, rows): bf16 or fp32 with unit stride in V, and `rows` rows if given."""
+    V = logits.shape[-1]
+    lg = logits.reshape(-1, V) if logits.dim() != 2 else logits
+    if logits.dtype not in (BF16, torch.float32) or lg.stride(1) != 1 or (rows is not None and lg.shape[0] != rows):
+        raise RuntimeError(f"vlp_b200: {what} logits must be bf16 or fp32 [rows, V] with unit column stride{rows_rule}")
+    return lg, V, lg.shape[0]
+
+
+def _check_bias(bias, logits, V):
+    if bias is not None and (bias.dtype != logits.dtype or bias.shape != (V,) or not bias.is_contiguous()):
+        raise RuntimeError("vlp_b200: the logit bias must be a contiguous [V] tensor of the logits' dtype")
+
+
+def _ignore_set(ignore, used=True):
+    """The n-gram ignore set (int32 device tensor of word ids, or None) as (pointer, count): (None, 0) when empty or not used."""
+    if ignore is not None and (ignore.dtype != torch.int32 or ignore.dim() != 1 or not ignore.is_contiguous()):
+        raise RuntimeError("vlp_b200: the n-gram ignore set must be a contiguous 1-D int32 tensor of word ids")
+    n = ignore.numel() if ignore is not None and used else 0
+    return (ignore.data_ptr() if n else None), n
+
+
+def _check_histories(hist_in, hist_out, rows, what, rows_name):
+    """Two contiguous int32 [rows, T_cap] word histories; returns T_cap."""
+    if hist_in is None or hist_out is None or hist_in.shape != hist_out.shape or hist_out.dim() != 2 or hist_out.shape[0] != rows \
+            or hist_in.dtype != torch.int32 or hist_out.dtype != torch.int32 or not (hist_in.is_contiguous() and hist_out.is_contiguous()):
+        raise RuntimeError(f"vlp_b200: {what} histories must be two contiguous int32 [{rows_name}, T_cap] tensors")
+    return hist_out.shape[1]
+
+
+def _beam_traces(wid, ptr, score, eos, f, slots_name):
+    """Beam traces wid / ptr (int64) and score / eos (fp32), contiguous [T, B, slots], at frame f: ((T, B, slots), frame f-1's four
+    rows, or four None at f = 0)."""
+    if wid.dim() != 3 or any(t.shape != wid.shape or not t.is_contiguous() for t in (wid, ptr, score, eos)) \
+            or wid.dtype != torch.int64 or ptr.dtype != torch.int64 or score.dtype != torch.float32 or eos.dtype != torch.float32:
+        raise RuntimeError(f"vlp_b200: beam traces must be contiguous [T, B, {slots_name}] tensors: int64 word ids and pointers, fp32 "
+                           "scores and eos flags")
+    T = wid.shape[0]
+    if not 0 <= f < T:
+        raise ValueError(f"vlp_b200: frame {f} outside the traces' {T} frames")
+    return wid.shape, ((wid[f - 1], ptr[f - 1], score[f - 1], eos[f - 1]) if f else (None,) * 4)
+
+
+# ------------------------------------------------------------------------------------------------
 # beam search
 # ------------------------------------------------------------------------------------------------
 def beam_ngram_block(hist_in, hist_out, ptr, wid, f, n, ignore, logp):
@@ -635,25 +688,20 @@ def beam_ngram_block(hist_in, hist_out, ptr, wid, f, n, ignore, logp):
     hist_in[parent] + wid of every hypothesis (ptr / wid: int64 [B, K] back pointers and word ids of frame f-1); if f >= n, logp
     (fp32, [B*K, ..., V] with unit stride in V) gets -10000 added in place at each hypothesis' repeated-n-gram completions.
     ignore: int32 device tensor of exempt word ids, or None."""
-    for t, what in ((hist_in, "n-gram history"), (hist_out, "n-gram history"), (ptr, "beam back pointers"), (wid, "beam word ids"),
-                    (logp, "beam log-probabilities")) + (() if ignore is None else ((ignore, "n-gram ignore set"),)):
-        _require_cuda(t, what)
+    _require_cuda_all((hist_in, "n-gram history"), (hist_out, "n-gram history"), (ptr, "beam back pointers"), (wid, "beam word ids"),
+                      (logp, "beam log-probabilities"), (ignore, "n-gram ignore set"))
     B, K = wid.shape
-    rows, T_cap = hist_out.shape
+    rows = B * K
+    T_cap = _check_histories(hist_in, hist_out, rows, "n-gram", "B*K")
     V = logp.shape[-1]
-    if rows != B * K or hist_out.dtype != torch.int32 or not hist_out.is_contiguous() or hist_in.shape != hist_out.shape \
-            or hist_in.dtype != torch.int32 or not hist_in.is_contiguous():
-        raise RuntimeError("vlp_b200: n-gram histories must be two contiguous int32 [B*K, T_cap] tensors")
     if ptr.dtype != torch.int64 or wid.dtype != torch.int64 or not (ptr.is_contiguous() and wid.is_contiguous()) or ptr.shape != wid.shape:
         raise RuntimeError("vlp_b200: back pointers and word ids must be contiguous int64 [B, K] tensors")
     lp = logp.view(rows, -1) if logp.dim() != 2 else logp
     if logp.dtype != torch.float32 or lp.stride(1) != 1 or lp.shape[0] != rows:
         raise RuntimeError("vlp_b200: beam log-probabilities must be fp32 [B*K, V] rows with unit column stride")
-    if ignore is not None and (ignore.dtype != torch.int32 or ignore.dim() != 1 or not ignore.is_contiguous()):
-        raise RuntimeError("vlp_b200: the n-gram ignore set must be a contiguous 1-D int32 tensor of word ids")
-    n_ign = 0 if ignore is None else ignore.numel()
+    ign, n_ign = _ignore_set(ignore)
     L.call("vlpk_beam_ngram_block", rows, K, int(f), T_cap, int(n), hist_in.data_ptr(), hist_out.data_ptr(), ptr.data_ptr(),
-           wid.data_ptr(), ignore.data_ptr() if n_ign else None, n_ign, lp.data_ptr(), lp.stride(0), V, L.stream())
+           wid.data_ptr(), ign, n_ign, lp.data_ptr(), lp.stride(0), V, L.stream())
 
 
 # ------------------------------------------------------------------------------------------------
@@ -670,32 +718,22 @@ def sample_tokens(logits, bias, mode, topk, topp, seed, f, seq, score, finished,
     seq[row, :f] when ngram > 0 and [EOS] when block_eos, keeps the top-k words or the top-p nucleus and draws one with the
     Philox uniform keyed by (seed; f, row).  seq: int64 [rows, T] receives column f; score: fp32 [rows, T] or None; finished: int32
     [rows]; live: int32 [1], decremented once per row that draws eos_id.  ignore: int32 device tensor of exempt word ids, or None."""
-    tensors = ((logits, "logits"), (seq, "sampled ids"), (finished, "finished flags"), (live, "live-row count"))
-    for t, what in tensors + tuple((t, w) for t, w in ((bias, "logit bias"), (score, "scores"), (ignore, "n-gram ignore set"))
-                                   if t is not None):
-        _require_cuda(t, what)
+    _require_cuda_all((logits, "logits"), (seq, "sampled ids"), (finished, "finished flags"), (live, "live-row count"),
+                      (bias, "logit bias"), (score, "scores"), (ignore, "n-gram ignore set"))
     if mode not in SAMPLE_MODES:
         raise ValueError(f"vlp_b200: sampling mode must be one of {sorted(SAMPLE_MODES)}, got {mode!r}")
-    V = logits.shape[-1]
-    lg = logits.reshape(-1, V) if logits.dim() != 2 else logits
-    rows = lg.shape[0]
-    if logits.dtype not in (BF16, torch.float32) or lg.stride(1) != 1:
-        raise RuntimeError("vlp_b200: sampling logits must be bf16 or fp32 [rows, V] with unit column stride")
-    if bias is not None and (bias.dtype != logits.dtype or bias.shape != (V,) or not bias.is_contiguous()):
-        raise RuntimeError("vlp_b200: the logit bias must be a contiguous [V] tensor of the logits' dtype")
+    lg, V, rows = _logit_rows(logits, "sampling")
+    _check_bias(bias, logits, V)
     if seq.dtype != torch.int64 or seq.dim() != 2 or seq.shape[0] != rows or not seq.is_contiguous():
         raise RuntimeError("vlp_b200: sampled ids must be a contiguous int64 [rows, T] tensor")
     if score is not None and (score.dtype != torch.float32 or score.shape != seq.shape or not score.is_contiguous()):
         raise RuntimeError("vlp_b200: sampling scores must be a contiguous fp32 tensor shaped like the ids")
     if finished.dtype != torch.int32 or finished.shape != (rows,) or live.dtype != torch.int32 or live.numel() != 1:
         raise RuntimeError("vlp_b200: finished flags must be int32 [rows] and the live-row count an int32 [1] tensor")
-    if ignore is not None and (ignore.dtype != torch.int32 or ignore.dim() != 1 or not ignore.is_contiguous()):
-        raise RuntimeError("vlp_b200: the n-gram ignore set must be a contiguous 1-D int32 tensor of word ids")
-    n_ign = 0 if ignore is None else ignore.numel()
+    ign, n_ign = _ignore_set(ignore)
     L.call("vlpk_sample_tokens", rows, V, lg.data_ptr(), lg.stride(0), L.ptr(bias), int(logits.dtype == torch.float32), SAMPLE_MODES[mode],
            int(topk), float(topp), int(seed) & 0xFFFFFFFFFFFFFFFF, int(f), seq.data_ptr(), seq.shape[1], L.ptr(score), finished.data_ptr(),
-           live.data_ptr(), int(eos_id), int(pad_id), int(bool(block_eos)), int(ngram), ignore.data_ptr() if n_ign else None, n_ign,
-           L.stream())
+           live.data_ptr(), int(eos_id), int(pad_id), int(bool(block_eos)), int(ngram), ign, n_ign, L.stream())
 
 
 # ------------------------------------------------------------------------------------------------
@@ -709,42 +747,21 @@ def diverse_beam_step(logits, bias, f, G, penalty, wid, ptr, score, eos, top_w, 
     written and frame f-1 read.  top_w (int32) / top_lp (fp32): contiguous [B*K, K] scratch.  ngram > 0: duplicate-n-gram blocking
     over the int32 [B*K, T_cap] histories hist_in (frame f-1) and hist_out (frame f), two different tensors used in turn; ignore:
     int32 device tensor of exempt word ids, or None.  block_eos: the frame is below min_len."""
-    tensors = ((logits, "logits"), (wid, "beam word ids"), (ptr, "beam back pointers"), (score, "beam scores"), (eos, "beam eos flags"),
-               (top_w, "top-K scratch"), (top_lp, "top-K scratch"))
-    extra = ((bias, "logit bias"), (ignore, "n-gram ignore set"), (hist_in, "n-gram history"), (hist_out, "n-gram history"))
-    for t, what in tensors + tuple((t, w) for t, w in extra if t is not None):
-        _require_cuda(t, what)
-    if wid.dim() != 3 or any(t.shape != wid.shape or not t.is_contiguous() for t in (wid, ptr, score, eos)) \
-            or wid.dtype != torch.int64 or ptr.dtype != torch.int64 or score.dtype != torch.float32 or eos.dtype != torch.float32:
-        raise RuntimeError("vlp_b200: beam traces must be contiguous [T, B, K] tensors: int64 word ids and pointers, fp32 scores and "
-                           "eos flags")
-    T, B, K = wid.shape
-    if not 0 <= f < T:
-        raise ValueError(f"vlp_b200: frame {f} outside the traces' {T} frames")
-    V = logits.shape[-1]
-    lg = logits.reshape(-1, V) if logits.dim() != 2 else logits
-    if logits.dtype not in (BF16, torch.float32) or lg.stride(1) != 1 or lg.shape[0] != (B if f == 0 else B * K):
-        raise RuntimeError("vlp_b200: diverse-beam logits must be bf16 or fp32 [rows, V] with unit column stride, rows = B at frame 0 "
-                           "and B*K after")
-    if bias is not None and (bias.dtype != logits.dtype or bias.shape != (V,) or not bias.is_contiguous()):
-        raise RuntimeError("vlp_b200: the logit bias must be a contiguous [V] tensor of the logits' dtype")
+    _require_cuda_all((logits, "logits"), (wid, "beam word ids"), (ptr, "beam back pointers"), (score, "beam scores"),
+                      (eos, "beam eos flags"), (top_w, "top-K scratch"), (top_lp, "top-K scratch"), (bias, "logit bias"),
+                      (ignore, "n-gram ignore set"), (hist_in, "n-gram history"), (hist_out, "n-gram history"))
+    (T, B, K), prev = _beam_traces(wid, ptr, score, eos, f, "K")
+    lg, V, _ = _logit_rows(logits, "diverse-beam", B if f == 0 else B * K, ", rows = B at frame 0 and B*K after")
+    _check_bias(bias, logits, V)
     if top_w.dtype != torch.int32 or top_lp.dtype != torch.float32 or top_w.shape != (B * K, K) or top_lp.shape != (B * K, K) \
             or not (top_w.is_contiguous() and top_lp.is_contiguous()):
         raise RuntimeError("vlp_b200: the top-K scratch must be contiguous int32 and fp32 [B*K, K] tensors")
-    T_cap = T
-    if ngram:
-        if hist_in is None or hist_out is None or hist_in.shape != hist_out.shape or hist_out.dim() != 2 or hist_out.shape[0] != B * K \
-                or hist_in.dtype != torch.int32 or hist_out.dtype != torch.int32 or not (hist_in.is_contiguous() and hist_out.is_contiguous()):
-            raise RuntimeError("vlp_b200: n-gram histories must be two contiguous int32 [B*K, T_cap] tensors")
-        T_cap = hist_out.shape[1]
-    if ignore is not None and (ignore.dtype != torch.int32 or ignore.dim() != 1 or not ignore.is_contiguous()):
-        raise RuntimeError("vlp_b200: the n-gram ignore set must be a contiguous 1-D int32 tensor of word ids")
-    n_ign = 0 if ignore is None or not ngram else ignore.numel()
-    prev = (wid[f - 1], ptr[f - 1], score[f - 1], eos[f - 1]) if f else (None,) * 4
+    T_cap = _check_histories(hist_in, hist_out, B * K, "n-gram", "B*K") if ngram else T
+    ign, n_ign = _ignore_set(ignore, used=bool(ngram))
     L.call("vlpk_diverse_beam_step", B, K, int(G), int(f), V, lg.data_ptr(), lg.stride(0), L.ptr(bias), int(logits.dtype == torch.float32),
            float(penalty), int(eos_id), int(bool(block_eos)), T_cap, int(ngram), L.ptr(hist_in if ngram else None),
-           L.ptr(hist_out if ngram else None), ignore.data_ptr() if n_ign else None, n_ign, *(L.ptr(t) for t in prev), top_w.data_ptr(),
-           top_lp.data_ptr(), wid[f].data_ptr(), ptr[f].data_ptr(), score[f].data_ptr(), eos[f].data_ptr(), L.stream())
+           L.ptr(hist_out if ngram else None), ign, n_ign, *(L.ptr(t) for t in prev), top_w.data_ptr(), top_lp.data_ptr(),
+           wid[f].data_ptr(), ptr[f].data_ptr(), score[f].data_ptr(), eos[f].data_ptr(), L.stream())
 
 
 # ------------------------------------------------------------------------------------------------
@@ -759,52 +776,31 @@ def constrained_beam_step(logits, bias, f, cons, wid, ptr, score, eos, top_w, to
     contiguous [B*S*K, K + C*A] scratch, top_dest (int32) [B*S*K, C*A].  hist_in / hist_out: the int32 [B*S*K, T_cap] histories of
     frames f-1 and f, two different tensors used in turn (needed at f >= 1, whatever ngram).  ngram > 0: duplicate-n-gram blocking;
     ignore: int32 device tensor of exempt word ids, or None.  block_eos: the frame is below min_len."""
-    tensors = ((logits, "logits"), (cons, "constraint table"), (wid, "beam word ids"), (ptr, "beam back pointers"), (score, "beam scores"),
-               (eos, "beam eos flags"), (top_w, "top-K scratch"), (top_lp, "top-K scratch"), (top_dest, "top-K scratch"))
-    extra = ((bias, "logit bias"), (ignore, "n-gram ignore set"), (hist_in, "word history"), (hist_out, "word history"))
-    for t, what in tensors + tuple((t, w) for t, w in extra if t is not None):
-        _require_cuda(t, what)
+    _require_cuda_all((logits, "logits"), (cons, "constraint table"), (wid, "beam word ids"), (ptr, "beam back pointers"),
+                      (score, "beam scores"), (eos, "beam eos flags"), (top_w, "top-K scratch"), (top_lp, "top-K scratch"),
+                      (top_dest, "top-K scratch"), (bias, "logit bias"), (ignore, "n-gram ignore set"), (hist_in, "word history"),
+                      (hist_out, "word history"))
     if cons.dim() != 4 or cons.dtype != torch.int64 or not cons.is_contiguous():
         raise RuntimeError("vlp_b200: the constraint table must be a contiguous int64 [B, C, A, P] tensor")
     Bc, C, A, P = cons.shape
-    if wid.dim() != 3 or any(t.shape != wid.shape or not t.is_contiguous() for t in (wid, ptr, score, eos)) \
-            or wid.dtype != torch.int64 or ptr.dtype != torch.int64 or score.dtype != torch.float32 or eos.dtype != torch.float32:
-        raise RuntimeError("vlp_b200: beam traces must be contiguous [T, B, S*K] tensors: int64 word ids and pointers, fp32 scores and "
-                           "eos flags")
-    T, B, SK = wid.shape
+    (T, B, SK), prev = _beam_traces(wid, ptr, score, eos, f, "S*K")
     if Bc != B or C < 1 or SK % (1 << C):
         raise RuntimeError(f"vlp_b200: a constraint table [{Bc}, {C}, ...] does not match traces of {B} images and {SK} slots "
                            "(2^C states of K beams)")
     K = SK >> C
-    if not 0 <= f < T:
-        raise ValueError(f"vlp_b200: frame {f} outside the traces' {T} frames")
-    V = logits.shape[-1]
-    lg = logits.reshape(-1, V) if logits.dim() != 2 else logits
-    if logits.dtype not in (BF16, torch.float32) or lg.stride(1) != 1 or lg.shape[0] != (B if f == 0 else B * SK):
-        raise RuntimeError("vlp_b200: constrained-beam logits must be bf16 or fp32 [rows, V] with unit column stride, rows = B at frame 0 "
-                           "and B*S*K after")
-    if bias is not None and (bias.dtype != logits.dtype or bias.shape != (V,) or not bias.is_contiguous()):
-        raise RuntimeError("vlp_b200: the logit bias must be a contiguous [V] tensor of the logits' dtype")
+    lg, V, _ = _logit_rows(logits, "constrained-beam", B if f == 0 else B * SK, ", rows = B at frame 0 and B*S*K after")
+    _check_bias(bias, logits, V)
     W = K + C * A
     if top_w.dtype != torch.int32 or top_lp.dtype != torch.float32 or top_dest.dtype != torch.int32 or top_w.shape != (B * SK, W) \
             or top_lp.shape != (B * SK, W) or top_dest.shape != (B * SK, C * A) \
             or not (top_w.is_contiguous() and top_lp.is_contiguous() and top_dest.is_contiguous()):
         raise RuntimeError("vlp_b200: the top-K scratch must be contiguous int32 / fp32 [B*S*K, K + C*A] and int32 [B*S*K, C*A] tensors")
-    T_cap = T
-    if hist_out is not None or f:
-        if hist_in is None or hist_out is None or hist_in.shape != hist_out.shape or hist_out.dim() != 2 or hist_out.shape[0] != B * SK \
-                or hist_in.dtype != torch.int32 or hist_out.dtype != torch.int32 or not (hist_in.is_contiguous() and hist_out.is_contiguous()):
-            raise RuntimeError("vlp_b200: word histories must be two contiguous int32 [B*S*K, T_cap] tensors")
-        T_cap = hist_out.shape[1]
-    if ignore is not None and (ignore.dtype != torch.int32 or ignore.dim() != 1 or not ignore.is_contiguous()):
-        raise RuntimeError("vlp_b200: the n-gram ignore set must be a contiguous 1-D int32 tensor of word ids")
-    n_ign = 0 if ignore is None or not ngram else ignore.numel()
-    prev = (wid[f - 1], ptr[f - 1], score[f - 1], eos[f - 1]) if f else (None,) * 4
+    T_cap = _check_histories(hist_in, hist_out, B * SK, "word", "B*S*K") if hist_out is not None or f else T
+    ign, n_ign = _ignore_set(ignore, used=bool(ngram))
     a = L.VlpkConstrainedBeamArgs(B=B, K=K, C=C, A=A, P=P, f=int(f), V=V, logits=lg.data_ptr(), ld=lg.stride(0), bias=L.ptr(bias),
                                   fp32=int(logits.dtype == torch.float32), eos_id=int(eos_id), block_eos=int(bool(block_eos)), T_cap=T_cap,
-                                  n=int(ngram), hist_in=L.ptr(hist_in), hist_out=L.ptr(hist_out),
-                                  ignore=ignore.data_ptr() if n_ign else None, n_ignore=n_ign, cons=cons.data_ptr(),
-                                  prev_wid=L.ptr(prev[0]), prev_ptr=L.ptr(prev[1]), prev_score=L.ptr(prev[2]), prev_eos=L.ptr(prev[3]),
-                                  top_w=top_w.data_ptr(), top_lp=top_lp.data_ptr(), top_dest=top_dest.data_ptr(), wid=wid[f].data_ptr(),
-                                  ptr=ptr[f].data_ptr(), score=score[f].data_ptr(), eos=eos[f].data_ptr())
+                                  n=int(ngram), hist_in=L.ptr(hist_in), hist_out=L.ptr(hist_out), ignore=ign, n_ignore=n_ign,
+                                  cons=cons.data_ptr(), prev_wid=L.ptr(prev[0]), prev_ptr=L.ptr(prev[1]), prev_score=L.ptr(prev[2]),
+                                  prev_eos=L.ptr(prev[3]), top_w=top_w.data_ptr(), top_lp=top_lp.data_ptr(), top_dest=top_dest.data_ptr(),
+                                  wid=wid[f].data_ptr(), ptr=ptr[f].data_ptr(), score=score[f].data_ptr(), eos=eos[f].data_ptr())
     L.call("vlpk_constrained_beam_step", L.C.byref(a), L.stream())
