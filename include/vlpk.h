@@ -449,6 +449,9 @@ int vlpk_sample_tokens(int rows, int V, const void* logits, int64_t ld, const vo
  *   groups      g = 0 .. G-1 in turn: group g's parents are beams [g*Kg, (g+1)*Kg) (row b at f = 0); it keeps the Kg (parent, word)
  *     pairs with the largest cand - diversity_penalty * cnt(w), cnt(w) = beams of groups < g that chose w in this frame; ties go
  *     to the lower parent, then the lower word.  Its r-th pair becomes beam g*Kg + r.
+ *   NaN          ranks above every number (as torch.topk ranks it), and NaNs tie.  A row with a NaN or +inf x, or whose every x is
+ *     -inf, has a NaN logsumexp, so its logp is NaN (but at eos_id under block_eos): its pairs rank first, lower parent and word
+ *     first, and every word id written stays in [0, V).
  *   traces      wid / ptr int64 [B, K] (ptr a beam index in [0, K), 0 at f = 0), score fp32 [B, K] the unpenalised cand, eos fp32
  *     [B, K] (wid == eos_id).  top_w int32 / top_lp fp32 [rows, K] are scratch (each row's top K words).
  * Bitwise reproducible.  Returns < 0 without launching for K outside [1, 64], G not dividing K, V < K, ld < V, a penalty that is
@@ -475,6 +478,8 @@ int vlpk_diverse_beam_step(int B, int K, int G, int f, int V, const void* logits
  *   dest(i, w)   s_i ∪ {j : w completes an alternative a of j}: a[-1] == w and the row's last len(a) - 1 words equal a[:-1].
  *   selection    state s' keeps the K (row, word) pairs with dest == s' and the largest finite cand, ties to the lower parent slot, then
  *     the lower word; its r-th pair becomes slot s'*K + r.  Slots it cannot fill are empty: word 0, pointer 0, score -inf, eos 0.
+ *     Non-finite cands are dropped: a row with a NaN or +inf x, or whose every x is -inf, has a NaN logsumexp and offers no pair
+ *     but its eos_id under block_eos (logp -10000).
  *   traces       wid / ptr int64 [B, S*K] (ptr a slot in [0, S*K), 0 at f = 0), score fp32 [B, S*K] the cand, eos fp32 [B, S*K]
  *     (wid == eos_id).  top_w int32 / top_lp fp32 [rows, K + C*A] and top_dest int32 [rows, C*A] are scratch: each row's top K
  *     words that keep it in its state, then its completing words and their destinations.

@@ -33,7 +33,8 @@ def _cand(lp_rows, prev_score, prev_eos, first, dtype):
 
 
 def _merge(parents, words, cands, K, G, lam, dtype):
-    """Groups g = 0 .. G-1 over per-group candidate arrays (parents, words, cands of group g) -> wid, ptr, score [K], margin: the
+    """Groups g = 0 .. G-1 over per-group candidate arrays (parents, words, cands of group g), NaN ranked above every number as the
+    kernel ranks it -> wid, ptr, score [K], margin: the
     smallest gap between consecutive penalised values among each group's Kg + 1 best.  An exact tie between two words of the same
     parent and penalty does not count: both values come from the same row's logsumexp, parent score and penalty, so any
     implementation that rounds a row consistently sees the same tie and breaks it by word id."""
@@ -46,7 +47,8 @@ def _merge(parents, words, cands, K, G, lam, dtype):
         for q in wid[:g * Kg]:
             cnt += (w == q)
         pen = (c - (dtype(lam) * cnt).astype(dtype)).astype(dtype)
-        order = np.lexsort((w, p, -pen))
+        nan = np.isnan(pen)
+        order = np.lexsort((w, p, np.where(nan, 0, -pen), ~nan))          # NaN ranks above every number, then ties by (parent, word)
         sel = order[:Kg]
         wid[g * Kg:(g + 1) * Kg], ptr[g * Kg:(g + 1) * Kg], score[g * Kg:(g + 1) * Kg] = w[sel], p[sel], c[sel]
         top = order[:Kg + 1]

@@ -246,18 +246,19 @@ __device__ __forceinline__ void row_logp(const Args& a, int row, bool blocked, c
   }
 }
 
-// The K words of val [V] ranked first by (value descending, word ascending), written in rank order to out_w / out_lp [0:K]: a
-// threshold on order_key(val) by binary search over the key's bits plus a scan of the ties in index order (no sort).  Each
-// thread's chunk of val must be complete; the search starts from the maximum, which skips NaNs (the constrained kernel's
-// excluded words).  redf / redi: [33], prei: [SAMPLE_THREADS + 1], sel_w / sel_lp: [K] shared.
-__device__ __forceinline__ void row_top_k(const float* val, int V, int K, int* out_w, float* out_lp, float* redf, int* redi,
-                                          int* prei, int* sel_w, float* sel_lp) {
+// The K words of val [V] ranked first by (order_key(value) descending, word ascending), written in rank order to out_w / out_lp
+// [0:K]: a threshold on order_key(val) by binary search over the key's bits plus a scan of the ties in index order (no sort).  The
+// key orders every float, NaN included: the canonical NaN of a non-finite row ranks above +inf (as torch.topk ranks NaN), and the
+// constrained kernel's excluded words (key 0) below everything, so exactly K words are kept whatever the row holds (V >= K).  Each
+// thread's chunk of val must be complete.  redi: [33], prei: [SAMPLE_THREADS + 1], sel_w / sel_lp: [K] shared.
+__device__ __forceinline__ void row_top_k(const float* val, int V, int K, int* out_w, float* out_lp, int* redi, int* prei, int* sel_w,
+                                          float* sel_lp) {
   const int tid = threadIdx.x;
   const Chunk ch = row_chunk(V);
   const int lo = ch.lo, hi = ch.hi;
-  float top = -INFINITY;
-  for (int v = lo; v < hi; ++v) top = fmaxf(top, val[v]);
-  top = block_reduce(top, redf, [](float p, float q) { return fmaxf(p, q); });
+  unsigned top = 0;
+  for (int v = lo; v < hi; ++v) top = max(top, order_key(val[v]));
+  top = block_reduce(top, reinterpret_cast<unsigned*>(redi), [](unsigned p, unsigned q) { return max(p, q); });
 
   // tau = the largest key with at least K words at or above it
   auto count = [&](unsigned t) {
@@ -265,7 +266,7 @@ __device__ __forceinline__ void row_top_k(const float* val, int V, int K, int* o
     for (int v = lo; v < hi; ++v) c += order_key(val[v]) >= t;
     return block_reduce(c, redi, [](int p, int q) { return p + q; });
   };
-  const unsigned tau = threshold_key(order_key(top), [&](unsigned t) { return count(t) >= K; });
+  const unsigned tau = threshold_key(top, [&](unsigned t) { return count(t) >= K; });
   const int take = K - (tau == 0xffffffffu ? 0 : count(tau + 1));   // words tied at tau to keep, lowest index first
 
   int ties = 0;
@@ -456,8 +457,10 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
 //            top_w / top_lp [row, 0:K].
 // diverse_beam_merge_kernel, one CTA per image: groups choose in order g = 0 .. G-1.  Group g's candidates are its parents'
 //   (beams [g*Kg, (g+1)*Kg); row b at f = 0) row top K with cand = logp + eos_prev * -10000 + score_prev (cand = logp at f = 0);
-//   it keeps the Kg with the largest cand - lambda * cnt(w), cnt(w) = beams of groups < g that chose w in this frame, ties to the
-//   lower parent then the lower word, in rank order as beams g*Kg ..  The traces get the unpenalised cand.
+//   it keeps the Kg with the largest cand - lambda * cnt(w), cnt(w) = beams of groups < g that chose w in this frame, NaN ranked
+//   above every number, ties to the lower parent then the lower word, in rank order as beams g*Kg ..  The traces get the
+//   unpenalised cand.  A row with a NaN or +inf logit, or with every logit -inf, has a NaN logsumexp: its logp is NaN (but at a
+//   block_eos [EOS]), its top K are its lowest NaN words, and its candidates rank first, in (parent, word) order.
 // Group g penalises at most g*Kg <= K - Kg words, so any (row, word) outside the row's top K has at least Kg unpenalised words of
 // the same row ranked strictly ahead of it: the row top K hold every pair a group can keep.  Every sum runs in a fixed order
 // (chunk, then a fixed shuffle tree) and the merge only compares, so a frame is bitwise reproducible.
@@ -481,8 +484,7 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) diverse_beam_rows_kernel(Diver
     if (a.f >= a.n) blocked = ngram_candidates(hist, a.f, a.n, V, a.ignore, a.n_ignore, bits);
   }
   row_logp<T>(a, row, blocked, bits, val, redf);
-  row_top_k(val, V, K, a.top_w + static_cast<size_t>(row) * K, a.top_lp + static_cast<size_t>(row) * K, redf, redi, prei, sel_w,
-            sel_lp);
+  row_top_k(val, V, K, a.top_w + static_cast<size_t>(row) * K, a.top_lp + static_cast<size_t>(row) * K, redi, prei, sel_w, sel_lp);
 }
 
 __global__ void __launch_bounds__(MERGE_THREADS) diverse_beam_merge_kernel(DiverseBeamArgs a) {
@@ -517,7 +519,9 @@ __global__ void __launch_bounds__(MERGE_THREADS) diverse_beam_merge_kernel(Diver
       for (int d = 0; d < nc && r < Kg; ++d) {
         const float u = pen[d];
         const int pd = d / K;
-        r += u > v || (u == v && (pd < pc || (pd == pc && word[d] < w)));
+        const bool ahead = isnan(u) ? !isnan(v) : u > v;             // NaN first: a total order, so each rank has one candidate
+        const bool tied = u == v || (isnan(u) && isnan(v));
+        r += ahead || (tied && (pd < pc || (pd == pc && word[d] < w)));
       }
       if (r < Kg) {
         const int k = g * Kg + r;
@@ -625,7 +629,7 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) constrained_beam_rows_kernel(V
     if (used) val[w] = __int_as_float(-1);                         // a NaN whose order_key is 0
   }
   __syncthreads();
-  row_top_k(val, V, K, a.top_w + out, a.top_lp + out, redf, redi, prei, sel_w, sel_lp);
+  row_top_k(val, V, K, a.top_w + out, a.top_lp + out, redi, prei, sel_w, sel_lp);
 }
 
 size_t cbs_merge_smem_bytes(int K, int C, int A) {                   // one state's candidates at most: value, parent, word
