@@ -48,6 +48,28 @@ def import_reference_optimization():
     return o
 
 
+class bool_masked_fill:
+    """Context manager for running the reference's region masking (mask_image_regions=True, modeling.py:1050-1057) on a modern
+    torch.  The reference builds its region mask with `.byte()` and passes it to Tensor.masked_fill; torch 1.x accepted a uint8 mask
+    as a boolean one, torch 2 raises "masked_fill_ only supports boolean masks".  Inside the block Tensor.masked_fill converts a
+    uint8 mask to bool (the semantics the code was written for) and is otherwise untouched; it is restored on exit."""
+
+    def __enter__(self):
+        import torch
+        self._orig = orig = torch.Tensor.masked_fill
+
+        def masked_fill(t, mask, value):
+            return orig(t, mask.bool() if mask.dtype == torch.uint8 else mask, value)
+
+        torch.Tensor.masked_fill = masked_fill
+        return self
+
+    def __exit__(self, *exc):
+        import torch
+        torch.Tensor.masked_fill = self._orig
+        return False
+
+
 def build_reference_model(dims, state_dict, tasks="img2txt", decoder=False, **decoder_kw):
     """Instantiate the reference's BertForPreTrainingLossMask / BertForSeq2SeqDecoder (enable_butd=True) and
     load `state_dict`.  modeling.py:1008-1014 reads detectron_weights/fc7_{w,b}.pkl from the CWD at

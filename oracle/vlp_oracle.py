@@ -155,30 +155,57 @@ def loss_mask_and_normalize(loss, mask, drop_worst_ratio):
     return (keep_loss / denom).sum()
 
 
+def mask_regions(x, vis_masked_pos):
+    """modeling.py:1050-1056 — rows vis_masked_pos - 1 of the projected [B, R, H] regions set to 0."""
+    m = torch.zeros(x.shape[0], x.shape[1], 1, dtype=torch.bool, device=x.device)
+    for b in range(vis_masked_pos.size(0)):
+        for j in range(vis_masked_pos.size(1)):
+            m[b, vis_masked_pos[b, j] - 1] = True
+    return x.masked_fill(m, 0.0)
+
+
+def region_pretext_loss(vis, vpe, pooled, vis_masked_pos):
+    """modeling.py:1113-1131 (enable_butd) — the "Selfie-like" pretext: for each masked region, the UNMASKED projected position
+    encoding plus the pooled output scored against the UNMASKED projected features of every masked region of its sample; the loss
+    is the mean over samples of the mean -log-softmax of the matching pair."""
+    idx = (vis_masked_pos - 1).unsqueeze(-1)
+    feats = torch.gather(vis, 1, idx.expand(-1, -1, vis.size(-1)))
+    enc = torch.gather(vpe, 1, idx.expand(-1, -1, vpe.size(-1))) + pooled.unsqueeze(1)
+    sim = F.log_softmax(torch.matmul(enc, feats.permute(0, 2, 1)), dim=-1)
+    return torch.stack([-sim[i].diag().mean() for i in range(sim.size(0))]).mean()
+
+
 def pretraining_loss(sd, dims, batch, tasks="img2txt", drop_worst_ratio=0.0, p_hidden=0.0, p_attn=0.0, training=False,
-                     return_all=False):
-    """BertForPreTrainingLossMask.forward, modeling.py:1033-1143 (mask_image_regions=False branch)."""
+                     return_all=False, mask_image_regions=False):
+    """BertForPreTrainingLossMask.forward, modeling.py:1033-1143.  mask_image_regions: the encoder sees the projected features and
+    position encodings of batch["vis_masked_pos"] as zeros (:1050-1057) and the second loss is the region pretext (:1113-1131)."""
     kw = dict(p_hidden=p_hidden, p_attn=p_attn, training=training)
     vis, vpe = region_projections(sd, batch["img"], batch["vis_pe"], p_hidden, training)
+    in_vis, in_vpe = vis, vpe
+    if mask_image_regions:
+        in_vis, in_vpe = mask_regions(vis, batch["vis_masked_pos"]), mask_regions(vpe, batch["vis_masked_pos"])
     ext = extended_attention_mask(batch["input_mask"], dtype=vis.dtype)   # parameter dtype, modeling.py:830-831
-    emb = embeddings(sd, vis, vpe, batch["input_ids"], batch["segment_ids"], len_vis_input=dims.regions, p=p_hidden, training=training)
+    emb = embeddings(sd, in_vis, in_vpe, batch["input_ids"], batch["segment_ids"], len_vis_input=dims.regions, p=p_hidden,
+                     training=training)
     outs = encoder(sd, dims.layers, emb, ext, dims.heads, **kw)
     seq = outs[-1]
+    pooled = pooler(sd, seq)
     pos = batch["masked_pos"]
     gathered = torch.gather(seq, 1, pos.unsqueeze(2).expand(-1, -1, seq.size(-1)))          # :1068-1069
     logits = lm_head(sd, gathered)
     ce = F.cross_entropy(logits.transpose(1, 2).float(), batch["masked_ids"], reduction="none")  # :1108-1109
     mlm = loss_mask_and_normalize(ce.float(), batch["masked_weights"], drop_worst_ratio)
     zero = mlm.new_zeros(1)
+    pretext = region_pretext_loss(vis, vpe, pooled, batch["vis_masked_pos"]) if mask_image_regions else zero
     if tasks == "vqa2":                                                                      # :1135-1141
         e = seq[:, 0] * seq[:, dims.regions + 1]
         pred = linear(torch.relu(linear(e, sd, "ans_classifier.0")), sd, "ans_classifier.2")
         vqa = F.binary_cross_entropy_with_logits(pred, batch["ans_labels"]) * batch["ans_labels"].size(1)
-        losses = (zero, zero, vqa)
+        losses = (zero, pretext, vqa)
     else:
-        losses = (mlm, zero, zero)
+        losses = (mlm, pretext, zero)
     if return_all:
-        return losses, {"embedding": emb, "layers": outs, "logits": logits, "pooled": pooler(sd, seq)}
+        return losses, {"embedding": emb, "layers": outs, "logits": logits, "pooled": pooled}
     return losses
 
 

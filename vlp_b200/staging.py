@@ -34,9 +34,25 @@ def mask_descriptor(len_b, mode):
     return lb, md
 
 
+def loader_mask(len_b, mode, len_a, L_):
+    """bool [B, L, L]: the self-attention mask seq2seq_loader.py:291-301 builds for text lengths len_b [B] and modes [B] (1 = seq2seq,
+    0 = bidirectional) — the matrix the packed mask of `mask_descriptor(len_b, mode)` stands for."""
+    len_b, mode = torch.as_tensor(len_b), torch.as_tensor(mode)
+    st = len_a + 2
+    en = (st + 1 + len_b.to(torch.int64)).view(-1, 1, 1)
+    i = torch.arange(L_, device=len_b.device).view(1, -1, 1)
+    j = torch.arange(L_, device=len_b.device).view(1, 1, -1)
+    s2s = (j < st) | ((i >= st) & (i < en) & (j >= st) & (j <= i))
+    bi = (j < en).expand(-1, L_, -1)
+    return torch.where(mode.view(-1, 1, 1) != 0, s2s, bi)
+
+
 def describe_mask(input_mask, len_a):
     """Recover (len_b, mode) from a loader-built [B,L,L] 0/1 mask (seq2seq_loader.py:291-301) — for callers that still receive the
-    matrix from an unmodified loader; O(B*L) host work.  s2s rows past the text keep only the prefix, bi rows are all identical."""
+    matrix from an unmodified loader.  s2s rows past the text keep only the prefix, bi rows are all identical.  ValueError unless the
+    matrix is exactly loader_mask(len_b, mode): a matrix of another form — one that blocks the key columns of masked regions (what
+    seq2seq_loader.py:303-304 means to do for --vis_mask_prob), or one whose layout len_a does not describe — has no (len_b, mode)
+    descriptor, and reading one off it would stand for a different mask.  O(B*L*L) work on the matrix's device."""
     m = input_mask
     B, Lm, _ = m.shape
     st = len_a + 2
@@ -45,7 +61,13 @@ def describe_mask(input_mask, len_a):
     en = diag.sum(-1)
     first_text_row = m[:, st]                                  # s2s: attends to [0, st]; bi: [0, en)
     s2s = (first_text_row.sum(-1) == st + 1) & (en > st + 1) | ((en == st + 1) & (last_row.sum(-1) == st) & (Lm > st + 1))
-    return (en - len_a - 3).to(torch.int32), s2s.to(torch.int32)
+    len_b = (en - len_a - 3).clamp_min(0)
+    bad = (m != loader_mask(len_b, s2s, len_a, Lm).to(m.dtype)).flatten(1).any(1) | (en < st + 1)
+    if bool(bad.any()):
+        raise ValueError(f"vlp_b200: the attention mask of sample(s) {bad.nonzero().flatten().tolist()[:8]} is not a loader mask of "
+                         f"{len_a} regions (seq2seq_loader.py:291-301) — a matrix with blocked region columns has no "
+                         f"(len_b, mode) descriptor")
+    return len_b.to(torch.int32), s2s.to(torch.int32)
 
 
 class PackedAttentionMask:
@@ -169,7 +191,9 @@ class BatchStager:
     captions_per_image=G > 1: batches of B images x G seq2seq captions for BertForPreTrainingLossMask(..., captions_per_image=G).
     "img" / "vis_pe" have B rows, the text fields B * G rows (pair b * G + g is image b's caption g), and either "len_b" (int32
     [B * G], with "mode" if the loader gives it) or the loader's "input_mask" matrices (read on the host through describe_mask, not
-    copied); a bidirectional pair is refused with ValueError.  b["input_mask"] is a GroupedCaptionMask."""
+    copied); a bidirectional pair is refused with ValueError.  b["input_mask"] is a GroupedCaptionMask.  Reading matrices costs host
+    time on the step's path — describe_mask compares every element, about 8 ms of one Xeon core for 64 pairs at L = 123 — so loaders
+    that can should pass "len_b"."""
 
     def __init__(self, device, len_vis_input=100, max_len=123, feature_dtype=BF16, depth=2, captions_per_image=1):
         self.device = torch.device(device)

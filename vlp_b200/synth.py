@@ -102,10 +102,15 @@ def attention_mask(d: VlpDims, text_len, mode):
     return m
 
 
-def make_batch(d: VlpDims, batch, seed=1234, mode="s2s", ragged=False, tasks="img2txt"):
+def make_batch(d: VlpDims, batch, seed=1234, mode="s2s", ragged=False, tasks="img2txt", vis_mask_prob=0.0):
     """The 12 fields of one training batch (SURVEY.md §3.1 input contract), CPU tensors, fp32 features.
 
-    mode: "s2s", "bi" or "mix" (per-sample Bernoulli(0.75 s2s / 0.25 bi), README.md:120)."""
+    mode: "s2s", "bi" or "mix" (per-sample Bernoulli(0.75 s2s / 0.25 bi), README.md:120).
+    vis_mask_prob > 0 draws region masking as the loader does with --vis_mask_prob (seq2seq_loader.py:267-269):
+    vis_masked_pos [B, int(R * vis_mask_prob)] holds distinct regions in [1, R] (row of the region, no padding).  The attention
+    mask stays the plain one: the loader's `input_mask[:, vis_masked_pos].fill_(0)` (:303-304, "block the masked visual feature")
+    fills the copy that indexing with an index array returns, so its matrix keeps those key columns.  The draws come after all
+    others, so every other field equals the batch drawn with vis_mask_prob 0, whose vis_masked_pos is empty."""
     g = torch.Generator().manual_seed(seed)
     L, R, T = d.seq_len, d.regions, d.text
     P = 1 if tasks == "vqa2" else d.max_pred
@@ -149,11 +154,15 @@ def make_batch(d: VlpDims, batch, seed=1234, mode="s2s", ragged=False, tasks="im
             ans[b, cols] = vals[torch.randint(0, 4, (n,), generator=g)]
     else:
         ans = torch.zeros(batch, 1)
+    vis_masked_pos = torch.zeros(batch, 0, dtype=torch.long)
+    n_vis = int(R * vis_mask_prob)
+    if n_vis > 0:
+        vis_masked_pos = torch.stack([torch.randperm(R, generator=g)[:n_vis] + 1 for _ in range(batch)])
     return {
         "input_ids": input_ids, "segment_ids": segment_ids, "input_mask": input_mask,
         "masked_ids": masked_ids, "masked_pos": masked_pos, "masked_weights": masked_weights,
         "is_next": torch.full((batch,), -1, dtype=torch.long), "task_idx": task_idx,
-        "img": vis_feats, "vis_masked_pos": torch.zeros(batch, 0, dtype=torch.long), "vis_pe": vis_pe, "ans_labels": ans,
+        "img": vis_feats, "vis_masked_pos": vis_masked_pos, "vis_pe": vis_pe, "ans_labels": ans,
     }
 
 
