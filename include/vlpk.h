@@ -513,6 +513,34 @@ typedef struct VlpkConstrainedBeamArgs {
 } VlpkConstrainedBeamArgs;
 int vlpk_constrained_beam_step(const VlpkConstrainedBeamArgs* args, void* stream);
 
+/* Prompted captions: the three row selectors above for decodes whose captions start with given words (a prompt of t_b words for
+ * the image of each row, padded to a width Tp shared by the batch).  Each prompted entry point takes its selector's arguments and
+ *   hist_off    Tp >= 0.  Every row's word history has hist_off + g entries at generated word g: its prompt right-aligned behind
+ *               Tp - t_b entries of -1 (a word id that matches no word and is never a candidate), then the generated words, so the
+ *               duplicate-n-gram rule and the constraint tail match see prompt + continuation.
+ *   eos_until   int32 [rows] or NULL: [EOS] is blocked (as block_eos) while g + 1 <= eos_until[row] (min_len - t_b); NULL: never.
+ * vlpk_sample_tokens_prompt: f = hist_off + g and seq[row, :hist_off] holds the row's prompt history; the draw is keyed by
+ *   (seed; g, row), as an unprompted decode keys word g.  Refused (< 0, no launch) for hist_off outside [0, f].
+ * vlpk_diverse_beam_step_prompt / vlpk_constrained_beam_step_prompt: f is the trace frame g; at f = 0 row b of hist_in ([B, T_cap],
+ *   read when n > 0, and always for the constrained search) holds image b's hist_off prompt entries, and from f = 1 on the carry runs
+ *   over hist_off + f entries (prev_ptr is read at f = 1 too).  A constraint the prompt contains is met from the start when the
+ *   caller zeroes its alternatives for that image; a phrase may begin in the prompt.  Refused for hist_off < 0 or f + hist_off >=
+ *   T_cap, and for a NULL hist_in or prev_ptr that is needed.
+ * Each runs its own prompted instantiation of the selector's rows kernel; the unprompted entry points are unchanged. */
+typedef struct VlpkPromptRows {
+  int32_t hist_off;                  /* Tp: prompt entries at the start of every history */
+  const int32_t* eos_until;          /* [rows] [EOS] blocked while g + 1 <= eos_until[row], or NULL */
+} VlpkPromptRows;
+int vlpk_sample_tokens_prompt(int rows, int V, const void* logits, int64_t ld, const void* bias, int fp32, int mode, int topk, float topp,
+                              uint64_t seed, int f, int64_t* seq, int T_cap, float* score, int32_t* finished, int32_t* live, int eos_id,
+                              int pad_id, int n, const int32_t* ignore, int n_ignore, const VlpkPromptRows* prompt, void* stream);
+int vlpk_diverse_beam_step_prompt(int B, int K, int G, int f, int V, const void* logits, int64_t ld, const void* bias, int fp32,
+                                  float diversity_penalty, int eos_id, int T_cap, int n, const int32_t* hist_in, int32_t* hist_out,
+                                  const int32_t* ignore, int n_ignore, const int64_t* prev_wid, const int64_t* prev_ptr,
+                                  const float* prev_score, const float* prev_eos, int32_t* top_w, float* top_lp, int64_t* wid, int64_t* ptr,
+                                  float* score, float* eos, const VlpkPromptRows* prompt, void* stream);
+int vlpk_constrained_beam_step_prompt(const VlpkConstrainedBeamArgs* args, const VlpkPromptRows* prompt, void* stream);
+
 /* utilities */
 int vlpk_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 int vlpk_colsum(const void* x, int64_t ld, int64_t M, int N, float* out, void* stream);

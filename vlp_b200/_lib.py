@@ -60,6 +60,10 @@ class VlpkConstrainedBeamArgs(C.Structure):
                                    "score", "eos")]
 
 
+class VlpkPromptRows(C.Structure):
+    _fields_ = [("hist_off", C.c_int32), ("eos_until", c_void_p)]
+
+
 # name -> (restype, argtypes); mirrors include/vlpk.h one to one
 _P = c_void_p
 _SIGS = {
@@ -144,6 +148,11 @@ _SIGS = {
     "vlpk_diverse_beam_step": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, c_i64, _P, c_int, c_float, c_int, c_int, c_int, c_int, _P,
                                        _P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "vlpk_constrained_beam_step": (c_int, [C.POINTER(VlpkConstrainedBeamArgs), _P]),
+    "vlpk_sample_tokens_prompt": (c_int, [c_int, c_int, _P, c_i64, _P, c_int, c_int, c_int, c_float, c_u64, c_int, _P, c_int, _P, _P, _P,
+                                          c_int, c_int, c_int, _P, c_int, C.POINTER(VlpkPromptRows), _P]),
+    "vlpk_diverse_beam_step_prompt": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, c_i64, _P, c_int, c_float, c_int, c_int, c_int, _P,
+                                              _P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.POINTER(VlpkPromptRows), _P]),
+    "vlpk_constrained_beam_step_prompt": (c_int, [C.POINTER(VlpkConstrainedBeamArgs), C.POINTER(VlpkPromptRows), _P]),
     "vlpk_f32_to_bf16": (c_int, [_P, _P, c_i64, _P]),
     "vlpk_colsum": (c_int, [_P, c_i64, c_i64, c_int, _P, _P]),
     "vlpk_debug_dropout_mask": (c_int, [C.POINTER(VlpkDropout), c_u64, c_i64, _P, _P]),

@@ -19,7 +19,8 @@ import torch
 import torch.nn.functional as F
 
 from . import ops
-from .decode import DecodeState, _ignore_tensor, expand_task_idx, new_attention_maps
+from .decode import (DecodeState, _ignore_tensor, expand_task_idx, new_attention_maps, prompt_constraints, prompt_eos_until, prompt_history,
+                     prompt_lengths, with_prompt)
 
 
 def _dup_ngram_candidates(seq, n, ignore):
@@ -66,31 +67,57 @@ def _padded_traces(out, sc, wi, pt, out_len):
         out[k] = padded
 
 
-def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, output_attentions=False):
+def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, output_attentions=False,
+                prompt=None):
     """output_attentions: out["attentions"] [B, out_len - in_len, layers, heads, out_len] holds, for frame t of pred_seq, the [MASK]-row
-    maps of step t taken from the row its hypothesis continued (beam_maps)."""
+    maps of step t taken from the row its hypothesis continued (beam_maps).
+    prompt [B, Tp] (Tp >= 1): the search runs out_len - in_len - Tp frames after the prompt's prefill (decode.DecodeState).  Every
+    hypothesis' n-gram history starts with its image's prompt (decode.prompt_history: Tp + g entries at frame g, so frame 0 is
+    blocked too), [EOS] is blocked while t_b + g + 1 <= min_len, and pred_seq / nbest_seq hold the t_b prompt words before the
+    generated ones.  The traces and scores are those of the generated words only."""
     K = dec.search_beam_size
     B, in_len = input_ids.shape
     out_len = token_type_ids.shape[1]
     dev = input_ids.device
     N = dec.num_return_sequences
     # N > 1: the K hypotheses of an image share its prefix K/V; a reorder moves slot-table entries, not cache rows
-    state = DecodeState(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, K if N > 1 else None)
+    state = DecodeState(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, K if N > 1 else None, prompt)
+    Tp = 0 if prompt is None else prompt.shape[1]
     total_scores, beam_eos, step_ids, step_ptrs = [], [], [], []
     if dec.forbid_duplicate_ngrams:
         ngram, ignore = int(dec.ngram_size), _ignore_tensor(dec, dev)
         hist = [torch.empty(B * K, out_len - in_len, dtype=torch.int32, device=dev) for _ in range(2)]    # word histories, in turn
     # per step t, the [MASK]-row maps of its B*K input rows (step 0: B rows, written at rows b*K)
     maps = new_attention_maps(dec, out_len - in_len, B * K, out_len, dev) if output_attentions else None
-    curr_ids = input_ids
-    for frame in range(out_len - in_len):
+    if Tp:
+        lens = prompt_lengths(prompt)
+        row_lens = lens                                                   # t_b of every row: B rows at frame 0, B*K after
+    curr_ids = state.first_ids
+    for frame in range(state.frames):
         scores, _ = dec.cls(state.step(curr_ids, _step_maps(maps, frame, B, K)), None, task_idx=task_idx)
         logp = F.log_softmax(scores.float(), dim=-1)                      # [B or B*K, 1, V]
-        if dec.forbid_duplicate_ngrams and frame >= 1:
-            # history of frame `frame` from the previous frame's words and back pointers; blocks in place once it holds n words
-            ops.beam_ngram_block(hist[(frame - 1) % 2], hist[frame % 2], step_ptrs[-1], step_ids[-1], frame, ngram, ignore, logp)
-        if dec.min_len and (frame + 1 <= dec.min_len):
-            logp[:, :, dec.eos_id] = -10000.0
+        if Tp:
+            if dec.forbid_duplicate_ngrams:
+                if frame == 0:
+                    # the prompt alone is frame 0's history: one row per image, its own parent, its last entry fed as the word
+                    seed = prompt_history(prompt, 1, out_len - in_len)
+                    ops.beam_ngram_block(seed, torch.empty_like(seed), torch.zeros(B, 1, dtype=torch.int64, device=dev),
+                                         seed[:, Tp - 1:Tp].to(torch.int64), Tp, ngram, ignore, logp)
+                    hist[0] = seed.repeat_interleave(K, 0)                # frame 1's parents: each image's rows
+                else:
+                    ops.beam_ngram_block(hist[(frame - 1) % 2], hist[frame % 2], step_ptrs[-1], step_ids[-1], Tp + frame, ngram, ignore,
+                                         logp)
+            if dec.min_len:
+                block = (row_lens + frame + 1 <= dec.min_len).view(-1, 1)
+                logp[:, :, dec.eos_id] = torch.where(block, torch.full_like(logp[:, :, dec.eos_id], -10000.0), logp[:, :, dec.eos_id])
+            if frame == 0:
+                row_lens = lens.repeat_interleave(K)
+        else:
+            if dec.forbid_duplicate_ngrams and frame >= 1:
+                # history of frame `frame` from the previous frame's words and back pointers; blocks in place once it holds n words
+                ops.beam_ngram_block(hist[(frame - 1) % 2], hist[frame % 2], step_ptrs[-1], step_ids[-1], frame, ngram, ignore, logp)
+            if dec.min_len and (frame + 1 <= dec.min_len):
+                logp[:, :, dec.eos_id] = -10000.0
         kk_scores, kk_ids = torch.topk(logp, k=K)                          # [*, 1, K]
         if frame == 0:
             k_ids = kk_ids.reshape(B, K)
@@ -115,11 +142,15 @@ def beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids,
     _padded_traces(out, sc, wi, pt, out_len)
     if N > 1:
         out["nbest_seq"], out["nbest_scores"] = nbest(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len, N)
+    if Tp:
+        for k in ("pred_seq", "nbest_seq"):
+            if k in out:
+                out[k] = with_prompt(prompt, out[k])
     return out
 
 
 def diverse_beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None,
-                        output_attentions=False):
+                        output_attentions=False, prompt=None):
     """Diverse beam search (Vijayakumar et al., AAAI 2018): the K = dec.search_beam_size beams of an image in G = dec.num_beam_groups
     groups of Kg = K / G.  Every frame, the groups choose in turn; group g extends its own beams and ranks each (parent, word) by its
     beam score minus dec.diversity_penalty times the number of beams of groups < g that chose the word in this frame.  The traces keep
@@ -128,30 +159,41 @@ def diverse_beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, posit
     and the min_len [EOS] block included; nothing synchronises with the host.
 
     Output: beam_search's dict (pred_seq, scores, wids, ptrs; attentions, nbest_seq / nbest_scores as there), plus group_seq int64
-    [B, G, out_len] and group_scores fp32 [B, G]: the final-selection rule applied to each group's Kg beams alone."""
+    [B, G, out_len] and group_scores fp32 [B, G]: the final-selection rule applied to each group's Kg beams alone.
+    prompt [B, Tp] (Tp >= 1): as beam_search's, through vlpk_diverse_beam_step_prompt; group_seq holds the prompt words too."""
     K, G = dec.search_beam_size, dec.num_beam_groups
     B, in_len = input_ids.shape
     out_len = token_type_ids.shape[1]
-    T = out_len - in_len
     dev = input_ids.device
     N = dec.num_return_sequences
-    state = DecodeState(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, K if N > 1 else None)
+    state = DecodeState(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, K if N > 1 else None, prompt)
+    T, Tp = state.frames, state.prefix_len - in_len
     ngram = int(dec.ngram_size) if dec.forbid_duplicate_ngrams else 0
     ignore = _ignore_tensor(dec, dev) if ngram else None
-    hist = [torch.empty(B * K, T, dtype=torch.int32, device=dev) for _ in range(2)] if ngram else [None, None]
+    hist = [torch.empty(B * K, T + Tp, dtype=torch.int32, device=dev) for _ in range(2)] if ngram else [None, None]
+    if Tp:
+        seed = prompt_history(prompt, 1, T + Tp)
+        eos_until = [prompt_eos_until(prompt, 1, dec.min_len), prompt_eos_until(prompt, K, dec.min_len)]
     sc, eos = (torch.zeros(T, B, K, dtype=torch.float32, device=dev) for _ in range(2))
     wi, pt = (torch.zeros(T, B, K, dtype=torch.int64, device=dev) for _ in range(2))
     top_w = torch.empty(B * K, K, dtype=torch.int32, device=dev)
     top_lp = torch.empty(B * K, K, dtype=torch.float32, device=dev)
     pred = dec.cls.predictions
     maps = new_attention_maps(dec, T, B * K, out_len, dev) if output_attentions else None
-    curr_ids = input_ids
+    curr_ids = state.first_ids
     for frame in range(T):
         h = pred.select_task(pred.transform(state.step(curr_ids, _step_maps(maps, frame, B, K)).to(pred.decoder.weight.dtype)), task_idx)
         logits = pred.decoder(h)                                          # [B or B*K, 1, V]; the kernel adds the bias
-        ops.diverse_beam_step(logits, pred.bias.to(logits.dtype), frame, G, dec.diversity_penalty, wi, pt, sc, eos, top_w, top_lp,
-                              dec.eos_id, block_eos=bool(dec.min_len) and frame + 1 <= dec.min_len, ngram=ngram, ignore=ignore,
-                              hist_in=hist[(frame - 1) % 2], hist_out=hist[frame % 2])
+        if Tp:
+            ops.diverse_beam_step(logits, pred.bias.to(logits.dtype), frame, G, dec.diversity_penalty, wi, pt, sc, eos, top_w, top_lp,
+                                  dec.eos_id, ngram=ngram, ignore=ignore, hist_in=seed if frame == 0 else hist[(frame - 1) % 2],
+                                  hist_out=hist[frame % 2], prompt=(Tp, eos_until[min(frame, 1)]))
+            if frame == 0 and ngram:
+                hist[0] = seed.repeat_interleave(K, 0)                    # frame 1's parents: each image's rows
+        else:
+            ops.diverse_beam_step(logits, pred.bias.to(logits.dtype), frame, G, dec.diversity_penalty, wi, pt, sc, eos, top_w, top_lp,
+                                  dec.eos_id, block_eos=bool(dec.min_len) and frame + 1 <= dec.min_len, ngram=ngram, ignore=ignore,
+                                  hist_in=hist[(frame - 1) % 2], hist_out=hist[frame % 2])
         task_idx = _follow_beams(state, frame, pt[frame], task_idx)
         curr_ids = wi[frame].reshape(B * K, 1)
 
@@ -162,11 +204,20 @@ def diverse_beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, posit
     if N > 1:
         out["nbest_seq"], out["nbest_scores"] = nbest(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len, N)
     out["group_seq"], out["group_scores"] = group_best(sc, wi, pt, dec.eos_id, dec.length_penalty, out_len, G)
+    return _prompted(out, prompt, ("pred_seq", "nbest_seq", "group_seq"))
+
+
+def _prompted(out, prompt, keys):
+    """out with the prompt's words placed before the generated words of every returned caption in keys (decode.with_prompt)."""
+    if prompt is not None:
+        for k in keys:
+            if k in out:
+                out[k] = with_prompt(prompt, out[k])
     return out
 
 
 def constrained_beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, cons, task_idx=None,
-                            output_attentions=False):
+                            output_attentions=False, prompt=None):
     """Constrained beam search (Anderson et al., EMNLP 2017): captions that must contain given words or phrases.  cons: int64 [B, C, A,
     P] on the device, 0-padded: constraint j of image b is met when one of its A alternatives (each a run of up to P word ids) occurs as
     a contiguous run of the generated words; a constraint with no alternative is met from the start.  A hypothesis' state is the set s
@@ -183,21 +234,29 @@ def constrained_beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, p
                        state has none, the best of the states with the most constraints met (higher value, then lower state);
       constraints_met  bool [B]: the accept state had a candidate;
       state_seq        int64 [B, S, out_len] and state_scores fp32 [B, S]: each state's own best (-inf where it has none);
-      nbest_seq / nbest_scores (num_return_sequences N > 1): the accept state's N best."""
+      nbest_seq / nbest_scores (num_return_sequences N > 1): the accept state's N best.
+    prompt [B, Tp] (Tp >= 1): as beam_search's, through vlpk_constrained_beam_step_prompt: a constraint one of whose alternatives the
+    prompt contains is met from the start (decode.prompt_constraints: each image starts in its own state), a phrase may begin in the
+    prompt and end in the continuation, and constraints_met refers to the whole caption."""
     K, C = dec.search_beam_size, cons.shape[1]
     S = 1 << C
     SK = S * K
     B, in_len = input_ids.shape
     out_len = token_type_ids.shape[1]
-    T = out_len - in_len
     dev = input_ids.device
     N = dec.num_return_sequences
     W = K + C * cons.shape[2]
     # one copy of each image's prefix K/V for its S*K hypotheses; the attention maps come from per-hypothesis caches
-    state = DecodeState(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, None if output_attentions else SK)
+    state = DecodeState(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, None if output_attentions else SK,
+                        prompt)
+    T, Tp = state.frames, state.prefix_len - in_len
     ngram = int(dec.ngram_size) if dec.forbid_duplicate_ngrams else 0
     ignore = _ignore_tensor(dec, dev) if ngram else None
-    hist = [torch.empty(B * SK, T, dtype=torch.int32, device=dev) for _ in range(2)]       # the constraint match reads them always
+    hist = [torch.empty(B * SK, T + Tp, dtype=torch.int32, device=dev) for _ in range(2)]  # the constraint match reads them always
+    if Tp:
+        cons = prompt_constraints(cons, prompt)
+        seed = prompt_history(prompt, 1, T + Tp)
+        eos_until = [prompt_eos_until(prompt, 1, dec.min_len), prompt_eos_until(prompt, SK, dec.min_len)]
     sc, eos = (torch.zeros(T, B, SK, dtype=torch.float32, device=dev) for _ in range(2))
     wi, pt = (torch.zeros(T, B, SK, dtype=torch.int64, device=dev) for _ in range(2))
     top_w = torch.empty(B * SK, W, dtype=torch.int32, device=dev)
@@ -205,13 +264,20 @@ def constrained_beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, p
     top_dest = torch.empty(B * SK, W - K, dtype=torch.int32, device=dev)
     pred = dec.cls.predictions
     maps = new_attention_maps(dec, T, B * SK, out_len, dev) if output_attentions else None
-    curr_ids = input_ids
+    curr_ids = state.first_ids
     for frame in range(T):
         h = pred.select_task(pred.transform(state.step(curr_ids, _step_maps(maps, frame, B, SK)).to(pred.decoder.weight.dtype)), task_idx)
         logits = pred.decoder(h)                                          # [B or B*S*K, 1, V]; the kernel adds the bias
-        ops.constrained_beam_step(logits, pred.bias.to(logits.dtype), frame, cons, wi, pt, sc, eos, top_w, top_lp, top_dest, dec.eos_id,
-                                  block_eos=bool(dec.min_len) and frame + 1 <= dec.min_len, ngram=ngram, ignore=ignore,
-                                  hist_in=hist[(frame - 1) % 2], hist_out=hist[frame % 2])
+        if Tp:
+            ops.constrained_beam_step(logits, pred.bias.to(logits.dtype), frame, cons, wi, pt, sc, eos, top_w, top_lp, top_dest,
+                                      dec.eos_id, ngram=ngram, ignore=ignore, hist_in=seed if frame == 0 else hist[(frame - 1) % 2],
+                                      hist_out=hist[frame % 2], prompt=(Tp, eos_until[min(frame, 1)]))
+            if frame == 0:
+                hist[0] = seed.repeat_interleave(SK, 0)                   # frame 1's parents: each image's rows
+        else:
+            ops.constrained_beam_step(logits, pred.bias.to(logits.dtype), frame, cons, wi, pt, sc, eos, top_w, top_lp, top_dest,
+                                      dec.eos_id, block_eos=bool(dec.min_len) and frame + 1 <= dec.min_len, ngram=ngram, ignore=ignore,
+                                      hist_in=hist[(frame - 1) % 2], hist_out=hist[frame % 2])
         task_idx = _follow_beams(state, frame, pt[frame], task_idx)
         curr_ids = wi[frame].reshape(B * SK, 1)
 
@@ -231,7 +297,7 @@ def constrained_beam_search(dec, vis_feats, vis_pe, input_ids, token_type_ids, p
     if N > 1:
         out["nbest_seq"], out["nbest_scores"] = nbest(sc, wi, pt, dec.eos_id, lp, out_len, N, beams=slice((S - 1) * K, SK))
     out["state_seq"], out["state_scores"] = state_seq, state_scores
-    return out
+    return _prompted(out, prompt, ("pred_seq", "nbest_seq", "state_seq"))
 
 
 def state_choice(state_scores):

@@ -1025,6 +1025,52 @@ int vlpk_constrained_beam_step(const VlpkConstrainedBeamArgs* args, void* stream
   return launch_constrained_beam_step(*args, S(stream));
 }
 
+static PromptRows prompt_rows(const VlpkPromptRows& p) {
+  PromptRows r;
+  r.hist_off = p.hist_off;
+  r.eos_until = p.eos_until;
+  return r;
+}
+
+int vlpk_sample_tokens_prompt(int rows, int V, const void* logits, int64_t ld, const void* bias, int fp32, int mode, int topk, float topp,
+                              uint64_t seed, int f, int64_t* seq, int T_cap, float* score, int32_t* finished, int32_t* live, int eos_id,
+                              int pad_id, int n, const int32_t* ignore, int n_ignore, const VlpkPromptRows* prompt, void* stream) {
+  VLPK_CHECK_ARG(prompt, "sample_tokens_prompt: null prompt rows");
+  SampleArgs a;
+  a.rows = rows; a.V = V; a.logits = logits; a.ld = ld; a.bias = bias; a.fp32 = fp32;
+  a.mode = mode; a.topk = topk; a.topp = topp; a.seed = seed;
+  a.f = f; a.seq = reinterpret_cast<long long*>(seq); a.T_cap = T_cap; a.score = score;
+  a.finished = finished; a.live = live; a.eos_id = eos_id; a.pad_id = pad_id;
+  a.n = n; a.ignore = ignore; a.n_ignore = n_ignore;
+  const PromptRows p = prompt_rows(*prompt);
+  return launch_sample(a, S(stream), &p);
+}
+
+int vlpk_diverse_beam_step_prompt(int B, int K, int G, int f, int V, const void* logits, int64_t ld, const void* bias, int fp32,
+                                  float diversity_penalty, int eos_id, int T_cap, int n, const int32_t* hist_in, int32_t* hist_out,
+                                  const int32_t* ignore, int n_ignore, const int64_t* prev_wid, const int64_t* prev_ptr,
+                                  const float* prev_score, const float* prev_eos, int32_t* top_w, float* top_lp, int64_t* wid, int64_t* ptr,
+                                  float* score, float* eos, const VlpkPromptRows* prompt, void* stream) {
+  VLPK_CHECK_ARG(prompt, "diverse_beam_step_prompt: null prompt rows");
+  DiverseBeamArgs a;
+  a.B = B; a.K = K; a.G = G; a.f = f; a.V = V;
+  a.logits = logits; a.ld = ld; a.bias = bias; a.fp32 = fp32;
+  a.lambda = diversity_penalty; a.eos_id = eos_id;
+  a.T_cap = T_cap; a.n = n; a.hist_in = hist_in; a.hist_out = hist_out; a.ignore = ignore; a.n_ignore = n_ignore;
+  a.prev_wid = reinterpret_cast<const long long*>(prev_wid); a.prev_ptr = reinterpret_cast<const long long*>(prev_ptr);
+  a.prev_score = prev_score; a.prev_eos = prev_eos;
+  a.top_w = top_w; a.top_lp = top_lp;
+  a.wid = reinterpret_cast<long long*>(wid); a.ptr = reinterpret_cast<long long*>(ptr); a.score = score; a.eos = eos;
+  const PromptRows p = prompt_rows(*prompt);
+  return launch_diverse_beam_step(a, S(stream), &p);
+}
+
+int vlpk_constrained_beam_step_prompt(const VlpkConstrainedBeamArgs* args, const VlpkPromptRows* prompt, void* stream) {
+  VLPK_CHECK_ARG(args && prompt, "constrained_beam_step_prompt: null argument struct");
+  const PromptRows p = prompt_rows(*prompt);
+  return launch_constrained_beam_step(*args, S(stream), &p);
+}
+
 int vlpk_colsum(const void* x, int64_t ld, int64_t M, int N, float* out, void* stream) {
   VLPK_CHECK_ARG(x && out, "colsum: null pointer");
   return launch_colsum(x, ld, M, N, out, S(stream));

@@ -318,8 +318,8 @@ __device__ __forceinline__ void row_top_k(const float* val, int V, int K, int* o
 // Each thread owns one contiguous chunk of the row in shared memory and every sum is taken in a fixed order (chunk, then a
 // fixed shuffle tree), so the result depends on (seed, f, row, logits) only: not on the batch, the grid or the run.
 // Finished rows write pad_id and score 0; a row that draws eos_id is marked finished and decrements *live.
-template <typename T>
-__global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
+template <typename T, bool PROMPT>
+__device__ __forceinline__ void sample_rows(const SampleArgs& a, const PromptRows& p) {
   __shared__ float redf[33], pref[SAMPLE_THREADS + 1];
   __shared__ int redi[33], prei[SAMPLE_THREADS + 1];
   const int V = a.V, tid = threadIdx.x, row = blockIdx.x;
@@ -340,6 +340,8 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
     for (int t = tid; t < a.f; t += SAMPLE_THREADS) hist[t] = to_word(out[t]);
     blocked = ngram_candidates(hist, a.f, a.n, V, a.ignore, a.n_ignore, bits);
   }
+  const int draw_f = PROMPT ? a.f - p.hist_off : 0;                 // prompted: the generated word's frame g keys the draw
+  const int prompt_eos = PROMPT && p.eos_until ? draw_f + 1 <= p.eos_until[row] : 0;
 
   // x, coalesced, and its maximum (order-free)
   const T* lrow = static_cast<const T*>(a.logits) + static_cast<size_t>(row) * a.ld;
@@ -348,7 +350,7 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
   for (int v = tid; v < V; v += SAMPLE_THREADS) {
     float x = head_logit(lrow, bias, v);
     if (blocked && ((bits[v >> 5] >> (v & 31)) & 1u)) x += -10000.0f;
-    if (a.block_eos && v == a.eos_id) x = -10000.0f;
+    if ((PROMPT ? prompt_eos : a.block_eos) && v == a.eos_id) x = -10000.0f;
     val[v] = x;
     mx = fmaxf(mx, x);
   }
@@ -399,7 +401,7 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
   }
   block_exclusive_scan(kept, redf, pref);
 
-  const uint4 r = Philox::gen(a.seed, static_cast<unsigned long long>(a.f), static_cast<unsigned long long>(row));
+  const uint4 r = Philox::gen(a.seed, static_cast<unsigned long long>(PROMPT ? draw_f : a.f), static_cast<unsigned long long>(row));
   const float u = static_cast<float>(r.x >> 8) * (1.0f / 16777216.0f);
   const float goal = u * pref[SAMPLE_THREADS];
   int found = INT_MAX;
@@ -443,6 +445,28 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
   }
 }
 
+template <typename T>
+__global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) { sample_rows<T, false>(a, PromptRows{}); }
+
+// Prompted rows: seq[row, :hist_off] holds the row's prompt right-aligned behind -1 entries, f = hist_off + g for generated word g,
+// the draw is keyed by (seed; g, row) and [EOS] is blocked while g + 1 <= eos_until[row].
+template <typename T>
+__global__ void __launch_bounds__(SAMPLE_THREADS) sample_prompt_kernel(SampleArgs a, PromptRows p) { sample_rows<T, true>(a, p); }
+
+// The history of a prompted beam row at trace frame f, hf = hist_off + f entries (the prompt right-aligned behind -1 entries, then
+// the generated words): at f = 0, row `row` of hist_in (one per image) is read into seq; after, it is carried from the parent as
+// carry_history does.  The caller orders seq with a barrier before reading it.
+template <typename I64>
+__device__ __forceinline__ void prompt_history(const int* hist_in, int* hist_out, int* seq, const I64* prev_ptr, const I64* prev_wid,
+                                               int row, int width, int f, int hf, int T_cap) {
+  if (f == 0) {
+    const int* src = hist_in + static_cast<size_t>(row) * T_cap;
+    for (int t = threadIdx.x; t < hf; t += blockDim.x) seq[t] = src[t];
+  } else {
+    carry_history(hist_in, hist_out, seq, prev_ptr, prev_wid, row, width, hf, T_cap);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------------------------
 // Diverse beam search (Vijayakumar et al., AAAI 2018) of one frame f: K beams per image in G groups of Kg = K / G, with a Hamming
 // diversity penalty lambda.  Two launches.
@@ -467,8 +491,8 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_kernel(SampleArgs a) {
 constexpr int MERGE_THREADS = 256;
 constexpr int DIVERSE_MAX_CAND = DIVERSE_MAX_BEAMS * DIVERSE_MAX_BEAMS;       // Kg * K <= K * K candidates per group
 
-template <typename T>
-__global__ void __launch_bounds__(SAMPLE_THREADS) diverse_beam_rows_kernel(DiverseBeamArgs a) {
+template <typename T, bool PROMPT>
+__device__ __forceinline__ void diverse_rows(const DiverseBeamArgs& a, const PromptRows& p) {
   __shared__ float redf[33];
   __shared__ int redi[33], prei[SAMPLE_THREADS + 1];
   __shared__ int sel_w[DIVERSE_MAX_BEAMS];
@@ -479,12 +503,32 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) diverse_beam_rows_kernel(Diver
   row_smem(V, val, bits, hist);
 
   bool blocked = false;
-  if (a.n > 0 && a.f >= 1) {                                         // uniform
-    carry_history(a.hist_in, a.hist_out, hist, a.prev_ptr, a.prev_wid, row, K, a.f, a.T_cap);
-    if (a.f >= a.n) blocked = ngram_candidates(hist, a.f, a.n, V, a.ignore, a.n_ignore, bits);
+  if constexpr (PROMPT) {
+    const int hf = a.f + p.hist_off;
+    if (a.n > 0) {                                                   // uniform
+      prompt_history(a.hist_in, a.hist_out, hist, a.prev_ptr, a.prev_wid, row, K, a.f, hf, a.T_cap);
+      if (hf >= a.n) blocked = ngram_candidates(hist, hf, a.n, V, a.ignore, a.n_ignore, bits);
+    }
+    DiverseBeamArgs b = a;
+    if (p.eos_until) b.block_eos = a.f + 1 <= p.eos_until[row];
+    row_logp<T>(b, row, blocked, bits, val, redf);
+  } else {
+    if (a.n > 0 && a.f >= 1) {                                       // uniform
+      carry_history(a.hist_in, a.hist_out, hist, a.prev_ptr, a.prev_wid, row, K, a.f, a.T_cap);
+      if (a.f >= a.n) blocked = ngram_candidates(hist, a.f, a.n, V, a.ignore, a.n_ignore, bits);
+    }
+    row_logp<T>(a, row, blocked, bits, val, redf);
   }
-  row_logp<T>(a, row, blocked, bits, val, redf);
   row_top_k(val, V, K, a.top_w + static_cast<size_t>(row) * K, a.top_lp + static_cast<size_t>(row) * K, redi, prei, sel_w, sel_lp);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(SAMPLE_THREADS) diverse_beam_rows_kernel(DiverseBeamArgs a) { diverse_rows<T, false>(a, PromptRows{}); }
+
+// Prompted rows: histories of hist_off + f entries (prompt_history), [EOS] blocked while f + 1 <= eos_until[row].
+template <typename T>
+__global__ void __launch_bounds__(SAMPLE_THREADS) diverse_beam_rows_prompt_kernel(DiverseBeamArgs a, PromptRows p) {
+  diverse_rows<T, true>(a, p);
 }
 
 __global__ void __launch_bounds__(MERGE_THREADS) diverse_beam_merge_kernel(DiverseBeamArgs a) {
@@ -567,8 +611,8 @@ __device__ __forceinline__ int cbs_root_state(const VlpkConstrainedBeamArgs& a, 
   return s;
 }
 
-template <typename T>
-__global__ void __launch_bounds__(SAMPLE_THREADS) constrained_beam_rows_kernel(VlpkConstrainedBeamArgs a) {
+template <typename T, bool PROMPT>
+__device__ __forceinline__ void constrained_rows(const VlpkConstrainedBeamArgs& a, const PromptRows& p) {
   __shared__ float redf[33];
   __shared__ int redi[33], prei[SAMPLE_THREADS + 1];
   __shared__ int sel_w[CBS_MAX_BEAMS];
@@ -584,18 +628,23 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) constrained_beam_rows_kernel(V
   unsigned* bits; int* hist;
   row_smem(V, val, bits, hist);
 
-  if (f >= 1) carry_history(a.hist_in, a.hist_out, hist, a.prev_ptr, a.prev_wid, row, SK, f, a.T_cap);      // uniform
+  const int hf = PROMPT ? f + p.hist_off : f;                      // the history's length
+  if constexpr (PROMPT) {
+    prompt_history(a.hist_in, a.hist_out, hist, a.prev_ptr, a.prev_wid, row, SK, f, hf, a.T_cap);
+  } else {
+    if (f >= 1) carry_history(a.hist_in, a.hist_out, hist, a.prev_ptr, a.prev_wid, row, SK, f, a.T_cap);      // uniform
+  }
   __syncthreads();
-  const bool blocked = a.n > 0 && f >= a.n && ngram_candidates(hist, f, a.n, V, a.ignore, a.n_ignore, bits);
+  const bool blocked = a.n > 0 && hf >= a.n && ngram_candidates(hist, hf, a.n, V, a.ignore, a.n_ignore, bits);
 
   if (tid < CA) {                                                    // alternative tid: constraint tid / A
     const int64_t* alt = a.cons + (static_cast<size_t>(b) * CA + tid) * a.P;
     int len = 0;
     while (len < a.P && alt[len] != 0) ++len;
     int w = -1;
-    if (len > 0 && len - 1 <= f && !((state >> (tid / a.A)) & 1) && alt[len - 1] >= 0 && alt[len - 1] < V) {
+    if (len > 0 && len - 1 <= hf && !((state >> (tid / a.A)) & 1) && alt[len - 1] >= 0 && alt[len - 1] < V) {
       bool match = true;
-      for (int t = 0; t < len - 1 && match; ++t) match = hist[f - (len - 1) + t] == alt[t];
+      for (int t = 0; t < len - 1 && match; ++t) match = hist[hf - (len - 1) + t] == alt[t];
       if (match) w = static_cast<int>(alt[len - 1]);
     }
     hit[tid] = w;
@@ -617,7 +666,13 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) constrained_beam_rows_kernel(V
     n_comp = m;
   }
 
-  row_logp<T>(a, row, blocked, bits, val, redf);
+  if constexpr (PROMPT) {
+    VlpkConstrainedBeamArgs e = a;
+    if (p.eos_until) e.block_eos = f + 1 <= p.eos_until[row];
+    row_logp<T>(e, row, blocked, bits, val, redf);
+  } else {
+    row_logp<T>(a, row, blocked, bits, val, redf);
+  }
   __syncthreads();
   const size_t out = static_cast<size_t>(row) * W;
   if (tid < CA) {                                                    // completing entries, then out of the top-K search
@@ -630,6 +685,19 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) constrained_beam_rows_kernel(V
   }
   __syncthreads();
   row_top_k(val, V, K, a.top_w + out, a.top_lp + out, redi, prei, sel_w, sel_lp);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(SAMPLE_THREADS) constrained_beam_rows_kernel(VlpkConstrainedBeamArgs a) {
+  constrained_rows<T, false>(a, PromptRows{});
+}
+
+// Prompted rows: histories of hist_off + f entries (prompt_history), read always, so a phrase may begin in the prompt; [EOS] blocked
+// while f + 1 <= eos_until[row].  A constraint the prompt already contains is met from the start through the table (its
+// alternatives zeroed for that image by the caller).
+template <typename T>
+__global__ void __launch_bounds__(SAMPLE_THREADS) constrained_beam_rows_prompt_kernel(VlpkConstrainedBeamArgs a, PromptRows p) {
+  constrained_rows<T, true>(a, p);
 }
 
 size_t cbs_merge_smem_bytes(int K, int C, int A) {                   // one state's candidates at most: value, parent, word
@@ -709,15 +777,15 @@ int allow_dynamic_smem(int bytes) {
 }
 
 // One CTA of SAMPLE_THREADS per row, with `smem` bytes of row_smem, of the fp32 or the bf16 instantiation of a row kernel.
-template <auto KernelF, auto KernelB, typename Args>
-int launch_rows(int rows, size_t smem, cudaStream_t s, const Args& a) {
+template <auto KernelF, auto KernelB, typename Args, typename... Extra>
+int launch_rows(int rows, size_t smem, cudaStream_t s, const Args& a, const Extra&... extra) {
   LaunchScope scope(CAT_MISC, (a.fp32 ? 8.0 : 4.0) * rows * a.V, s);
   if (a.fp32) {
     VLPK_TRY(allow_dynamic_smem<KernelF>(static_cast<int>(SAMPLE_SMEM_MAX)));
-    KernelF<<<rows, SAMPLE_THREADS, smem, s>>>(a);
+    KernelF<<<rows, SAMPLE_THREADS, smem, s>>>(a, extra...);
   } else {
     VLPK_TRY(allow_dynamic_smem<KernelB>(static_cast<int>(SAMPLE_SMEM_MAX)));
-    KernelB<<<rows, SAMPLE_THREADS, smem, s>>>(a);
+    KernelB<<<rows, SAMPLE_THREADS, smem, s>>>(a, extra...);
   }
   VLPK_CUDA(cudaGetLastError());
   return 0;
@@ -735,7 +803,7 @@ int check_frame(const char* name, int V, int fp32, int T_cap, int f, int n, int 
 
 }  // namespace
 
-int launch_sample(const SampleArgs& a, cudaStream_t s) {
+int launch_sample(const SampleArgs& a, cudaStream_t s, const PromptRows* p) {
   VLPK_CHECK_ARG(a.rows >= 0 && a.V >= 1 && a.ld >= a.V, "sample: rows=%d V=%d ld=%lld (ld must be >= V >= 1)", a.rows, a.V, a.ld);
   VLPK_CHECK_ARG(a.mode == SAMPLE_TOPK || a.mode == SAMPLE_TOPP, "sample: mode=%d (0 top-k, 1 top-p)", a.mode);
   VLPK_CHECK_ARG(a.mode != SAMPLE_TOPK || (a.topk >= 1 && a.topk <= SAMPLE_MAX_TOPK), "sample: topk=%d outside [1, %d]", a.topk,
@@ -744,11 +812,14 @@ int launch_sample(const SampleArgs& a, cudaStream_t s) {
   const size_t smem = row_smem_bytes(a.T_cap, a.V);
   VLPK_TRY(check_frame("sample", a.V, a.fp32, a.T_cap, a.f, a.n, a.n_ignore, a.ignore, smem));
   VLPK_CHECK_ARG(a.logits && a.seq && a.finished && a.live, "sample: null pointer (logits, seq, finished, live)");
+  VLPK_CHECK_ARG(!p || (p->hist_off >= 0 && p->hist_off <= a.f), "sample: prompt width hist_off=%d outside [0, f=%d]", p ? p->hist_off : 0,
+                 a.f);
   if (a.rows == 0) return 0;
+  if (p) return launch_rows<sample_prompt_kernel<float>, sample_prompt_kernel<bf16>>(a.rows, smem, s, a, *p);
   return launch_rows<sample_kernel<float>, sample_kernel<bf16>>(a.rows, smem, s, a);
 }
 
-int launch_diverse_beam_step(const DiverseBeamArgs& a, cudaStream_t s) {
+int launch_diverse_beam_step(const DiverseBeamArgs& a, cudaStream_t s, const PromptRows* p) {
   VLPK_CHECK_ARG(a.B >= 0 && a.K >= 1 && a.K <= DIVERSE_MAX_BEAMS, "diverse_beam_step: B=%d K=%d (K must lie in [1, %d])", a.B, a.K,
                  DIVERSE_MAX_BEAMS);
   VLPK_CHECK_ARG(a.G >= 1 && a.K % a.G == 0, "diverse_beam_step: G=%d groups do not divide K=%d beams", a.G, a.K);
@@ -763,19 +834,26 @@ int launch_diverse_beam_step(const DiverseBeamArgs& a, cudaStream_t s) {
                  a.f);
   const bool hist = a.n > 0 && a.f >= 1;
   VLPK_CHECK_ARG(!hist || (a.hist_out && a.prev_wid), "diverse_beam_step: null pointer (hist_out, prev_wid are needed at f=%d)", a.f);
-  VLPK_CHECK_ARG(!hist || a.f == 1 || (a.hist_in && a.prev_ptr), "diverse_beam_step: null pointer (hist_in, prev_ptr are needed at f=%d)",
-                 a.f);
+  VLPK_CHECK_ARG(!hist || (a.f == 1 && !p) || (a.hist_in && a.prev_ptr),
+                 "diverse_beam_step: null pointer (hist_in, prev_ptr are needed at f=%d)", a.f);
   VLPK_CHECK_ARG(!hist || a.hist_in != a.hist_out, "diverse_beam_step: hist_in and hist_out must be different buffers");
+  VLPK_CHECK_ARG(!p || (p->hist_off >= 0 && a.f + p->hist_off < a.T_cap), "diverse_beam_step: prompt width hist_off=%d with f=%d outside "
+                 "T_cap=%d", p ? p->hist_off : 0, a.f, a.T_cap);
+  VLPK_CHECK_ARG(!p || a.n == 0 || a.hist_in, "diverse_beam_step: null pointer (hist_in holds the prompts' histories)");
   if (a.B == 0) return 0;
   const int rows = a.f == 0 ? a.B : a.B * a.K;
-  VLPK_TRY((launch_rows<diverse_beam_rows_kernel<float>, diverse_beam_rows_kernel<bf16>>(rows, smem, s, a)));
+  if (p) {
+    VLPK_TRY((launch_rows<diverse_beam_rows_prompt_kernel<float>, diverse_beam_rows_prompt_kernel<bf16>>(rows, smem, s, a, *p)));
+  } else {
+    VLPK_TRY((launch_rows<diverse_beam_rows_kernel<float>, diverse_beam_rows_kernel<bf16>>(rows, smem, s, a)));
+  }
   LaunchScope scope(CAT_MISC, 8.0 * rows * a.K, s);
   diverse_beam_merge_kernel<<<a.B, MERGE_THREADS, 0, s>>>(a);
   VLPK_CUDA(cudaGetLastError());
   return 0;
 }
 
-int launch_constrained_beam_step(const VlpkConstrainedBeamArgs& a, cudaStream_t s) {
+int launch_constrained_beam_step(const VlpkConstrainedBeamArgs& a, cudaStream_t s, const PromptRows* p) {
   VLPK_CHECK_ARG(a.C >= 1 && a.C <= CBS_MAX_CONSTRAINTS && a.A >= 1 && a.A <= CBS_MAX_ALTS && a.P >= 1 && a.P <= CBS_MAX_WORDS,
                  "constrained_beam_step: C=%d A=%d P=%d (C in [1, %d], A in [1, %d], P in [1, %d])", a.C, a.A, a.P, CBS_MAX_CONSTRAINTS,
                  CBS_MAX_ALTS, CBS_MAX_WORDS);
@@ -789,11 +867,18 @@ int launch_constrained_beam_step(const VlpkConstrainedBeamArgs& a, cudaStream_t 
                  "constrained_beam_step: null pointer (logits, cons, top_w, top_lp, top_dest, wid, ptr, score, eos)");
   VLPK_CHECK_ARG(a.f == 0 || (a.prev_score && a.prev_eos && a.prev_wid && a.hist_out),
                  "constrained_beam_step: null pointer (prev_score, prev_eos, prev_wid, hist_out are needed at f=%d)", a.f);
-  VLPK_CHECK_ARG(a.f <= 1 || (a.hist_in && a.prev_ptr), "constrained_beam_step: null pointer (hist_in, prev_ptr are needed at f=%d)", a.f);
+  VLPK_CHECK_ARG((a.f <= 1 && !p) || (a.hist_in && (a.f == 0 || a.prev_ptr)),
+                 "constrained_beam_step: null pointer (hist_in, prev_ptr are needed at f=%d)", a.f);
   VLPK_CHECK_ARG(a.f == 0 || a.hist_in != a.hist_out, "constrained_beam_step: hist_in and hist_out must be different buffers");
+  VLPK_CHECK_ARG(!p || (p->hist_off >= 0 && a.f + p->hist_off < a.T_cap), "constrained_beam_step: prompt width hist_off=%d with f=%d "
+                 "outside T_cap=%d", p ? p->hist_off : 0, a.f, a.T_cap);
   if (a.B == 0) return 0;
   const int SK = a.K << a.C, rows = a.f == 0 ? a.B : a.B * SK;
-  VLPK_TRY((launch_rows<constrained_beam_rows_kernel<float>, constrained_beam_rows_kernel<bf16>>(rows, smem, s, a)));
+  if (p) {
+    VLPK_TRY((launch_rows<constrained_beam_rows_prompt_kernel<float>, constrained_beam_rows_prompt_kernel<bf16>>(rows, smem, s, a, *p)));
+  } else {
+    VLPK_TRY((launch_rows<constrained_beam_rows_kernel<float>, constrained_beam_rows_kernel<bf16>>(rows, smem, s, a)));
+  }
   VLPK_TRY(allow_dynamic_smem<constrained_beam_merge_kernel>(static_cast<int>(cbs_merge_smem_bytes(CBS_MAX_BEAMS, 2, CBS_MAX_ALTS))));
   LaunchScope scope(CAT_MISC, 8.0 * rows * (a.K + a.C * a.A), s);
   constrained_beam_merge_kernel<<<dim3(1 << a.C, a.B), MERGE_THREADS, cbs_merge_smem_bytes(a.K, a.C, a.A), s>>>(a);

@@ -51,7 +51,14 @@ struct SampleArgs {
   int n_ignore = 0;
 };
 
-int launch_sample(const SampleArgs& a, cudaStream_t s);
+// Prompted rows of the row kernels (vlpk.h, VlpkPromptRows): histories start with hist_off prompt entries, and [EOS] is blocked per
+// row while the generated word's frame g satisfies g + 1 <= eos_until[row] (eos_until null: block_eos as without a prompt).
+struct PromptRows {
+  int hist_off = 0;
+  const int* eos_until = nullptr;
+};
+
+int launch_sample(const SampleArgs& a, cudaStream_t s, const PromptRows* p = nullptr);
 
 // Diverse beam search: one frame's selection, K beams per image in G groups with a Hamming penalty (see decode.cu).
 constexpr int DIVERSE_MAX_BEAMS = SAMPLE_MAX_TOPK;
@@ -85,11 +92,11 @@ struct DiverseBeamArgs {
   float* eos = nullptr;
 };
 
-int launch_diverse_beam_step(const DiverseBeamArgs& a, cudaStream_t s);
+int launch_diverse_beam_step(const DiverseBeamArgs& a, cudaStream_t s, const PromptRows* p = nullptr);
 
 // Constrained beam search: one frame's selection, K beams in each of the 2^C constraint states (see decode.cu and vlpk.h).
 constexpr int CBS_MAX_CONSTRAINTS = 4, CBS_MAX_ALTS = 4, CBS_MAX_WORDS = 8, CBS_MAX_BEAMS = 64, CBS_MAX_SLOTS = 256;
 
-int launch_constrained_beam_step(const VlpkConstrainedBeamArgs& a, cudaStream_t s);
+int launch_constrained_beam_step(const VlpkConstrainedBeamArgs& a, cudaStream_t s, const PromptRows* p = nullptr);
 
 }  // namespace vlpk

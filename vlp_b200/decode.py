@@ -143,6 +143,119 @@ def check_constraints(cons, vocab_size, beam_size, max_words=None, values=True):
         raise ValueError(f"vlp_b200: a constraint alternative is longer than the {max_words} words the decode generates")
 
 
+def prompt_table(prompt):
+    """The host int64 [1, Tp] prompt of a list of word ids shared by every image; ValueError for anything else."""
+    if isinstance(prompt, (str, bytes)) or not isinstance(prompt, (list, tuple)) \
+            or any(isinstance(w, bool) or not isinstance(w, int) for w in prompt):
+        raise ValueError("vlp_b200: prompt must be a list of word ids")
+    return torch.tensor([list(prompt)], dtype=torch.int64).reshape(1, len(prompt))
+
+
+def check_prompt(prompt, batch, vocab_size, max_words, eos_id, mask_word_id, values=True):
+    """ValueError, before anything is launched, for a prompt table the decoder does not take: prompt_ids must be an int64 [B, Tp] or
+    [1, Tp] tensor with Tp < max_words (out_len - in_len: at least one word is generated); with values, read from a host copy, its
+    ids must lie in [1, vocab_size) with 0 only as padding after a row's words, and no row may hold eos_id or mask_word_id."""
+    if not torch.is_tensor(prompt) or prompt.dim() != 2 or prompt.dtype != torch.int64:
+        raise ValueError("vlp_b200: prompt_ids must be an int64 tensor [B, Tp] (or [1, Tp] for every image) of word ids, 0-padded")
+    if prompt.shape[0] not in (1, batch):
+        raise ValueError(f"vlp_b200: prompt_ids for {prompt.shape[0]} images, the batch has {batch}")
+    if prompt.shape[1] >= max_words:
+        raise ValueError(f"vlp_b200: a prompt of width Tp={prompt.shape[1]} leaves no word of the {max_words} the decode generates "
+                         "(Tp < out_len - in_len needed)")
+    if not values:
+        return
+    p = prompt.cpu()
+    if bool(((p < 0) | (p >= vocab_size)).any()):
+        raise ValueError(f"vlp_b200: prompt word ids must lie in [1, {vocab_size}) (0 is padding)")
+    if bool(((p[:, 1:] != 0) & (p[:, :-1] == 0)).any()):
+        raise ValueError("vlp_b200: a prompt row has a 0 (padding) before a word id")
+    for name, w in (("eos_id", eos_id), ("mask_word_id", mask_word_id)):
+        if bool((p == int(w)).any()):
+            raise ValueError(f"vlp_b200: a prompt holds the decoder's {name} ({int(w)})")
+
+
+def check_prompt_mode(sampling_method, num_beam_groups=1, constraints=False, use_kv_cache=True, output_attentions=False):
+    """ValueError for decode settings that do not take a prompt: prompted captions run in every decode mode over the K/V caches,
+    without attention maps."""
+    if not use_kv_cache:
+        raise ValueError("vlp_b200: a prompt needs use_kv_cache (the prompts run in the step-0 prefill of the K/V caches)")
+    if output_attentions:
+        raise ValueError("vlp_b200: output_attentions is not available with a prompt")
+
+
+def prompt_lengths(prompt):
+    """t_b, the number of words of each prompt row [B] (int64): its non-zero entries, which come first."""
+    return (prompt != 0).sum(1)
+
+
+def prompt_columns(prompt, in_len, out_len):
+    """The gap layout of a prompted decode, column space -> position space, for B images with prompts prompt [B, Tp] of t_b words:
+    column c of image b holds
+      c < in_len                      the image prefix, position c;
+      in_len <= c < in_len + t_b      prompt word c - in_len, position c;
+      in_len + t_b <= c < in_len + Tp a gap (PAD id, masked out as a key for every row), position c;
+      c >= in_len + Tp                the [MASK] of frame c - in_len - Tp and the words after it, position c - (Tp - t_b).
+    Returns (pos [B, out_len] int64, gap [B, out_len] bool)."""
+    B, Tp = prompt.shape
+    lens = prompt_lengths(prompt).unsqueeze(1)
+    c = torch.arange(out_len, device=prompt.device).unsqueeze(0)
+    pos = torch.where(c < in_len + Tp, c, c - (Tp - lens))
+    gap = (c >= in_len + lens) & (c < in_len + Tp)
+    return pos, gap
+
+
+def with_prompt(prompt, seq, fill=None):
+    """seq [B, ..., L] whose column g holds frame g's generated word -> the caption: image b's t_b prompt words (or `fill`, e.g. 0 for
+    per-word scores), then seq shifted right by t_b.  Columns shifted past L hold padding and drop off."""
+    B, L = seq.shape[0], seq.shape[-1]
+    view = (B,) + (1,) * (seq.dim() - 1)
+    lens = prompt_lengths(prompt).view(view)
+    j = torch.arange(L, device=seq.device)
+    shifted = seq.gather(-1, (j - lens).clamp_min(0).expand(seq.shape))
+    if fill is None:
+        head = prompt.new_zeros(B, L)
+        head[:, :prompt.shape[1]] = prompt
+        head = head.view(B, *([1] * (seq.dim() - 2)), L).to(seq.dtype)
+    else:
+        head = torch.full_like(seq, fill)
+    return torch.where(j < lens, head, shifted)
+
+
+def prompt_history(prompt, rows_per_image, width):
+    """The n-gram history of a prompted beam search before its first generated word, int32 [B * rows_per_image, width]: each
+    image's prompt right-aligned in columns [0, Tp) behind Tp - t_b entries of -1 (a word id that matches no word and is never a
+    candidate), repeated for its rows.  A history of Tp + g entries at frame g then holds the same n-grams as the t_b + g words
+    of the caption."""
+    B, Tp = prompt.shape
+    lens = prompt_lengths(prompt).unsqueeze(1)
+    j = torch.arange(Tp, device=prompt.device).unsqueeze(0)
+    right = prompt.gather(1, (j - (Tp - lens)).clamp_min(0))
+    hist = torch.full((B, width), -1, dtype=torch.int32, device=prompt.device)
+    hist[:, :Tp] = torch.where(j >= Tp - lens, right, torch.full_like(right, -1)).to(torch.int32)
+    return hist.repeat_interleave(rows_per_image, 0)
+
+
+def prompt_eos_until(prompt, rows_per_image, min_len):
+    """The prompted selectors' per-row [EOS] block: int32 [B * rows_per_image], min_len - t_b (frame g is blocked while g + 1 <= it),
+    or None without min_len."""
+    if not min_len:
+        return None
+    return (int(min_len) - prompt_lengths(prompt)).to(torch.int32).repeat_interleave(rows_per_image)
+
+
+def prompt_constraints(cons, prompt):
+    """The constraint table of a prompted constrained search: constraint j of image b is met from the start when one of its
+    alternatives occurs as a contiguous run of image b's prompt words, and its alternatives are then zeroed for that image (the
+    search's root state holds it).  Device ops only.  cons [B, C, A, P], prompt [B, Tp] -> [B, C, A, P]."""
+    B, C, A, P = cons.shape
+    words = torch.where(prompt != 0, prompt, torch.full_like(prompt, -1))
+    windows = torch.cat((words, words.new_full((B, P), -1)), 1).unfold(1, P, 1)           # [B, Tp + 1, P]
+    alt = cons.unsqueeze(3)                                                              # [B, C, A, 1, P]
+    hit = ((alt == 0) | (alt == windows.view(B, 1, 1, -1, P))).all(-1) & (cons[..., :1] != 0)   # [B, C, A, Tp + 1]
+    met = hit.flatten(2).any(-1)                                                         # [B, C]
+    return cons.masked_fill(met.view(B, C, 1, 1), 0)
+
+
 class DecodeState:
     """A decode's per-sequence inputs and what persists between its steps; the only code that knows how a step's rows reach the
     encoder.  The history is one of:
@@ -150,19 +263,35 @@ class DecodeState:
       - the reference's data flow (use_kv_cache False, modeling.py:273-277): the embeddings and every layer's output of the rows
         decoded so far, re-projected to K and V at every step;
       - with shared_prefix = G: a SharedPrefixCache of G hypotheses per image, one copy of each image prefix's K/V.
-    It holds one row per image until expand(G), B*G rows after."""
+    It holds one row per image until expand(G), B*G rows after.
 
-    def __init__(self, dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, shared_prefix=None):
+    prompt: int64 [B, Tp], Tp >= 1 (prompt_columns): step 0 feeds first_ids = input_ids ‖ the Tp prompt columns ‖ [MASK], and the
+    per-sequence inputs are taken in column space (positions, token types and the attention mask gathered at each column's position,
+    gap columns masked out as keys), built here once with device ops only.  The decode then runs `frames` = out_len - in_len - Tp
+    steps; a shared prefix cache holds the prompt columns in each image's prefix, P = in_len + Tp."""
+
+    def __init__(self, dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, shared_prefix=None, prompt=None):
         self.dec, self.vis_feats, self.vis_pe = dec, vis_feats, vis_pe
         self.token_type_ids, self.position_ids, self.attention_mask = token_type_ids, position_ids, attention_mask
         B, self.in_len = input_ids.shape
         out_len = token_type_ids.shape[1]
+        self.first_ids = input_ids
+        self.prefix_len = self.in_len
+        if prompt is not None:
+            self.prefix_len += prompt.shape[1]
+            self.first_ids = torch.cat((input_ids, prompt.to(input_ids.dtype)), dim=1)
+            pos, gap = prompt_columns(prompt, self.in_len, out_len)
+            self.token_type_ids, self.position_ids = token_type_ids.gather(1, pos), position_ids.gather(1, pos)
+            m = attention_mask.gather(1, pos.unsqueeze(2).expand(B, out_len, attention_mask.shape[2]))
+            m = m.gather(2, pos.unsqueeze(1).expand(B, out_len, out_len))
+            self.attention_mask = torch.where(gap.unsqueeze(1), torch.zeros_like(m), m)
+        self.frames = out_len - self.prefix_len
         self.mask_ids = input_ids[:, :1] * 0 + dec.mask_word_id
-        self.next_pos = self.in_len
+        self.next_pos = self.prefix_len
         self.shared = shared_prefix is not None
         self.prev_emb = self.prev_layers = None
         if self.shared:
-            self.caches = SharedPrefixCache(len(dec.bert.encoder.layer), B, shared_prefix, self.in_len, out_len - self.in_len,
+            self.caches = SharedPrefixCache(len(dec.bert.encoder.layer), B, shared_prefix, self.prefix_len, out_len - self.prefix_len,
                                             dec.config.hidden_size, input_ids.device)
         else:
             self.caches = dec.new_kv_caches(B, input_ids.device, out_len) if dec.use_kv_cache else None
@@ -210,7 +339,7 @@ class DecodeState:
     def reorder(self, parent):
         """Beam step: hypothesis i continues hypothesis parent[i] (int64 [rows]), whose history it takes over."""
         if self.shared:
-            self.caches.reorder(parent, self.next_pos - self.in_len - 2)      # the frame of the word the last step fed
+            self.caches.reorder(parent, self.next_pos - self.prefix_len - 2)      # the frame of the word the last step fed
         elif self.caches is not None:
             self.caches = [c.index_select(0, parent) for c in self.caches]
         else:
@@ -244,16 +373,17 @@ def _ignore_tensor(dec, dev):
 
 
 def greedy_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, sample_mode="greedy",
-                  output_attentions=False):
+                  output_attentions=False, prompt=None):
     """The reference's greedy / sample_mode="sample" loop (modeling.py:1210-1252): (ids, scores) [B, out_len - in_len], the arg-max
     words and their logits, or the drawn words and their log-probabilities; with output_attentions also the maps, as
-    BertForSeq2SeqDecoder.forward describes."""
-    state = DecodeState(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask)
+    BertForSeq2SeqDecoder.forward describes.  prompt [B, Tp] (Tp >= 1): the loop runs out_len - in_len - Tp frames after the prompt's
+    prefill, and row b of ids holds image b's t_b prompt words (score 0), then its generated words, then 0."""
+    state = DecodeState(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, prompt=prompt)
     B, in_len = input_ids.shape
     out_len = token_type_ids.shape[1]
     maps = new_attention_maps(dec, B, out_len - in_len, out_len, input_ids.device) if output_attentions else None
-    curr_ids, output_ids, output_probs = input_ids, [], []
-    for frame in range(out_len - in_len):
+    curr_ids, output_ids, output_probs = state.first_ids, [], []
+    for frame in range(state.frames):
         prediction_scores, _ = dec.cls(state.step(curr_ids, None if maps is None else maps[:, frame]), None, task_idx=task_idx)
         if sample_mode == "greedy":
             probs, curr_ids = torch.max(prediction_scores, dim=-1)
@@ -266,11 +396,14 @@ def greedy_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_id
         output_ids.append(curr_ids)
         output_probs.append(probs)
     out = torch.cat(output_ids, dim=1), torch.cat(output_probs, dim=1)
+    if prompt is not None:
+        pad = (0, prompt.shape[1])
+        out = with_prompt(prompt, F.pad(out[0], pad)), with_prompt(prompt, F.pad(out[1], pad), fill=0)
     return out if maps is None else out + (maps,)
 
 
 def sample_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, seed=None,
-                  output_attentions=False):
+                  output_attentions=False, prompt=None):
     """Top-k and top-p (nucleus) sampling on the device.  `sampling_method="topk"` keeps the `topk` most likely words of every step,
     `"topp"` the smallest set whose probability reaches `topp`; one word is drawn from the kept set, renormalised.  The head's decoder
     runs without its bias, and one vlpk_sample_tokens launch per step adds the bias, applies the duplicate-n-gram blocking of beam
@@ -288,7 +421,11 @@ def sample_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_id
     image's prefix (shared_prefix.py).  A row that draws [EOS] is finished; its later positions hold PAD_ID with score 0.  Outside
     CUDA-graph capture the loop also stops once every row is finished: each step copies the device's count of live rows to pinned
     host memory and the loop reads it once the copy's event has completed (a non-blocking query, never a synchronisation), so it
-    stops a step or two after the last [EOS]."""
+    stops a step or two after the last [EOS].
+
+    prompt [B, Tp] (Tp >= 1): out_len - in_len - Tp frames after the prompt's prefill; each row's history starts with its image's
+    prompt (vlpk_sample_tokens_prompt), so n-gram blocking and min_len count it, and the draw of generated word g stays keyed by
+    (seed; g, r).  ids / scores hold the t_b prompt words (score 0), then the sampled words."""
     seed = dec.seed if seed is None else seed
     B, in_len = input_ids.shape
     out_len = token_type_ids.shape[1]
@@ -300,8 +437,12 @@ def sample_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_id
     # N > 1: row b * N + j is sample j of image b, drawn exactly as row b * N + j of the batch repeated with repeat_interleave(N)
     N = dec.num_return_sequences
     R = B * N
+    Tp = 0 if prompt is None else prompt.shape[1]
     ids = torch.full((R, T), PAD_ID, dtype=torch.int64, device=dev)
     scores = torch.zeros(R, T, dtype=torch.float32, device=dev)
+    if Tp:
+        ids[:, :Tp] = prompt_history(prompt, N, Tp)                      # the rows' histories start with their prompts
+        prompt_rows = (Tp, prompt_eos_until(prompt, N, dec.min_len))
     finished = torch.zeros(R, dtype=torch.int32, device=dev)
     live = torch.full((1,), R, dtype=torch.int32, device=dev)
     poll = None
@@ -309,11 +450,11 @@ def sample_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_id
         poll, polled = torch.empty(1, dtype=torch.int32, pin_memory=True), None
     if N > 1:
         task_idx = expand_task_idx(task_idx, B, N)
-    state = DecodeState(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, N if N > 1 else None)
+    state = DecodeState(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, N if N > 1 else None, prompt)
     maps = new_attention_maps(dec, B, T, out_len, dev) if output_attentions else None
-    curr_ids = input_ids
+    curr_ids = state.first_ids
     dec.last_decode_steps = 0
-    for frame in range(T):
+    for frame in range(state.frames):
         if poll is not None and polled is not None and polled.query():
             if int(poll[0]) == 0:
                 break                                                  # every row has drawn [EOS]: the rest stays padding
@@ -324,20 +465,30 @@ def sample_decode(dec, vis_feats, vis_pe, input_ids, token_type_ids, position_id
             # here on every input is per sample (the attention mask stays per image: the shared cache reads it so).  The rows keep
             # the prefill output's row stride too, as a slice of the repeated batch's output would: the head's GEMMs pick their
             # kernels by shape and strides, and a contiguous copy rounds differently at BERT-base sizes.
-            full = last.new_empty(R, in_len + 1, last.shape[2])
+            full = last.new_empty(R, state.prefix_len + 1, last.shape[2])
             full[:, -1:] = last.repeat_interleave(N, 0)
             last = full[:, -1:]
             state.expand(N)
         h = pred.select_task(pred.transform(last.to(pred.decoder.weight.dtype)), task_idx)
         logits = pred.decoder(h)                                       # [R, 1, V]; the bias is added inside the sampling kernel
-        ops.sample_tokens(logits, pred.bias.to(logits.dtype), dec.sampling_method, dec.topk, dec.topp, seed, frame, ids, scores, finished,
-                          live, dec.eos_id, PAD_ID, block_eos=bool(dec.min_len) and frame + 1 <= dec.min_len, ngram=ngram, ignore=ignore)
+        if Tp:
+            ops.sample_tokens(logits, pred.bias.to(logits.dtype), dec.sampling_method, dec.topk, dec.topp, seed, Tp + frame, ids, scores,
+                              finished, live, dec.eos_id, PAD_ID, ngram=ngram, ignore=ignore, prompt=prompt_rows)
+        else:
+            ops.sample_tokens(logits, pred.bias.to(logits.dtype), dec.sampling_method, dec.topk, dec.topp, seed, frame, ids, scores,
+                              finished, live, dec.eos_id, PAD_ID, block_eos=bool(dec.min_len) and frame + 1 <= dec.min_len, ngram=ngram,
+                              ignore=ignore)
         if poll is not None and polled is None:
             poll.copy_(live, non_blocking=True)
             polled = torch.cuda.Event()
             polled.record()
-        curr_ids = ids[:, frame:frame + 1]
+        curr_ids = ids[:, Tp + frame:Tp + frame + 1]
         dec.last_decode_steps += 1
+    if Tp:
+        ids = F.pad(ids[:, Tp:], (0, Tp), value=PAD_ID)
+        scores = F.pad(scores[:, Tp:], (0, Tp))
+        view = (B, N, T) if N > 1 else (B, T)
+        return with_prompt(prompt, ids.view(view)), with_prompt(prompt, scores.view(view), fill=0)
     if N > 1:
         return ids.view(B, N, T), scores.view(B, N, T)
     return (ids, scores) if maps is None else (ids, scores, maps)

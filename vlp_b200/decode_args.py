@@ -10,7 +10,7 @@ A script that already defines one of these options (decode_img2txt.py has its ow
 import argparse
 
 from . import ops
-from .decode import CONSTRAINT_LIMITS, SAMPLING_METHODS, check_decode
+from .decode import CONSTRAINT_LIMITS, SAMPLING_METHODS, check_decode, check_prompt_mode
 
 
 def constraint_spec(text):
@@ -45,6 +45,8 @@ _OPTIONS = (
     ("--constraints", dict(type=constraint_spec, default=None, help="constrained beam search: words or phrases every caption must "
                                                                    "contain, e.g. 'dog,dogs|frisbee' ('|' separates constraints, "
                                                                    "',' the alternatives of one)")),
+    ("--prompt", dict(type=str, default=None, help="prompted captions: every caption starts with these words, e.g. 'a photo of' "
+                                                   "(greedy decode and beam search)")),
 )
 
 
@@ -64,6 +66,8 @@ def check_decode_args(args):
     check_decode(args.sampling_method, args.topk, args.topp, args.beam_size, args.num_return_sequences, args.forbid_duplicate_ngrams,
                  args.ngram_size, ngram_in_greedy=True, num_beam_groups=args.num_beam_groups, diversity_penalty=args.diversity_penalty,
                  constraints=getattr(args, "constraints", None) is not None)
+    if getattr(args, "prompt", None):
+        check_prompt_mode(args.sampling_method, args.num_beam_groups, getattr(args, "constraints", None) is not None)
 
 
 def parse_decode_args(parser, argv=None):
@@ -78,8 +82,8 @@ def parse_decode_args(parser, argv=None):
 
 def decoder_kwargs(args, tokenizer=None):
     """BertForSeq2SeqDecoder keyword arguments of the parsed options.  tokenizer (convert_tokens_to_ids) maps --forbid_ignore_word
-    to word ids, as decode_img2txt.py does, and tokenizes every --constraints alternative into wordpieces (tokenize, then
-    convert_tokens_to_ids); without one both options must be empty."""
+    to word ids, as decode_img2txt.py does, and tokenizes every --constraints alternative and the --prompt into wordpieces (tokenize,
+    then convert_tokens_to_ids); without one these options must be empty."""
     check_decode_args(args)
     ignore = None
     if args.forbid_ignore_word:
@@ -99,4 +103,8 @@ def decoder_kwargs(args, tokenizer=None):
         if tokenizer is None:
             raise ValueError("vlp_b200: --constraints needs a tokenizer to map its words to wordpiece ids")
         kw["constraints"] = [[list(tokenizer.convert_tokens_to_ids(tokenizer.tokenize(a))) for a in c] for c in args.constraints]
+    if getattr(args, "prompt", None) is not None:
+        if tokenizer is None:
+            raise ValueError("vlp_b200: --prompt needs a tokenizer to map its words to wordpiece ids")
+        kw["prompt"] = list(tokenizer.convert_tokens_to_ids(tokenizer.tokenize(args.prompt)))
     return kw

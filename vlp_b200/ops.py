@@ -711,13 +711,26 @@ SAMPLE_MODES = {"topk": 0, "topp": 1}
 MAX_TOPK = 64
 
 
+def _prompt_rows(prompt, rows):
+    """prompt = (hist_off, eos_until): the VlpkPromptRows of a prompted selector call; eos_until an int32 device tensor [rows] or
+    None."""
+    hist_off, eos_until = prompt
+    if eos_until is not None:
+        _require_cuda(eos_until, "[EOS] block lengths")
+        if eos_until.dtype != torch.int32 or eos_until.shape != (rows,) or not eos_until.is_contiguous():
+            raise RuntimeError(f"vlp_b200: [EOS] block lengths must be a contiguous int32 [{rows}] tensor")
+    return L.VlpkPromptRows(hist_off=int(hist_off), eos_until=L.ptr(eos_until))
+
+
 def sample_tokens(logits, bias, mode, topk, topp, seed, f, seq, score, finished, live, eos_id, pad_id=0, block_eos=False, ngram=0,
-                  ignore=None):
+                  ignore=None, prompt=None):
     """One frame of top-k / top-p sampling (vlpk_sample_tokens): for every row of logits ([rows, ..., V], unit stride in V, bf16 or
     fp32, without the head's bias), adds bias ([V], same dtype, or None), blocks the duplicate n-grams of the row's history
     seq[row, :f] when ngram > 0 and [EOS] when block_eos, keeps the top-k words or the top-p nucleus and draws one with the
     Philox uniform keyed by (seed; f, row).  seq: int64 [rows, T] receives column f; score: fp32 [rows, T] or None; finished: int32
-    [rows]; live: int32 [1], decremented once per row that draws eos_id.  ignore: int32 device tensor of exempt word ids, or None."""
+    [rows]; live: int32 [1], decremented once per row that draws eos_id.  ignore: int32 device tensor of exempt word ids, or None.
+    prompt: (hist_off, eos_until) for a prompted decode (vlpk_sample_tokens_prompt): seq[:, :hist_off] holds the rows' prompt
+    histories, f = hist_off + g, the draw is keyed by (seed; g, row) and eos_until [rows] replaces block_eos."""
     _require_cuda_all((logits, "logits"), (seq, "sampled ids"), (finished, "finished flags"), (live, "live-row count"),
                       (bias, "logit bias"), (score, "scores"), (ignore, "n-gram ignore set"))
     if mode not in SAMPLE_MODES:
@@ -731,6 +744,12 @@ def sample_tokens(logits, bias, mode, topk, topp, seed, f, seq, score, finished,
     if finished.dtype != torch.int32 or finished.shape != (rows,) or live.dtype != torch.int32 or live.numel() != 1:
         raise RuntimeError("vlp_b200: finished flags must be int32 [rows] and the live-row count an int32 [1] tensor")
     ign, n_ign = _ignore_set(ignore)
+    if prompt is not None:
+        L.call("vlpk_sample_tokens_prompt", rows, V, lg.data_ptr(), lg.stride(0), L.ptr(bias), int(logits.dtype == torch.float32),
+               SAMPLE_MODES[mode], int(topk), float(topp), int(seed) & 0xFFFFFFFFFFFFFFFF, int(f), seq.data_ptr(), seq.shape[1],
+               L.ptr(score), finished.data_ptr(), live.data_ptr(), int(eos_id), int(pad_id), int(ngram), ign, n_ign,
+               L.C.byref(_prompt_rows(prompt, rows)), L.stream())
+        return
     L.call("vlpk_sample_tokens", rows, V, lg.data_ptr(), lg.stride(0), L.ptr(bias), int(logits.dtype == torch.float32), SAMPLE_MODES[mode],
            int(topk), float(topp), int(seed) & 0xFFFFFFFFFFFFFFFF, int(f), seq.data_ptr(), seq.shape[1], L.ptr(score), finished.data_ptr(),
            live.data_ptr(), int(eos_id), int(pad_id), int(bool(block_eos)), int(ngram), ign, n_ign, L.stream())
@@ -740,13 +759,15 @@ def sample_tokens(logits, bias, mode, topk, topp, seed, f, seq, score, finished,
 # diverse beam search
 # ------------------------------------------------------------------------------------------------
 def diverse_beam_step(logits, bias, f, G, penalty, wid, ptr, score, eos, top_w, top_lp, eos_id, block_eos=False, ngram=0, ignore=None,
-                      hist_in=None, hist_out=None):
+                      hist_in=None, hist_out=None, prompt=None):
     """The selection of diverse-beam frame f (vlpk_diverse_beam_step): K beams per image in G groups with a Hamming penalty.  logits:
     the head's decoder outputs without its bias, [rows, ..., V] with unit stride in V, bf16 or fp32, rows = B at f = 0 and B*K after;
     bias: [V] of the same dtype, or None.  wid / ptr (int64) and score / eos (fp32): the traces, contiguous [T, B, K]; frame f is
     written and frame f-1 read.  top_w (int32) / top_lp (fp32): contiguous [B*K, K] scratch.  ngram > 0: duplicate-n-gram blocking
     over the int32 [B*K, T_cap] histories hist_in (frame f-1) and hist_out (frame f), two different tensors used in turn; ignore:
-    int32 device tensor of exempt word ids, or None.  block_eos: the frame is below min_len."""
+    int32 device tensor of exempt word ids, or None.  block_eos: the frame is below min_len.
+    prompt: (hist_off, eos_until) for a prompted decode (vlpk_diverse_beam_step_prompt): histories of hist_off + f entries, at f = 0
+    hist_in [B, T_cap] (the images' prompt histories), and eos_until [rows] in place of block_eos."""
     _require_cuda_all((logits, "logits"), (wid, "beam word ids"), (ptr, "beam back pointers"), (score, "beam scores"),
                       (eos, "beam eos flags"), (top_w, "top-K scratch"), (top_lp, "top-K scratch"), (bias, "logit bias"),
                       (ignore, "n-gram ignore set"), (hist_in, "n-gram history"), (hist_out, "n-gram history"))
@@ -756,8 +777,18 @@ def diverse_beam_step(logits, bias, f, G, penalty, wid, ptr, score, eos, top_w, 
     if top_w.dtype != torch.int32 or top_lp.dtype != torch.float32 or top_w.shape != (B * K, K) or top_lp.shape != (B * K, K) \
             or not (top_w.is_contiguous() and top_lp.is_contiguous()):
         raise RuntimeError("vlp_b200: the top-K scratch must be contiguous int32 and fp32 [B*K, K] tensors")
-    T_cap = _check_histories(hist_in, hist_out, B * K, "n-gram", "B*K") if ngram else T
+    if prompt is not None and f == 0 and ngram:
+        T_cap = _check_histories(hist_in, hist_in, B, "prompt", "B")
+    else:
+        T_cap = _check_histories(hist_in, hist_out, B * K, "n-gram", "B*K") if ngram else T + (0 if prompt is None else int(prompt[0]))
     ign, n_ign = _ignore_set(ignore, used=bool(ngram))
+    if prompt is not None:
+        L.call("vlpk_diverse_beam_step_prompt", B, K, int(G), int(f), V, lg.data_ptr(), lg.stride(0), L.ptr(bias),
+               int(logits.dtype == torch.float32), float(penalty), int(eos_id), T_cap, int(ngram), L.ptr(hist_in if ngram else None),
+               L.ptr(hist_out if ngram else None), ign, n_ign, *(L.ptr(t) for t in prev), top_w.data_ptr(), top_lp.data_ptr(),
+               wid[f].data_ptr(), ptr[f].data_ptr(), score[f].data_ptr(), eos[f].data_ptr(),
+               L.C.byref(_prompt_rows(prompt, B if f == 0 else B * K)), L.stream())
+        return
     L.call("vlpk_diverse_beam_step", B, K, int(G), int(f), V, lg.data_ptr(), lg.stride(0), L.ptr(bias), int(logits.dtype == torch.float32),
            float(penalty), int(eos_id), int(bool(block_eos)), T_cap, int(ngram), L.ptr(hist_in if ngram else None),
            L.ptr(hist_out if ngram else None), ign, n_ign, *(L.ptr(t) for t in prev), top_w.data_ptr(), top_lp.data_ptr(),
@@ -768,14 +799,16 @@ def diverse_beam_step(logits, bias, f, G, penalty, wid, ptr, score, eos, top_w, 
 # constrained beam search
 # ------------------------------------------------------------------------------------------------
 def constrained_beam_step(logits, bias, f, cons, wid, ptr, score, eos, top_w, top_lp, top_dest, eos_id, block_eos=False, ngram=0, ignore=None,
-                          hist_in=None, hist_out=None):
+                          hist_in=None, hist_out=None, prompt=None):
     """The selection of constrained-beam frame f (vlpk_constrained_beam_step): K beams in each of the S = 2^C constraint states of an
     image.  logits: the head's decoder outputs without its bias, [rows, ..., V] with unit stride in V, bf16 or fp32, rows = B at f = 0
     and B*S*K after; bias: [V] of the same dtype, or None.  cons: contiguous int64 [B, C, A, P] constraint table.  wid / ptr (int64)
     and score / eos (fp32): the traces, contiguous [T, B, S*K]; frame f is written and frame f-1 read.  top_w (int32) / top_lp (fp32):
     contiguous [B*S*K, K + C*A] scratch, top_dest (int32) [B*S*K, C*A].  hist_in / hist_out: the int32 [B*S*K, T_cap] histories of
     frames f-1 and f, two different tensors used in turn (needed at f >= 1, whatever ngram).  ngram > 0: duplicate-n-gram blocking;
-    ignore: int32 device tensor of exempt word ids, or None.  block_eos: the frame is below min_len."""
+    ignore: int32 device tensor of exempt word ids, or None.  block_eos: the frame is below min_len.
+    prompt: (hist_off, eos_until) for a prompted decode (vlpk_constrained_beam_step_prompt): histories of hist_off + f entries, at
+    f = 0 hist_in [B, T_cap] (the images' prompt histories), and eos_until [rows] in place of block_eos."""
     _require_cuda_all((logits, "logits"), (cons, "constraint table"), (wid, "beam word ids"), (ptr, "beam back pointers"),
                       (score, "beam scores"), (eos, "beam eos flags"), (top_w, "top-K scratch"), (top_lp, "top-K scratch"),
                       (top_dest, "top-K scratch"), (bias, "logit bias"), (ignore, "n-gram ignore set"), (hist_in, "word history"),
@@ -795,7 +828,10 @@ def constrained_beam_step(logits, bias, f, cons, wid, ptr, score, eos, top_w, to
             or top_lp.shape != (B * SK, W) or top_dest.shape != (B * SK, C * A) \
             or not (top_w.is_contiguous() and top_lp.is_contiguous() and top_dest.is_contiguous()):
         raise RuntimeError("vlp_b200: the top-K scratch must be contiguous int32 / fp32 [B*S*K, K + C*A] and int32 [B*S*K, C*A] tensors")
-    T_cap = _check_histories(hist_in, hist_out, B * SK, "word", "B*S*K") if hist_out is not None or f else T
+    if prompt is not None and f == 0:
+        T_cap = _check_histories(hist_in, hist_in, B, "prompt", "B")
+    else:
+        T_cap = _check_histories(hist_in, hist_out, B * SK, "word", "B*S*K") if hist_out is not None or f else T
     ign, n_ign = _ignore_set(ignore, used=bool(ngram))
     a = L.VlpkConstrainedBeamArgs(B=B, K=K, C=C, A=A, P=P, f=int(f), V=V, logits=lg.data_ptr(), ld=lg.stride(0), bias=L.ptr(bias),
                                   fp32=int(logits.dtype == torch.float32), eos_id=int(eos_id), block_eos=int(bool(block_eos)), T_cap=T_cap,
@@ -803,4 +839,7 @@ def constrained_beam_step(logits, bias, f, cons, wid, ptr, score, eos, top_w, to
                                   cons=cons.data_ptr(), prev_wid=L.ptr(prev[0]), prev_ptr=L.ptr(prev[1]), prev_score=L.ptr(prev[2]),
                                   prev_eos=L.ptr(prev[3]), top_w=top_w.data_ptr(), top_lp=top_lp.data_ptr(), top_dest=top_dest.data_ptr(),
                                   wid=wid[f].data_ptr(), ptr=ptr[f].data_ptr(), score=score[f].data_ptr(), eos=eos[f].data_ptr())
+    if prompt is not None:
+        L.call("vlpk_constrained_beam_step_prompt", L.C.byref(a), L.C.byref(_prompt_rows(prompt, B if f == 0 else B * SK)), L.stream())
+        return
     L.call("vlpk_constrained_beam_step", L.C.byref(a), L.stream())

@@ -24,7 +24,8 @@ from torch import nn
 from . import ops
 from .staging import GroupedCaptionMask
 from .beam import beam_search, constrained_beam_search, diverse_beam_search
-from .decode import check_constraints, check_decode, constraint_table, greedy_decode, sample_decode
+from .decode import (check_constraints, check_decode, check_prompt, check_prompt_mode, constraint_table, greedy_decode, prompt_table,
+                     sample_decode)
 from .score import score_caption_matrix, score_captions
 
 logger = logging.getLogger(__name__)
@@ -915,7 +916,7 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
 
     def __init__(self, config, mask_word_id=0, num_labels=2, search_beam_size=1, length_penalty=1.0, eos_id=0, forbid_duplicate_ngrams=False,
                  forbid_ignore_set=None, ngram_size=3, min_len=0, enable_butd=False, len_vis_input=49, sampling_method="beam_search", topk=1,
-                 topp=1.0, seed=0, num_return_sequences=1, num_beam_groups=1, diversity_penalty=0.0, constraints=None):
+                 topp=1.0, seed=0, num_return_sequences=1, num_beam_groups=1, diversity_penalty=0.0, constraints=None, prompt=None):
         super().__init__(config)
         self.bert = BertModelIncr(config)
         self.cls = BertPreTrainingHeads(config, self.bert.embeddings.word_embeddings.weight, num_labels=num_labels)
@@ -942,6 +943,10 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         self.constraints = None if constraints is None else constraint_table(constraints)
         if self.constraints is not None:
             check_constraints(self.constraints, config.vocab_size, search_beam_size)
+        # prompt: a list of word ids every caption starts with (prompted decode); forward's `prompt_ids` overrides it per call.
+        self.prompt = None if prompt is None else prompt_table(prompt)
+        if self.prompt is not None and self.prompt.shape[1]:
+            check_prompt_mode(sampling_method, num_beam_groups, constraints is not None)
         self.sampling_method, self.topk, self.topp, self.seed = sampling_method, topk, topp, seed
         self.num_return_sequences = num_return_sequences
         self.num_beam_groups, self.diversity_penalty = num_beam_groups, diversity_penalty
@@ -954,7 +959,7 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         return [torch.empty(batch, rows, 2 * H, device=device, dtype=torch.bfloat16) for _ in self.bert.encoder.layer]
 
     def forward(self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx=None, sample_mode="greedy",
-                seed=None, output_attentions=False, constraints=None):
+                seed=None, output_attentions=False, constraints=None, prompt_ids=None):
         """seed: the sampling seed of this call (sampling_method "topk" / "topp"); None uses self.seed.
         output_attentions: greedy / sample / top-k / top-p decode return (ids, scores, attentions) and beam search adds
         out["attentions"]: fp32 [B, out_len - in_len, layers, heads, out_len], for every output word the attention probabilities of the
@@ -966,7 +971,16 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
         constraints: int64 [B, C, A, P] (or [1, C, A, P] for every image), 0-padded word ids, this call's constraints in place of
         the constructor's: constrained beam search, whose out also holds out["constraints_met"] bool [B], out["state_seq"] int64
         [B, 2^C, out_len] and out["state_scores"] fp32 [B, 2^C] (beam.constrained_beam_search).  A device tensor's ids are checked
-        from a host copy, except while a CUDA graph is being captured."""
+        from a host copy, except while a CUDA graph is being captured.
+        prompt_ids: int64 [B, Tp] (or [1, Tp] for every image), this call's prompt in place of the constructor's: row b holds the t_b
+        words image b's caption starts with, then 0-padding (ragged lengths, t_b = 0 included).  Every decode mode continues each
+        prompt: step 0 runs the prompts' columns in the prefill (decode.DecodeState), every image
+        generates up to out_len - in_len - Tp words, the n-gram blocking and min_len count the prompt as the caption's first words,
+        and ids / pred_seq / nbest_seq hold the t_b prompt words (per-word score 0), then the generated words, then 0.  The beam
+        traces and scores are those of the generated words.  None, or width 0, is the unprompted decode.  ValueError (before any
+        launch, ids checked as constraints are) for ids outside [1, V), eos_id or mask_word_id in a prompt, a 0 before a word, a row
+        count other than 1 or B, Tp >= out_len - in_len, use_kv_cache False and output_attentions.  Sampling draws stay keyed by
+        (seed; generated word, row); a constraint the prompt contains is met from the start."""
         self.cls.predictions.check_task_idx(task_idx)          # before anything is launched
         _check_seq_len(self.config, token_type_ids.size(1))
         cons = self.constraints if constraints is None else constraints
@@ -975,18 +989,39 @@ class BertForSeq2SeqDecoder(PreTrainedBertModel, _RegionProjections):
                      num_beam_groups=self.num_beam_groups, diversity_penalty=self.diversity_penalty, constraints=cons is not None)
         if cons is not None:
             cons = self._constraint_tensor(cons, constraints is None, input_ids, token_type_ids.size(1) - input_ids.size(1))
+        prompt = self.prompt if prompt_ids is None else prompt_ids
+        if prompt is not None:
+            prompt = self._prompt_tensor(prompt, prompt_ids is None, input_ids, token_type_ids.size(1) - input_ids.size(1), cons is not None,
+                                         output_attentions)
         with torch.no_grad():
             vis_feats, vis_pe = self.project_regions(vis_feats, vis_pe)
             inputs = (self, vis_feats, vis_pe, input_ids, token_type_ids, position_ids, attention_mask, task_idx)
             if self.sampling_method != "beam_search":
-                return sample_decode(*inputs, seed, output_attentions=output_attentions)
+                return sample_decode(*inputs, seed, output_attentions=output_attentions, prompt=prompt)
             if cons is not None:
-                return constrained_beam_search(*inputs[:-1], cons, task_idx, output_attentions=output_attentions)
+                return constrained_beam_search(*inputs[:-1], cons, task_idx, output_attentions=output_attentions, prompt=prompt)
             if self.num_beam_groups > 1:
-                return diverse_beam_search(*inputs, output_attentions=output_attentions)
+                return diverse_beam_search(*inputs, output_attentions=output_attentions, prompt=prompt)
             if self.search_beam_size > 1:
-                return beam_search(*inputs, output_attentions=output_attentions)
-            return greedy_decode(*inputs, sample_mode, output_attentions=output_attentions)
+                return beam_search(*inputs, output_attentions=output_attentions, prompt=prompt)
+            return greedy_decode(*inputs, sample_mode, output_attentions=output_attentions, prompt=prompt)
+
+    def _prompt_tensor(self, prompt, shared, input_ids, max_words, constrained, output_attentions):
+        """Checks a prompt and returns it as a contiguous int64 [B, Tp] tensor on the decode's device, or None for width 0 (the
+        unprompted decode).  The constructor's prompt (shared) is copied to each device once and kept, as the constraint table is."""
+        B, dev = input_ids.size(0), input_ids.device
+        capturing = dev.type == "cuda" and torch.cuda.is_current_stream_capturing()
+        check_prompt(prompt, B, self.config.vocab_size, max_words, self.eos_id, self.mask_word_id, values=not capturing)
+        if prompt.size(1) == 0:
+            return None
+        check_prompt_mode(self.sampling_method, self.num_beam_groups, constrained, self.use_kv_cache, output_attentions)
+        if shared:
+            cache = self.__dict__.setdefault("_prompt_cache", {})
+            key = (str(dev), tuple(prompt.flatten().tolist()), tuple(prompt.shape))
+            if key not in cache:
+                cache[key] = prompt.to(dev)
+            prompt = cache[key]
+        return prompt.to(dev).expand(B, prompt.size(1)).contiguous()
 
     def _constraint_tensor(self, cons, shared, input_ids, max_words):
         """Checks a constraint table and returns it as a contiguous int64 [B, C, A, P] tensor on the decode's device.  The
