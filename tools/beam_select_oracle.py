@@ -18,8 +18,10 @@ expf's 2 ulp and the rounding of x - mx (together (4 + |x - mx|) * 2^-24 relativ
 A row with a NaN or +inf x, or whose every x is -inf, has a NaN L: every lp is NaN (but a block_eos [EOS]).
 
 carry states the history carry (carry_history): hist_out[i] = hist_in[(i / width) * width + p] ‖ prev_wid[i], p = prev_ptr[i] (0 at
-f = 1); a pointer outside [0, width) gives -1 words and an id outside int32 gives -1.  The merges are diverse_beam_oracle.merge and
-constrained_beam_oracle.merge, fp32-exact already.  Nothing here calls the kernels or reads the reference."""
+f = 1); a pointer outside [0, width) gives -1 words and an id outside int32 gives -1.  prompt_carry states the prompted rows'
+history (prompt_history): hist_off prompt entries, then the generated words; eos_blocked the prompted rows' [EOS] rule.  The merges
+are diverse_beam_oracle.merge and constrained_beam_oracle.merge, fp32-exact already.  Nothing here calls the kernels or reads the
+reference."""
 import math
 
 import numpy as np
@@ -181,6 +183,25 @@ def carry(hist_in, prev_ptr, prev_wid, width, f):
         out[:, :f - 1] = np.where(ok[:, None], np.asarray(hist_in, dtype=np.int64)[src, :f - 1], -1)
     out[:, f - 1] = to_word(prev_wid)
     return out
+
+
+def prompt_carry(hist_in, prev_ptr, prev_wid, width, f, hist_off):
+    """The history of a prompted row at trace frame f, hist_off + f entries: at f = 0 row i is hist_in[i, :hist_off] (one row per
+    image, its prompt right-aligned behind -1 entries); at f >= 1 it is carry(..., hist_off + f), so prev_ptr is read whenever
+    hist_off + f > 1 (from f = 1 on when hist_off > 0)."""
+    if f == 0:
+        return np.asarray(hist_in, dtype=np.int64)[:, :hist_off].copy()
+    return carry(hist_in, prev_ptr, prev_wid, width, hist_off + f)
+
+
+def eos_blocked(eos_until, g, rows):
+    """bool [rows]: the prompted rows whose [EOS] is blocked at generated word g: g + 1 <= eos_until[i]; none when eos_until is
+    None (never blocked, whatever an unprompted call's block_eos would say)."""
+    if eos_until is None:
+        return np.zeros(rows, bool)
+    e = np.asarray(eos_until, dtype=np.int64).reshape(-1)
+    assert e.size == rows, (e.size, rows)
+    return g + 1 <= e
 
 
 def ngram_blocked(hists, n, ignore, V):

@@ -510,7 +510,7 @@ __device__ __forceinline__ void diverse_rows(const DiverseBeamArgs& a, const Pro
       if (hf >= a.n) blocked = ngram_candidates(hist, hf, a.n, V, a.ignore, a.n_ignore, bits);
     }
     DiverseBeamArgs b = a;
-    if (p.eos_until) b.block_eos = a.f + 1 <= p.eos_until[row];
+    b.block_eos = p.eos_until && a.f + 1 <= p.eos_until[row];         // eos_until alone: NULL never blocks
     row_logp<T>(b, row, blocked, bits, val, redf);
   } else {
     if (a.n > 0 && a.f >= 1) {                                       // uniform
@@ -668,7 +668,7 @@ __device__ __forceinline__ void constrained_rows(const VlpkConstrainedBeamArgs& 
 
   if constexpr (PROMPT) {
     VlpkConstrainedBeamArgs e = a;
-    if (p.eos_until) e.block_eos = f + 1 <= p.eos_until[row];
+    e.block_eos = p.eos_until && f + 1 <= p.eos_until[row];           // eos_until alone: NULL never blocks, whatever args.block_eos
     row_logp<T>(e, row, blocked, bits, val, redf);
   } else {
     row_logp<T>(a, row, blocked, bits, val, redf);

@@ -52,7 +52,7 @@ struct SampleArgs {
 };
 
 // Prompted rows of the row kernels (vlpk.h, VlpkPromptRows): histories start with hist_off prompt entries, and [EOS] is blocked per
-// row while the generated word's frame g satisfies g + 1 <= eos_until[row] (eos_until null: block_eos as without a prompt).
+// row while the generated word's frame g satisfies g + 1 <= eos_until[row] (eos_until null: never; the args' block_eos is not read).
 struct PromptRows {
   int hist_off = 0;
   const int* eos_until = nullptr;

@@ -711,9 +711,11 @@ SAMPLE_MODES = {"topk": 0, "topp": 1}
 MAX_TOPK = 64
 
 
-def _prompt_rows(prompt, rows):
+def _prompt_rows(prompt, rows, block_eos):
     """prompt = (hist_off, eos_until): the VlpkPromptRows of a prompted selector call; eos_until an int32 device tensor [rows] or
-    None."""
+    None (never blocked).  A prompted call takes its [EOS] block from eos_until alone: ValueError for block_eos with a prompt."""
+    if block_eos:
+        raise ValueError("vlp_b200: a prompted selector blocks [EOS] by eos_until (prompt[1]), not block_eos")
     hist_off, eos_until = prompt
     if eos_until is not None:
         _require_cuda(eos_until, "[EOS] block lengths")
@@ -730,7 +732,8 @@ def sample_tokens(logits, bias, mode, topk, topp, seed, f, seq, score, finished,
     Philox uniform keyed by (seed; f, row).  seq: int64 [rows, T] receives column f; score: fp32 [rows, T] or None; finished: int32
     [rows]; live: int32 [1], decremented once per row that draws eos_id.  ignore: int32 device tensor of exempt word ids, or None.
     prompt: (hist_off, eos_until) for a prompted decode (vlpk_sample_tokens_prompt): seq[:, :hist_off] holds the rows' prompt
-    histories, f = hist_off + g, the draw is keyed by (seed; g, row) and eos_until [rows] replaces block_eos."""
+    histories, f = hist_off + g, the draw is keyed by (seed; g, row) and eos_until [rows] (or None: never) replaces block_eos,
+    which must then be False."""
     _require_cuda_all((logits, "logits"), (seq, "sampled ids"), (finished, "finished flags"), (live, "live-row count"),
                       (bias, "logit bias"), (score, "scores"), (ignore, "n-gram ignore set"))
     if mode not in SAMPLE_MODES:
@@ -748,7 +751,7 @@ def sample_tokens(logits, bias, mode, topk, topp, seed, f, seq, score, finished,
         L.call("vlpk_sample_tokens_prompt", rows, V, lg.data_ptr(), lg.stride(0), L.ptr(bias), int(logits.dtype == torch.float32),
                SAMPLE_MODES[mode], int(topk), float(topp), int(seed) & 0xFFFFFFFFFFFFFFFF, int(f), seq.data_ptr(), seq.shape[1],
                L.ptr(score), finished.data_ptr(), live.data_ptr(), int(eos_id), int(pad_id), int(ngram), ign, n_ign,
-               L.C.byref(_prompt_rows(prompt, rows)), L.stream())
+               L.C.byref(_prompt_rows(prompt, rows, block_eos)), L.stream())
         return
     L.call("vlpk_sample_tokens", rows, V, lg.data_ptr(), lg.stride(0), L.ptr(bias), int(logits.dtype == torch.float32), SAMPLE_MODES[mode],
            int(topk), float(topp), int(seed) & 0xFFFFFFFFFFFFFFFF, int(f), seq.data_ptr(), seq.shape[1], L.ptr(score), finished.data_ptr(),
@@ -787,7 +790,7 @@ def diverse_beam_step(logits, bias, f, G, penalty, wid, ptr, score, eos, top_w, 
                int(logits.dtype == torch.float32), float(penalty), int(eos_id), T_cap, int(ngram), L.ptr(hist_in if ngram else None),
                L.ptr(hist_out if ngram else None), ign, n_ign, *(L.ptr(t) for t in prev), top_w.data_ptr(), top_lp.data_ptr(),
                wid[f].data_ptr(), ptr[f].data_ptr(), score[f].data_ptr(), eos[f].data_ptr(),
-               L.C.byref(_prompt_rows(prompt, B if f == 0 else B * K)), L.stream())
+               L.C.byref(_prompt_rows(prompt, B if f == 0 else B * K, block_eos)), L.stream())
         return
     L.call("vlpk_diverse_beam_step", B, K, int(G), int(f), V, lg.data_ptr(), lg.stride(0), L.ptr(bias), int(logits.dtype == torch.float32),
            float(penalty), int(eos_id), int(bool(block_eos)), T_cap, int(ngram), L.ptr(hist_in if ngram else None),
@@ -840,6 +843,7 @@ def constrained_beam_step(logits, bias, f, cons, wid, ptr, score, eos, top_w, to
                                   prev_eos=L.ptr(prev[3]), top_w=top_w.data_ptr(), top_lp=top_lp.data_ptr(), top_dest=top_dest.data_ptr(),
                                   wid=wid[f].data_ptr(), ptr=ptr[f].data_ptr(), score=score[f].data_ptr(), eos=eos[f].data_ptr())
     if prompt is not None:
-        L.call("vlpk_constrained_beam_step_prompt", L.C.byref(a), L.C.byref(_prompt_rows(prompt, B if f == 0 else B * SK)), L.stream())
+        rows = _prompt_rows(prompt, B if f == 0 else B * SK, block_eos)
+        L.call("vlpk_constrained_beam_step_prompt", L.C.byref(a), L.C.byref(rows), L.stream())
         return
     L.call("vlpk_constrained_beam_step", L.C.byref(a), L.stream())
